@@ -9,6 +9,7 @@ Contract (see the task statement): `python bench.py --gpus N --steps K --warmup 
   vq           : the second headline metric (VQ argmin GB/s, algorithmic bytes) measured live
   cpu_baseline : the CPU oracle (a restatement of the reference; kind "port") timed on this box's host cores
 `--impl reference` times that same CPU implementation alone and prints the line with "impl": "reference".
+`--dump-outputs DIR` writes what the last timed step computed (decoder output, losses, parameter gradients) as DIR/<name>.npy.
 Workload = BASELINE.json configs[1]; synthetic data (torch.rand images, seeded default-init weights, N(0,1) codebook,
 q_counter past the re-init window so the real VQ branch runs — SURVEY.md 8d). Proxy loss: L1 + codebook term.
 """
@@ -40,11 +41,12 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], bf16=d["bf16_tflops"], bf16_sustained=d["bf16_tflops_sustained"], src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, src="fallback")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 / FP16; never reached, only a scale
+    return dict(hbm=3350.0, bf16=989.0, bf16_sustained=989.0, src="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks/throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -225,7 +227,7 @@ def dominant_kernel_roofline(dev, pk):
         y = torch.empty_like(x)
         wt = ops._packed_conv_weight(w, w, 128, 128, False, dev, False, True)
         fn = lambda: L.call("mas_conv3x3_fprop_tc16h", x16, L.t4(x16), wt, b, None, y, L.t4(y), None, None)
-        main = entry("shift_gemm_t16 (TMA-fed tcgen05 kind::f16, fp32 accumulate) conv3x3 128->128 @256^2 x32",
+        main = entry("shift_gemm_t16 (TMA-fed wgmma fp16, fp32 accumulate) conv3x3 128->128 @256^2 x32",
                      time_kernel(fn, iters=6, warm=3), 2.0 * BATCH * RES * RES * 128 + 4.0 * BATCH * RES * RES * 128 + wbytes,
                      "conv3x3_tma_128_128_256_bytes_per_launch")
         dy = torch.randn(BATCH, 128, RES, RES, device=dev).contiguous(memory_format=torch.channels_last) * 1e-6
@@ -240,7 +242,7 @@ def dominant_kernel_roofline(dev, pk):
     xa = ops.amax(x) if fmt == "f16" else None
     fn = lambda: ops.conv3x3_raw(x, w, b, None, L.CONV_S1, x_amax=xa)
     kname = {"f16": "shift_gemm_tc<9,f16> (register-staged fp16 operands; strided / upsampling / unshadowed layers)",
-             "tf32": "shift_gemm_tc<9> (tcgen05 TF32)", "fp32": "conv_fprop_simt (fp32 FFMA)"}[fmt] + " conv3x3 128->128 @256^2 x32"
+             "tf32": "shift_gemm_tc<9> (wgmma TF32)", "fp32": "conv_fprop_simt (fp32 FFMA)"}[fmt] + " conv3x3 128->128 @256^2 x32"
     staged = entry(kname, time_kernel(fn, iters=6, warm=3), 4.0 * BATCH * RES * RES * 256 + 4 * 128 * 128 * 9,
                    "conv3x3_128_128_256_bytes_per_launch")
     if fmt == "f16" and ops.conv_tma_on():
@@ -253,8 +255,8 @@ def dominant_kernel_roofline(dev, pk):
 
 def attn_metric(dev, pk):
     """AttnBlock (modules.py:139-191) at the model's shape: batch 32, C = 512, 16x16 tokens; forward and backward of the
-    whole block (GroupNorm, q/k/v and proj_out 1x1 GEMMs on TF32 tcgen05, the fused QK^T -> softmax -> PV core, the four
-    gradients of the two contractions on the 3xTF32 tcgen05 GEMM, residual, next-norm statistics). Algorithmic FLOPs per image forward: 0.671 GFLOP
+    whole block (GroupNorm, q/k/v and proj_out 1x1 GEMMs on TF32 wgmma, the fused QK^T -> softmax -> PV core, the four
+    gradients of the two contractions on the 3xTF32 wgmma GEMM, residual, next-norm statistics). Algorithmic FLOPs per image forward: 0.671 GFLOP
     (SURVEY.md 8d), backward = 2x; the 3xTF32 passes are not counted."""
     from models import modules as M
     torch.manual_seed(0)
@@ -279,7 +281,7 @@ def ffma_peak(dev):
     """fp32 FMA-pipe peak measured live (mas_ffma_probe, CUDA events): the roofline of the exact-fp32 VQ distance kernel."""
     import ctypes
     from mas_b200 import _lib as L
-    scratch = torch.empty(148 * 4 * 512, device=dev)
+    scratch = torch.empty(132 * 4 * 512, device=dev)
     fl = ctypes.c_double(0.0)
     fn = lambda: L.call("mas_ffma_probe", scratch, 2048, ctypes.cast(ctypes.pointer(fl), ctypes.c_void_p))
     sec = time_kernel(fn, iters=5, warm=2)
@@ -324,7 +326,7 @@ def vq_metric(dev, pk, sweep=True):
     return {"rows": at32["rows"], "ms": at32["ms"], "gb_per_s": at32["gb_per_s"], "tflop_per_s": at32["tflop_per_s"],
             "hbm_frac": at32["hbm_frac"], "ffma_frac": at32["ffma_frac"], "tensor_frac_3pass": at32["tensor_frac_3pass"],
             "ffma_peak_tflops_measured": round(peak, 2),
-            "kernel": "vq_filter_tc (tcgen05 kind::f16, 2 x fp16 operand split) + vq_resolve (exact fp32 re-evaluation)",
+            "kernel": "vq_filter_tc (wgmma fp16, 2 x fp16 operand split) + vq_resolve (exact fp32 re-evaluation)",
             "bound": "tensor pipe for the filter (3 MMAs per K step); an exact all-pairs evaluation is bound by the fp32 FFMA pipe",
             "all_pairs_ffma_kernel": exact, "sweep": pts}
 
@@ -402,7 +404,7 @@ def transformer_metric(dev, pk, batch=8, steps=3, warmup=2):
     return {"metric": "token transformer training step (fwd + cross-entropy + bwd), sequence tokens/s", "value": round(batch * S / sec, 1),
             "unit": "tokens/s", "batch": batch, "seq_len": S, "ms_per_step": round(sec * 1e3, 3), "loss": round(float(loss.detach()), 5),
             "model_tflops": round(flops / sec / 1e12, 1), "gpu_launches_per_step": (_lib.launch_count() - l0) // steps,
-            "tcgen05_launches_per_step": (_lib.tc_launch_count() - t0) // steps,
+            "tensor_core_launches_per_step": (_lib.tc_launch_count() - t0) // steps,
             "kernels": "rows_gemm_t16 / rows_wgrad_t16 (TMA-fed fp16 Linear layers), attn_causal_fwd (fused causal attention core), "
                        "gemm3_tc (3xTF32 attention gradients, causal block skipping), mas_ce_* (fused cross-entropy)",
             "kernel_rooflines": roofs}
@@ -411,6 +413,33 @@ def transformer_metric(dev, pk, batch=8, steps=3, warmup=2):
 def _fmt():
     from mas_b200 import ops
     return "fp16 (3x3 convolutions) / tf32 (1x1)" if ops.get_operand_format() == "f16" else "tf32"
+
+
+DUMP_BYTES = 64 << 20          # all arrays of --dump-outputs together
+DUMP_SAMPLE = 4096             # sampled entries per gradient (2048x that of a larger decoder output)
+
+
+def dump_outputs(path, last, model):
+    """What the timed path computed in its last step, as DIR/<name>.npy: decoder output `dec`, codebook loss `diff`, proxy
+    loss `loss` (only the gradients when the step was replayed from a CUDA graph), every parameter gradient's norm
+    `grad_norms` (float64, named-parameter order) and `grad_sample` (seeded positions). Inputs and weights are seeded, so two
+    builds run with the same arguments can be compared array for array."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    g = torch.Generator().manual_seed(2024)
+    pick = lambda t, k: t if t.numel() <= k else t[torch.randint(t.numel(), (k,), generator=g).to(t.device)]
+    out = {k: v.detach() if k == "dec" else v.detach().reshape(-1) for k, v in last.items()}
+    if "dec" in out and out["dec"].numel() > 2048 * DUMP_SAMPLE:
+        out["dec"] = pick(out["dec"].reshape(-1), 2048 * DUMP_SAMPLE)
+    grads = [prm.grad.detach().reshape(-1) for prm in model.parameters() if prm.grad is not None]
+    out["grad_norms"] = torch.stack([gr.double().norm() for gr in grads])
+    out["grad_sample"] = torch.cat([pick(gr, DUMP_SAMPLE) for gr in grads])
+    total = 0
+    for name, t in out.items():
+        a = t.cpu().numpy().astype(np.float64 if t.dtype == torch.float64 else np.float32)
+        total += a.nbytes
+        assert total <= DUMP_BYTES, "--dump-outputs: arrays exceed %d bytes" % DUMP_BYTES
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 def main():
@@ -426,6 +455,8 @@ def main():
     ap.add_argument("--profile", action="store_true", help="print per-entry-point CUDA-event times of one extra step")
     ap.add_argument("--step-only", action="store_true",
                     help="skip the per-kernel blocks (roofline / VQ sweep / AttnBlock / CPU baseline): launch-list captures under ncu")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write what the last timed step computed as DIR/<name>.npy (see dump_outputs)")
     ap.add_argument("--graph", action="store_true",
                     help="single GPU: replay the step from one CUDA graph (mas_b200.graph.GraphedStep) instead of launching from Python")
     args = ap.parse_args()
@@ -458,15 +489,19 @@ def main():
         img_host = torch.rand(B, 3, RES, RES, generator=gen).pin_memory()
     img_dev = img_host.to(dev)
 
+    last = {}
+
     def step(img):
         net.zero_grad(set_to_none=True)
         dec, diff = net(img)
+        last.update(dec=dec, diff=diff)
         if seg:
             from mas_b200 import ops
             loss = ops.BCELogitsFn.apply(dec, img, pos_w) + diff     # losses/loss_seg.py:15-22
         else:
             loss = (img - dec).abs().mean() + diff
         loss.backward()
+        last["loss"] = loss
         return loss
 
     def timed(fn, warmup, steps):
@@ -490,9 +525,8 @@ def main():
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
         return float(ms) * 1e-3, _lib.launch_count() - l0
 
-    # --graph (single GPU): the step is captured once into a CUDA graph (mas_b200.graph.GraphedStep) and replayed.  Measured
-    # on B200 at batch 32 it is within run-to-run noise of eager launching (the GPU is never starved: ~110 ms of kernels per
-    # step against ~45 ms of host launch work), so the default stays eager, which is also what the DDP runs (N > 1) use.
+    # --graph (single GPU): the step is captured once into a CUDA graph (mas_b200.graph.GraphedStep) and replayed; the default
+    # is eager launching, which is also what the DDP runs (N > 1) use.
     gs, graph_note = None, "eager (every kernel launched from Python through the C-ABI)"
     if world == 1 and args.graph:
         from mas_b200.graph import GraphedStep
@@ -517,6 +551,8 @@ def main():
     clocks = sampler.stop() if rank == 0 else None
     if gs is not None:
         launches = gs.launches_per_step * args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last, model)
 
     def e2e_step():
         if gs is not None:
@@ -549,11 +585,11 @@ def main():
     if seg:
         line = {"metric": SEG_METRIC, "value": value, "unit": "images/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
                 "ms_per_step": sec / args.steps * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-                "dtype": "%s tcgen05 operands, fp32 accumulate / storage" % _fmt(), "data": "synthetic",
+                "dtype": "%s wgmma operands, fp32 accumulate / storage" % _fmt(), "data": "synthetic",
                 "config": {"workload": "VQ-SEG 256x256, 159-channel maps, codebook=1024 dim=256, batch %d/GPU (BASELINE configs[3])" % B,
                            "global_batch": B * world, "parallelism": "dp%d" % world, "launch": graph_note,
                            "loss": "weighted BCE-with-logits (pos_weight 20 on channels 153-157) + codebook loss, kernels mas_bce_cl_*",
-                           "edge_layers": "159-channel conv_in / conv_out zero-padded to 160 / 2x128 channels on the fp16 tcgen05 kernels"},
+                           "edge_layers": "159-channel conv_in / conv_out zero-padded to 160 / 2x128 channels on the fp16 wgmma kernels"},
                 "e2e": {"value": e2e, "unit": "images/s", "h2d_bytes_per_step": B * 159 * RES * RES * 4, "d2h_bytes_per_step": 4,
                         "ms_per_step": sec_e2e / args.steps * 1e3},
                 "gpu_launches": int(launches), "clocks": clocks, "roofline": roof}
@@ -565,11 +601,11 @@ def main():
     attn = attn_metric(dev, pk)
     line = {"metric": METRIC, "value": value, "unit": "images/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": sec / args.steps * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
-            "dtype": "%s tcgen05 operands (11-bit significand), fp32 accumulate / storage; 3xTF32 for the attention contractions; fp32 FFMA for VQ argmin and edge layers" % _fmt(),
+            "dtype": "%s wgmma operands (11-bit significand), fp32 accumulate / storage; 3xTF32 for the attention contractions; fp32 FFMA for VQ argmin and edge layers" % _fmt(),
             "data": "synthetic",
             "config": {"workload": "VQ-IMG 256x256 codebook=8192 dim=256 batch %d/GPU (BASELINE configs[1])" % B,
                        "global_batch": B * world, "parallelism": "dp%d" % world, "launch": graph_note,
-                       "l2": "per-step working set >> 126 MB L2 (one 128x256x256 activation at batch 32 is 1.07 GB); no explicit flush",
+                       "l2": "per-step working set >> 50 MB L2 (one 128x256x256 activation at batch 32 is 1.07 GB); no explicit flush",
                        "optimizer": "excluded (metric is enc+VQ+dec fwd+bwd, BASELINE.md section 3)"},
             "e2e": {"value": e2e, "unit": "images/s", "h2d_bytes_per_step": B * 3 * RES * RES * 4, "d2h_bytes_per_step": 4,
                     "ms_per_step": sec_e2e / args.steps * 1e3},

@@ -1,4 +1,4 @@
-/* mas_b200.h — C-ABI of the B200-native VQ-IMG hot path (libmas_b200.so).
+/* mas_b200.h — C-ABI of the H100-native VQ-IMG hot path (libmas_b200.so).
  *
  * The reference (CasualGANPapers/Make-A-Scene) is pure Python/PyTorch and has NO native interface;
  * every arithmetic step of its hot path is a stock ATen/cuDNN/cuBLAS call issued from
@@ -38,10 +38,10 @@ extern "C" {
 #define MAS_CONV_ZS 3 /* zero-stuffed x2 input (data gradient of MAS_CONV_S2), stride 1 pad 1             */
 
 /* Implementation selector for the contraction kernels. */
-#define MAS_IMPL_AUTO 0  /* tcgen05 (TF32 operands, fp32 accumulate) when the shape is eligible, else SIMT */
+#define MAS_IMPL_AUTO 0  /* wgmma (TF32 operands, fp32 accumulate) when the shape is eligible, else SIMT */
 #define MAS_IMPL_SIMT 1  /* fp32 FFMA kernels (exact fp32; also the on-GPU checker for the tensor path)      */
-#define MAS_IMPL_TC 2    /* tcgen05 only; MAS_ERR_UNSUPPORTED if the shape is not eligible                   */
-#define MAS_IMPL_TC3 3   /* mas_gemm only, explicit selection: fp32-accurate 3xTF32 operand-split tcgen05 GEMM
+#define MAS_IMPL_TC 2    /* wgmma only; MAS_ERR_UNSUPPORTED if the shape is not eligible                   */
+#define MAS_IMPL_TC3 3   /* mas_gemm only, explicit selection: fp32-accurate 3xTF32 operand-split wgmma GEMM
                           * (csrc/contract_tc3.cu; the AttnBlock token contractions run on it)                  */
 
 typedef struct mas_tensor4 {
@@ -53,7 +53,7 @@ int mas_version(void);
 const char* mas_last_error(void);
 /* Number of kernels this library has launched in the calling process (bench.py's gpu_launches). */
 int64_t mas_launch_count(void);
-/* ... of which kernels that issue tcgen05 tensor-core MMAs (the driver's evidence that the tensor path ran). */
+/* ... of which kernels that issue wgmma tensor-core MMAs (the driver's evidence that the tensor path ran). */
 int64_t mas_tc_launch_count(void);
 
 /* Measurement aid for bench.py: runs a pure-FFMA kernel (16 independent chains per thread, 148*4 blocks of 512 threads,
@@ -106,7 +106,7 @@ int mas_pack_conv3x3(const float* w_oihw, float* w_packed, int Cout, int Cin, in
                      int round_tf32, void* stream);
 int mas_conv3x3_fprop(const float* x, mas_tensor4 xs, const float* w_packed, const float* bias,
                       const float* residual, float* y, mas_tensor4 ys, int mode, int impl, void* stream);
-/* Tensor-core (tcgen05, TF32 operands / fp32 accumulate in TMEM) form of the same convolution for dense NHWC
+/* Tensor-core (wgmma, TF32 operands / fp32 accumulate) form of the same convolution for dense NHWC
  * tensors with Cin % 8 == 0, Cout % 128 == 0, Hout % 16 == 0, Wout % 8 == 0 and mode S1 / UP / ZS
  * (mas_conv3x3_tc_eligible).  w_tc comes from mas_pack_conv3x3_tc (transpose=1: data-gradient operand with
  * flipped taps); the packed image is what one cp.async.bulk per pipeline stage drops into shared memory. */
@@ -121,7 +121,7 @@ int mas_pack_conv3x3_tc(const float* w_oihw, float* w_tc, int Cout, int Cin, int
 int mas_conv3x3_fprop_tc(const float* x, mas_tensor4 xs, const float* w_tc, const float* bias,
                          const float* residual, float* y, mas_tensor4 ys, int mode, const float* gn_table,
                          int gn_silu, float* stats_part, void* stream);
-/* fp16-operand form of the same kernel (tcgen05 kind::f16, fp32 accumulate): an fp16 significand has the 11 bits of a TF32
+/* fp16-operand form of the same kernel (wgmma kind::f16, fp32 accumulate): an fp16 significand has the 11 bits of a TF32
  * one, so the rounding of the operands is the same as on the TF32 path, while one MMA instruction (and one byte of
  * shared-memory operand traffic, the kernel's limiter) carries twice the FLOPs.  The narrower exponent range is handled by
  * a power-of-two operand scale derived ON THE DEVICE from x_amax (a device scalar holding max|x|, from mas_amax; NULL = no
@@ -175,14 +175,14 @@ int mas_gemm_rows_f16(const void* x_f16, int64_t M, int K, const void* w_tc16, f
 size_t mas_wgrad_rows_f16_ws_bytes(int64_t M, int N, int K);
 int mas_wgrad_rows_f16(const void* x_f16, const void* dy_f16, int64_t M, int N, int K, float* dw, float* dbias,
                        const float* x_amax, const float* dy_amax, void* ws, size_t ws_bytes, void* stream);
-/* Diagnostic: one tcgen05.mma D[128x32] = A[128x8].B[32x8]^T with A from shared memory (a_src=0) or tensor memory
+/* Diagnostic: wgmma D[128x32] = A[128x8].B[32x8]^T (TF32, 2 x m64) with A from shared memory (a_src=0) or registers
  * (a_src=1) and B K-major (b_layout=0) or MN-major (1; 2 = LBO/SBO fields swapped). Used by the tests to pin the
- * descriptor conventions the production kernels rely on. b_layout=99: B descriptor bits / instruction descriptor /
+ * descriptor conventions the production kernels rely on. b_layout=99: B descriptor bits (sm_100 encoding) /
  * start offset are taken verbatim from raw_* and the B region holds its own word indices (address reveal). */
 int mas_tc_probe(const float* A, const float* B, float* D, int a_src, int b_layout, uint64_t raw_desc,
                  uint32_t raw_idesc, int raw_off, void* stream);
 /* fp16 address-reveal form: D[k][n] (k < 16, n < 32; D is [128][32]) = index of the half the tensor core reads for element
- * (n, k) of a B operand described by the raw descriptor / instruction descriptor, from a region filled with 0..2047. */
+ * (n, k) of a B operand described by the raw descriptor (MN-major when bit 16 of raw_idesc is set), from a region filled with 0..2047. */
 int mas_tc_probe16(float* D, uint64_t raw_desc, uint32_t raw_idesc, int raw_off, void* stream);
 /* Weight gradient, written in the reference's [Cout,Cin,3,3] layout; dbias [Cout] may be NULL.
  * x is the convolution's (already normalised+activated) input, dy the output gradient. */
@@ -265,7 +265,7 @@ int mas_softmax_backward(const float* p, const float* dp, float* ds, int64_t row
  * reference layout ([C, C(,1,1)] row-major, biases [C]).  hn, qkv, P, O are outputs of the forward that the caller
  * keeps for the backward.  stats_part (or NULL): statistics partials of `out` for the next GroupNorm
  * ([N*HW/128][4][C/4][2], tensor path and HW % 128 == 0 only).  dqkv_w [3C, C] / dqkv_b [3C] hold the q, k, v gradients
- * back to back.  The 1x1 convolutions use the tcgen05 row GEMM / weight-gradient kernels when C % 128 == 0 (impl as
+ * back to back.  The 1x1 convolutions use the wgmma row GEMM / weight-gradient kernels when C % 128 == 0 (impl as
  * MAS_IMPL_*); QK^T, PV and their gradients are strict fp32 like torch.bmm (modules.py:180,186). */
 size_t mas_attnblock_ws_bytes(int N, int HW, int C, int G);
 int mas_attnblock_forward(const float* x, int N, int HW, int C, int G, const float* mean, const float* rstd,
@@ -366,8 +366,8 @@ int mas_embed3_forward(const float* t0, const int64_t* id0, const float* t1, con
 int mas_embed3_backward(const float* dout, const int64_t* id0, float* d0, const int64_t* id1, float* d1,
                         const int64_t* id2, float* d2, int64_t R, int H, int seg, int total, int off, void* stream);
 /* Causal self-attention core of the token transformer, fused (transformer.py:77-103; csrc/attn_causal.cu): per (sequence,
- * head, 128-query tile) S = q k^T * scale in tensor memory -> causal softmax in registers -> P (written once, [B,heads,S,S],
- * zeros above the diagonal: the backward reads it) -> ctx = P v accumulated in tensor memory.  qkv [B,S,3*heads*hd] fused
+ * head, 128-query tile) S = q k^T * scale in registers -> causal softmax on the accumulator fragment -> P (written once, [B,heads,S,S],
+ * zeros above the diagonal: the backward reads it) -> ctx = P v accumulated in registers.  qkv [B,S,3*heads*hd] fused
  * q|k|v, ctx [B,S,heads*hd], amax = device scalar max|qkv| (mas_amax).  Needs hd == 64 and S % 128 == 0
  * (MAS_ERR_UNSUPPORTED otherwise: the caller runs the GEMM / softmax sequence).  2 x fp16 operand split = fp32-level accuracy. */
 int mas_attn_causal_forward(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads, int hd,

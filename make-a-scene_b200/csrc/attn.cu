@@ -2,7 +2,7 @@
 //   GN -> q,k,v 1x1 -> softmax(q^T k / sqrt(C)) over keys -> v.P^T -> proj_out 1x1 -> + x
 // enqueued on the caller's stream from caller-provided buffers. The q/k/v projections run as ONE row GEMM against the
 // concatenated [3C, C] weight (forward: N = 3C; data gradient: K = 3C; weight gradient: Cout = 3C), the 1x1 convolutions
-// go to the tcgen05 row-GEMM / weight-gradient kernels when the shape is eligible, and the two batched token contractions
+// go to the wgmma row-GEMM / weight-gradient kernels when the shape is eligible, and the two batched token contractions
 // (QK^T and PV, plus their four gradients) keep fp32-level accuracy like the reference's torch.bmm (modules.py:180,186):
 // 3xTF32 operand splitting on the tensor cores (contract_tc3.cu), or the FFMA kernel for extents off its tiles.
 #include <stdlib.h>
@@ -35,8 +35,8 @@ __global__ void cat3_kernel(const float* __restrict__ a, const float* __restrict
 }
 size_t al(size_t v) { return (v + 255) / 256 * 256; }
 bool rows_on_tc(int impl, int N, int K) { return impl != MAS_IMPL_SIMT && N % 128 == 0 && K % 32 == 0; }
-// implementation of the token contractions (QK^T, PV and their four gradients): the operand-split 3xTF32 tcgen05 GEMM
-// (contract_tc3.cu: fp32-level accuracy like the reference's strict-fp32 torch.bmm, validated against fp64 on B200) when the
+// implementation of the token contractions (QK^T, PV and their four gradients): the operand-split 3xTF32 wgmma GEMM
+// (contract_tc3.cu: fp32-level accuracy like the reference's strict-fp32 torch.bmm, validated against fp64) when the
 // extents fit its tiles, else the strict-fp32 FFMA kernel. MAS_ATTN_TC3=0 forces the FFMA kernel (A/B measurements).
 int bmm_impl(int impl, int HW, int C) {
   static const bool off = [] { const char* e = getenv("MAS_ATTN_TC3"); return e && e[0] == '0'; }();
@@ -100,7 +100,7 @@ int mas_attnblock_forward(const float* x, int N, int HW, int C, int G, const flo
     for (int i = 0; i < 3; ++i)
       if (int e = mas_gemm(hn, ws_[i], qkv + i * c, (int)M, C, C, 1, c, c, 3 * c, 0, 0, 0, 0, 1, 1.f, bs_[i], nullptr, impl, stream)) return e;
   }
-  // fused core (attn_fused.cu): S = scale q k^T in tensor memory -> softmax in registers -> P (TMEM A operand) -> O = P v
+  // fused core (attn_fused.cu): S = scale q k^T in registers -> softmax on the fragment -> P (shared memory) -> O = P v
   static const bool fused_off = [] { const char* e = getenv("MAS_ATTN_FUSED"); return e && e[0] == '0'; }();
   if (!fused_off && impl != MAS_IMPL_SIMT && attn_core_fused_ok(HW, C)) {
     float* amax = wpk;   // scratch: the packed QKV weight is dead once the QKV GEMM is enqueued (stream order), proj re-packs later

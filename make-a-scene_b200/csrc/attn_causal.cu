@@ -1,128 +1,42 @@
 // Causal self-attention core of the token transformer, fused (transformer.py:77-103): for one (sequence, head, tile of 128
 // queries)
 //     S = (q k^T) / sqrt(hd)  ->  P = softmax_rows(S restricted to keys <= query)  ->  ctx = P v
-// in ONE kernel over the fused [B, S, 3H] q|k|v activation: the scores live in tensor memory only, the softmax runs in registers
-// (thread = query row), P goes back to tensor memory as the A operand of the second contraction (and once to global memory, for
-// the backward), ctx is accumulated in tensor memory over the key blocks.  Only the causal key blocks (<= the query tile) are
-// visited.  Same arithmetic as the AttnBlock core (attn_fused.cu): the reference runs both contractions in strict fp32, so
-// operands are split into two fp16 numbers (x*s = h + l, 22 bits) and every K step issues three kind::f16 MMAs (hh + lh + hl).
+// in ONE kernel over the fused [B, S, 3H] q|k|v activation: the scores live in the accumulator registers only, the softmax
+// runs on the accumulator fragment, P goes to shared memory as the A operand of the second contraction (and once to global
+// memory, for the backward), ctx is accumulated in registers over the key blocks.  Only the causal key blocks (<= the query
+// tile) are visited.  Same arithmetic as the AttnBlock core (attn_fused.cu): the reference runs both contractions in strict
+// fp32, so operands are split into two fp16 numbers (x*s = h + l, 22 bits) and every K step issues three fp16 wgmma
+// (hh + lh + hl).
 //
-//   * grid = (S / 128 query tiles - heaviest first, heads, B); 13 warps: 0-3 softmax / epilogue (thread = row = TMEM lane),
-//     4-11 producers, 12 MMA issuer (+ TMEM alloc).
+//   * grid = (S / 128 query tiles - heaviest first, heads, B); two warpgroups, warpgroup g owns query rows 64 g .. 64 g + 63
+//     of the tile; both stage the operands (generic loads, split, st.shared).
 //   * two passes over the key blocks of 128: pass 0 computes the row maxima and sums online (scores only), pass 1 recomputes the
-//     scores, writes the normalised probabilities (global fp32 + split into TMEM) and accumulates ctx += P_blk v_blk.  The score
-//     contraction is cheap (K = 64), recomputing it is what keeps P exactly normalised without rescaling the accumulator.
-//   * tensor memory: scores [0,128), P hi [128,192) / lo [192,256) (two keys per 32-bit column), ctx [256,320).
-//   * shared memory: the Q tile (resident) + a 2-stage ring of K / V tiles (hi and lo images), K-major planes
-//     [c/8][row][8 halves] for Q and K, MN-major planes [c/8][key][8 channels] for V (staged untransposed).
+//     scores, writes the normalised probabilities (global fp32 + split into shared memory) and accumulates ctx += P_blk v_blk.
+//     The score contraction is cheap (K = 64), recomputing it is what keeps P exactly normalised without rescaling the
+//     accumulator.
+//   * shared memory: the Q tile (resident) + a 2-stage ring of K / V tiles (hi and lo images) + the P block, K-major planes
+//     [c/8][row][8 halves] for Q, K and P, MN-major planes [c/8][key][8 channels] for V (staged untransposed).
 #include <cuda_fp16.h>
 
 #include "mas_common.cuh"
+#include "wgmma.cuh"
 
 namespace mas {
 namespace attnc {
 
 constexpr int BM = 128, BK = 128, HD = 64, STAGES = 2;
-constexpr int NEPI = 128, NPROD = 256, NTHREADS = NEPI + NPROD + 32;
+constexpr int NPROD = 256, NTHREADS = 256;
 constexpr int PITCH_K = BK * 16 + 32;            // bytes between 8-channel planes of a Q / K tile (rows = queries / keys)
 constexpr int K_HALF = (HD / 8) * PITCH_K;       // one image (hi or lo)
 constexpr int PITCH_V = BK * 16 + 16;            // MN-major V tile: plane = 8 channels, rows = the block's 128 keys
 constexpr int V_HALF = (HD / 8) * PITCH_V;
 constexpr int TILE = 2 * K_HALF;                 // hi + lo (the V tile is slightly smaller)
 static_assert(2 * V_HALF <= TILE, "V tile must fit a ring stage");
-constexpr uint32_t COL_S = 0, COL_PH = 128, COL_PL = 192, COL_O = 256;
+constexpr int PITCH_P = BM * 16 + 32;            // bytes between 8-key planes of the P block (rows = queries)
+constexpr int P_HALF = (BK / 8) * PITCH_P;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,"
-      "%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,"
-      "%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// shared-memory matrix descriptor, no swizzle, sm_100 version field = 1 (conventions pinned by tests/test_gpu_tc_probe.py, as in
-// attn_fused.cu).  K-major: LBO = bytes between 8-element K groups (planes), SBO = bytes between 8-row groups.  MN-major: LBO =
-// bytes between 8-element K groups, SBO = between 8-element MN groups (planes).
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) |
-         (1ull << 46);
-}
-__host__ __device__ constexpr uint32_t idesc_f16(int n, bool b_mn) {
-  return (1u << 4) | (b_mn ? (1u << 16) : 0u) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
 __device__ __forceinline__ float split_scale(const float* amax, float* inv) {
   float s = 1.f, i = 1.f;
   const uint32_t b = __float_as_uint(*amax);
@@ -164,236 +78,179 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* q_tile = smem;                                   // resident Q tile (hi, lo)
   uint8_t* ring = smem + TILE;                              // STAGES x TILE
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ring + (size_t)STAGES * TILE);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 5);
-  const uint32_t bar_base = smem_u32(bars);
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t q_full = bar_base + 8u * (2 * STAGES), s_full = q_full + 8u, s_free = q_full + 16u, p_ready = q_full + 24u,
-                 pv_done = q_full + 32u;
+  uint8_t* p_blk = ring + (size_t)STAGES * TILE;            // P block (hi, lo)
+  const uint32_t q_base = smem_u32(q_tile), ring_base = smem_u32(ring), p_base = smem_u32(p_blk);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = warp >> 2, fk = lane & 3;
   const int S = p.S, heads = p.heads, H = heads * HD, C3 = 3 * H;
   const int qt = (int)gridDim.x - 1 - (int)blockIdx.x;      // heaviest query tiles first
   const int h = blockIdx.y, b = blockIdx.z;
   const int q0 = qt * BM, nkb = qt + 1;                     // causal: key blocks 0 .. qt
   const float* base = p.qkv + (size_t)b * S * C3 + h * HD;
-
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), NPROD);
-      mbar_init(empty_bar(s), 1);
-    }
-    mbar_init(q_full, NPROD);
-    mbar_init(s_full, 1);
-    mbar_init(s_free, NEPI);
-    mbar_init(p_ready, NEPI);
-    mbar_init(pv_done, 1);
-    fence_barrier_init();
-  }
-  if (warp == 12) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows frow, frow + 8 (query within the tile)
+  const uint32_t a_rows = (uint32_t)(wgi * 64 * 16);          // this warpgroup's rows inside a K-major plane
   float inv_s;
   const float sc = split_scale(p.amax, &inv_s);
   constexpr float P_SCALE = 16384.0f, P_INV = 1.0f / 16384.0f;    // probabilities in [0, 1] -> [0, 2^14]
+  const int pt = tid;
 
-  if (warp < 4) {
-    // ===================== softmax (two passes over the key blocks), then the epilogue of ctx =====================
-    const uint32_t lane_addr = (uint32_t)(warp * 32) << 16;
-    const int rit = warp * 32 + lane;                          // row within the query tile
-    const int row = q0 + rit;                                  // query index within the sequence
-    float* prow = p.P + (((size_t)b * heads + h) * S + row) * S;
-    for (int c = nkb * BK; c < S; c += 4) *reinterpret_cast<float4*>(prow + c) = make_float4(0.f, 0.f, 0.f, 0.f);   // masked key blocks
-    const float ss = p.scale * inv_s * inv_s;                  // accumulator -> scale * q.k
-    float m = -INFINITY, l = 0.f, rl = 0.f;
-    int it = 0;
-    for (int pass = 0; pass < 2; ++pass) {
-      for (int kb = 0; kb < nkb; ++kb, ++it) {
-        mbar_wait(s_full, (uint32_t)(it & 1));
-        tc_fence_after();
-        const bool diag = kb == qt;                            // the only block with masked entries
-        if (pass == 0) {
-          for (int cb = 0; cb < BK / 32; ++cb) {
-            float v[32];
-            tmem_ld32(tmem_base + lane_addr + COL_S + (uint32_t)(cb * 32), v);
-            float cm = -INFINITY;
+  // a [128 rows x 64 channels] fp32 tile of the q / k / v third -> hi / lo images; 1024 items of 8 channels, 4 per thread:
+  // item = (row, oct) with oct fastest: 8 lanes read one row's 256 contiguous bytes; all loads of a tile in flight together.
+  // The caller has retired every MMA that read dst (wait<0> in both warpgroups, then the barrier below).
+  auto fill = [&](uint8_t* dst, int third, int row0, int pitch, int half) {
+    float4 v0[4], v1[4];
 #pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              v[j] = (diag && cb * 32 + j > rit) ? -INFINITY : v[j] * ss;
-              cm = fmaxf(cm, v[j]);
-            }
-            const float mn = fmaxf(m, cm);
-            if (mn > -INFINITY) {                              // (a fully masked chunk before any visible key cannot occur: key 0 is visible)
-              float add = 0.f;
-#pragma unroll
-              for (int j = 0; j < 32; ++j) add += expf(v[j] - mn);
-              l = l * expf(m - mn) + add;
-              m = mn;
-            }
-          }
-          tc_fence_before();
-          mbar_arrive(s_free);
-          if (kb == nkb - 1) rl = 1.0f / l;
-        } else {
-          if (kb > 0) {                                        // the previous block's P V MMAs have read the P columns
-            mbar_wait(pv_done, (uint32_t)((kb - 1) & 1));
-            tc_fence_after();
-          }
-          float* pblk = prow + kb * BK;
-          for (int cb = 0; cb < BK / 64; ++cb) {               // 64 keys -> 32 packed hi words + 32 packed lo words
-            uint32_t hi[32], lo[32];
-#pragma unroll
-            for (int hb = 0; hb < 2; ++hb) {
-              float v[32];
-              tmem_ld32(tmem_base + lane_addr + COL_S + (uint32_t)(cb * 64 + hb * 32), v);
-#pragma unroll
-              for (int j = 0; j < 32; ++j) v[j] = (diag && cb * 64 + hb * 32 + j > rit) ? 0.f : expf(v[j] * ss - m) * rl;
-#pragma unroll
-              for (int j = 0; j < 32; j += 4)
-                *reinterpret_cast<float4*>(pblk + cb * 64 + hb * 32 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-#pragma unroll
-              for (int j = 0; j < 16; ++j) split2(v[2 * j], v[2 * j + 1], P_SCALE, &hi[hb * 16 + j], &lo[hb * 16 + j]);
-            }
-            tmem_st32(tmem_base + lane_addr + COL_PH + (uint32_t)(cb * 32), hi);
-            tmem_st32(tmem_base + lane_addr + COL_PL + (uint32_t)(cb * 32), lo);
-          }
-          tmem_st_wait();
-          tc_fence_before();
-          mbar_arrive(s_free);
-          mbar_arrive(p_ready);
-        }
-      }
+    for (int i = 0; i < 4; ++i) {
+      const int itm = pt + i * NPROD, oct = itm & 7, r = itm >> 3;
+      const float4* src = reinterpret_cast<const float4*>(base + (size_t)(row0 + r) * C3 + third * H + oct * 8);
+      v0[i] = __ldg(src);
+      v1[i] = __ldg(src + 1);
     }
-    // ctx tile: TMEM columns [256, 320) -> registers -> the row's 64 channels (256 contiguous bytes per thread)
-    mbar_wait(pv_done, (uint32_t)((nkb - 1) & 1));
-    tc_fence_after();
-    const float oscale = inv_s * P_INV;
-    float* orow = p.ctx + ((size_t)b * S + row) * H + h * HD;
+    __syncthreads();
 #pragma unroll
-    for (int cb = 0; cb < HD / 32; ++cb) {
-      float v[32];
-      tmem_ld32(tmem_base + lane_addr + COL_O + (uint32_t)(cb * 32), v);
-#pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        *reinterpret_cast<float4*>(orow + cb * 32 + j) = make_float4(v[j] * oscale, v[j + 1] * oscale, v[j + 2] * oscale, v[j + 3] * oscale);
+    for (int i = 0; i < 4; ++i) {
+      const int itm = pt + i * NPROD, oct = itm & 7, r = itm >> 3;
+      uint4 hh, ll;
+      split8(v0[i], v1[i], sc, &hh, &ll);
+      uint8_t* d = dst + oct * pitch + r * 16;
+      *reinterpret_cast<uint4*>(d) = hh;
+      *reinterpret_cast<uint4*>(d + half) = ll;
     }
-    tc_fence_before();
-  } else if (warp < 12) {
-    // ===================== producers =====================
-    const int pt = tid - NEPI;
-    // a [128 rows x 64 channels] fp32 tile of the q / k / v third -> hi / lo images; 1024 items of 8 channels, 4 per thread:
-    // item = (row, oct) with oct fastest: 8 lanes read one row's 256 contiguous bytes; all loads of a tile in flight together
-    auto fill = [&](uint8_t* dst, int third, int row0, int pitch, int half) {
-      float4 v0[4], v1[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int itm = pt + i * NPROD, oct = itm & 7, r = itm >> 3;
-        const float4* src = reinterpret_cast<const float4*>(base + (size_t)(row0 + r) * C3 + third * H + oct * 8);
-        v0[i] = __ldg(src);
-        v1[i] = __ldg(src + 1);
-      }
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int itm = pt + i * NPROD, oct = itm & 7, r = itm >> 3;
-        uint4 hh, ll;
-        split8(v0[i], v1[i], sc, &hh, &ll);
-        uint8_t* d = dst + oct * pitch + r * 16;
-        *reinterpret_cast<uint4*>(d) = hh;
-        *reinterpret_cast<uint4*>(d + half) = ll;
-      }
-    };
-    fill(q_tile, 0, q0, PITCH_K, K_HALF);
     fence_proxy_async();
-    mbar_arrive(q_full);
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int pass = 0; pass < 2; ++pass) {
-      for (int kb = 0; kb < nkb; ++kb) {
-        mbar_wait(empty_bar(stage), phase ^ 1);
-        fill(ring + (size_t)stage * TILE, 1, kb * BK, PITCH_K, K_HALF);          // K block: K-major planes
-        fence_proxy_async();
-        mbar_arrive(full_bar(stage));
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        if (pass == 1) {
-          mbar_wait(empty_bar(stage), phase ^ 1);
-          fill(ring + (size_t)stage * TILE, 2, kb * BK, PITCH_V, V_HALF);        // V block: MN-major planes [c/8][key][8 channels]
-          fence_proxy_async();
-          mbar_arrive(full_bar(stage));
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
+    __syncthreads();
+  };
+
+  // masked key blocks of the saved probabilities
+  {
+    float* pt0 = p.P + (((size_t)b * heads + h) * S + q0) * S;
+    const int cols = S - nkb * BK;
+    for (int i = tid; i < BM * (cols / 4); i += NTHREADS) {
+      const int r = i / (cols / 4), c4 = i - r * (cols / 4);
+      *reinterpret_cast<float4*>(pt0 + (size_t)r * S + nkb * BK + c4 * 4) = make_float4(0.f, 0.f, 0.f, 0.f);
     }
-  } else {
-    // ===================== MMA issuer (warp-uniform loop, one elected lane issues) =====================
-    constexpr uint32_t idesc_s = idesc_f16(BK, false), idesc_o = idesc_f16(HD, true);
-    const uint32_t q_base = smem_u32(q_tile), ring_base = smem_u32(ring);
-    mbar_wait(q_full, 0);
-    tc_fence_after();
-    int stage = 0, it = 0;
-    uint32_t phase = 0;
-    for (int pass = 0; pass < 2; ++pass) {
-      for (int kb = 0; kb < nkb; ++kb, ++it) {
-        // ---- scores of this key block -> TMEM columns [0, 128) ----
-        mbar_wait(full_bar(stage), phase);
-        if (it > 0) mbar_wait(s_free, (uint32_t)((it - 1) & 1));   // the softmax warps have read the previous scores
-        tc_fence_after();
-        {
-          const uint32_t st = ring_base + (uint32_t)stage * TILE;
-          if (elect_one()) {
+  }
+  fill(q_tile, 0, q0, PITCH_K, K_HALF);
+
+  const float ss = p.scale * inv_s * inv_s;                  // accumulator -> scale * q.k
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, rl[2] = {0.f, 0.f};
+  float sacc[BK / 2], oacc[HD / 2];
+  int stage = 0;
+  for (int pass = 0; pass < 2; ++pass) {
+    for (int kb = 0; kb < nkb; ++kb) {
+      // ---- scores of this key block ----
+      uint8_t* st = ring + (size_t)stage * TILE;
+      fill(st, 1, kb * BK, PITCH_K, K_HALF);          // K block: K-major planes
+      {
+        const uint32_t sa = ring_base + (uint32_t)stage * TILE;
+        wg::fence();
 #pragma unroll
-            for (int k16 = 0; k16 < HD / 16; ++k16) {
-              const uint64_t qh = make_desc(q_base + (uint32_t)(k16 * 2 * PITCH_K), PITCH_K, 128);
-              const uint64_t ql = make_desc(q_base + (uint32_t)(K_HALF + k16 * 2 * PITCH_K), PITCH_K, 128);
-              const uint64_t kh = make_desc(st + (uint32_t)(k16 * 2 * PITCH_K), PITCH_K, 128);
-              const uint64_t kl = make_desc(st + (uint32_t)(K_HALF + k16 * 2 * PITCH_K), PITCH_K, 128);
-              mma_f16_ss(tmem_base + COL_S, qh, kh, idesc_s, k16 > 0 ? 1u : 0u);
-              mma_f16_ss(tmem_base + COL_S, ql, kh, idesc_s, 1u);
-              mma_f16_ss(tmem_base + COL_S, qh, kl, idesc_s, 1u);
-            }
-            mma_commit(empty_bar(stage));
-            mma_commit(s_full);
-          }
-          __syncwarp();
+        for (int k16 = 0; k16 < HD / 16; ++k16) {
+          const uint64_t qh = wg::desc(q_base + a_rows + (uint32_t)(k16 * 2 * PITCH_K), PITCH_K, 128);
+          const uint64_t ql = wg::desc(q_base + a_rows + (uint32_t)(K_HALF + k16 * 2 * PITCH_K), PITCH_K, 128);
+          const uint64_t kh = wg::desc(sa + (uint32_t)(k16 * 2 * PITCH_K), PITCH_K, 128);
+          const uint64_t kl = wg::desc(sa + (uint32_t)(K_HALF + k16 * 2 * PITCH_K), PITCH_K, 128);
+          wg::wgmma_f16_ss_n128<0, 0>(sacc, qh, kh, k16 > 0 ? 1u : 0u);
+          wg::wgmma_f16_ss_n128<0, 0>(sacc, ql, kh, 1u);
+          wg::wgmma_f16_ss_n128<0, 0>(sacc, qh, kl, 1u);
         }
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        if (pass == 1) {
-          // ---- ctx += P_blk V_blk: A = P from tensor memory (TS mode), B = the V tile, MN-major ----
-          mbar_wait(full_bar(stage), phase);
-          mbar_wait(p_ready, (uint32_t)(kb & 1));
-          tc_fence_after();
-          const uint32_t st = ring_base + (uint32_t)stage * TILE;
-          if (elect_one()) {
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs<BK / 2>(sacc);
+      }
+      if (++stage == STAGES) stage = 0;
+      const bool diag = kb == qt;                            // the only block with masked entries
+      if (pass == 0) {
+        // online maximum / sum over this thread's columns of its two rows; the four lanes of a row are combined at the end
 #pragma unroll
-            for (int k16 = 0; k16 < BK / 16; ++k16) {
-              const uint32_t acol = (uint32_t)(k16 * 8);       // 16 keys = 8 packed columns
-              // MN-major B: K groups (8 keys) are 128 bytes apart inside a plane, N groups are the planes
-              const uint64_t vh = make_desc(st + (uint32_t)(k16 * 256), 128, PITCH_V);
-              const uint64_t vl = make_desc(st + (uint32_t)(V_HALF + k16 * 256), 128, PITCH_V);
-              mma_f16_ts(tmem_base + COL_O, tmem_base + COL_PH + acol, vh, idesc_o, (kb > 0 || k16 > 0) ? 1u : 0u);
-              mma_f16_ts(tmem_base + COL_O, tmem_base + COL_PL + acol, vh, idesc_o, 1u);
-              mma_f16_ts(tmem_base + COL_O, tmem_base + COL_PH + acol, vl, idesc_o, 1u);
+        for (int i = 0; i < 2; ++i) {
+          const int rit = frow + 8 * i;
+          float cm = -INFINITY;
+#pragma unroll
+          for (int j = 0; j < BK / 8; ++j)
+#pragma unroll
+            for (int c = 0; c < 2; ++c) {
+              const int key = 8 * j + 2 * fk + c;
+              const float v = (diag && key > rit) ? -INFINITY : sacc[4 * j + 2 * i + c] * ss;
+              sacc[4 * j + 2 * i + c] = v;
+              cm = fmaxf(cm, v);
             }
-            mma_commit(empty_bar(stage));
-            mma_commit(pv_done);
+          const float mn = fmaxf(m[i], cm);
+          if (mn > -INFINITY) {
+            float add = 0.f;
+#pragma unroll
+            for (int j = 0; j < BK / 8; ++j) add += expf(sacc[4 * j + 2 * i] - mn) + expf(sacc[4 * j + 2 * i + 1] - mn);
+            l[i] = l[i] * expf(m[i] - mn) + add;
+            m[i] = mn;
           }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
         }
+        if (kb == nkb - 1) {
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+#pragma unroll
+            for (int x = 1; x <= 2; x <<= 1) {
+              const float om = __shfl_xor_sync(0xffffffffu, m[i], x), ol = __shfl_xor_sync(0xffffffffu, l[i], x);
+              const float mn = fmaxf(m[i], om);
+              l[i] = (m[i] > -INFINITY ? l[i] * expf(m[i] - mn) : 0.f) + (om > -INFINITY ? ol * expf(om - mn) : 0.f);
+              m[i] = mn;
+            }
+            rl[i] = 1.0f / l[i];
+          }
+        }
+      } else {
+        // probabilities: global (fp32) and the split P block in shared memory (the previous block's P V MMAs have retired:
+        // the barrier in fill() above)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int rit = frow + 8 * i;
+          float* prow = p.P + (((size_t)b * heads + h) * S + q0 + rit) * S + kb * BK + 2 * fk;
+#pragma unroll
+          for (int j = 0; j < BK / 8; ++j) {
+            const int key = 8 * j + 2 * fk;
+            const float a = (diag && key > rit) ? 0.f : expf(sacc[4 * j + 2 * i] * ss - m[i]) * rl[i];
+            const float c = (diag && key + 1 > rit) ? 0.f : expf(sacc[4 * j + 2 * i + 1] * ss - m[i]) * rl[i];
+            *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(a, c);
+            uint32_t hi, lo;
+            split2(a, c, P_SCALE, &hi, &lo);
+            uint8_t* d = p_blk + (size_t)j * PITCH_P + rit * 16 + fk * 4;
+            *reinterpret_cast<uint32_t*>(d) = hi;
+            *reinterpret_cast<uint32_t*>(d + P_HALF) = lo;
+          }
+        }
+        // ---- ctx += P_blk V_blk: A = P (K-major), B = the V tile, MN-major ----
+        uint8_t* sv = ring + (size_t)stage * TILE;
+        fill(sv, 2, kb * BK, PITCH_V, V_HALF);        // V block: MN-major planes [c/8][key][8 channels]; fences the P stores too
+        const uint32_t vb = ring_base + (uint32_t)stage * TILE;
+        wg::fence();
+#pragma unroll
+        for (int k16 = 0; k16 < BK / 16; ++k16) {
+          const uint64_t ph = wg::desc(p_base + a_rows + (uint32_t)(k16 * 2 * PITCH_P), PITCH_P, 128);
+          const uint64_t pl = wg::desc(p_base + a_rows + (uint32_t)(P_HALF + k16 * 2 * PITCH_P), PITCH_P, 128);
+          // MN-major B: K groups (8 keys) are 128 bytes apart inside a plane, N groups are the planes
+          const uint64_t vh = wg::desc(vb + (uint32_t)(k16 * 256), 128, PITCH_V);
+          const uint64_t vl = wg::desc(vb + (uint32_t)(V_HALF + k16 * 256), 128, PITCH_V);
+          wg::wgmma_f16_ss_n64<0, 1>(oacc, ph, vh, (kb > 0 || k16 > 0) ? 1u : 0u);
+          wg::wgmma_f16_ss_n64<0, 1>(oacc, pl, vh, 1u);
+          wg::wgmma_f16_ss_n64<0, 1>(oacc, ph, vl, 1u);
+        }
+        wg::commit();
+        wg::wait<0>();
+        wg::fence_regs<HD / 2>(oacc);
+        if (++stage == STAGES) stage = 0;
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 12) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // ctx tile: straight from the fragment
+  const float oscale = inv_s * P_INV;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float* orow = p.ctx + ((size_t)b * S + q0 + frow + 8 * i) * H + h * HD + 2 * fk;
+#pragma unroll
+    for (int j = 0; j < HD / 8; ++j)
+      *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(oacc[4 * j + 2 * i] * oscale, oacc[4 * j + 2 * i + 1] * oscale);
   }
 }
 
-constexpr size_t SMEM_BYTES = (size_t)TILE * (1 + STAGES) + (2 * STAGES + 5) * 8 + 16;
+constexpr size_t SMEM_BYTES = (size_t)TILE * (1 + STAGES) + 2 * (size_t)P_HALF;
 
 }  // namespace attnc
 

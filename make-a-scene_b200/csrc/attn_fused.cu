@@ -1,134 +1,43 @@
 // AttnBlock core, fused (modules.py:175-187): for one image and one tile of 128 queries
 //     S = scale * Q K^T  ->  P = softmax_rows(S)  ->  O = P V
-// in ONE kernel: S lives in tensor memory only, the softmax runs in registers (thread = query row), P goes back to tensor
-// memory as the A operand of the second contraction (and once to global memory, for the backward), O is accumulated in the
-// columns S occupied.  The reference runs both contractions in strict fp32 (torch.bmm): operands are split into two fp16
-// numbers (x*s = h + l, 22 bits; power-of-two scales from the tensors' largest magnitude) and every K step issues three
-// kind::f16 MMAs (hh + lh + hl), accumulated in fp32 - the same arithmetic as the VQ filter (vq_tc.cu).
+// in ONE kernel: S lives in the accumulator registers only, the softmax runs on the accumulator fragment, P goes to shared
+// memory as the A operand of the second contraction (and once to global memory, for the backward).  The reference runs both
+// contractions in strict fp32 (torch.bmm): operands are split into two fp16 numbers (x*s = h + l, 22 bits; power-of-two
+// scales from the tensors' largest magnitude) and every K step issues three fp16 wgmma (hh + lh + hl), accumulated in fp32 -
+// the same arithmetic as the VQ filter (vq_tc.cu).
 //
-//   * grid = (HW / 128 query tiles, N images); 13 warps: 0-3 softmax / epilogue (thread = row = TMEM lane), 4-11 producers,
-//     12 MMA issuer (+ TMEM alloc).
-//   * phase 1: Q and K chunks of 32 channels are converted by the producers into K-major planes [k/8][row][8 halves]
-//     (hi and lo), 2-stage full / empty mbarrier ring, 6 MMAs (M 128, N = HW, K 16) per chunk into TMEM columns [0, HW).
-//   * softmax: three passes over the row in tensor memory (max, sum of exp, normalise); P -> global (fp32) and, split,
-//     -> TMEM columns [256, 256 + HW) (hi: HW/2 columns, lo: HW/2 columns).
-//   * phase 2: O = P V in halves of 256 channels: A = P from tensor memory (TS mode), B = V chunks of 32 keys staged
-//     UNTRANSPOSED as MN-major planes [c/8][key][8 channels] (tests/test_gpu_tc_probe.py::test_reveal_raw_f16), 6 MMAs per
-//     chunk into columns [0, 256); the epilogue warps drain a half (smem transpose -> coalesced rows) while the next runs.
+//   * grid = (HW / 128 query tiles, N images); two warpgroups, warpgroup g owns query rows 64 g .. 64 g + 63 of the tile and
+//     both stage the operands (generic loads, split, st.shared) into a 2-stage ring.
+//   * phase 1: Q and K chunks of 32 channels as K-major planes [k/8][row][8 halves] (hi and lo), 6 wgmma.m64nHWk16 per chunk.
+//   * softmax on the fragment (a row is spread over the four lanes of a quad): P -> global (fp32) and, split, -> shared
+//     memory planes [key/8][row][8 halves] (hi, lo) over the idle phase-1 ring.
+//   * phase 2: O = P V in halves of 256 channels: A = P (K-major), B = V chunks of 32 keys staged UNTRANSPOSED as MN-major
+//     planes [c/8][key][8 channels], 6 wgmma.m64n256k16 per chunk; each half is stored straight from the fragment.
 #include <cuda_fp16.h>
 
 #include "mas_common.cuh"
+#include "wgmma.cuh"
 
 namespace mas {
 namespace attnf {
 
 constexpr int BM = 128, KC = 32, STAGES = 2;
-constexpr int NEPI = 128, NPROD = 256, NTHREADS = NEPI + NPROD + 32;
+constexpr int NPROD = 256, NTHREADS = 256;
 constexpr int HWMAX = 256;                       // keys (= accumulator columns of S)
 constexpr int PITCH_Q = BM * 16 + 32;            // bytes between 8-channel planes of the Q chunk
 constexpr int PITCH_K = HWMAX * 16 + 32;         // ... of the K chunk (rows = keys)
 constexpr int Q_HALF = (KC / 8) * PITCH_Q, K_HALF = (KC / 8) * PITCH_K;
 constexpr int STAGE1 = 2 * Q_HALF + 2 * K_HALF;  // phase-1 stage: Q hi, Q lo, K hi, K lo
+constexpr int PITCH_P = BM * 16 + 32;            // bytes between 8-key planes of P
+constexpr int P_HALF = (HWMAX / 8) * PITCH_P;
+constexpr int REGION1 = (STAGES * STAGE1 > 2 * P_HALF) ? STAGES * STAGE1 : 2 * P_HALF;   // phase-1 ring, then P
 constexpr int NV = 256;                          // channels of one O half (N of the phase-2 MMAs)
 constexpr int PITCH_V = KC * 16 + 16;            // phase 2, MN-major: plane = 8 channels, rows = the chunk's 32 keys (16 B skew)
 constexpr int V_HALF = (NV / 8) * PITCH_V;
 constexpr int STAGE2 = 2 * V_HALF;
-constexpr int STAGE = STAGE1 > STAGE2 ? STAGE1 : STAGE2;
-constexpr int EP_LD = 36;
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// one lane of the (converged) warp: true for exactly one thread.  The MMA-issuing warps run their loops warp-uniformly (operand
-// descriptors stay in uniform registers) and only the issue itself is predicated on this.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,"
-      "%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,"
-      "%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// shared-memory matrix descriptor, no swizzle, sm_100 version field = 1.  K-major: LBO = bytes between 8-element K groups
-// (planes), SBO = bytes between 8-row groups.  MN-major: LBO = bytes between 8-element K groups, SBO = between 8-element
-// MN groups (planes).
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) |
-         (1ull << 46);
-}
-__host__ __device__ constexpr uint32_t idesc_f16(int n, bool b_mn) {
-  return (1u << 4) | (b_mn ? (1u << 16) : 0u) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
-}
 __device__ __forceinline__ float split_scale(const float* amax, float* inv) {
   float s = 1.f, i = 1.f;
   const uint32_t b = __float_as_uint(*amax);
@@ -167,248 +76,187 @@ struct Params {
 };
 
 template <int HW>
+__device__ __forceinline__ void mma_s(float* d, uint64_t a, uint64_t b, uint32_t acc) {
+  if (HW == 256) wg::wgmma_f16_ss_n256<0, 0>(d, a, b, acc);
+  else wg::wgmma_f16_ss_n128<0, 0>(d, a, b, acc);
+}
+
+template <int HW>
 __global__ void __launch_bounds__(NTHREADS, 1) attn_core_fwd(const Params p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  float* patches = reinterpret_cast<float*>(smem + (size_t)STAGES * STAGE);      // 4 warps x [32][EP_LD]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(patches + 4 * 32 * EP_LD);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  const uint32_t smem_base = smem_u32(smem), bar_base = smem_u32(bars);
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t s_full = bar_base + 8u * (2 * STAGES), p_ready = s_full + 8u, o_full = s_full + 16u, o_empty = s_full + 24u;
+  uint8_t* vring = smem + REGION1;
+  const uint32_t smem_base = smem_u32(smem), v_base = smem_u32(vring);
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = warp >> 2, fk = lane & 3;
   const int C = p.C, C3 = 3 * C;
   const int n = blockIdx.y, q0 = blockIdx.x * BM;
   const float* base = p.qkv + (size_t)n * HW * C3;
   const int nchunk1 = C / KC, nchunk2 = HW / KC, nhalf = C / NV;
-
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), NPROD);
-      mbar_init(empty_bar(s), 1);
-    }
-    mbar_init(s_full, 1);
-    mbar_init(p_ready, NEPI);
-    mbar_init(o_full, 1);
-    mbar_init(o_empty, NEPI);
-    fence_barrier_init();
-  }
-  if (warp == 12) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows frow, frow + 8 (query within the tile)
+  const uint32_t a_rows = (uint32_t)(wgi * 64 * 16);          // this warpgroup's rows inside a K-major plane
   float inv_s;
   const float sc = split_scale(p.amax, &inv_s);
   constexpr float P_SCALE = 16384.0f, P_INV = 1.0f / 16384.0f;    // probabilities in [0, 1] -> [0, 2^14]
-  const uint32_t pcol = tmem_base + 256, phalf = (uint32_t)(HW >> 1);
+  const int pt = tid;
 
-  if (warp < 4) {
-    // ===================== softmax, then the epilogue of O =====================
-    const uint32_t lane_addr = (uint32_t)(warp * 32) << 16;
-    const int row = q0 + warp * 32 + lane;                      // query index within the image
-    mbar_wait(s_full, 0);
-    tc_fence_after();
-    const float ss = p.scale * inv_s * inv_s;                   // accumulator -> scale * q.k
-    float mx = -INFINITY;
-    for (int cb = 0; cb < HW / 32; ++cb) {
-      float v[32];
-      tmem_ld32(tmem_base + lane_addr + (uint32_t)(cb * 32), v);
+  // ---- phase 1: S = Q K^T over chunks of 32 channels ----
+  float acc[HW / 2];
+  int stage = 0;
+  for (int c = 0; c < nchunk1; ++c) {
+    // items: (row, oct) with oct fastest: 4 lanes read one row's 128 contiguous bytes; all loads of a chunk in flight together
+    constexpr int NI1 = (BM + HW) * (KC / 8) / NPROD;
+    float4 v0[NI1], v1[NI1];
 #pragma unroll
-      for (int j = 0; j < 32; ++j) mx = fmaxf(mx, v[j] * ss);
+    for (int i = 0; i < NI1; ++i) {
+      const int it = pt + i * NPROD, oct = it & 3, r = it >> 2;
+      const bool isq = r < BM;
+      const int rr = isq ? r : r - BM;
+      const float4* src = reinterpret_cast<const float4*>(base + (size_t)(isq ? q0 + rr : rr) * C3 + (isq ? 0 : C) + c * KC + oct * 8);
+      v0[i] = __ldg(src);
+      v1[i] = __ldg(src + 1);
     }
-    float sum = 0.f;
-    for (int cb = 0; cb < HW / 32; ++cb) {
-      float v[32];
-      tmem_ld32(tmem_base + lane_addr + (uint32_t)(cb * 32), v);
+    if (c > 0) __syncthreads();   // both warpgroups have retired the MMAs that last read this stage (wait<1> below)
+    uint8_t* st = smem + (size_t)stage * STAGE1;
 #pragma unroll
-      for (int j = 0; j < 32; ++j) sum += expf(v[j] * ss - mx);
+    for (int i = 0; i < NI1; ++i) {
+      const int it = pt + i * NPROD, oct = it & 3, r = it >> 2;
+      const bool isq = r < BM;
+      const int rr = isq ? r : r - BM;
+      uint4 h, l;
+      split8(v0[i], v1[i], sc, &h, &l);
+      uint8_t* dh = isq ? st + oct * PITCH_Q + rr * 16 : st + 2 * Q_HALF + oct * PITCH_K + rr * 16;
+      *reinterpret_cast<uint4*>(dh) = h;
+      *reinterpret_cast<uint4*>(dh + (isq ? Q_HALF : K_HALF)) = l;
     }
-    const float rs = 1.0f / sum;
-    float* prow = p.P + ((size_t)n * HW + row) * HW;
-    for (int cb = 0; cb < HW / 64; ++cb) {                       // 64 keys -> 32 packed hi words + 32 packed lo words
-      uint32_t hi[32], lo[32];
+    fence_proxy_async();
+    __syncthreads();
+    const uint32_t sa = smem_base + (uint32_t)stage * STAGE1;
+    wg::fence();
 #pragma unroll
-      for (int hb = 0; hb < 2; ++hb) {
-        float v[32];
-        tmem_ld32(tmem_base + lane_addr + (uint32_t)(cb * 64 + hb * 32), v);
+    for (int k16 = 0; k16 < KC / 16; ++k16) {
+      const uint64_t qh = wg::desc(sa + a_rows + (uint32_t)(k16 * 2 * PITCH_Q), PITCH_Q, 128);
+      const uint64_t ql = wg::desc(sa + a_rows + (uint32_t)(Q_HALF + k16 * 2 * PITCH_Q), PITCH_Q, 128);
+      const uint64_t kh = wg::desc(sa + (uint32_t)(2 * Q_HALF + k16 * 2 * PITCH_K), PITCH_K, 128);
+      const uint64_t kl = wg::desc(sa + (uint32_t)(2 * Q_HALF + K_HALF + k16 * 2 * PITCH_K), PITCH_K, 128);
+      mma_s<HW>(acc, qh, kh, (c > 0 || k16 > 0) ? 1u : 0u);
+      mma_s<HW>(acc, ql, kh, 1u);
+      mma_s<HW>(acc, qh, kl, 1u);
+    }
+    wg::commit();
+    wg::wait<STAGES - 1>();
+    if (++stage == STAGES) stage = 0;
+  }
+  wg::wait<0>();
+  wg::fence_regs<HW / 2>(acc);
+
+  // ---- softmax: row frow + 8 i is spread over the four lanes of this quad (keys 8 j + 2 fk + {0, 1}) ----
+  const float ss = p.scale * inv_s * inv_s;                   // accumulator -> scale * q.k
+  float mx[2] = {-INFINITY, -INFINITY}, sum[2] = {0.f, 0.f};
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = expf(v[j] * ss - mx) * rs;
+  for (int j = 0; j < HW / 8; ++j)
 #pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<float4*>(prow + cb * 64 + hb * 32 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
+    for (int i = 0; i < 2; ++i) mx[i] = fmaxf(mx[i], fmaxf(acc[4 * j + 2 * i] * ss, acc[4 * j + 2 * i + 1] * ss));
 #pragma unroll
-        for (int j = 0; j < 16; ++j) split2(v[2 * j], v[2 * j + 1], P_SCALE, &hi[hb * 16 + j], &lo[hb * 16 + j]);
+  for (int i = 0; i < 2; ++i) {
+    mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 1));
+    mx[i] = fmaxf(mx[i], __shfl_xor_sync(0xffffffffu, mx[i], 2));
+  }
+#pragma unroll
+  for (int j = 0; j < HW / 8; ++j)
+#pragma unroll
+    for (int i = 0; i < 2; ++i)
+#pragma unroll
+      for (int cc = 0; cc < 2; ++cc) {
+        const float e = expf(acc[4 * j + 2 * i + cc] * ss - mx[i]);
+        acc[4 * j + 2 * i + cc] = e;
+        sum[i] += e;
       }
-      tmem_st32(pcol + lane_addr + (uint32_t)(cb * 32), hi);
-      tmem_st32(pcol + lane_addr + phalf + (uint32_t)(cb * 32), lo);
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    sum[i] += __shfl_xor_sync(0xffffffffu, sum[i], 1);
+    sum[i] += __shfl_xor_sync(0xffffffffu, sum[i], 2);
+  }
+  __syncthreads();   // every MMA of phase 1 has completed in both warpgroups: the ring becomes the P planes
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    const float rs = 1.0f / sum[i];
+    const int row = frow + 8 * i;
+    float* prow = p.P + ((size_t)n * HW + q0 + row) * HW + 2 * fk;
+#pragma unroll
+    for (int j = 0; j < HW / 8; ++j) {
+      const float a = acc[4 * j + 2 * i] * rs, b = acc[4 * j + 2 * i + 1] * rs;
+      *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(a, b);
+      uint32_t hi, lo;
+      split2(a, b, P_SCALE, &hi, &lo);
+      uint8_t* d = smem + (size_t)j * PITCH_P + row * 16 + fk * 4;
+      *reinterpret_cast<uint32_t*>(d) = hi;
+      *reinterpret_cast<uint32_t*>(d + P_HALF) = lo;
     }
-    tmem_st_wait();
-    tc_fence_before();
-    mbar_arrive(p_ready);
-    // O halves: TMEM columns [0, 256) -> registers -> per-warp smem transpose -> 128-byte row segments
-    const float oscale = inv_s * P_INV;
-    float* patch = patches + warp * (32 * EP_LD);
-    const int sub_r = lane >> 3, sub_c = lane & 7;
-    float* orow0 = p.O + ((size_t)n * HW + q0 + warp * 32) * C;
-    for (int half = 0; half < nhalf; ++half) {
-      mbar_wait(o_full, (uint32_t)(half & 1));
-      tc_fence_after();
-      for (int cb = 0; cb < NV / 32; ++cb) {
-        float v[32];
-        tmem_ld32(tmem_base + lane_addr + (uint32_t)(cb * 32), v);
-        if (cb == NV / 32 - 1) {       // the accumulator is in registers: the MMAs of the next half may overwrite it
-          tc_fence_before();
-          mbar_arrive(o_empty);
-        }
-        __syncwarp();
+  }
+  fence_proxy_async();
+
+  // ---- phase 2: O = P V, 256 channels at a time, 32 keys per chunk ----
+  const float oscale = inv_s * P_INV;
+  float* oacc = acc;   // HW == 256: the S registers are free again; HW == 128: a separate set
+  float oacc_own[HW == 256 ? 1 : NV / 2];
+  if (HW != 256) oacc = oacc_own;
+  stage = 0;
+  int it2 = 0;
+  for (int half = 0; half < nhalf; ++half) {
+    for (int c = 0; c < nchunk2; ++c, ++it2) {
+      constexpr int NI2 = KC * (NV / 8) / NPROD;
+      float4 v0[NI2], v1[NI2];
 #pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<float4*>(patch + lane * EP_LD + j) =
-              make_float4(v[j] * oscale, v[j + 1] * oscale, v[j + 2] * oscale, v[j + 3] * oscale);
-        __syncwarp();
-#pragma unroll
-        for (int i = 0; i < 8; ++i) {
-          const int r = i * 4 + sub_r;
-          *reinterpret_cast<float4*>(orow0 + (size_t)r * C + half * NV + cb * 32 + sub_c * 4) =
-              *reinterpret_cast<const float4*>(patch + r * EP_LD + sub_c * 4);
-        }
-      }
-    }
-  } else if (warp < 12) {
-    // ===================== producers =====================
-    const int pt = tid - NEPI;
-    int stage = 0;
-    uint32_t phase = 0;
-    // ---- phase 1: Q [128 x 32] and K [HW x 32] chunks, K-major planes ----
-    for (int c = 0; c < nchunk1; ++c) {
-      mbar_wait(empty_bar(stage), phase ^ 1);
-      uint8_t* st = smem + (size_t)stage * STAGE;
-      // items: (row, oct) with oct fastest: 4 lanes read one row's 128 contiguous bytes; all loads of a chunk in flight together
-      constexpr int NI1 = (BM + HW) * (KC / 8) / NPROD;
-      float4 v0[NI1], v1[NI1];
-#pragma unroll
-      for (int i = 0; i < NI1; ++i) {
-        const int it = pt + i * NPROD, oct = it & 3, r = it >> 2;
-        const bool isq = r < BM;
-        const int rr = isq ? r : r - BM;
-        const float4* src = reinterpret_cast<const float4*>(base + (size_t)(isq ? q0 + rr : rr) * C3 + (isq ? 0 : C) + c * KC + oct * 8);
+      for (int i = 0; i < NI2; ++i) {
+        const int it = pt + i * NPROD, oc = it % (NV / 8), key = it / (NV / 8);   // consecutive lanes: consecutive 32 bytes of one key's row
+        const float4* src = reinterpret_cast<const float4*>(base + (size_t)(c * KC + key) * C3 + 2 * C + half * NV + oc * 8);
         v0[i] = __ldg(src);
         v1[i] = __ldg(src + 1);
       }
+      __syncthreads();   // first chunk: P is complete; later: the MMAs that last read this stage have retired
+      uint8_t* st = vring + (size_t)stage * STAGE2;
 #pragma unroll
-      for (int i = 0; i < NI1; ++i) {
-        const int it = pt + i * NPROD, oct = it & 3, r = it >> 2;
-        const bool isq = r < BM;
-        const int rr = isq ? r : r - BM;
+      for (int i = 0; i < NI2; ++i) {
+        const int it = pt + i * NPROD, oc = it % (NV / 8), key = it / (NV / 8);
         uint4 h, l;
         split8(v0[i], v1[i], sc, &h, &l);
-        uint8_t* dh = isq ? st + oct * PITCH_Q + rr * 16 : st + 2 * Q_HALF + oct * PITCH_K + rr * 16;
+        uint8_t* dh = st + oc * PITCH_V + key * 16;
         *reinterpret_cast<uint4*>(dh) = h;
-        *reinterpret_cast<uint4*>(dh + (isq ? Q_HALF : K_HALF)) = l;
+        *reinterpret_cast<uint4*>(dh + V_HALF) = l;
       }
       fence_proxy_async();
-      mbar_arrive(full_bar(stage));
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-    }
-    // ---- phase 2: V chunks [32 keys x 256 channels], MN-major planes [c/8][key][8 channels] ----
-    for (int half = 0; half < nhalf; ++half) {
-      for (int c = 0; c < nchunk2; ++c) {
-        mbar_wait(empty_bar(stage), phase ^ 1);
-        uint8_t* st = smem + (size_t)stage * STAGE;
-        constexpr int NI2 = KC * (NV / 8) / NPROD;
-        float4 v0[NI2], v1[NI2];
+      __syncthreads();
+      const uint32_t sv = v_base + (uint32_t)stage * STAGE2;
+      wg::fence();
 #pragma unroll
-        for (int i = 0; i < NI2; ++i) {
-          const int it = pt + i * NPROD, oc = it % (NV / 8), key = it / (NV / 8);   // consecutive lanes: consecutive 32 bytes of one key's row
-          const float4* src = reinterpret_cast<const float4*>(base + (size_t)(c * KC + key) * C3 + 2 * C + half * NV + oc * 8);
-          v0[i] = __ldg(src);
-          v1[i] = __ldg(src + 1);
-        }
-#pragma unroll
-        for (int i = 0; i < NI2; ++i) {
-          const int it = pt + i * NPROD, oc = it % (NV / 8), key = it / (NV / 8);
-          uint4 h, l;
-          split8(v0[i], v1[i], sc, &h, &l);
-          uint8_t* dh = st + oc * PITCH_V + key * 16;
-          *reinterpret_cast<uint4*>(dh) = h;
-          *reinterpret_cast<uint4*>(dh + V_HALF) = l;
-        }
-        fence_proxy_async();
-        mbar_arrive(full_bar(stage));
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      for (int k16 = 0; k16 < KC / 16; ++k16) {
+        const uint32_t poff = (uint32_t)((c * KC / 8 + k16 * 2) * PITCH_P);
+        const uint64_t ph = wg::desc(smem_base + a_rows + poff, PITCH_P, 128);
+        const uint64_t pl = wg::desc(smem_base + a_rows + (uint32_t)P_HALF + poff, PITCH_P, 128);
+        // MN-major B: K groups (8 keys) are 128 bytes apart inside a plane, N groups are the planes
+        const uint64_t vh = wg::desc(sv + (uint32_t)(k16 * 256), 128, PITCH_V);
+        const uint64_t vl = wg::desc(sv + (uint32_t)(V_HALF + k16 * 256), 128, PITCH_V);
+        wg::wgmma_f16_ss_n256<0, 1>(oacc, ph, vh, (c > 0 || k16 > 0) ? 1u : 0u);
+        wg::wgmma_f16_ss_n256<0, 1>(oacc, pl, vh, 1u);
+        wg::wgmma_f16_ss_n256<0, 1>(oacc, ph, vl, 1u);
       }
+      wg::commit();
+      wg::wait<STAGES - 1>();
+      if (++stage == STAGES) stage = 0;
     }
-  } else {
-    // ===================== MMA issuer (warp-uniform loop, one elected lane issues) =====================
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      constexpr uint32_t idesc1 = idesc_f16(HW, false);
-      for (int c = 0; c < nchunk1; ++c) {
-        mbar_wait(full_bar(stage), phase);
-        tc_fence_after();
-        const uint32_t st = smem_base + (uint32_t)stage * STAGE;
-        if (elect_one()) {
+    wg::wait<0>();
+    wg::fence_regs<NV / 2>(oacc);
 #pragma unroll
-          for (int k16 = 0; k16 < KC / 16; ++k16) {
-            const uint64_t qh = make_desc(st + (uint32_t)(k16 * 2 * PITCH_Q), PITCH_Q, 128);
-            const uint64_t ql = make_desc(st + (uint32_t)(Q_HALF + k16 * 2 * PITCH_Q), PITCH_Q, 128);
-            const uint64_t kh = make_desc(st + (uint32_t)(2 * Q_HALF + k16 * 2 * PITCH_K), PITCH_K, 128);
-            const uint64_t kl = make_desc(st + (uint32_t)(2 * Q_HALF + K_HALF + k16 * 2 * PITCH_K), PITCH_K, 128);
-            mma_f16_ss(tmem_base, qh, kh, idesc1, (c > 0 || k16 > 0) ? 1u : 0u);
-            mma_f16_ss(tmem_base, ql, kh, idesc1, 1u);
-            mma_f16_ss(tmem_base, qh, kl, idesc1, 1u);
-          }
-          mma_commit(empty_bar(stage));
-          if (c == nchunk1 - 1) mma_commit(s_full);
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      mbar_wait(p_ready, 0);
-      tc_fence_after();
-      constexpr uint32_t idesc2 = idesc_f16(NV, true);
-      const uint32_t phalf_cols = (uint32_t)(HW >> 1);
-      for (int half = 0; half < nhalf; ++half) {
-        if (half > 0) {
-          mbar_wait(o_empty, (uint32_t)((half - 1) & 1));
-          tc_fence_after();
-        }
-        for (int c = 0; c < nchunk2; ++c) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t st = smem_base + (uint32_t)stage * STAGE;
-          if (elect_one()) {
+    for (int i = 0; i < 2; ++i) {
+      float* orow = p.O + ((size_t)n * HW + q0 + frow + 8 * i) * C + half * NV + 2 * fk;
 #pragma unroll
-            for (int k16 = 0; k16 < KC / 16; ++k16) {
-              const uint32_t acol = (uint32_t)((c * KC + k16 * 16) >> 1);
-              // MN-major B: K groups (8 keys) are 128 bytes apart inside a plane, N groups are the planes
-              const uint64_t vh = make_desc(st + (uint32_t)(k16 * 256), 128, PITCH_V);
-              const uint64_t vl = make_desc(st + (uint32_t)(V_HALF + k16 * 256), 128, PITCH_V);
-              mma_f16_ts(tmem_base, tmem_base + 256 + acol, vh, idesc2, (c > 0 || k16 > 0) ? 1u : 0u);
-              mma_f16_ts(tmem_base, tmem_base + 256 + phalf_cols + acol, vh, idesc2, 1u);
-              mma_f16_ts(tmem_base, tmem_base + 256 + acol, vl, idesc2, 1u);
-            }
-            mma_commit(empty_bar(stage));
-            if (c == nchunk2 - 1) mma_commit(o_full);
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
+      for (int j = 0; j < NV / 8; ++j)
+        *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(oacc[4 * j + 2 * i] * oscale, oacc[4 * j + 2 * i + 1] * oscale);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 12) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
-constexpr size_t SMEM_BYTES = (size_t)STAGES * STAGE + 4 * 32 * EP_LD * sizeof(float) + (2 * STAGES + 4) * 8 + 16;
+constexpr size_t SMEM_BYTES = (size_t)REGION1 + (size_t)STAGES * STAGE2;
 
 }  // namespace attnf
 

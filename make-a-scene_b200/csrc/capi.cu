@@ -1,4 +1,4 @@
-// C-ABI dispatch for the contraction entry points (include/mas_b200.h): picks the tcgen05 path
+// C-ABI dispatch for the contraction entry points (include/mas_b200.h): picks the wgmma path
 // (contract_tc.cu) when the shape is eligible and impl allows, else the fp32 SIMT path.
 #include "mas_common.cuh"
 
@@ -11,7 +11,7 @@ int conv_wgrad_simt_launch(const float* x, mas_tensor4 xs, const float* dy, mas_
 int gemm_simt_launch(const float* A, const float* B, float* C, int M, int N, int K, int batch, int64_t lda, int64_t ldb, int64_t ldc,
                      int64_t sa, int64_t sb, int64_t sc, int ta, int tb, float alpha, const float* bias, const float* res,
                      cudaStream_t st);
-// tcgen05 path; return MAS_ERR_UNSUPPORTED (without touching g_err semantics) when not eligible
+// wgmma path; return MAS_ERR_UNSUPPORTED (without touching g_err semantics) when not eligible
 
 int gemm_tc_launch(const float* A, const float* B, float* C, int M, int N, int K, int batch, int64_t lda, int64_t ldb, int64_t ldc,
                    int64_t sa, int64_t sb, int64_t sc, int ta, int tb, float alpha, const float* bias, const float* res,

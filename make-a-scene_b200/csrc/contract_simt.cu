@@ -1,7 +1,7 @@
 // fp32 FFMA (SIMT) contraction kernels: 3x3 convolution family (fprop / data-grad via packed weights /
 // weight-grad), batched GEMM (1x1 convolutions, attention bmm).  Exact fp32: these are both the
 // general-shape path (edge layers: Cin=3, Cout=3, NCHW views, odd sizes) and the on-GPU checker for the
-// tcgen05 path (contract_tc.cu).  Reference call sites: modules.py:44-81,93-117,145-164,179,186.
+// wgmma path (contract_tc.cu).  Reference call sites: modules.py:44-81,93-117,145-164,179,186.
 #include "mas_common.cuh"
 
 namespace mas {
@@ -496,7 +496,7 @@ int conv3x3_fprop_simt_launch(const float* x, mas_tensor4 xs, const float* w, co
 }
 
 static int wgrad_splits(int64_t M, int tiles, int ntap) {
-  int64_t want = cdiv(148 * 4, (int64_t)tiles * ntap);
+  int64_t want = cdiv(NUM_SMS * 4, (int64_t)tiles * ntap);
   int64_t maxs = cdiv(M, 256);
   int64_t s = want < 1 ? 1 : want;
   if (s > maxs) s = maxs;

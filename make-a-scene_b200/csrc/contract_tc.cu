@@ -1,5 +1,5 @@
-// tcgen05 (5th-gen tensor core) contraction kernels for sm_100a: fp16 operands (3x3 family; same 11-bit significand as TF32,
-// power-of-two operand scales derived on the device) or TF32 operands (1x1 row GEMM, A/B switch), fp32 accumulation in TMEM.
+// Hopper tensor-core (wgmma) contraction kernels for sm_90a: fp16 operands (3x3 family; same 11-bit significand as TF32,
+// power-of-two operand scales derived on the device) or TF32 operands (1x1 row GEMM, A/B switch), fp32 accumulation in registers.
 //
 //   conv3x3 family / row GEMM as a "shift-GEMM":
 //     D[m, n] = sum_{tap} sum_{k} A[slot(m) + shift(tap), k] * B_tap[n, k]
@@ -13,11 +13,10 @@
 //     gradient) and the GroupNorm+SiLU prologue are just a different slot->pixel map / register transform.
 //   * B operand (weights): pre-packed in global memory in the exact shared-memory image and pulled in with ONE
 //     cp.async.bulk (TMA bulk copy, mbarrier complete_tx) per stage.
-//   * two co-resident CTAs per SM, two M tiles (256 pixels, 256 TMEM columns) and a 2-stage ring each: one CTA's epilogue /
-//     pipeline fill overlaps the other's main loop.  warps 0-7 producers then epilogue (tcgen05.ld -> smem transpose ->
-//     bias / residual / GroupNorm statistics -> global), warp 8 = single-thread MMA issuer (+TMEM alloc/dealloc), warp 9 =
-//     bulk-copy issuer; full/empty mbarrier ring.  shift_gemm_p16 is the persistent one-CTA-per-SM variant (opt-in).
-//   * wgrad_tc: the weight gradient (K = pixels): dy through TMA -> tensor memory (TS mode), the activation halo as an
+//   * one CTA per SM, two M tiles (256 pixels) and a 2-stage ring: warps 0-7 (two warpgroups) stage A, then each issues the
+//     wgmma of its 64 rows of both tiles and runs the epilogue (registers -> shared-memory image -> bias / residual / GroupNorm
+//     statistics -> global); the last warpgroup issues the weight bulk copies; full/empty mbarrier ring.
+//   * wgrad_tc: the weight gradient (K = pixels): dy through TMA -> the wgmma A register fragment, the activation halo as an
 //     MN-major fp16 operand (untransposed) or a transposed TF32 one.
 //
 // Reference call sites replaced: nn.Conv2d 3x3 (modules.py:93-104), Upsample/Downsample data paths
@@ -29,13 +28,13 @@
 
 #include "mas_common.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace mas {
 namespace tc {
 
-constexpr int TILES_MAX = 4;   // M tiles per CTA: 4 (all 512 TMEM columns, 1 CTA/SM) or 2 (256 columns, 2 CTAs/SM)
 constexpr int NPROD = 256;     // producer threads (warps 0-7)
-constexpr int NTHREADS = 320;  // + MMA warp + bulk-copy warp
+constexpr int NTHREADS = 384;  // + the bulk-copy warpgroup (one issuing thread; its registers go to the producers)
 constexpr int STAGES_CONV = 3;
 
 enum { MAP_S1 = 0, MAP_UP = 2, MAP_ZS = 3, MAP_ROWS = 4 };
@@ -72,7 +71,7 @@ struct Params {
 // F16 = false: TF32 operands (fp32 words, 4 channels per 16-byte chunk, K = 8 per MMA).
 // F16 = true : fp16 operands converted by the producers (8 channels per 16-byte chunk, K = 16 per MMA); KC still counts channels.
 template <int TAPS, int KC, int STAGES, int TILES, bool F16>
-__global__ void __launch_bounds__(NTHREADS, (TILES == 2) ? 2 : 1) shift_gemm_tc(const Params p) {
+__global__ void __launch_bounds__(NTHREADS, 1) shift_gemm_tc(const Params p) {
   constexpr int EPC = F16 ? 8 : 4;                      // channels per 16-byte operand chunk
   constexpr int SLOTS = (TAPS == 9) ? 180 : 132;        // staged pixels per tile (18x10 halo | 128 rows + pad)
   constexpr int ROWP = (TAPS == 9) ? 10 : 8;            // staged pixels per image row
@@ -88,17 +87,17 @@ __global__ void __launch_bounds__(NTHREADS, (TILES == 2) ? 2 : 1) shift_gemm_tc(
   constexpr int ITEMS = TILES * SLOTS * QUADS;          // 16-byte operand chunks staged per K chunk
   constexpr int LPI = F16 ? 2 : 1;                      // float4 global loads per staged chunk
   constexpr int PER_THREAD = (ITEMS + NPROD - 1) / NPROD;
+  constexpr int ACC_LD = BN + 4;                        // floats per row of the staged accumulator image
   static_assert((SLOTS % 8) == 4, "A plane pitch must be 64 mod 128 bytes for conflict-free producer stores");
+  static_assert(BM * ACC_LD * 4 <= STAGES * STAGE, "one tile's accumulators are staged in the idle operand ring");
 
   extern __shared__ __align__(1024) uint8_t smem[];
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * STAGE);
-  // bars[0..S) full, bars[S..2S) empty, bars[2S] accumulator ready; then the TMEM base address word
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
+  // bars[0..S) full, bars[S..2S) empty
   const uint32_t smem_base = smem_u32(smem);
   const uint32_t bar_base = smem_u32(bars);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t accum_bar = bar_base + 8u * (2 * STAGES);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int64_t tile0 = (int64_t)blockIdx.x * TILES;
@@ -108,19 +107,15 @@ __global__ void __launch_bounds__(NTHREADS, (TILES == 2) ? 2 : 1) shift_gemm_tc(
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), NPROD + 1);
-      mbar_init(empty_bar(s), 1);
+      mbar_init(empty_bar(s), NPROD);
     }
-    mbar_init(accum_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 8) tmem_alloc(smem_u32(tmem_slot), TILES * BN);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   if (warp < 8) {
     // ===================== producers: stage A (input pixels) =====================
+    wg::regs_inc<wg::MMA_REGS>();
     const float* src[PER_THREAD];
     const float* tab[(TAPS == 9) ? PER_THREAD : 1];   // prologue table pointers (3x3 convolutions only)
     uint32_t dst[PER_THREAD];
@@ -163,7 +158,13 @@ __global__ void __launch_bounds__(NTHREADS, (TILES == 2) ? 2 : 1) shift_gemm_tc(
         }
       }
     }
-    int stage = 0;
+    const int wgi = warp >> 2;             // warpgroup: accumulator rows 64 wgi .. 64 wgi + 63 of each tile
+    float acc[TILES][BN / 2];
+#pragma unroll
+    for (int tl = 0; tl < TILES; ++tl)
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[tl][i] = 0.f;
+    int stage = 0, prev = 0;
     uint32_t phase = 0;
     float inv_scale = 1.f;
     const float in_scale = F16 ? operand_scale(p.x_amax, &inv_scale) : 1.f;
@@ -220,6 +221,31 @@ __global__ void __launch_bounds__(NTHREADS, (TILES == 2) ? 2 : 1) shift_gemm_tc(
       }
       fence_proxy_async();  // make the generic-proxy stores visible to the tensor core (async proxy)
       mbar_arrive(full_bar(stage));
+      // every producer's stores and the weight copy have landed: this warpgroup's MMAs over the stage
+      mbar_wait(full_bar(stage), phase);
+      const uint32_t st = smem_base + (uint32_t)stage * STAGE;
+      const uint64_t a_base = wg::desc(st + (uint32_t)(wgi * 8 * SBO_A), LBO_A, SBO_A);
+      const uint64_t b_base = wg::desc(st + A_STAGE, LBO_B, 128);
+      wg::fence();
+#pragma unroll
+      for (int tl = 0; tl < TILES; ++tl) {
+#pragma unroll
+        for (int t = 0; t < TAPS; ++t) {
+          const uint32_t tapoff = (TAPS == 9) ? (uint32_t)(((t / 3) * 10 + (t % 3)) * 16) : 0u;
+#pragma unroll
+          for (int k8 = 0; k8 < KC / (2 * EPC); ++k8) {   // one MMA = two 16-byte chunks of K (8 tf32 | 16 fp16)
+            const uint64_t ad = a_base + (uint64_t)((tl * A_TILE + tapoff + k8 * 2 * LBO_A) >> 4);
+            const uint64_t bd = b_base + (uint64_t)((t * B_TAP + k8 * 2 * LBO_B) >> 4);
+            if (F16) wg::wgmma_f16_ss_n128<0, 0>(acc[tl], ad, bd, 1u);
+            else wg::wgmma_tf32_ss_n128(acc[tl], ad, bd, 1u);
+          }
+        }
+      }
+      wg::commit();
+      // the MMAs of the previous chunk have read their stage: release it to the producers and the weight copy
+      wg::wait<1>();
+      if (kc > 0) mbar_arrive(empty_bar(prev));
+      prev = stage;
       if (++stage == STAGES) { stage = 0; phase ^= 1; }
     };
     gload(0, va);
@@ -232,24 +258,32 @@ __global__ void __launch_bounds__(NTHREADS, (TILES == 2) ? 2 : 1) shift_gemm_tc(
         if (kc + 3 < nchunks) gload(kc + 3, vb);
       }
     }
+    wg::wait<0>();
+#pragma unroll
+    for (int tl = 0; tl < TILES; ++tl) wg::fence_regs<BN / 2>(acc[tl]);
     const float alpha = p.alpha * inv_scale;
 
-    // ===================== epilogue: TMEM -> registers -> smem transpose -> coalesced global stores =====================
-    // A thread owns one pixel row of the accumulator (32 consecutive channels per tcgen05.ld); writing that directly
-    // makes every store instruction touch 32 different 128-byte lines with 16 bytes each.  Each warp instead bounces
-    // its 32x32 block through a private shared-memory patch (the pipeline stages are idle by now) so that 8 lanes
-    // cover one full line: 4 lines per store instruction, and the residual is read the same way.
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    const int lane_grp = warp & 3;           // TMEM lanes [32*lane_grp, +32)
+    // ===================== epilogue: registers -> shared-memory accumulator image -> coalesced global stores =====================
+    // The fragment of a thread is scattered over 16 rows; the tile is staged as a [128][BN] image in the (now idle) operand
+    // ring so that each warp can then read a 32-row x 32-channel block with 8 lanes per pixel row: 4 lines per store
+    // instruction, and the residual is read the same way.
+    const int lane_grp = warp & 3;           // accumulator rows [32*lane_grp, +32)
     const int chalf = warp >> 2;             // column half of the 128-wide tile
-    constexpr int EP_LD = 36;                // floats per staged row (144 B: conflict-free 16-byte accesses)
-    float* patch = reinterpret_cast<float*>(smem) + warp * (32 * EP_LD);
+    float* img = reinterpret_cast<float*>(smem);
     const int sub_r = lane >> 3, sub_c = lane & 7;
-#pragma unroll 1
+    const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+#pragma unroll
     for (int tl = 0; tl < TILES; ++tl) {
       const int64_t tile = tile0 + tl;
-      if (tile >= p.total_tiles) break;     // warp-uniform
+      if (tile >= p.total_tiles) break;     // block-uniform
+      wg::bar_sync(1, NPROD);               // the previous tile's image has been read (first tile: every MMA has completed)
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j)
+#pragma unroll
+        for (int i = 0; i < 2; ++i)
+          *reinterpret_cast<float2*>(img + (frow + 8 * i) * ACC_LD + 8 * j + fcol) =
+              make_float2(acc[tl][4 * j + 2 * i] * alpha, acc[tl][4 * j + 2 * i + 1] * alpha);
+      wg::bar_sync(1, NPROD);
       int64_t pix_base = 0;                 // pixel index of accumulator row 0 of this tile (image maps: per-row formula)
       int tx_ = 0, ty_ = 0, n_img = 0;
       if (TAPS == 9) {
@@ -261,14 +295,6 @@ __global__ void __launch_bounds__(NTHREADS, (TILES == 2) ? 2 : 1) shift_gemm_tc(
 #pragma unroll 1
       for (int cc = 0; cc < 2; ++cc) {
         const int col = chalf * 64 + cc * 32;
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)(tl * BN + col), v);
-        __syncwarp();
-#pragma unroll
-        for (int j = 0; j < 32; j += 4)
-          *reinterpret_cast<float4*>(patch + lane * EP_LD + j) =
-              make_float4(v[j] * alpha, v[j + 1] * alpha, v[j + 2] * alpha, v[j + 3] * alpha);
-        __syncwarp();
         float4 bq = make_float4(0.f, 0.f, 0.f, 0.f);
         if (p.bias) bq = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + col + sub_c * 4));
         float st_s = 0.f, st_q = 0.f;
@@ -280,7 +306,7 @@ __global__ void __launch_bounds__(NTHREADS, (TILES == 2) ? 2 : 1) shift_gemm_tc(
           if (TAPS == 9) pix = ((int64_t)n_img * p.Hout + ty_ * 16 + (m >> 3)) * p.Wout + tx_ * 8 + (m & 7);
           else pix = pix_base + m;
           if (TAPS == 9 || pix < (int64_t)p.N * p.Hout * p.Wout) {
-            float4 o = *reinterpret_cast<const float4*>(patch + row * EP_LD + sub_c * 4);
+            float4 o = *reinterpret_cast<const float4*>(img + m * ACC_LD + col + sub_c * 4);
             o.x += bq.x; o.y += bq.y; o.z += bq.z; o.w += bq.w;
             const int64_t off = pix * p.ldy + n0 + col + sub_c * 4;
             if (n0 + col + sub_c * 4 >= p.Cstore) continue;   // padded output channels (4-channel granularity)
@@ -306,48 +332,10 @@ __global__ void __launch_bounds__(NTHREADS, (TILES == 2) ? 2 : 1) shift_gemm_tc(
         }
       }
     }
-    tc_fence_before();
-  } else if (warp == 8) {
-    // ===================== MMA issuer =====================
-    // warp-uniform loop (descriptors stay in uniform registers), one elected lane issues: see conv_tma.cu
-    {
-      constexpr uint32_t idesc = F16 ? make_idesc_f16(BN) : make_idesc(BN);
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kc = 0; kc < nchunks; ++kc) {
-        mbar_wait(full_bar(stage), phase);
-        tc_fence_after();
-        // one base descriptor per operand per stage; every MMA of the stage is (base + compile-time constant): the
-        // start-address field is the low 14 bits (address >> 4) and never carries out for < 256 KB of shared memory
-        const uint32_t a_st = smem_base + (uint32_t)stage * STAGE;
-        const uint64_t a_base = make_desc(a_st, LBO_A, SBO_A);
-        const uint64_t b_base = make_desc(a_st + A_STAGE, LBO_B, 128);
-        const uint32_t acc0 = (kc > 0) ? 1u : 0u;
-        if (elect_one()) {
-#pragma unroll
-          for (int tl = 0; tl < TILES; ++tl) {
-#pragma unroll
-            for (int t = 0; t < TAPS; ++t) {
-              const uint32_t tapoff = (TAPS == 9) ? (uint32_t)(((t / 3) * 10 + (t % 3)) * 16) : 0u;
-#pragma unroll
-              for (int k8 = 0; k8 < KC / (2 * EPC); ++k8) {   // one MMA = two 16-byte chunks of K (8 tf32 | 16 fp16)
-                const uint64_t ad = a_base + (uint64_t)((tl * A_TILE + tapoff + k8 * 2 * LBO_A) >> 4);
-                const uint64_t bd = b_base + (uint64_t)((t * B_TAP + k8 * 2 * LBO_B) >> 4);
-                if (F16) mma_f16_ss(tmem_base + (uint32_t)(tl * BN), ad, bd, idesc, (t > 0 || k8 > 0) ? 1u : acc0);
-                else mma_tf32_ss(tmem_base + (uint32_t)(tl * BN), ad, bd, idesc, (t > 0 || k8 > 0) ? 1u : acc0);
-              }
-            }
-          }
-          mma_commit(empty_bar(stage));  // frees the smem stage when these MMAs have read it
-          if (kc == nchunks - 1) mma_commit(accum_bar);  // all accumulators complete
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-    }
   } else {
     // ===================== weight bulk-copy issuer (one thread) =====================
-    if (lane == 0) {
+    wg::regs_dec<wg::COPY_REGS>();
+    if (warp == 8 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       const float* wsrc = p.wpk + (size_t)blockIdx.y * nchunks * (B_STAGE / 4);
@@ -360,312 +348,6 @@ __global__ void __launch_bounds__(NTHREADS, (TILES == 2) ? 2 : 1) shift_gemm_tc(
     }
     __syncwarp();
   }
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TILES * BN);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------------------
-// Persistent form of the fp16-operand 3x3 kernel (the production path).  ncu on shift_gemm_tc<9,16,2,2,true> (profiles/
-// r02_ncu_conv_f16.md): tensor pipe 43 % active, the producers' global-load latency and the per-CTA prologue / epilogue
-// exposed because a CTA owns one pair of tiles and a 2-stage ring.  Here ONE CTA per SM walks a list of work items
-// (pair of 128-pixel tiles x 128 output channels):
-//   * 4-stage operand ring that keeps running ACROSS work items: the producers of item i+1 fill stages while the MMAs of
-//     item i drain them (no pipeline fill / drain per tile pair);
-//   * two accumulator sets in tensor memory (2 x 256 columns): dedicated epilogue warps drain set b while the MMAs of the
-//     next item run into set b^1;
-//   * warps 0-7 producers (register-staged A operand, ping-pong prefetch), 8-11 epilogue, 12 MMA issuer, 13 weight bulk copies.
-// Same operand layouts, packed weights, slot maps (S1 / UP / ZS), GroupNorm prologue and statistics epilogue as shift_gemm_tc.
-constexpr int P_STAGES = 4;
-constexpr int P_NTHREADS = 14 * 32;
-constexpr int P_EPI0 = 8;      // first epilogue warp (8 % 4 == 0: warp w owns TMEM lanes 32 * (w % 4))
-
-__global__ void __launch_bounds__(P_NTHREADS, 1) shift_gemm_p16(const Params p) {
-  constexpr int KC = 16, EPC = 8, TILES = 2, TAPS = 9;
-  constexpr int SLOTS = 180, ROWP = 10;
-  constexpr int LBO_A = SLOTS * 16, SBO_A = ROWP * 16;
-  constexpr int A_TILE = (KC / EPC) * LBO_A, A_STAGE = TILES * A_TILE;
-  constexpr int LBO_B = BN * 16, B_TAP = (KC / EPC) * LBO_B, B_STAGE = TAPS * B_TAP;
-  constexpr int STAGE = A_STAGE + B_STAGE;
-  constexpr int QUADS = KC / EPC;
-  constexpr int ITEMS = TILES * SLOTS * QUADS;
-  constexpr int PER_THREAD = (ITEMS + NPROD - 1) / NPROD;
-  constexpr int EP_LD = 36;
-
-  extern __shared__ __align__(1024) uint8_t smem[];
-  float* patches = reinterpret_cast<float*>(smem + (size_t)P_STAGES * STAGE);                  // 4 warps x [32][EP_LD]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(patches + 4 * 32 * EP_LD);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * P_STAGES + 4);
-  const uint32_t smem_base = smem_u32(smem), bar_base = smem_u32(bars);
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (P_STAGES + s); };
-  auto accf_bar = [&](int b) { return bar_base + 8u * (2 * P_STAGES + b); };
-  auto acce_bar = [&](int b) { return bar_base + 8u * (2 * P_STAGES + 2 + b); };
-
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int nchunks = p.Cin / KC;
-  const int n_tiles = p.Cout / BN;
-  const int64_t ngroups = (p.total_tiles + TILES - 1) / TILES;
-  const int64_t nitems = ngroups * n_tiles;       // work item = (group of two M tiles, output-channel tile); channel tile fastest
-
-  if (tid == 0) {
-    for (int s = 0; s < P_STAGES; ++s) {
-      mbar_init(full_bar(s), NPROD + 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(accf_bar(b), 1);
-      mbar_init(acce_bar(b), 128);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 12) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-
-  if (warp < 8) {
-    // ===================== producers =====================
-    // (A variant with 128-byte-per-pixel "wide" loads - eight lanes per pixel, a double K chunk per step - measured 1.8x
-    // SLOWER: 1.25 vs 0.70 ms on the dominant layer; the narrow 32-byte pieces with two register sets stay.)
-    float inv_scale = 1.f;
-    const float in_scale = operand_scale(p.x_amax, &inv_scale);
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-      const int64_t tile0 = (item / n_tiles) * TILES;
-      const float* src[PER_THREAD];
-      const float* tab[PER_THREAD];
-      uint32_t dst[PER_THREAD];
-#pragma unroll
-      for (int i = 0; i < PER_THREAD; ++i) {
-        const int it = tid + i * NPROD;
-        src[i] = nullptr;
-        tab[i] = nullptr;
-        dst[i] = 0xFFFFFFFFu;
-        if (it < ITEMS) {
-          const int q = it % QUADS, rest = it / QUADS, slot = rest % SLOTS, tl = rest / SLOTS;
-          dst[i] = (uint32_t)(tl * A_TILE + q * LBO_A + slot * 16);
-          const int64_t tile = tile0 + tl;
-          if (tile < p.total_tiles) {
-            const int tx_ = (int)(tile % p.tiles_x), ty_ = (int)((tile / p.tiles_x) % p.tiles_y);
-            const int n = (int)(tile / ((int64_t)p.tiles_x * p.tiles_y));
-            const int r = slot / 10, c = slot % 10;
-            const int vy = ty_ * 16 - 1 + r, vx = tx_ * 8 - 1 + c;
-            int iy = vy, ix = vx;
-            bool ok;
-            if (p.map == MAP_S1) {
-              ok = (unsigned)vy < (unsigned)p.Hin && (unsigned)vx < (unsigned)p.Win;
-            } else if (p.map == MAP_UP) {
-              ok = (unsigned)vy < (unsigned)(2 * p.Hin) && (unsigned)vx < (unsigned)(2 * p.Win);
-              iy = vy >> 1; ix = vx >> 1;
-            } else {  // MAP_ZS
-              ok = vy >= 0 && vx >= 0 && (vy & 1) && (vx & 1) && (vy >> 1) < p.Hin && (vx >> 1) < p.Win;
-              iy = vy >> 1; ix = vx >> 1;
-            }
-            if (ok) {
-              src[i] = p.x + ((int64_t)(n * p.Hin + iy) * p.Win + ix) * p.ldx + q * EPC;
-              if (p.gn_table) tab[i] = p.gn_table + ((size_t)n * p.Cin + q * EPC) * 2;
-            }
-          }
-        }
-      }
-      float4 va[PER_THREAD][2], vb[PER_THREAD][2];
-      auto gload = [&](int kc, float4 (*v)[2]) {
-#pragma unroll
-        for (int i = 0; i < PER_THREAD; ++i) {
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            v[i][h] = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (src[i]) v[i][h] = ldg_l2pf(reinterpret_cast<const float4*>(src[i] + (size_t)kc * KC) + h);
-          }
-        }
-      };
-      auto consume = [&](int kc, float4 (*v)[2]) {
-        if (p.gn_table) {
-#pragma unroll
-          for (int i = 0; i < PER_THREAD; ++i) {
-            if (tab[i]) {
-#pragma unroll
-              for (int h = 0; h < 2; ++h) {
-                const float4* tp = reinterpret_cast<const float4*>(tab[i] + (size_t)kc * KC * 2) + 2 * h;
-                const float4 t0 = __ldg(tp);
-                const float4 t1 = __ldg(tp + 1);
-                float a0 = fmaf(v[i][h].x, t0.x, t0.y), a1 = fmaf(v[i][h].y, t0.z, t0.w);
-                float a2 = fmaf(v[i][h].z, t1.x, t1.y), a3 = fmaf(v[i][h].w, t1.z, t1.w);
-                if (p.gn_silu) { a0 = silu_f(a0); a1 = silu_f(a1); a2 = silu_f(a2); a3 = silu_f(a3); }
-                v[i][h] = make_float4(a0, a1, a2, a3);
-              }
-            }
-          }
-        }
-        mbar_wait(empty_bar(stage), phase ^ 1);
-        uint8_t* a_st = smem + (size_t)stage * STAGE;
-#pragma unroll
-        for (int i = 0; i < PER_THREAD; ++i) {
-          if (dst[i] != 0xFFFFFFFFu) {
-            const float4 lo = v[i][0], hi = v[i][1];
-            *reinterpret_cast<uint4*>(a_st + dst[i]) =
-                make_uint4(pack_h2(lo.x * in_scale, lo.y * in_scale), pack_h2(lo.z * in_scale, lo.w * in_scale),
-                           pack_h2(hi.x * in_scale, hi.y * in_scale), pack_h2(hi.z * in_scale, hi.w * in_scale));
-          }
-        }
-        fence_proxy_async();
-        mbar_arrive(full_bar(stage));
-        if (++stage == P_STAGES) { stage = 0; phase ^= 1; }
-      };
-      gload(0, va);
-      if (nchunks > 1) gload(1, vb);
-      for (int kc = 0; kc < nchunks; kc += 2) {
-        consume(kc, va);
-        if (kc + 2 < nchunks) gload(kc + 2, va);
-        if (kc + 1 < nchunks) {
-          consume(kc + 1, vb);
-          if (kc + 3 < nchunks) gload(kc + 3, vb);
-        }
-      }
-    }
-  } else if (warp < 12) {
-    // ===================== epilogue warps: drain one accumulator set while the other is being filled =====================
-    float inv_scale = 1.f;
-    operand_scale(p.x_amax, &inv_scale);
-    const float alpha = p.alpha * inv_scale;
-    const int lane_grp = warp & 3;
-    float* patch = patches + lane_grp * (32 * EP_LD);
-    const int sub_r = lane >> 3, sub_c = lane & 7;
-    int buf = 0;
-    uint32_t ph[2] = {0u, 0u};
-    for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-      const int64_t tile0 = (item / n_tiles) * TILES;
-      const int n0 = (int)(item % n_tiles) * BN;
-      mbar_wait(accf_bar(buf), ph[buf]);
-      ph[buf] ^= 1u;
-      tc_fence_after();
-#pragma unroll 1
-      for (int tl = 0; tl < TILES; ++tl) {
-        const int64_t tile = tile0 + tl;
-        const bool live = tile < p.total_tiles;           // warp-uniform
-        const int tx_ = (int)(tile % p.tiles_x), ty_ = (int)((tile / p.tiles_x) % p.tiles_y);
-        const int n_img = (int)(tile / ((int64_t)p.tiles_x * p.tiles_y));
-#pragma unroll 1
-        for (int cb = 0; cb < BN / 32; ++cb) {
-          const int col = cb * 32;
-          float v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)(buf * TILES * BN + tl * BN + col), v);
-          if (tl == TILES - 1 && cb == BN / 32 - 1) {
-            // everything this thread needs from the accumulator set is in registers: hand it back to the MMA warp now
-            tc_fence_before();
-            mbar_arrive(acce_bar(buf));
-          }
-          if (!live) continue;
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            *reinterpret_cast<float4*>(patch + lane * EP_LD + j) =
-                make_float4(v[j] * alpha, v[j + 1] * alpha, v[j + 2] * alpha, v[j + 3] * alpha);
-          __syncwarp();
-          float4 bq = make_float4(0.f, 0.f, 0.f, 0.f);
-          if (p.bias) bq = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + col + sub_c * 4));
-          float st_s = 0.f, st_q = 0.f;
-#pragma unroll
-          for (int i = 0; i < 8; ++i) {
-            const int row = i * 4 + sub_r;
-            const int m = lane_grp * 32 + row;
-            const int64_t pix = ((int64_t)n_img * p.Hout + ty_ * 16 + (m >> 3)) * p.Wout + tx_ * 8 + (m & 7);
-            float4 o = *reinterpret_cast<const float4*>(patch + row * EP_LD + sub_c * 4);
-            o.x += bq.x; o.y += bq.y; o.z += bq.z; o.w += bq.w;
-            const int64_t off = pix * p.ldy + n0 + col + sub_c * 4;
-            if (n0 + col + sub_c * 4 >= p.Cstore) continue;   // padded output channels (4-channel granularity)
-            if (p.res) {
-              const float4 r4 = __ldg(reinterpret_cast<const float4*>(p.res + off));
-              o.x += r4.x; o.y += r4.y; o.z += r4.z; o.w += r4.w;
-            }
-            *reinterpret_cast<float4*>(p.y + off) = o;
-            st_s += (o.x + o.y) + (o.z + o.w);
-            st_q = fmaf(o.x, o.x, fmaf(o.y, o.y, fmaf(o.z, o.z, fmaf(o.w, o.w, st_q))));
-          }
-          if (p.stats_part) {
-            st_s += __shfl_xor_sync(0xffffffffu, st_s, 8);
-            st_q += __shfl_xor_sync(0xffffffffu, st_q, 8);
-            st_s += __shfl_xor_sync(0xffffffffu, st_s, 16);
-            st_q += __shfl_xor_sync(0xffffffffu, st_q, 16);
-            if (lane < 8) {
-              float* sp = p.stats_part + (((size_t)tile * 4 + lane_grp) * (p.Cout >> 2) + ((n0 + col) >> 2) + sub_c) * 2;
-              sp[0] = st_s;
-              sp[1] = st_q;
-            }
-          }
-        }
-      }
-      buf ^= 1;
-    }
-  } else if (warp == 12) {
-    // ===================== MMA issuer (warp-uniform loop, one elected lane issues) =====================
-    {
-      constexpr uint32_t idesc = make_idesc_f16(BN);
-      int stage = 0, buf = 0;
-      uint32_t phase = 0, eph[2] = {0u, 0u};
-      for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-        mbar_wait(acce_bar(buf), eph[buf] ^ 1);     // the epilogue warps have read this accumulator set (first use: passes)
-        eph[buf] ^= 1u;
-        tc_fence_after();
-        const uint32_t acc = tmem_base + (uint32_t)(buf * TILES * BN);
-        for (int kc = 0; kc < nchunks; ++kc) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t a_st = smem_base + (uint32_t)stage * STAGE;
-          const uint64_t a_base = make_desc(a_st, LBO_A, SBO_A);
-          const uint64_t b_base = make_desc(a_st + A_STAGE, LBO_B, 128);
-          const uint32_t acc0 = (kc > 0) ? 1u : 0u;
-          if (elect_one()) {
-#pragma unroll
-            for (int tl = 0; tl < TILES; ++tl) {
-#pragma unroll
-              for (int t = 0; t < TAPS; ++t) {
-                const uint32_t tapoff = (uint32_t)(((t / 3) * 10 + (t % 3)) * 16);
-                const uint64_t ad = a_base + (uint64_t)((tl * A_TILE + tapoff) >> 4);
-                const uint64_t bd = b_base + (uint64_t)((t * B_TAP) >> 4);
-                mma_f16_ss(acc + (uint32_t)(tl * BN), ad, bd, idesc, t > 0 ? 1u : acc0);
-              }
-            }
-            mma_commit(empty_bar(stage));
-            if (kc == nchunks - 1) mma_commit(accf_bar(buf));
-          }
-          __syncwarp();
-          if (++stage == P_STAGES) { stage = 0; phase ^= 1; }
-        }
-        buf ^= 1;
-      }
-    }
-  } else {
-    // ===================== weight bulk-copy issuer (one thread) =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-        const float* wsrc = p.wpk + (size_t)(item % n_tiles) * nchunks * (B_STAGE / 4);
-        for (int kc = 0; kc < nchunks; ++kc) {
-          mbar_wait(empty_bar(stage), phase ^ 1);
-          mbar_expect_tx(full_bar(stage), B_STAGE);
-          bulk_g2s(smem_base + (uint32_t)stage * STAGE + A_STAGE, wsrc + (size_t)kc * (B_STAGE / 4), B_STAGE, full_bar(stage));
-          if (++stage == P_STAGES) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-    __syncwarp();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 12) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-constexpr size_t p16_smem_bytes() {
-  return (size_t)P_STAGES * (2 * 2 * 180 * 16 + 9 * 2 * BN * 16) + 4 * 32 * 36 * 4 + (2 * P_STAGES + 4) * 8 + 16;
 }
 
 template <int TAPS, int KC, int STAGES, int TILES, bool F16>
@@ -748,20 +430,21 @@ __global__ void pack_weights_tc_pair(const float* __restrict__ w, float* __restr
 
 
 // ------------------------------------------------------------------------------------------------------------
-// Weight gradient on tcgen05:  dW[tap][co][ci] = sum_pixels dy[p][co] * xa[p + tap][ci]
-//   D (TMEM, 9 accumulators of 128 co x NT ci)  +=  A (TMEM: dy^T, lanes = co, columns = pixels)  x  B (smem: xa halo)
-//   * The reduction (K) dimension is the PIXEL index.  A lives in tensor memory (tcgen05.st from registers: lane = co makes
-//     the global reads of dy[p][co0..co0+127] coalesced and the transpose free), so the nine taps re-read it at no
-//     shared-memory cost; B is the same staged halo the forward kernel uses ([ci/4][slot][4 floats], here an
-//     MN-major operand whose K stride is one 16-byte pixel slot), and a tap is a start-address shift of the descriptor.
-//   * unit of pipelining = 8x8 output pixels (halo 10x10): 9 taps x 8 image rows = 72 MMAs of 128 x NT x 8.
+// Weight gradient on the Hopper tensor cores:  dW[tap][co][ci] = sum_pixels dy[p][co] * xa[p + tap][ci]
+//   D (registers, 3 | 1 accumulators of 64 co x 3 NT ci per warpgroup)  +=  A (registers: dy^T, rows = co, K = pixels)  x
+//   B (smem: xa halo)
+//   * The reduction (K) dimension is the PIXEL index.  A is read by each MMA warpgroup straight from the staged dy tile into
+//     the wgmma register fragment (rows = co: the transpose is free), so the three kernel rows re-read it at no
+//     shared-memory cost; B is the same staged halo the forward kernel uses ([ci/4][slot][4 floats], here a K-major
+//     operand whose K stride is one 16-byte pixel chunk), and a tap is a start-address shift of the descriptor.
+//   * unit of pipelining = 8x8 output pixels (halo 10x10): 3 kernel rows x 8 image rows = 24 MMAs of 64 x 96 x 8 per warpgroup.
 //   * CTA = (128 co) x (NT ci) x (a contiguous range of units); partial results go to the split-K workspace that the
-//     SIMT path also uses and are reduced deterministically; the per-channel sums of dy (bias gradient) fall out of
-//     the A loader for free.
+//     SIMT path also uses and are reduced deterministically; the per-channel sums of dy (bias gradient) are taken from the
+//     staged dy tile.
 constexpr int WG_NT = 32;
 constexpr int WG_STAGES = 3;
 constexpr int WG_SLOTS = 100;          // 10 x 10 halo
-constexpr int WG_THREADS = 14 * 32;    // 8 producer warps, 4 A-loader warps, 1 MMA warp, 1 bulk-copy warp
+constexpr int WG_THREADS = 12 * 32;    // 8 producer / MMA warps, the dy copy warpgroup
 constexpr int WG_DY_STAGE = 64 * 128 * 4;  // staged dy tile: 64 pixels x 128 channels fp32
 
 struct WParams {
@@ -783,48 +466,42 @@ struct WParams {
 // TAPS == 9: 3x3 convolution (unit = 8x8 output pixels, halo 10x10).  TAPS == 1: 1x1 convolution / row GEMM
 // (unit = 64 consecutive rows, no halo).
 // F16 (3x3 only): both operands converted to fp16 on their way to the tensor core (dy scaled by a power of two from
-// p.dy_amax); a 16-byte chunk of B then holds 8 pixels = one halo row segment, one MMA (K = 16) covers two image rows
-// of the unit, and A packs two pixels per TMEM column.
+// p.dy_amax); a 16-byte chunk of B then holds 8 pixels = one halo row segment and one MMA (K = 16) covers two image rows
+// of the unit.
 template <int TAPS, bool PRO, bool F16>
 __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc(const WParams p, const __grid_constant__ CUtensorMap dy_map) {
   static_assert(!F16 || TAPS == 9, "the fp16-operand weight-gradient kernel is the 3x3 one");
-  // B (the shifted operand) must be K-major with K = pixel: tests/test_gpu_tc_probe.py shows that kind::tf32 returns
-  // zeros for MN-major shared-memory operands, so the halo is staged TRANSPOSED ([ci][pixel], 4 pixels per 16-byte
-  // chunk) once per horizontal tap offset dx (3 copies); vertical offsets are whole-chunk K advances of the descriptor.
+  // B (the shifted operand) must be K-major with K = pixel for TF32 (wgmma transposes 16-bit operands only), so the halo is
+  // staged TRANSPOSED ([ci][pixel], 4 pixels per 16-byte chunk) once per horizontal tap offset dx (3 copies); vertical
+  // offsets are whole-chunk K advances of the descriptor.
   // Channel ci = 4q + j of the tile sits in operand row n = 8j + q: the 8 lanes of a store phase (q = 0..7) then hit 8
-  // different bank groups, and the epilogue undoes the permutation in registers.
+  // different bank groups, and the epilogue undoes the permutation.
   // One MMA covers the three horizontal taps of a kernel row: its N = 3 x NT operand rows are [dx][channel], laid out
   // per 4-pixel chunk as 3*NT/8 consecutive 128-byte core matrices, so a single descriptor (SBO = 128, LBO = chunk
-  // pitch) spans all three dx copies.  (N = 32 MMAs are issue-bound: ~4x slower than their 16-cycle math.)
+  // pitch) spans all three dx copies.
   constexpr int NT = (TAPS == 9) ? WG_NT : 128, QUADS = NT / 4;
   constexpr int SLOTS = (TAPS == 9) ? WG_SLOTS : 64;
   constexpr int COPIES = (TAPS == 9) ? 3 : 1;
   constexpr int LBO_B = COPIES * NT * 16;                  // TF32: bytes between 16-byte chunks (4 pixels)
-  // fp16: kind::f16 DOES take MN-major shared-memory operands (tests/test_gpu_tc_probe.py::test_reveal_raw_f16: element (n, k)
-  // sits at (n%8)*2 + (k%8)*16 + (k/8)*LBO + (n/8)*SBO bytes), so the halo is staged UNTRANSPOSED, as planes
-  // [dx copy][ci/8][slot][8 channels]: a pixel's 8 channels are one 16-byte store per dx copy (copy dx holds the halo shifted
-  // left by dx pixels) instead of 24 two-byte stores; K groups are image rows (LBO = the 160-byte halo row), N groups are the
-  // 12 (dx, ci/8) planes (SBO = plane pitch), a vertical tap is a start-address advance of one halo row.
+  // fp16: the halo is staged UNTRANSPOSED (an MN-major operand: element (n, k) sits at (n%8)*2 + (k%8)*16 + (k/8)*LBO +
+  // (n/8)*SBO bytes), as planes [dx copy][ci/8][slot][8 channels]: a pixel's 8 channels are one 16-byte store per dx copy (copy
+  // dx holds the halo shifted left by dx pixels) instead of 24 two-byte stores; K groups are image rows (LBO = the 160-byte
+  // halo row), N groups are the 12 (dx, ci/8) planes (SBO = plane pitch), a vertical tap is a start-address advance of one
+  // halo row.
   constexpr int P16 = SLOTS * 16 + 32;                     // plane pitch (32-byte skew: conflict-free 16-byte stores)
   constexpr int B_STAGE = F16 ? 12 * P16 : ((TAPS == 9) ? 20 : 16) * LBO_B;
-  constexpr int A_COLS = F16 ? 32 : 64;                    // TMEM columns of one staged dy tile (64 pixels)
   constexpr int ITEMS = SLOTS * QUADS, PER_THREAD = (ITEMS + NPROD - 1) / NPROD;
-  constexpr uint32_t ACC_COLS = TAPS * NT;
   constexpr int NMMA = COPIES * NT;                        // N of one MMA (96 | 128)
-  // instruction descriptor: D=f32, A=tf32 (TMEM, K-major), B=tf32 K-major, M=128, N=NMMA
-  constexpr uint32_t idesc = F16 ? (make_idesc_f16(NMMA) | (1u << 16))   // bit 16: B operand MN-major
-                                 : ((1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(NMMA >> 3) << 17) | ((uint32_t)(BM >> 4) << 24));
+  constexpr int NACC = (TAPS == 9) ? 3 : 1;                // accumulators: one per kernel row
+  constexpr int KSTEPS = F16 ? 4 : 8;                      // MMAs per kernel row and unit (K = 16 | 8 pixels)
 
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* dy_smem = smem + (size_t)WG_STAGES * B_STAGE;   // [WG_STAGES][64 pixels][128 co] fp32, filled by cp.async.bulk
+  uint8_t* dy_smem = smem + (size_t)WG_STAGES * B_STAGE;   // [WG_STAGES][64 pixels][128 co] fp32 (or halves), filled by TMA
   uint64_t* bars = reinterpret_cast<uint64_t*>(dy_smem + (size_t)WG_STAGES * WG_DY_STAGE);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 4 * WG_STAGES + 1);
   const uint32_t smem_base = smem_u32(smem), bar_base = smem_u32(bars);
   auto fullB = [&](int s) { return bar_base + 8u * s; };
-  auto fullA = [&](int s) { return bar_base + 8u * (WG_STAGES + s); };
-  auto empty = [&](int s) { return bar_base + 8u * (2 * WG_STAGES + s); };
-  auto fullD = [&](int s) { return bar_base + 8u * (3 * WG_STAGES + s); };
-  const uint32_t accum_bar = bar_base + 8u * (4 * WG_STAGES);
+  auto empty = [&](int s) { return bar_base + 8u * (WG_STAGES + s); };
+  auto fullD = [&](int s) { return bar_base + 8u * (2 * WG_STAGES + s); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ci0 = blockIdx.x * NT, co0 = blockIdx.y * BM, split = blockIdx.z;
@@ -834,21 +511,87 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc(const WParams p, const
   if (tid == 0) {
     for (int s = 0; s < WG_STAGES; ++s) {
       mbar_init(fullB(s), NPROD);
-      mbar_init(fullA(s), 128);
-      mbar_init(empty(s), 1);
+      mbar_init(empty(s), NPROD);
       mbar_init(fullD(s), 1);
     }
-    mbar_init(accum_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 12) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp < 8 && F16) {
-    // ============ producers, fp16: x halo -> shared memory planes [dx][ci/8][slot][8 channels] (no transposition) ============
+  if (warp < 8) {
+    wg::regs_inc<wg::MMA_REGS>();
+    const int wgi = warp >> 2;
+    const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2), fk = lane & 3;   // fragment row (co) and K quad of this thread
+    float acc[NACC][NMMA / 2];
+#pragma unroll
+    for (int a = 0; a < NACC; ++a)
+#pragma unroll
+      for (int i = 0; i < NMMA / 2; ++i) acc[a][i] = 0.f;
+    float bsum = 0.f;
+    const bool want_bias = p.bpart != nullptr && blockIdx.x == 0 && tid < 128;   // thread tid sums channel co0 + tid
+    float a_inv = 1.f;
+    const float a_scale = F16 ? operand_scale(p.dy_amax, &a_inv) : 1.f;
+    // all producers have staged B and the dy tile has landed: this warpgroup's MMAs of unit u
+    auto mma_unit = [&](int64_t u, int stage, uint32_t phase) {
+      mbar_wait(fullB(stage), phase);
+      mbar_wait(fullD(stage), phase);
+      const uint8_t* dyt = dy_smem + (size_t)stage * WG_DY_STAGE;
+      const bool shadow = F16 && p.dy_f16;
+      if (want_bias) {   // the bias gradient falls out of ONE ci-tile's pass over dy (the other ci tiles see the same dy)
+        if (shadow) {
+          const __half* dh = reinterpret_cast<const __half*>(dyt) + tid;
+          for (int j = 0; j < 64; j += 2) bsum += __half2float(dh[j * 128]) + __half2float(dh[(j + 1) * 128]);
+        } else {
+          const float* df = reinterpret_cast<const float*>(dyt) + tid;
+          for (int j = 0; j < 64; ++j) bsum += (TAPS == 9 || u * 64 + j < p.rows) ? df[j * 128] : 0.f;
+        }
+      }
+      // A fragments of the unit: a[ks][0..3] = dy^T rows (frow, frow + 8) x pixels of K step ks
+      uint32_t a[KSTEPS][4];
+#pragma unroll
+      for (int ks = 0; ks < KSTEPS; ++ks) {
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+          const int co = frow + 8 * (h & 1);
+          if (F16) {
+            const int px = ks * 16 + 2 * fk + 8 * (h >> 1);
+            if (shadow) {
+              const unsigned short* dh = reinterpret_cast<const unsigned short*>(dyt) + co;
+              a[ks][h] = (uint32_t)dh[px * 128] | ((uint32_t)dh[(px + 1) * 128] << 16);
+            } else {
+              const float* df = reinterpret_cast<const float*>(dyt) + co;
+              a[ks][h] = pack_h2(df[px * 128] * a_scale, df[(px + 1) * 128] * a_scale);
+            }
+          } else {
+            const int px = ks * 8 + fk + 4 * (h >> 1);
+            const float v = reinterpret_cast<const float*>(dyt)[px * 128 + co];
+            a[ks][h] = __float_as_uint((TAPS == 9 || u * 64 + px < p.rows) ? v : 0.f);
+          }
+        }
+      }
+      const uint32_t b_st = smem_base + (uint32_t)stage * B_STAGE;
+      const uint64_t b_base = wg::desc(b_st, LBO_B, 128);
+      const uint64_t b16 = wg::desc(b_st, 160, P16);   // MN-major: LBO = K-group (halo row) pitch, SBO = N-group (plane) pitch
+      wg::fence();
+#pragma unroll
+      for (int ks = 0; ks < KSTEPS; ++ks) {
+#pragma unroll
+        for (int dyy = 0; dyy < NACC; ++dyy) {
+          if (F16) {   // K = 16 pixels = image rows (2 ks, 2 ks + 1) of the unit: halo rows 2 ks + dy, 2 ks + dy + 1
+            wg::wgmma_f16_rs_n96<1>(acc[dyy], a[ks], b16 + (uint64_t)(((2 * ks + dyy) * 160) >> 4), 1u);
+          } else if (TAPS == 9) {   // image row ks + dy starts at chunk 2 (ks + dy); the three dx taps are the N blocks
+            wg::wgmma_tf32_rs_n96(acc[dyy], a[ks], b_base + (uint64_t)(((ks + dyy) * 2 * LBO_B) >> 4), 1u);
+          } else {
+            wg::wgmma_tf32_rs_n128(acc[dyy], a[ks], b_base + (uint64_t)((ks * 2 * LBO_B) >> 4), 1u);
+          }
+        }
+      }
+      wg::commit();
+      wg::wait<0>();   // the A fragments are reloaded for the next unit
+      mbar_arrive(empty(stage));
+    };
+    if (F16) {
+      // ============ producers, fp16: x halo -> shared memory planes [dx][ci/8][slot][8 channels] (no transposition) ============
     constexpr int OCTS = NT / 8, ITEMS16 = SLOTS * OCTS, PT16 = (ITEMS16 + NPROD - 1) / NPROD;   // 400 items, 2 per thread
     int sl_r[PT16], sl_c[PT16], sl_o[PT16];
 #pragma unroll
@@ -941,28 +684,11 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc(const WParams p, const
       }
       fence_proxy_async();
       mbar_arrive(fullB(stage));
+      mma_unit(u, stage, phase);
       if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
     }
-    // epilogue (warps 0-3): accumulator column t*NT + j of lane co is dW[tap t][co][ci0 + j]
-    if (warp < 4) {
-      float inv = 1.f;
-      operand_scale(p.dy_amax, &inv);
-      mbar_wait(accum_bar, 0);
-      tc_fence_after();
-      const int co = co0 + warp * 32 + lane;
-#pragma unroll 1
-      for (int t = 0; t < TAPS; ++t) {
-        float* o = p.part + (((size_t)split * TAPS + t) * p.Cout + co) * p.Cin + ci0;
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(t * NT), v);
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          *reinterpret_cast<float4*>(o + q * 4) = make_float4(v[4 * q] * inv, v[4 * q + 1] * inv, v[4 * q + 2] * inv, v[4 * q + 3] * inv);
-      }
-      tc_fence_before();
-    }
-  } else if (warp < 8) {
-    // ============ producers: x halo / rows -> shared memory, transposed (K = pixel) ============
+    } else {
+      // ============ producers: x halo / rows -> shared memory, transposed (K = pixel) ============
     int it_r[PER_THREAD], it_c[PER_THREAD], it_q[PER_THREAD];
 #pragma unroll
     for (int i = 0; i < PER_THREAD; ++i) {
@@ -1072,109 +798,39 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc(const WParams p, const
       }
       fence_proxy_async();
       mbar_arrive(fullB(stage));
+      mma_unit(u, stage, phase);
       if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
     }
-    // ============ epilogue (warps 0-3): TAPS x [128 co x NT ci] partial sums -> workspace ============
-    if (warp < 4) {
-      float inv = 1.f;
-      if (F16) operand_scale(p.dy_amax, &inv);
-      mbar_wait(accum_bar, 0);
-      tc_fence_after();
-      const int co = co0 + warp * 32 + lane;
-#pragma unroll 1
-      for (int t = 0; t < TAPS; ++t) {
-        float* o = p.part + (((size_t)split * TAPS + t) * p.Cout + co) * p.Cin + ci0;
-        if (TAPS == 9) {
-          float v[32];
-          tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(t * NT), v);
+    }
 #pragma unroll
-          for (int q = 0; q < 8; ++q)
-            *reinterpret_cast<float4*>(o + q * 4) = make_float4(v[q] * inv, v[8 + q] * inv, v[16 + q] * inv, v[24 + q] * inv);
-        } else {
-          // NT = 128: column n = 32*j + q holds channel 4q + j; gather the four j-planes, 8 quads at a time
+    for (int a = 0; a < NACC; ++a) wg::fence_regs<NMMA / 2>(acc[a]);
+    if (want_bias) p.bpart[(size_t)split * p.Cout + co0 + tid] = (F16 && p.dy_f16) ? bsum * a_inv : bsum;
+    // ============ epilogue: TAPS x [128 co x NT ci] partial sums -> workspace ============
+    // acc[dyy][4 j + 2 i + c] = kernel row dyy, co frow + 8 i, operand row n = 8 j + 2 (lane % 4) + c = (dx, channel slot)
+    const float inv = F16 ? a_inv : 1.f;
 #pragma unroll
-          for (int qb = 0; qb < 32; qb += 8) {
-            float v0[8], v1[8], v2[8], v3[8];
-            const uint32_t tb = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)qb;
-            tmem_ld8(tb, v0);
-            tmem_ld8(tb + 32, v1);
-            tmem_ld8(tb + 64, v2);
-            tmem_ld8(tb + 96, v3);
+    for (int dyy = 0; dyy < NACC; ++dyy) {
 #pragma unroll
-            for (int q = 0; q < 8; ++q) *reinterpret_cast<float4*>(o + (qb + q) * 4) = make_float4(v0[q], v1[q], v2[q], v3[q]);
+      for (int i = 0; i < 2; ++i) {
+        const int co = co0 + frow + 8 * i;
+#pragma unroll
+        for (int j = 0; j < NMMA / 8; ++j) {
+#pragma unroll
+          for (int c = 0; c < 2; ++c) {
+            const int n = 8 * j + 2 * fk + c, dx = n / NT, nn = n % NT;
+            const int ci = F16 ? nn : 4 * (nn % QUADS) + nn / QUADS;
+            const int t = (TAPS == 9) ? dyy * 3 + dx : 0;
+            p.part[(((size_t)split * TAPS + t) * p.Cout + co) * p.Cin + ci0 + ci] = acc[dyy][4 * j + 2 * i + c] * inv;
           }
         }
       }
-      tc_fence_before();
     }
-  } else if (warp < 12) {
-    // ============ A loaders: dy tile (shared memory, landed by cp.async.bulk) -> registers -> tensor memory ============
-    // lane = co, column = pixel: reading smem "down a channel" is conflict-free and the transpose is free; the global
-    // latency is carried by the bulk copies of warp 13, so one group of four warps keeps up with the MMAs.
-    const int lg = warp & 3;          // TMEM lane group (warp % 4)
-    const int cl = lg * 32 + lane;    // channel within the 128-wide co tile
-    float bsum = 0.f;
-    const bool want_bias = p.bpart != nullptr && blockIdx.x == 0;
-    int stage = 0;
-    uint32_t phase = 0;
-    float a_inv;
-    const float a_scale = F16 ? operand_scale(p.dy_amax, &a_inv) : 1.f;
-    for (int64_t u = u0; u < u1; ++u) {
-      mbar_wait(fullD(stage), phase);   // implies the TMEM A stage is free too (the copy was issued after empty(stage))
-      const float* dys = reinterpret_cast<const float*>(dy_smem + (size_t)stage * WG_DY_STAGE) + cl;
-      if (F16 && p.dy_f16) {
-        // fp16 shadow: the staged tile is [64 pixels][128 channels] halves, already scaled: two pixels of this lane's channel
-        // are packed into a column as they are (no multiply, no conversion, half the shared-memory bytes)
-        const unsigned short* dh = reinterpret_cast<const unsigned short*>(dy_smem + (size_t)stage * WG_DY_STAGE) + cl;
-        float w[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const uint32_t lo = dh[(2 * j) * 128], hi = dh[(2 * j + 1) * 128];
-          w[j] = __uint_as_float(lo | (hi << 16));
-          if (want_bias) bsum += __half2float(__ushort_as_half((unsigned short)lo)) + __half2float(__ushort_as_half((unsigned short)hi));
-        }
-        tc_fence_after();
-        tmem_st32(tmem_base + ((uint32_t)(lg * 32) << 16) + ACC_COLS + (uint32_t)(stage * A_COLS), w);
-        tmem_st_wait();
-        tc_fence_before();
-        mbar_arrive(fullA(stage));
-        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-        continue;
-      }
-      float v[64];
-      if (TAPS == 9) {
-#pragma unroll
-        for (int j = 0; j < 64; ++j) v[j] = dys[j * 128];
-      } else {
-#pragma unroll
-        for (int j = 0; j < 64; ++j) v[j] = (u * 64 + j < p.rows) ? dys[j * 128] : 0.f;
-      }
-      if (want_bias) {   // the bias gradient falls out of ONE ci-tile's pass over dy (the other ci tiles see the same dy)
-#pragma unroll
-        for (int j = 0; j < 64; ++j) bsum += v[j];
-      }
-      tc_fence_after();
-      const uint32_t ta = tmem_base + ((uint32_t)(lg * 32) << 16) + ACC_COLS + (uint32_t)(stage * A_COLS);
-      if (F16) {   // two consecutive pixels (K) of this lane's channel per 32-bit TMEM column
-        float w[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) w[j] = __uint_as_float(pack_h2(v[2 * j] * a_scale, v[2 * j + 1] * a_scale));
-        tmem_st32(ta, w);
-      } else {
-        tmem_st32(ta, v);
-        tmem_st32(ta + 32, v + 32);
-      }
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(fullA(stage));
-      if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-    }
-    if (want_bias) p.bpart[(size_t)split * p.Cout + co0 + cl] = (F16 && p.dy_f16) ? bsum * a_inv : bsum;
-  } else if (warp == 13) {
+  } else {
     // ============ dy TMA issuer (one thread): box [8 rows][8 pixels][128 co] (or [64 rows][128 co]) -> shared [64][128] ============
     // a tiled tensor map (cuTensorMapEncodeTiled on the host) lets ONE cp.async.bulk.tensor fetch the whole dy tile of a
     // unit for any Cout; rows beyond the matrix (1x1 tail) are zero-filled by the TMA unit.
-    if (lane == 0) {
+    wg::regs_dec<wg::COPY_REGS>();
+    if (warp == 8 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int64_t u = u0; u < u1; ++u) {
@@ -1192,87 +848,32 @@ __global__ void __launch_bounds__(WG_THREADS, 1) wgrad_tc(const WParams p, const
       }
     }
     __syncwarp();
-  } else {
-    // ============ MMA issuer ============
-    // the whole warp walks the loop (warp-uniform control flow keeps descriptors in uniform registers: the single-thread form
-    // spent ~23 instructions per MMA on vector adds and R2UR moves and could not run ahead of the tensor pipe); one elected
-    // lane issues the MMAs and the commits
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int64_t u = u0; u < u1; ++u) {
-        mbar_wait(fullB(stage), phase);
-        mbar_wait(fullA(stage), phase);
-        tc_fence_after();
-        const uint32_t b_st = smem_base + (uint32_t)stage * B_STAGE;
-        const uint32_t a_t = tmem_base + ACC_COLS + (uint32_t)(stage * A_COLS);
-        const uint64_t b_base = make_desc(b_st, LBO_B, 128);
-        const uint64_t b16 = make_desc(b_st, 160, P16);   // MN-major: LBO = K-group (halo row) pitch, SBO = N-group (plane) pitch
-        const uint32_t acc0 = (u > u0) ? 1u : 0u;
-        if (elect_one()) {
-          if (F16) {
-#pragma unroll
-            for (int r = 0; r < 8; r += 2) {     // K = 16 pixels = image rows (r, r+1) of the unit: halo rows r+dy, r+dy+1
-#pragma unroll
-              for (int dyy = 0; dyy < 3; ++dyy) {
-                const uint64_t bd = b16 + (uint64_t)(((r + dyy) * 160) >> 4);
-                mma_f16_ts(tmem_base + (uint32_t)(dyy * NMMA), a_t + (uint32_t)(r * 4), bd, idesc, r > 0 ? 1u : acc0);
-              }
-            }
-          } else {
-#pragma unroll
-            for (int r = 0; r < 8; ++r) {
-#pragma unroll
-              for (int dyy = 0; dyy < ((TAPS == 9) ? 3 : 1); ++dyy) {
-                // image row r + dy starts at chunk 2*(r+dy) (8 pixels = 2 chunks); the three dx taps are the N blocks
-                const uint64_t bd = b_base + (uint64_t)(((r + dyy) * 2 * LBO_B) >> 4);
-                mma_tf32_ts(tmem_base + (uint32_t)(dyy * NMMA), a_t + (uint32_t)(r * 8), bd, idesc, r > 0 ? 1u : acc0);
-              }
-            }
-          }
-          mma_commit(empty(stage));
-          if (u + 1 == u1) mma_commit(accum_bar);
-        }
-        __syncwarp();
-        if (++stage == WG_STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (u0 >= u1 && elect_one()) mma_commit(accum_bar);   // empty split: nothing was issued, the epilogue still waits
-      __syncwarp();
-    }
-  }
-  __syncthreads();
-  if (warp == 12) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
+
 // ------------------------------------------------------------------------------------------------------------
-// Single-MMA probe (tests/test_gpu_tc_probe.py): D[128 x 32] = A[128 x 8] * B[32 x 8]^T with the operand placement /
-// descriptor conventions selected at run time — pins the hardware semantics the production kernels rely on.
+// Single-MMA probe (tests/test_gpu_tc_probe.py): D[128 x 32] = A[128 x 8] * B[32 x 8]^T as two wgmma.m64n32k8 (rows 0-63,
+// 64-127) with the operand placement / descriptor conventions selected at run time - pins the addressing the production
+// kernels rely on.  a_src 1: A from registers (the wgrad_tc form).  b_layout 99: the B descriptor is the host's raw one
+// (sm_100 version bits 46-48 dropped; TF32 operands cannot be transposed, so no instruction descriptor applies).
 __global__ void __launch_bounds__(128, 1) mma_probe(const float* __restrict__ A, const float* __restrict__ B, float* __restrict__ D,
-                                                    int a_src, int b_layout, unsigned long long raw_desc, unsigned raw_idesc,
-                                                    int raw_off) {
-  __shared__ __align__(1024) uint8_t sm[16384];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tslot;
+                                                    int a_src, int b_layout, unsigned long long raw_desc, int raw_off) {
+  __shared__ __align__(1024) uint8_t sm[24576];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   float* sa = reinterpret_cast<float*>(sm);           // A: K-major, LBO = 2048 (128 rows * 16 B), SBO = 128
-  float* sb = reinterpret_cast<float*>(sm + 8192);    // B region
+  float* sb = reinterpret_cast<float*>(sm + 8192);    // B region (16 KB: any descriptor of the tests stays inside)
   constexpr int PL = 36 * 16;                         // plane pitch of the MN-major B layout (36 slots)
-  if (tid == 0) { mbar_init(smem_u32(&bar), 1); fence_barrier_init(); }
-  if (warp == 0) tmem_alloc(smem_u32(&tslot), 64);
-  // A[m][k] -> (k/4)*2048 + m*16 + (k%4)*4
-  for (int i = tid; i < 128 * 8; i += 128) {
+  for (int i = tid; i < 128 * 8; i += 128) {          // A[m][k] -> (k/4)*2048 + m*16 + (k%4)*4
     int m = i / 8, k = i % 8;
     sa[((k / 4) * 2048 + m * 16 + (k % 4) * 4) / 4] = A[i];
   }
-  const int raw = b_layout == 99;      // raw mode: descriptor high bits / idesc / start offset come from the host
+  const int raw = b_layout == 99;      // raw mode: descriptor high bits / start offset come from the host
   const int reveal = b_layout >= 10;   // address-reveal mode: B region holds its own word index
-  if (reveal) {
-    b_layout = raw ? 0 : b_layout - 10;
-    for (int i = tid; i < 2048; i += 128) sb[i] = (float)i;
-  } else {
+  if (reveal) b_layout = raw ? 0 : b_layout - 10;
+  for (int i = tid; i < 4096; i += 128) sb[i] = (reveal && i < 2048) ? (float)i : 0.f;
+  __syncthreads();
+  if (!reveal) {
     for (int i = tid; i < 32 * 8; i += 128) {
       int n = i / 8, k = i % 8;
       int off = (b_layout == 0) ? ((k / 4) * 512 + n * 16 + (k % 4) * 4) : ((n / 4) * PL + k * 16 + (n % 4) * 4);
@@ -1280,80 +881,67 @@ __global__ void __launch_bounds__(128, 1) mma_probe(const float* __restrict__ A,
     }
   }
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tb = tslot;
-  if (a_src == 1) {  // A -> TMEM columns [32, 40): lane = m, column = k (pad the x32 store with zeros)
-    float v[32];
+  uint64_t bd;
+  if (b_layout == 0) bd = wg::desc(smem_u32(sb), 512, 128);
+  else if (b_layout == 1) bd = wg::desc(smem_u32(sb), 160, PL);   // LBO field = K-group stride, SBO field = MN-quad stride
+  else bd = wg::desc(smem_u32(sb), PL, 160);                      // fields swapped
+  if (raw) bd = (raw_desc & ~(0x3FFFull | (7ull << 46))) | (uint64_t)(((smem_u32(sb) + (uint32_t)raw_off) >> 4) & 0x3FFF);
+  const int r = (warp & 3) * 16 + (lane >> 2), c = lane & 3;      // fragment rows r, r + 8; columns / K quads c, c + 4
+  float acc[2][16];
+  uint32_t a[2][4];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = j < 8 ? A[(warp * 32 + lane) * 8 + j] : 0.f;
-    tmem_st32(tb + ((uint32_t)(warp * 32) << 16) + 32, v);
-    tmem_st_wait();
-    tc_fence_before();
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int q = 0; q < 4; ++q) a[h][q] = __float_as_uint(A[(h * 64 + r + 8 * (q & 1)) * 8 + c + 4 * (q >> 1)]);
+  wg::fence();
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (a_src == 0) wg::wgmma_tf32_ss_n32(acc[h], wg::desc(smem_u32(sa) + h * 1024, 2048, 128), bd, 0u);
+    else wg::wgmma_tf32_rs_n32(acc[h], a[h], bd, 0u);
   }
-  __syncthreads();
-  tc_fence_after();
-  if (tid == 0) {
-    uint32_t idesc = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(32 >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-    if (b_layout != 0) idesc |= (1u << 16);
-    uint64_t bd;
-    if (b_layout == 0) bd = make_desc(smem_u32(sb), 512, 128);
-    else if (b_layout == 1) bd = make_desc(smem_u32(sb), 160, PL);   // LBO field = K-group stride, SBO field = MN-quad stride
-    else bd = make_desc(smem_u32(sb), PL, 160);                      // fields swapped
-    if (raw) {
-      bd = (raw_desc & ~0x3FFFull) | (uint64_t)(((smem_u32(sb) + (uint32_t)raw_off) >> 4) & 0x3FFF);
-      idesc = raw_idesc;
-    }
-    if (a_src == 0) mma_tf32_ss(tb, make_desc(smem_u32(sa), 2048, 128), bd, idesc, 0);
-    else mma_tf32_ts(tb, tb + 32, bd, idesc, 0);
-    mma_commit(smem_u32(&bar));
+  wg::commit();
+  wg::wait<0>();
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    wg::fence_regs<16>(acc[h]);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) D[(h * 64 + r + 8 * ((j >> 1) & 1)) * 32 + 8 * (j >> 2) + 2 * c + (j & 1)] = acc[h][j];
   }
-  mbar_wait(smem_u32(&bar), 0);
-  tc_fence_after();
-  float v[32];
-  tmem_ld32(tb + ((uint32_t)(warp * 32) << 16), v);
-  for (int j = 0; j < 32; ++j) D[(warp * 32 + lane) * 32 + j] = v[j];
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tb, 64);
 }
 
-// fp16 address-reveal probe: A (shared memory, K-major) selects k = m % 16 in row m; the B region (2048 halves) holds its own
-// half index; D[k][n] is therefore the index of the half the tensor core reads for element (n, k) of B under the raw shared-
-// memory descriptor / instruction descriptor supplied by the host (tests/test_gpu_tc_probe.py: MN-major conventions).
-__global__ void __launch_bounds__(128, 1) mma_probe16(float* __restrict__ D, unsigned long long raw_desc, unsigned raw_idesc, int raw_off) {
-  __shared__ __align__(1024) uint8_t sm[8192];
-  __shared__ __align__(8) uint64_t bar;
-  __shared__ uint32_t tslot;
+// fp16 address-reveal probe: A (shared memory, K-major) selects k = m % 16 in row m; the B region holds its own half index
+// (0 .. 2047); D[k][n] is therefore the index of the half the tensor core reads for element (n, k) of B under the raw shared-
+// memory descriptor supplied by the host, read MN-major when b_mn is set (tests/test_gpu_tc_probe.py).
+__global__ void __launch_bounds__(128, 1) mma_probe16(float* __restrict__ D, unsigned long long raw_desc, int b_mn, int raw_off) {
+  __shared__ __align__(1024) uint8_t sm[16384];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   __half* sa = reinterpret_cast<__half*>(sm);          // A: 128 x 16 halves, K-major [k/8][m][8]: LBO 2048, SBO 128
-  __half* sb = reinterpret_cast<__half*>(sm + 4096);   // B region: 2048 halves
-  if (tid == 0) { mbar_init(smem_u32(&bar), 1); fence_barrier_init(); }
-  if (warp == 0) tmem_alloc(smem_u32(&tslot), 64);
+  __half* sb = reinterpret_cast<__half*>(sm + 4096);   // B region (12 KB)
   for (int i = tid; i < 128 * 16; i += 128) {
     const int m = i / 16, k = i % 16;
     sa[(k / 8) * 1024 + m * 8 + (k % 8)] = __float2half((k == m % 16) ? 1.f : 0.f);
   }
-  for (int i = tid; i < 2048; i += 128) sb[i] = __float2half((float)i);
+  for (int i = tid; i < 6144; i += 128) sb[i] = __float2half(i < 2048 ? (float)i : 0.f);
   fence_proxy_async();
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tb = tslot;
-  if (tid == 0) {
-    const uint64_t bd = (raw_desc & ~0x3FFFull) | (uint64_t)(((smem_u32(sb) + (uint32_t)raw_off) >> 4) & 0x3FFF);
-    mma_f16_ss(tb, make_desc(smem_u32(sa), 2048, 128), bd, raw_idesc, 0);
-    mma_commit(smem_u32(&bar));
+  const uint64_t bd = (raw_desc & ~(0x3FFFull | (7ull << 46))) | (uint64_t)(((smem_u32(sb) + (uint32_t)raw_off) >> 4) & 0x3FFF);
+  float acc[2][16];
+  wg::fence();
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    if (b_mn) wg::wgmma_f16_ss_n32<0, 1>(acc[h], wg::desc(smem_u32(sa) + h * 1024, 2048, 128), bd, 0u);
+    else wg::wgmma_f16_ss_n32<0, 0>(acc[h], wg::desc(smem_u32(sa) + h * 1024, 2048, 128), bd, 0u);
   }
-  mbar_wait(smem_u32(&bar), 0);
-  tc_fence_after();
-  float v[32];
-  tmem_ld32(tb + ((uint32_t)(warp * 32) << 16), v);
-  for (int j = 0; j < 32; ++j) D[(warp * 32 + lane) * 32 + j] = v[j];
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tmem_dealloc(tb, 64);
+  wg::commit();
+  wg::wait<0>();
+  const int r = (warp & 3) * 16 + (lane >> 2), c = lane & 3;
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    wg::fence_regs<16>(acc[h]);
+#pragma unroll
+    for (int j = 0; j < 16; ++j) D[(h * 64 + r + 8 * ((j >> 1) & 1)) * 32 + 8 * (j >> 2) + 2 * c + (j & 1)] = acc[h][j];
+  }
 }
 
 }  // namespace tc
@@ -1402,8 +990,7 @@ int conv3x3_fprop_tc_launch(const float* x, mas_tensor4 xs, const float* w_tc, c
   p.gn_table = gn_table; p.gn_silu = gn_silu; p.stats_part = stats_part;
   p.x_amax = f16 ? x_amax : nullptr;
   if (gn_table && !al16p(gn_table)) return fail(MAS_ERR_INVALID_ARG, "tc conv: gn_table must be 16-byte aligned");
-  // two co-resident CTAs per SM (2 tiles / 256 TMEM columns / 2 stages each): one CTA's epilogue and pipeline fill
-  // overlap the other's main loop
+  // one CTA per SM: 2 tiles (2 x 64 accumulator registers per thread and tile half) and a 2-stage ring
   constexpr int T = 2, STG = 2;
   constexpr size_t smem = tc::smem_bytes<9, 8, STG, T, false>();
   static_assert(smem == tc::smem_bytes<9, 16, STG, T, true>(), "both operand formats stage the same bytes per K chunk");
@@ -1415,25 +1002,6 @@ int conv3x3_fprop_tc_launch(const float* x, mas_tensor4 xs, const float* w_tc, c
   }
   dim3 grid((unsigned)cdiv(p.total_tiles, T), (unsigned)(Cout / tc::BN));
   if (f16) {
-    // persistent one-CTA-per-SM form: validated (whole GPU suite green) and measured - 0.70 vs 0.67 ms on the dominant layer,
-    // 0.147 vs 0.159 ms on 256 channels @64^2: no net gain on the step, so it stays an explicit opt-in (MAS_CONV_PERSIST=1)
-    static const bool persist = [] { const char* e = getenv("MAS_CONV_PERSIST"); return e && e[0] == '1'; }();
-    if (persist) {
-      constexpr size_t psm = tc::p16_smem_bytes();
-      static std::atomic<uint64_t> pconf{0};
-      static int sm_count = 148;
-      if (first_on_device(pconf)) {
-        if (int e = set_smem(tc::shift_gemm_p16, psm)) return e;
-        int dev = 0;
-        cudaGetDevice(&dev);
-        cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
-        mark_device(pconf);
-      }
-      const int64_t nitems = cdiv(p.total_tiles, 2) * (Cout / tc::BN);
-      const unsigned g = (unsigned)(nitems < sm_count ? nitems : sm_count);
-      tc::shift_gemm_p16<<<g, tc::P_NTHREADS, psm, st>>>(p);
-      return launched_tc("shift_gemm_p16");
-    }
     tc::shift_gemm_tc<9, 16, STG, T, true><<<grid, tc::NTHREADS, smem, st>>>(p);
     return launched_tc("shift_gemm_tc<9,f16>");
   }
@@ -1481,7 +1049,7 @@ static bool wgrad_tc_ok(const mas_tensor4& xs, const mas_tensor4& dys, int mode,
   return dys.h == eh && dys.w == ew && xs.n == dys.n;
 }
 static int wgrad_tc_splits(int64_t cps, int64_t units) {
-  int64_t s = 148 / cps;
+  int64_t s = NUM_SMS / cps;
   if (s < 1) s = 1;
   if (s > units) s = units;
   const int64_t ups = cdiv(units, s);
@@ -1671,12 +1239,13 @@ int mas_gemm_rows_packed(const float* A, int64_t lda, const float* w_tc, float* 
 
 int mas_tc_probe(const float* A, const float* B, float* D, int a_src, int b_layout, uint64_t raw_desc, uint32_t raw_idesc,
                  int raw_off, void* stream) {
-  tc::mma_probe<<<1, 128, 0, S(stream)>>>(A, B, D, a_src, b_layout, (unsigned long long)raw_desc, raw_idesc, raw_off);
+  (void)raw_idesc;
+  tc::mma_probe<<<1, 128, 0, S(stream)>>>(A, B, D, a_src, b_layout, (unsigned long long)raw_desc, raw_off);
   return launched_tc("mma_probe");
 }
 
 int mas_tc_probe16(float* D, uint64_t raw_desc, uint32_t raw_idesc, int raw_off, void* stream) {
-  tc::mma_probe16<<<1, 128, 0, S(stream)>>>(D, (unsigned long long)raw_desc, raw_idesc, raw_off);
+  tc::mma_probe16<<<1, 128, 0, S(stream)>>>(D, (unsigned long long)raw_desc, (int)((raw_idesc >> 16) & 1), raw_off);
   return launched_tc("mma_probe16");
 }
 

@@ -1,108 +1,44 @@
-// Batched fp32-accurate GEMM on tcgen05 by operand splitting ("3xTF32"): for the contractions the reference runs in strict
-// fp32 (torch.bmm in AttnBlock, modules.py:180,186; the transformer's QK^T / PV, transformer.py:77-103) a single TF32 pass
-// (10-bit mantissa) is not acceptable, but
+// Batched fp32-accurate GEMM on the Hopper tensor cores by operand splitting ("3xTF32"): for the contractions the reference
+// runs in strict fp32 (torch.bmm in AttnBlock, modules.py:180,186; the transformer's QK^T / PV, transformer.py:77-103) a
+// single TF32 pass (10-bit mantissa) is not acceptable, but
 //     a = a_hi + a_lo,  b = b_hi + b_lo   (a_hi = tf32(a), a_lo = tf32(a - a_hi), same for b)
 //     a.b ~= a_hi.b_hi + a_lo.b_hi + a_hi.b_lo          (dropped term a_lo.b_lo ~ 2^-22 relative)
-// accumulated in fp32 in tensor memory recovers fp32-level accuracy at three MMAs per K step - still ~5x the FFMA rate.
+// accumulated in fp32 recovers fp32-level accuracy at three MMAs per K step - still several times the FFMA rate.
 //
 //   C[b][m,n] = alpha * sum_k opA(A[b])[m,k] * opB(B[b])[n,k]
 //   * CTA = one 128 x BN output tile (BN = 128, or 64 for 64-channel attention heads), full K, K chunks of 32
-//   * BOTH operands are staged by the producer warps straight from the activation tensors (no pack pass): generic loads,
-//     split into hi / lo in registers, st.shared into the K-major no-swizzle UMMA layout [k/4][row][4] (the layout the
+//   * BOTH operands are staged by the two warpgroups straight from the activation tensors (no pack pass): generic loads,
+//     split into hi / lo in registers, st.shared into the K-major no-swizzle wgmma layout [k/4][row][4] (the layout the
 //     convolution kernels use for their weight operand).  Either source orientation works: [row][k] (16-byte loads along
 //     k, one 16-byte store) or [k][row] (16-byte loads along rows, four 4-byte stores) - so Q.K^T, P.V and all four of
 //     their gradients run without a transposing copy.
-//   * warps 0-7 produce then run the epilogue (tcgen05.ld -> smem patch -> coalesced 16-byte stores), warp 8 lane 0 issues
-//     the MMAs (12 per chunk); 2-stage full/empty mbarrier ring; 128 TMEM columns.
+//   * warpgroup g issues the wgmma.m64nBNk8 of rows 64 g .. 64 g + 63 (12 per chunk) and keeps that half of the tile in
+//     registers; the loads of chunk k+1 and, with two stages, the stores of chunk k+1 overlap the MMAs of chunk k.
 //
 // Selected by impl = MAS_IMPL_TC3 of mas_gemm / mas_gemm_batched2: the AttnBlock backward and the token transformer's attention
 // contractions run on it (tests/test_gpu_gemm3.py, tests/test_gpu_transformer.py).
 #include <stdlib.h>
 
 #include "mas_common.cuh"
+#include "wgmma.cuh"
 
 namespace mas {
 namespace tc3 {
 
 constexpr int BM = 128, KC = 32;   // the N tile (128 or 64: attention heads of 64) and the ring depth are template parameters
-constexpr int NPROD = 256, NTHREADS = 288;   // 8 producer / epilogue warps + the MMA warp
+constexpr int NPROD = 256, NTHREADS = 256;   // two warpgroups: producers, MMA issuers and epilogue
 constexpr int SLOTS = 132;                   // row pitch of an operand plane in 16-byte units (132 % 8 == 4: conflict-free stores)
 constexpr int LBO = SLOTS * 16;              // bytes between k-quads
 constexpr int PLANE = (KC / 4) * LBO;        // one operand image (hi or lo) per stage: 16 896 B
 constexpr int STAGE = 4 * PLANE;             // A_hi, A_lo, B_hi, B_lo
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void mma_tf32_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// one lane of the (converged) warp: true for exactly one thread.  The MMA-issuing warps run their loops warp-uniformly (operand
-// descriptors stay in uniform registers) and only the issue itself is predicated on this.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,"
-      "%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// shared-memory matrix descriptor, no swizzle ("interleaved"), sm_100 version field = 1 (as in contract_tc.cu)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) |
-         (1ull << 46);
-}
-// instruction descriptor: D=f32, A=B=tf32, both K-major, M=128, N
-__host__ __device__ constexpr uint32_t make_idesc(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
+
+template <int BN>
+__device__ __forceinline__ void mma_tf32(float* d, uint64_t a, uint64_t b) {
+  if (BN == 128) wg::wgmma_tf32_ss_n128(d, a, b, 1u);
+  else wg::wgmma_tf32_ss_n64(d, a, b, 1u);
 }
 
 struct P3 {
@@ -129,22 +65,15 @@ struct Quad4 {
   float4 v[4];
 };
 
-// STAGES = 2: one CTA per SM, loads of chunk k+1 overlap the MMAs of chunk k.  STAGES = 1 (short reductions, K <= 64: the
-// attention heads' 64-wide contractions are two chunks): half the shared memory and a 113-register cap so that two or three
-// CTAs share an SM and overlap each other's load / MMA / epilogue phases instead.
+// STAGES = 2: one CTA per SM, the stores of chunk k+1 overlap the MMAs of chunk k.  STAGES = 1 (short reductions, K <= 64:
+// the attention heads' 64-wide contractions are two chunks): half the shared memory so that two or three CTAs share an SM
+// and overlap each other's load / MMA / epilogue phases instead.
 template <int BN, int STAGES>
 __global__ void __launch_bounds__(NTHREADS, STAGES == 1 ? 2 : 1) gemm3_tc(const P3 p) {
-  constexpr uint32_t IDESC = make_idesc(BN);
-  constexpr int TCOLS = BN < 32 ? 32 : BN;          // tensor-memory columns (power of two >= 32)
   constexpr int B_ITEMS = BN * (KC / 4) / NPROD;    // 16-byte items of the B operand per producer thread (4 or 2)
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)STAGES * STAGE);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 1);
-  const uint32_t smem_base = smem_u32(smem), bar_base = smem_u32(bars);
-  auto full_bar = [&](int s) { return bar_base + 8u * s; };
-  auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  const uint32_t accum_bar = bar_base + 8u * (2 * STAGES);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const uint32_t smem_base = smem_u32(smem);
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = warp >> 2;
   const int n0 = blockIdx.x * BN, m0 = blockIdx.y * BM;
   const int zo = (int)blockIdx.z / p.inner, zi = (int)blockIdx.z - zo * p.inner;
   const float* Ab = p.A + (int64_t)zo * p.sa2 + (int64_t)zi * p.sa;
@@ -157,25 +86,10 @@ __global__ void __launch_bounds__(NTHREADS, STAGES == 1 ? 2 : 1) gemm3_tc(const 
   else if (p.causal == 3 && n0 >= m0 + BM) kc1 = 0;
   const bool empty = kc0 >= kc1;          // block-uniform: nothing to contract, the tile is zero
 
-  if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(full_bar(s), NPROD);
-      mbar_init(empty_bar(s), 1);
-    }
-    mbar_init(accum_bar, 1);
-    fence_barrier_init();
-  }
-  if (warp == 8) tmem_alloc(smem_u32(tmem_slot), TCOLS);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  float acc[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
 
-  if (warp < 8) {
-    // ---------------- producers ----------------
-    // item i (0..3) of this thread, per operand:
-    //   k-contiguous source : quad q = item % 8 (k = 4q..4q+3), row = item / 8            -> one 16-byte store at [q][row]
-    //   row-contiguous      : k = item % 32, row quad rq = item / 32 (rows 4rq..4rq+3)    -> four 4-byte stores at [k/4][row+j][k%4]
     auto load_op = [&](const float* base, int64_t ld, int trans, int row0, int rows_total, int kc, Quad4& out, int nitems) {
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
@@ -223,7 +137,6 @@ __global__ void __launch_bounds__(NTHREADS, STAGES == 1 ? 2 : 1) gemm3_tc(const 
       }
     };
     int stage = 0;
-    uint32_t phase = 0;
     Quad4 an, bn;
     if (!empty) {
       load_op(Ab, p.lda, p.ta, m0, p.M, kc0, an, 4);
@@ -231,87 +144,53 @@ __global__ void __launch_bounds__(NTHREADS, STAGES == 1 ? 2 : 1) gemm3_tc(const 
     }
     for (int kc = kc0; kc < kc1; ++kc) {
       const Quad4 a = an, b = bn;
-      if (kc + 1 < kc1) {   // next chunk's loads fly while this one is split and stored
+      if (kc + 1 < kc1) {   // next chunk's loads fly while this one is split, stored and multiplied
         load_op(Ab, p.lda, p.ta, m0, p.M, kc + 1, an, 4);
         load_op(Bb, p.ldb, p.tb, n0, p.N, kc + 1, bn, B_ITEMS);
       }
-      mbar_wait(empty_bar(stage), phase ^ 1);
+      // the stage about to be overwritten was last read by the MMAs of chunk kc - STAGES: both warpgroups have waited for
+      // those (wait<STAGES - 1> below) before arriving here
+      if (kc > kc0) __syncthreads();
       uint8_t* st = smem + (size_t)stage * STAGE;
       store_op(st, st + PLANE, p.ta, a, 4);
       store_op(st + 2 * PLANE, st + 3 * PLANE, p.tb, b, B_ITEMS);
-      fence_proxy_async();
-      mbar_arrive(full_bar(stage));
-      if (++stage == STAGES) { stage = 0; phase ^= 1; }
-    }
-    // ---------------- epilogue ----------------
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    const int lane_grp = warp & 3, chalf = warp >> 2;
-    constexpr int EP_LD = 36;
-    float* patch = reinterpret_cast<float*>(smem) + warp * (32 * EP_LD);
-    const int sub_r = lane >> 3, sub_c = lane & 7;
-#pragma unroll 1
-    for (int cc = 0; cc < BN / 64; ++cc) {          // the two warp groups split the BN columns in halves of BN/2
-      const int col = chalf * (BN / 2) + cc * 32;
-      float v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(lane_grp * 32) << 16) + (uint32_t)col, v);
-      if (empty) {
+      fence_proxy_async();  // make the generic-proxy stores visible to the tensor core (async proxy)
+      __syncthreads();
+      const uint32_t sa = smem_base + (uint32_t)stage * STAGE;
+      // rows 64 g .. 64 g + 63 of A start 64 * 16 bytes into each k-quad plane
+      const uint64_t a_hi = wg::desc(sa + wgi * 1024, LBO, 128), a_lo = wg::desc(sa + PLANE + wgi * 1024, LBO, 128);
+      const uint64_t b_hi = wg::desc(sa + 2 * PLANE, LBO, 128), b_lo = wg::desc(sa + 3 * PLANE, LBO, 128);
+      wg::fence();
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0.f;
+      for (int k8 = 0; k8 < KC / 8; ++k8) {
+        const uint64_t ko = (uint64_t)((k8 * 2 * LBO) >> 4);
+        mma_tf32<BN>(acc, a_hi + ko, b_hi + ko);
+        mma_tf32<BN>(acc, a_lo + ko, b_hi + ko);
+        mma_tf32<BN>(acc, a_hi + ko, b_lo + ko);
       }
-      __syncwarp();
+      wg::commit();
+      wg::wait<STAGES - 1>();
+      if (++stage == STAGES) stage = 0;
+    }
+    wg::wait<0>();
+    wg::fence_regs<BN / 2>(acc);
+
+    // ---------------- epilogue: straight from the accumulator fragment ----------------
+    const int rbase = m0 + wgi * 64 + (warp & 3) * 16 + (lane >> 2);
+    float* cp = Cb + n0 + 2 * (lane & 3);
 #pragma unroll
-      for (int j = 0; j < 32; j += 4)
-        *reinterpret_cast<float4*>(patch + lane * EP_LD + j) =
-            make_float4(v[j] * p.alpha, v[j + 1] * p.alpha, v[j + 2] * p.alpha, v[j + 3] * p.alpha);
-      __syncwarp();
+    for (int i = 0; i < 2; ++i) {
+      const int m = rbase + 8 * i;
+      if (m < p.M) {
 #pragma unroll
-      for (int i = 0; i < 8; ++i) {
-        const int row = i * 4 + sub_r, m = m0 + lane_grp * 32 + row;
-        if (m < p.M)
-          *reinterpret_cast<float4*>(Cb + (int64_t)m * p.ldc + n0 + col + sub_c * 4) =
-              *reinterpret_cast<const float4*>(patch + row * EP_LD + sub_c * 4);
+        for (int j = 0; j < BN / 8; ++j)
+          *reinterpret_cast<float2*>(cp + (int64_t)m * p.ldc + 8 * j) = make_float2(acc[4 * j + 2 * i] * p.alpha, acc[4 * j + 2 * i + 1] * p.alpha);
       }
     }
-    tc_fence_before();
-  } else {
-    // ---------------- MMA issuer (warp-uniform loop, one elected lane issues) ----------------
-    {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kc = kc0; kc < kc1; ++kc) {
-        mbar_wait(full_bar(stage), phase);
-        tc_fence_after();
-        const uint32_t st = smem_base + (uint32_t)stage * STAGE;
-        const uint64_t a_hi = make_desc(st, LBO, 128), a_lo = make_desc(st + PLANE, LBO, 128);
-        const uint64_t b_hi = make_desc(st + 2 * PLANE, LBO, 128), b_lo = make_desc(st + 3 * PLANE, LBO, 128);
-        if (elect_one()) {
-#pragma unroll
-          for (int k8 = 0; k8 < KC / 8; ++k8) {
-            const uint64_t ko = (uint64_t)((k8 * 2 * LBO) >> 4);
-            mma_tf32_ss(tmem_base, a_hi + ko, b_hi + ko, IDESC, (kc > kc0 || k8 > 0) ? 1u : 0u);
-            mma_tf32_ss(tmem_base, a_lo + ko, b_hi + ko, IDESC, 1u);
-            mma_tf32_ss(tmem_base, a_hi + ko, b_lo + ko, IDESC, 1u);
-          }
-          mma_commit(empty_bar(stage));
-          if (kc == kc1 - 1) mma_commit(accum_bar);
-        }
-        __syncwarp();
-        if (++stage == STAGES) { stage = 0; phase ^= 1; }
-      }
-      if (empty && elect_one()) mma_commit(accum_bar);
-      __syncwarp();
-    }
-  }
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TCOLS);
-  }
 }
 
 template <int STAGES>
-constexpr size_t smem_bytes() { return (size_t)STAGES * STAGE + (2 * STAGES + 1) * 8 + 16; }
+constexpr size_t smem_bytes() { return (size_t)STAGES * STAGE; }
 
 }  // namespace tc3
 

@@ -1,22 +1,20 @@
-// 3x3 stride-1 convolution (fprop / data gradient) as a pure TMA + tcgen05 kernel: the A operand comes from an fp16 "shadow"
+// 3x3 stride-1 convolution (fprop / data gradient) as a pure TMA + wgmma kernel: the A operand comes from an fp16 "shadow"
 // of the activation (written channels-last by the producing kernel: GroupNorm(+SiLU) apply in the forward pass, GroupNorm
 // backward in the backward pass) instead of being converted by producer warps.
 //
-//   * one persistent CTA per SM walks work items (pair of 128-pixel tiles x 128 output channels), as shift_gemm_p16;
+//   * one persistent CTA per SM walks work items (pair of 128-pixel tiles x 128 output channels);
 //   * A: ONE cp.async.bulk.tensor (4-D map over [N][H][W][C] halves, box 1 x 18 x 10 x 64, 128-byte swizzle, out-of-image
 //     halo pixels zero-filled by the copy engine) per tile per 64-channel chunk.  The staged halo is [180 pixels][128 B];
 //     the nine taps and the four K = 16 steps of the chunk are descriptor start-address shifts ((ty*10+tx)*128 + k*32 bytes)
 //     over that one copy: the 8-row core group is eight horizontally adjacent pixels, the group stride (SBO) one staged image
-//     row = 1280 B.  Row-shifted starts under the 128-byte swizzle are address-exact on sm_100 (the XOR is taken from the
-//     absolute shared-memory address bits; tools/probe_sw128.py pins it);
+//     row = 1280 B;
 //   * B (weights): the same pre-packed no-swizzle stages as shift_gemm_tc (mas_pack_conv3x3_tc16), one bulk copy per
 //     16-channel step, ring of three;
-//   * operand roles are swapped (D^T = W x X^T: the packed weights are the M-side operand, the pixels the N side), so a TMEM
-//     lane is an output channel and a column a pixel: the epilogue's 32 lanes store 32 consecutive channels of one pixel -
-//     a full 128-byte line per instruction without a shared-memory transpose; bias and GroupNorm statistics are per-thread;
-//   * two accumulator sets in tensor memory (2 x 256 columns): eight epilogue warps drain set b (bias / residual /
-//     GroupNorm-statistics epilogue) while the MMAs of the next item fill set b^1;
-//   * warps 0-7 epilogue, warp 8 MMA issuer, warp 9 copy issuer: no thread of the CTA touches the operands.
+//   * operand roles are swapped (D^T = W x X^T: the packed weights are the M-side operand, the pixels the N side of
+//     wgmma.m64n256k16 / two m64n128k16): warpgroup g owns output channels 64 g .. 64 g + 63 of the tile, so bias and
+//     GroupNorm statistics are per-row scalars of the accumulator fragment;
+//   * warps 0-7 MMA + epilogue (two warpgroups), warp 8 copy issuer (its warpgroup hands its registers to the MMA ones): no
+//     thread of the CTA touches the operands; the copy issuer fills the rings of the next item while the warpgroups store the current one.
 //
 // Reference call sites replaced: nn.Conv2d 3x3 stride 1 (modules.py:93-104) forward and its data gradient.
 #include <cuda.h>
@@ -26,6 +24,7 @@
 
 #include "mas_common.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace mas {
 
@@ -33,8 +32,8 @@ PFN_cuTensorMapEncodeTiled tensor_map_encoder();   // contract_tc.cu
 
 namespace tc {
 
-constexpr int T_EPI_WARPS = 8;
-constexpr int T_THREADS = (T_EPI_WARPS + 2) * 32;
+constexpr int T_MMA_WARPS = 8;
+constexpr int T_THREADS = (T_MMA_WARPS + 4) * 32;   // + the copy-issuing warpgroup
 constexpr int T_ASTAGES = 2, T_BSTAGES = 3;
 constexpr int T_ATILE = 23 * 1024;                  // 18 x 10 halo pixels x 128 B = 23040, padded to the 1024-byte swizzle atom
 constexpr int T_ASTAGE = 2 * T_ATILE;               // pair of 16 x 8 tiles, or one 32 x 8 tile (34 x 10 halo = 43520 B)
@@ -52,10 +51,6 @@ struct HParams {
   float* stats_part;   // GroupNorm-statistics epilogue (see shift_gemm_tc), or null
   const float* x_amax; // amax the shadow's power-of-two scale was derived from (null: unscaled shadow)
 };
-
-__device__ __forceinline__ uint64_t make_desc_sw128(uint32_t saddr, uint32_t sbo_bytes) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46) | (2ull << 61);
-}
 
 // 16 x 8 tile (n, ty, tx) of half `hf` of work unit `u`; false when the unit's second tile does not exist (odd tile count)
 template <bool TALL>
@@ -78,8 +73,7 @@ __device__ __forceinline__ bool unit_tile(const HParams& p, int64_t u, int hf, i
 }
 
 // TALL: the unit is one 32 x 8 tile whose staged halo (34 x 10 pixels, uniform 1280-byte row pitch) is ONE N = 256 operand:
-// per K = 16 step and tap a single M128 x N256 MMA reads 4 KB of weights + 8 KB of pixels instead of 2 x (4 + 4) KB - the
-// SS-mode kernel is bound by exactly that operand traffic (measured: no change with the weight copies stubbed out).
+// per K = 16 step and tap a single m64n256 MMA per warpgroup instead of two m64n128 ones over the two halos of a pair.
 template <bool TALL>
 __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, const __grid_constant__ CUtensorMap x_map) {
   constexpr int TAPS = 9;
@@ -93,15 +87,11 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
   const uint32_t a_base = smem_base;
   const uint32_t b_base = a_base + T_ASTAGES * T_ASTAGE;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + T_ASTAGES * T_ASTAGE + T_BSTAGES * T_BSTAGE);
-  constexpr int NBARS = 2 * T_ASTAGES + 2 * T_BSTAGES + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + NBARS);
   const uint32_t bar_base = smem_u32(bars);
   auto afull = [&](int s) { return bar_base + 8u * s; };
   auto aempty = [&](int s) { return bar_base + 8u * (T_ASTAGES + s); };
   auto bfull = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + s); };
   auto bempty = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + T_BSTAGES + s); };
-  auto accf = [&](int b) { return bar_base + 8u * (2 * T_ASTAGES + 2 * T_BSTAGES + b); };
-  auto acce = [&](int b) { return bar_base + 8u * (2 * T_ASTAGES + 2 * T_BSTAGES + 2 + b); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int achunks = p.Cin / 64;
@@ -109,145 +99,120 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
   const int64_t nitems = p.units * n_tiles;       // channel tile fastest: the halo of a unit is re-read from L2
 
   if (tid == 0) {
-    for (int s = 0; s < T_ASTAGES; ++s) { mbar_init(afull(s), 1); mbar_init(aempty(s), 1); }
-    for (int s = 0; s < T_BSTAGES; ++s) { mbar_init(bfull(s), 1); mbar_init(bempty(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(accf(b), 1); mbar_init(acce(b), T_EPI_WARPS * 32); }
+    for (int s = 0; s < T_ASTAGES; ++s) { mbar_init(afull(s), 1); mbar_init(aempty(s), T_MMA_WARPS * 32); }
+    for (int s = 0; s < T_BSTAGES; ++s) { mbar_init(bfull(s), 1); mbar_init(bempty(s), T_MMA_WARPS * 32); }
     fence_barrier_init();
   }
-  if (warp == T_EPI_WARPS) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp < T_EPI_WARPS) {
-    // ===================== epilogue warps =====================
-    // The accumulator is D^T: TMEM lane = output channel, column = pixel (weights are the M-side operand).  A warp owns 32
-    // consecutive channels (lane quarter warp % 4) of one 16 x 8 half of the unit (warp / 4); for every pixel its 32 lanes
-    // store 32 consecutive floats = one full 128-byte line: coalesced without a shared-memory transpose, bias and GroupNorm
-    // statistics are per-thread scalars.
+  if (warp < T_MMA_WARPS) {
+    wg::regs_inc<wg::MMA_REGS>();
+    // ===================== MMA warpgroups, then epilogue =====================
+    // acc[64 h + 4 j + 2 i + c] = D^T[channel 64 wgi + 16 (warp % 4) + lane / 4 + 8 i][pixel 128 h + 8 j + 2 (lane % 4) + c]
     float inv_scale = 1.f;
     operand_scale(p.x_amax, &inv_scale);
     const float alpha = inv_scale;
-    const int quarter = warp & 3, hf = warp >> 2;
-    int buf = 0;
-    uint32_t ph[2] = {0u, 0u};
+    const int wgi = warp >> 2;
+    const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+    int as = 0, bs = 0, prev_b = 0, prev_a = -1;
+    uint32_t aph = 0, bph = 0;
+    float acc[128];
     for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-      int n_img, ty_, tx_;
-      const bool live = unit_tile<TALL>(p, item / n_tiles, hf, n_img, ty_, tx_);   // warp-uniform
-      const int ch = (int)(item % n_tiles) * BN + quarter * 32 + lane;
-      const bool st_ok = ch < p.Cstore;
-      const float bv = (p.bias && st_ok) ? __ldg(p.bias + ch) : 0.f;
-      const int64_t pix0 = ((int64_t)n_img * p.H + ty_ * 16) * p.W + tx_ * 8;
-      // residual: the 32 loads of a 32-pixel batch are issued ONE BATCH AHEAD (the first before the accumulator is even
-      // waited for), so 32 KB per SM are in flight - the epilogue was bound by this latency, not by the stores.  (An L2
-      // prefetch of the next item's residual tile on top of this measured SLOWER - 0.66 vs 0.61 ms - and fetched 44 % of the
-      // residual twice: the output stream evicts the prefetched lines.)
-      const int rs = p.W * (int)p.ldy, ps = (int)p.ldy;      // element strides of an image row / a pixel (tile-local: fits int)
-      const int64_t base0 = pix0 * p.ldy + ch;
-      const bool use_res = p.res != nullptr && live && st_ok;
-      float ra[32], rb[32];
-      auto rload = [&](int cb, float* r) {
-        const float* rp = p.res + base0 + (int64_t)(cb * 4) * rs;
-#pragma unroll
-        for (int j = 0; j < 32; ++j) r[j] = __ldg(rp + (j >> 3) * rs + (j & 7) * ps);
-      };
-      if (use_res) rload(0, ra);
-      mbar_wait(accf(buf), ph[buf]);
-      ph[buf] ^= 1u;
-      tc_fence_after();
-      auto batch = [&](int cb, const float* r) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * 256 + hf * 128 + cb * 32), v);
-        if (cb == 3) {
-          tc_fence_before();
-          mbar_arrive(acce(buf));     // this warp's share of the accumulator set is in registers
-        }
-        if (!live) return;
-        float st_s = 0.f, st_q = 0.f;
-        if (st_ok) {
-          float* yp = p.y + base0 + (int64_t)(cb * 4) * rs;
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            float o = fmaf(v[j], alpha, bv);
-            if (use_res) o += r[j];
-            yp[(j >> 3) * rs + (j & 7) * ps] = o;
-            st_s += o;
-            st_q = fmaf(o, o, st_q);
-          }
-        }
-        if (p.stats_part) {   // same partial layout as shift_gemm_tc: [16 x 8 tile][32-pixel group][channel quad][sum, sumsq]
-          st_s += __shfl_xor_sync(0xffffffffu, st_s, 1);
-          st_q += __shfl_xor_sync(0xffffffffu, st_q, 1);
-          st_s += __shfl_xor_sync(0xffffffffu, st_s, 2);
-          st_q += __shfl_xor_sync(0xffffffffu, st_q, 2);
-          if ((lane & 3) == 0) {
-            const size_t tile = ((size_t)n_img * p.tiles_y + ty_) * p.tiles_x + tx_;
-            float* sp = p.stats_part + ((tile * 4 + cb) * (p.Cout >> 2) + (ch >> 2)) * 2;
-            sp[0] = st_s;
-            sp[1] = st_q;
-          }
-        }
-      };
-      if (use_res) rload(1, rb);
-      batch(0, ra);
-      if (use_res) rload(2, ra);
-      batch(1, rb);
-      if (use_res) rload(3, rb);
-      batch(2, ra);
-      batch(3, rb);
-      buf ^= 1;
-    }
-  } else if (warp == T_EPI_WARPS) {
-    // ===================== MMA issuer =====================
-    // The whole warp walks the loop (warp-uniform control flow keeps the operand descriptors in uniform registers: one add
-    // per descriptor per MMA instead of a 64-bit vector add + five R2UR moves - the single-thread form spent ~23 instructions
-    // per MMA and could not run ahead of the tensor pipe); one elected lane issues the MMAs and commits.
-    {
-      constexpr uint32_t idesc = make_idesc_f16(TALL ? 256 : BN);
-      int as = 0, bs = 0, buf = 0;
-      uint32_t aph = 0, bph = 0, eph[2] = {0u, 0u};
-      for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-        mbar_wait(acce(buf), eph[buf] ^ 1);     // the epilogue warps have read this accumulator set (first use: passes)
-        eph[buf] ^= 1u;
-        tc_fence_after();
-        const uint32_t acc = tmem_base + (uint32_t)(buf * 256);
-        for (int c = 0; c < achunks; ++c) {
-          mbar_wait(afull(as), aph);
-          tc_fence_after();
-          const uint64_t xd0 = make_desc_sw128(a_base + (uint32_t)as * T_ASTAGE, 1280);
+      for (int c = 0; c < achunks; ++c) {
+        mbar_wait(afull(as), aph);
+        const uint64_t xd0 = wg::desc(a_base + (uint32_t)as * T_ASTAGE, 16, 1280, wg::SW_128);
 #pragma unroll 1
-          for (int sub = 0; sub < 4; ++sub) {
-            mbar_wait(bfull(bs), bph);
-            tc_fence_after();
-            const uint64_t wd0 = make_desc(b_base + (uint32_t)bs * T_BSTAGE, LBO_B, 128);
-            const uint64_t xds = xd0 + (uint64_t)((sub * 32) >> 4);
-            const uint32_t acc0 = (c > 0 || sub > 0) ? 1u : 0u;
-            if (elect_one()) {
+        for (int sub = 0; sub < 4; ++sub) {
+          mbar_wait(bfull(bs), bph);
+          const uint64_t wd0 = wg::desc(b_base + (uint32_t)bs * T_BSTAGE + (uint32_t)(wgi * 1024), LBO_B, 128);
+          const uint64_t xds = xd0 + (uint64_t)((sub * 32) >> 4);
+          const uint32_t acc0 = (c > 0 || sub > 0) ? 1u : 0u;
+          wg::fence();
 #pragma unroll
-              for (int t = 0; t < TAPS; ++t) {
-                const uint32_t tapoff = (uint32_t)(((t / 3) * 10 + (t % 3)) * 128);
-                const uint64_t wd = wd0 + (uint64_t)((t * B_TAP) >> 4);
-                const uint64_t xd = xds + (uint64_t)(tapoff >> 4);
-                // D^T = W x X^T: weights on the M side, pixels on the N side
-                mma_f16_ss(acc, wd, xd, idesc, t > 0 ? 1u : acc0);
-                if (!TALL) mma_f16_ss(acc + 128u, wd, xd + (uint64_t)(T_ATILE >> 4), idesc, t > 0 ? 1u : acc0);
-              }
-              mma_commit(bempty(bs));
-              if (sub == 3) mma_commit(aempty(as));
-              if (sub == 3 && c == achunks - 1) mma_commit(accf(buf));
+          for (int t = 0; t < TAPS; ++t) {
+            const uint32_t tapoff = (uint32_t)(((t / 3) * 10 + (t % 3)) * 128);
+            const uint64_t wd = wd0 + (uint64_t)((t * B_TAP) >> 4);
+            const uint64_t xd = xds + (uint64_t)(tapoff >> 4);
+            // D^T = W x X^T: weights on the M side, pixels on the N side
+            if (TALL) {
+              wg::wgmma_f16_ss_n256<0, 0>(acc, wd, xd, t > 0 ? 1u : acc0);
+            } else {
+              wg::wgmma_f16_ss_n128<0, 0>(acc, wd, xd, t > 0 ? 1u : acc0);
+              wg::wgmma_f16_ss_n128<0, 0>(acc + 64, wd, xd + (uint64_t)(T_ATILE >> 4), t > 0 ? 1u : acc0);
             }
-            __syncwarp();
-            if (++bs == T_BSTAGES) { bs = 0; bph ^= 1; }
           }
-          if (++as == T_ASTAGES) { as = 0; aph ^= 1; }
+          wg::commit();
+          // the previous step's MMAs have read their weight stage (and, after a chunk's last step, its halo stage)
+          wg::wait<1>();
+          if (c > 0 || sub > 0) {
+            mbar_arrive(bempty(prev_b));
+            if (prev_a >= 0) mbar_arrive(aempty(prev_a));
+          }
+          prev_b = bs;
+          prev_a = (sub == 3) ? as : -1;
+          if (++bs == T_BSTAGES) { bs = 0; bph ^= 1; }
         }
-        buf ^= 1;
+        if (++as == T_ASTAGES) { as = 0; aph ^= 1; }
+      }
+      wg::wait<0>();
+      wg::fence_regs<128>(acc);
+      mbar_arrive(bempty(prev_b));
+      mbar_arrive(aempty(prev_a));
+
+      const int ch_tile = (int)(item % n_tiles) * BN;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        int n_img, ty_, tx_;
+        const bool live = unit_tile<TALL>(p, item / n_tiles, h, n_img, ty_, tx_);   // block-uniform
+        if (!live) continue;
+        const int64_t pix0 = ((int64_t)n_img * p.H + ty_ * 16) * p.W + tx_ * 8;
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int ch = ch_tile + frow + 8 * i;
+          const bool st_ok = ch < p.Cstore;
+          const float bv = (p.bias && st_ok) ? __ldg(p.bias + ch) : 0.f;
+#pragma unroll
+          for (int cb = 0; cb < 4; ++cb) {         // 32-pixel groups = four image rows of the 16 x 8 tile
+            float st_s = 0.f, st_q = 0.f;
+#pragma unroll
+            for (int jj = 0; jj < 4; ++jj) {
+              const int j = cb * 4 + jj;           // pixel row j of the tile, columns fcol, fcol + 1
+              const int64_t off = (pix0 + (int64_t)j * p.W + fcol) * p.ldy + ch;
+#pragma unroll
+              for (int cc = 0; cc < 2; ++cc) {
+                float o = fmaf(acc[64 * h + 4 * j + 2 * i + cc], alpha, bv);
+                if (st_ok) {
+                  if (p.res) o += __ldg(p.res + off + cc * p.ldy);
+                  p.y[off + cc * p.ldy] = o;
+                  st_s += o;
+                  st_q = fmaf(o, o, st_q);
+                }
+              }
+            }
+            if (p.stats_part) {   // same partial layout as shift_gemm_tc: [16 x 8 tile][32-pixel group][channel quad][sum, sumsq]
+              st_s += __shfl_xor_sync(0xffffffffu, st_s, 1);   // the four lanes of a channel row: all 32 pixels
+              st_q += __shfl_xor_sync(0xffffffffu, st_q, 1);
+              st_s += __shfl_xor_sync(0xffffffffu, st_s, 2);
+              st_q += __shfl_xor_sync(0xffffffffu, st_q, 2);
+              st_s += __shfl_xor_sync(0xffffffffu, st_s, 4);   // four consecutive channel rows: the quad
+              st_q += __shfl_xor_sync(0xffffffffu, st_q, 4);
+              st_s += __shfl_xor_sync(0xffffffffu, st_s, 8);
+              st_q += __shfl_xor_sync(0xffffffffu, st_q, 8);
+              if ((lane & 15) == 0) {
+                const size_t tile = ((size_t)n_img * p.tiles_y + ty_) * p.tiles_x + tx_;
+                float* sp = p.stats_part + ((tile * 4 + cb) * (p.Cout >> 2) + (ch >> 2)) * 2;
+                sp[0] = st_s;
+                sp[1] = st_q;
+              }
+            }
+          }
+        }
       }
     }
   } else {
     // ===================== copy issuer (one thread): halos by tensor map, weight stages by bulk copy =====================
-    if (lane == 0) {
+    wg::regs_dec<wg::COPY_REGS>();
+    if (warp == T_MMA_WARPS && lane == 0) {
       int as = 0, bs = 0;
       uint32_t aph = 0, bph = 0;
       const int kchunks = p.Cin / 16;
@@ -274,35 +239,33 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
     }
     __syncwarp();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == T_EPI_WARPS) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 constexpr size_t t16_smem_bytes() {
-  return 1024 + (size_t)T_ASTAGES * T_ASTAGE + (size_t)T_BSTAGES * T_BSTAGE + (2 * T_ASTAGES + 2 * T_BSTAGES + 4) * 8 + 16;
+  return 1024 + (size_t)T_ASTAGES * T_ASTAGE + (size_t)T_BSTAGES * T_BSTAGE + (2 * T_ASTAGES + 2 * T_BSTAGES) * 8 + 16;
 }
 
 // ------------------------------------------------------------------------------------------------------------
 // Weight gradient of the 3x3 stride-1 convolution from the two fp16 shadows (activation x16, output gradient dy16 - already
 // scaled), dW[tap][co][ci] = sum_pixels dy[p][co] * x[p + tap][ci]; the reduction runs over PIXELS, so both operands are
 // "MN-major" in memory (channels contiguous, pixels strided):
-//   * A = dy^T in tensor memory (TS mode): the dy tile of a unit (8 x 8 pixels x 128 co, one tensor-map copy) is moved
-//     shared -> registers -> TMEM by four loader warps, two pixels per 32-bit column, lane = co (the transpose is free);
+//   * A = dy^T: the dy tile of a unit (8 x 8 pixels x 128 co) lands as two 64-channel tensor-map boxes under the 128-byte
+//     swizzle, an MN-major operand (K groups = image rows of 8 pixels, SBO = 1024 B); warpgroup g multiplies co 64 g .. 64 g + 63;
 //   * B = the activation halo exactly as the copy engine lands it under the 128-byte swizzle: [row][pixel][64 ci] with 128-byte
-//     pixel rows, read as an MN-major operand (K groups = image rows of 8 pixels, SBO = the 1280-byte halo row; probe:
-//     tools/probe_mn128.py).  A tap is a descriptor start shift (dx * 128 B); no producer warps, no dx copies;
-//   * a CTA owns one kernel ROW (3 horizontal taps) of a 128 co x NCI ci block: 3 x NCI accumulator columns, N = 64 MMAs
-//     (two per tap and K step for NCI = 128), K = 16 pixels = two image rows of the unit;
-//   * split-K over the units; partial sums (and the bias gradient from the dy loaders) go to the caller's workspace in the
-//     layout conv_wgrad_reduce expects.
+//     pixel rows, read as an MN-major operand (K groups = image rows of 8 pixels, SBO = the 1280-byte halo row).  A tap is a
+//     descriptor start shift (dx * 128 B); no producer warps, no dx copies;
+//   * a CTA owns one kernel ROW (3 horizontal taps) of a 128 co x 64 ci block: three m64n64 accumulators per warpgroup,
+//     K = 16 pixels = two image rows of the unit per MMA;
+//   * split-K over the units; partial sums (and the bias gradient, summed from the staged dy tile) go to the caller's
+//     workspace in the layout conv_wgrad_reduce expects.
 constexpr int WT_STAGES = 4;
+constexpr int WT_NCI = 64;                  // input channels per CTA (one swizzle atom of the halo)
 constexpr int WT_XATOM = 8 * 10 * 128;      // 8 halo rows x 10 pixels x 128 B (64 channels)
-constexpr int WT_DY = 64 * 128 * 2;         // 64 pixels x 128 co halves
-constexpr int WT_THREADS = 6 * 32;
+constexpr int WT_DYATOM = 64 * 128;         // 64 pixels x 64 co halves
+constexpr int WT_DY = 2 * WT_DYATOM;        // 64 pixels x 128 co halves
+constexpr int WT_THREADS = 12 * 32;
+constexpr int WT_STAGE = WT_XATOM + WT_DY;
+static_assert(WT_STAGE % 1024 == 0 && WT_XATOM % 1024 == 0, "stages must keep the swizzle atoms 1024-byte aligned");
 
 struct WTParams {
   float* part;      // [splits][9][Cout][Cin]
@@ -313,148 +276,112 @@ struct WTParams {
   const float* dy_amax;   // the magnitude dy16's power-of-two scale was derived from
 };
 
-template <int NCI>
 __global__ void __launch_bounds__(WT_THREADS, 1) wgrad_t16(const WTParams p, const __grid_constant__ CUtensorMap x_map,
                                                           const __grid_constant__ CUtensorMap dy_map) {
-  constexpr int XB = (NCI / 64) * WT_XATOM, STAGE = XB + WT_DY;
-  constexpr uint32_t ACC_COLS = 3 * NCI, A_COLS = 32;
-  static_assert(ACC_COLS + WT_STAGES * A_COLS <= 512, "tensor memory budget");
-  constexpr uint32_t idesc = make_idesc_f16(64) | (1u << 16);   // B operand MN-major
-
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
   const uint32_t smem_base = (raw_base + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (smem_base - raw_base);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)WT_STAGES * STAGE);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * WT_STAGES + 1);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)WT_STAGES * WT_STAGE);
   const uint32_t bar_base = smem_u32(bars);
   auto fullD = [&](int s) { return bar_base + 8u * s; };                      // copies of the stage have landed
-  auto fullA = [&](int s) { return bar_base + 8u * (WT_STAGES + s); };        // dy^T of the stage is in tensor memory
-  auto empty = [&](int s) { return bar_base + 8u * (2 * WT_STAGES + s); };    // the MMAs of the stage have completed
-  const uint32_t accum_bar = bar_base + 8u * (3 * WT_STAGES);
+  auto empty = [&](int s) { return bar_base + 8u * (WT_STAGES + s); };        // the MMAs of the stage have completed
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int dyy = blockIdx.x % 3, ci0 = (blockIdx.x / 3) * NCI, co0 = blockIdx.y * BM, split = blockIdx.z;
+  const int dyy = blockIdx.x % 3, ci0 = (blockIdx.x / 3) * WT_NCI, co0 = blockIdx.y * BM, split = blockIdx.z;
   const int64_t u0 = (int64_t)split * p.units_per_split;
   const int64_t u1 = min(p.total_units, u0 + p.units_per_split);
 
   if (tid == 0) {
-    for (int s = 0; s < WT_STAGES; ++s) { mbar_init(fullD(s), 1); mbar_init(fullA(s), 128); mbar_init(empty(s), 1); }
-    mbar_init(accum_bar, 1);
+    for (int s = 0; s < WT_STAGES; ++s) { mbar_init(fullD(s), 1); mbar_init(empty(s), 256); }
     fence_barrier_init();
   }
-  if (warp == 4) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp < 4) {
-    // ============ dy loaders, then epilogue ============
-    const int cl = warp * 32 + lane;          // channel within the co tile = TMEM lane
+  if (warp < 8) {
+    // ============ MMA warpgroups (bias-gradient sums by warpgroup 0), then epilogue ============
+    wg::regs_inc<wg::MMA_REGS>();
+    const int wgi = warp >> 2;
     float a_inv;
     operand_scale(p.dy_amax, &a_inv);
     float bsum = 0.f;
-    const bool want_bias = p.bpart != nullptr && blockIdx.x == 0;
-    int stage = 0;
+    const bool want_bias = p.bpart != nullptr && blockIdx.x == 0 && tid < 128;
+    float acc[3][32];
+#pragma unroll
+    for (int dx = 0; dx < 3; ++dx)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[dx][i] = 0.f;
+    int stage = 0, prev = 0;
     uint32_t phase = 0;
     for (int64_t u = u0; u < u1; ++u) {
       mbar_wait(fullD(stage), phase);
-      const unsigned short* dh = reinterpret_cast<const unsigned short*>(smem + (size_t)stage * STAGE + XB) + cl;
-      float w[32];
+      const uint32_t xs = smem_base + (uint32_t)stage * WT_STAGE;
+      // MN-major, 128-byte swizzle: K groups (8 pixels = one image row of the unit) are 1280 B (halo) / 1024 B (dy) apart
+      const uint64_t xd0 = wg::desc(xs, 16, 1280, wg::SW_128);
+      const uint64_t ad0 = wg::desc(xs + WT_XATOM + (uint32_t)(wgi * WT_DYATOM), 16, 1024, wg::SW_128);
+      wg::fence();
 #pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const uint32_t lo = dh[(2 * j) * 128], hi = dh[(2 * j + 1) * 128];
-        w[j] = __uint_as_float(lo | (hi << 16));
-        if (want_bias) bsum += __half2float(__ushort_as_half((unsigned short)lo)) + __half2float(__ushort_as_half((unsigned short)hi));
+      for (int r = 0; r < 8; r += 2) {          // K = 16 pixels: image rows r, r + 1 of the unit
+#pragma unroll
+        for (int dx = 0; dx < 3; ++dx)
+          wg::wgmma_f16_ss_n64<1, 1>(acc[dx], ad0 + (uint64_t)((r * 1024) >> 4), xd0 + (uint64_t)((r * 1280 + dx * 128) >> 4), 1u);
       }
-      tc_fence_after();
-      tmem_st32(tmem_base + ((uint32_t)(warp * 32) << 16) + ACC_COLS + (uint32_t)(stage * A_COLS), w);
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(fullA(stage));
-      if (++stage == WT_STAGES) { stage = 0; phase ^= 1; }
-    }
-    if (want_bias) p.bpart[(size_t)split * p.Cout + co0 + cl] = bsum * a_inv;
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int dx = 0; dx < 3; ++dx) {
-      float* o = p.part + (((size_t)split * 9 + dyy * 3 + dx) * p.Cout + co0 + cl) * p.Cin + ci0;
-#pragma unroll 1
-      for (int cb = 0; cb < NCI / 32; ++cb) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(dx * NCI + cb * 32), v);
-#pragma unroll
-        for (int q = 0; q < 8; ++q)
-          *reinterpret_cast<float4*>(o + cb * 32 + q * 4) =
-              make_float4(v[4 * q] * a_inv, v[4 * q + 1] * a_inv, v[4 * q + 2] * a_inv, v[4 * q + 3] * a_inv);
-      }
-    }
-    tc_fence_before();
-  } else if (warp == 4) {
-    // ============ MMA issuer (warp-uniform loop, one elected lane issues) ============
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int64_t u = u0; u < u1; ++u) {
-      mbar_wait(fullA(stage), phase);     // implies fullD: the halo of the stage has landed too
-      tc_fence_after();
-      const uint32_t xs = smem_base + (uint32_t)stage * STAGE;
-      const uint32_t a_t = tmem_base + ACC_COLS + (uint32_t)(stage * A_COLS);
-      // MN-major, 128-byte swizzle: K groups (8 pixels = one image row of the unit) are SBO = 1280 B apart
-      const uint64_t xd0 = (uint64_t)((xs >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1280 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-      const uint32_t acc0 = (u > u0) ? 1u : 0u;
-      if (elect_one()) {
-#pragma unroll
-        for (int r = 0; r < 8; r += 2) {          // K = 16 pixels: image rows r, r + 1 of the unit
-#pragma unroll
-          for (int dx = 0; dx < 3; ++dx) {
-#pragma unroll
-            for (int hf = 0; hf < NCI / 64; ++hf) {
-              const uint64_t xd = xd0 + (uint64_t)((hf * WT_XATOM + r * 1280 + dx * 128) >> 4);
-              mma_f16_ts(tmem_base + (uint32_t)(dx * NCI + hf * 64), a_t + (uint32_t)(r * 4), xd, idesc, r > 0 ? 1u : acc0);
-            }
-          }
+      wg::commit();
+      if (want_bias) {
+        // channel tid of the staged dy tile (swizzled: 16-byte chunk index XOR pixel % 8), pixels in pairs
+        const uint8_t* dyt = smem + (size_t)stage * WT_STAGE + WT_XATOM + (tid >> 6) * WT_DYATOM;
+        const int chk = (tid & 63) >> 3, e = tid & 7;
+#pragma unroll 4
+        for (int m = 0; m < 64; m += 2) {
+          const __half lo = *reinterpret_cast<const __half*>(dyt + m * 128 + ((chk ^ (m & 7)) << 4) + e * 2);
+          const __half hi = *reinterpret_cast<const __half*>(dyt + (m + 1) * 128 + ((chk ^ ((m + 1) & 7)) << 4) + e * 2);
+          bsum += __half2float(lo) + __half2float(hi);
         }
-        mma_commit(empty(stage));
-        if (u + 1 == u1) mma_commit(accum_bar);
       }
-      __syncwarp();
+      wg::wait<1>();
+      if (u > u0) mbar_arrive(empty(prev));
+      prev = stage;
       if (++stage == WT_STAGES) { stage = 0; phase ^= 1; }
     }
-    if (u0 >= u1 && elect_one()) mma_commit(accum_bar);
-    __syncwarp();
+    wg::wait<0>();
+#pragma unroll
+    for (int dx = 0; dx < 3; ++dx) wg::fence_regs<32>(acc[dx]);
+    if (want_bias) p.bpart[(size_t)split * p.Cout + co0 + tid] = bsum * a_inv;
+    const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+#pragma unroll
+    for (int dx = 0; dx < 3; ++dx) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float* o = p.part + (((size_t)split * 9 + dyy * 3 + dx) * p.Cout + co0 + frow + 8 * i) * p.Cin + ci0 + fcol;
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[dx][4 * j + 2 * i] * a_inv, acc[dx][4 * j + 2 * i + 1] * a_inv);
+      }
+    }
   } else {
     // ============ copy issuer (one thread): dy tile + activation halo rows of this kernel row ============
-    if (lane == 0) {
+    wg::regs_dec<wg::COPY_REGS>();
+    if (warp == 8 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int64_t u = u0; u < u1; ++u) {
         const int ux = (int)(u % p.units_x), uy = (int)((u / p.units_x) % p.units_y);
         const int n = (int)(u / ((int64_t)p.units_x * p.units_y));
-        const uint32_t dst = smem_base + (uint32_t)stage * STAGE;
+        const uint32_t dst = smem_base + (uint32_t)stage * WT_STAGE;
         mbar_wait(empty(stage), phase ^ 1);
-        mbar_expect_tx(fullD(stage), STAGE);
+        mbar_expect_tx(fullD(stage), WT_STAGE);
+        tma_load_4d(dst, &x_map, ci0, ux * 8 - 1, uy * 8 + dyy - 1, n, fullD(stage));
 #pragma unroll
-        for (int hf = 0; hf < NCI / 64; ++hf)
-          tma_load_4d(dst + (uint32_t)(hf * WT_XATOM), &x_map, ci0 + hf * 64, ux * 8 - 1, uy * 8 + dyy - 1, n, fullD(stage));
-        tma_load_4d(dst + XB, &dy_map, co0, ux * 8, uy * 8, n, fullD(stage));
+        for (int hf = 0; hf < 2; ++hf)
+          tma_load_4d(dst + WT_XATOM + (uint32_t)(hf * WT_DYATOM), &dy_map, co0 + hf * 64, ux * 8, uy * 8, n, fullD(stage));
         if (++stage == WT_STAGES) { stage = 0; phase ^= 1; }
       }
     }
     __syncwarp();
   }
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
-template <int NCI>
-constexpr size_t wt_smem_bytes() {
-  return 1024 + (size_t)WT_STAGES * ((NCI / 64) * WT_XATOM + WT_DY) + (3 * WT_STAGES + 1) * 8 + 16;
-}
+constexpr size_t wt_smem_bytes() { return 1024 + (size_t)WT_STAGES * WT_STAGE + 2 * WT_STAGES * 8 + 16; }
 
 // fp32 -> fp16 shadow (optionally scaled by the power-of-two operand scale of *amax): plain vectorised copy
 __global__ void to_half_kernel(const float4* __restrict__ x, uint2* __restrict__ y, int64_t n4, const float* __restrict__ amax) {
@@ -508,7 +435,7 @@ int conv3x3_fprop_tma16_launch(const void* x16, mas_tensor4 xs, const void* w_tc
 
   constexpr size_t smem = tc::t16_smem_bytes();
   static std::atomic<uint64_t> configured{0};
-  static int sm_count = 148;
+  static int sm_count = 132;
   if (first_on_device(configured)) {
     cudaError_t e = cudaFuncSetAttribute(tc::shift_gemm_t16<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::shift_gemm_t16<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
@@ -529,7 +456,7 @@ void conv_wgrad_reduce_launch(const float* part, int splits, int ntap, int Cout,
                               cudaStream_t st);   // contract_simt.cu
 
 static int wt_splits(int64_t cps, int64_t units) {
-  int64_t s = 148 / cps;
+  int64_t s = 132 / cps;
   if (s < 1) s = 1;
   if (s > units) s = units;
   const int64_t ups = cdiv(units, s);
@@ -542,8 +469,7 @@ bool conv_wgrad_t16_ok(mas_tensor4 xs, mas_tensor4 dys) {
 size_t conv_wgrad_t16_ws(mas_tensor4 xs, mas_tensor4 dys) {
   if (!conv_wgrad_t16_ok(xs, dys)) return 0;
   const int64_t coutk = cdiv(dys.c, tc::BM) * tc::BM;
-  const int nci = xs.c % 128 == 0 ? 128 : 64;
-  const size_t splits = wt_splits((coutk / tc::BM) * (xs.c / nci) * 3, dys.n * (dys.h / 8) * (dys.w / 8));
+  const size_t splits = wt_splits((coutk / tc::BM) * (xs.c / tc::WT_NCI) * 3, dys.n * (dys.h / 8) * (dys.w / 8));
   return splits * 9 * (size_t)coutk * xs.c * sizeof(float) + splits * (size_t)coutk * sizeof(float) + 256;
 }
 // x16: fp16 activation shadow; dy16: fp16 output-gradient shadow scaled by operand_scale(*dy_amax); dw/dbias sized for
@@ -557,8 +483,7 @@ int conv_wgrad_t16_launch(const void* x16, mas_tensor4 xs, const void* dy16, mas
   p.units_x = (int)(dys.w / 8); p.units_y = (int)(dys.h / 8);
   p.total_units = (int64_t)p.N * p.units_x * p.units_y;
   p.dy_amax = dy_amax;
-  const int nci = p.Cin % 128 == 0 ? 128 : 64;
-  const int splits = wt_splits((int64_t)(p.Cout / tc::BM) * (p.Cin / nci) * 3, p.total_units);
+  const int splits = wt_splits((int64_t)(p.Cout / tc::BM) * (p.Cin / tc::WT_NCI) * 3, p.total_units);
   p.units_per_split = cdiv(p.total_units, splits);
   p.part = (float*)ws;
   p.bpart = dbias ? (float*)ws + (size_t)splits * 9 * p.Cout * p.Cin : nullptr;
@@ -577,21 +502,19 @@ int conv_wgrad_t16_launch(const void* x16, mas_tensor4 xs, const void* dy16, mas
   {
     cuuint64_t dims[4] = {(cuuint64_t)dys.c, (cuuint64_t)dys.w, (cuuint64_t)dys.h, (cuuint64_t)dys.n};
     cuuint64_t strides[3] = {(cuuint64_t)dys.c * 2, (cuuint64_t)dys.w * dys.c * 2, (cuuint64_t)dys.h * dys.w * dys.c * 2};
-    cuuint32_t box[4] = {128, 8, 8, 1}, es[4] = {1, 1, 1, 1};
+    cuuint32_t box[4] = {64, 8, 8, 1}, es[4] = {1, 1, 1, 1};
     CUresult r = enc(&dmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(dy16), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (wgrad dy map) failed (%d)", (int)r);
   }
   static std::atomic<uint64_t> configured{0};
   if (first_on_device(configured)) {
-    cudaError_t e = cudaFuncSetAttribute(tc::wgrad_t16<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::wt_smem_bytes<128>());
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::wgrad_t16<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::wt_smem_bytes<64>());
+    cudaError_t e = cudaFuncSetAttribute(tc::wgrad_t16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::wt_smem_bytes());
     if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(wgrad_t16): %s", cudaGetErrorString(e));
     mark_device(configured);
   }
-  dim3 grid((unsigned)((p.Cin / nci) * 3), (unsigned)(p.Cout / tc::BM), (unsigned)splits);
-  if (nci == 128) tc::wgrad_t16<128><<<grid, tc::WT_THREADS, tc::wt_smem_bytes<128>(), st>>>(p, xmap, dmap);
-  else tc::wgrad_t16<64><<<grid, tc::WT_THREADS, tc::wt_smem_bytes<64>(), st>>>(p, xmap, dmap);
+  dim3 grid((unsigned)((p.Cin / tc::WT_NCI) * 3), (unsigned)(p.Cout / tc::BM), (unsigned)splits);
+  tc::wgrad_t16<<<grid, tc::WT_THREADS, tc::wt_smem_bytes(), st>>>(p, xmap, dmap);
   if (int e = launched_tc("wgrad_t16")) return e;
   conv_wgrad_reduce_launch((const float*)ws, splits, 9, p.Cout, p.Cin, dw, p.bpart, dbias, st);
   return launched("conv_wgrad_reduce");
@@ -602,7 +525,7 @@ int to_half_launch(const float* x, void* y, int64_t n, const float* amax, cudaSt
     return fail(MAS_ERR_INVALID_ARG, "to_half: n %% 4 == 0 and aligned pointers required");
   const int64_t n4 = n / 4;
   const int64_t blocks = cdiv(n4, 256);
-  tc::to_half_kernel<<<(unsigned)(blocks < 148 * 16 ? blocks : 148 * 16), 256, 0, st>>>(reinterpret_cast<const float4*>(x),
+  tc::to_half_kernel<<<(unsigned)(blocks < 132 * 16 ? blocks : 132 * 16), 256, 0, st>>>(reinterpret_cast<const float4*>(x),
                                                                                        reinterpret_cast<uint2*>(y), n4, amax);
   return launched("to_half");
 }

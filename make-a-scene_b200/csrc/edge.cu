@@ -220,7 +220,7 @@ static int edge_geom(EdgeGeom& g, mas_tensor4 small, mas_tensor4 big, const char
   g.sn = small.sn; g.sh = small.sh; g.sw = small.sw; g.sc = small.sc;
   return MAS_OK;
 }
-constexpr int EDGE_PBLOCKS = 148 * 4;
+constexpr int EDGE_PBLOCKS = NUM_SMS * 4;
 
 }  // namespace mas
 
@@ -299,7 +299,7 @@ int mas_edge_small_cout_wgrad(const float* a, mas_tensor4 at, const float* dys, 
 
 // ---------------------------------------------------------------------------------------------------- stride-2 conv via space-to-depth
 // Downsample (modules.py:74-78) = pad(0,1,0,1) + conv3x3 stride 2.  With X4[n,i,j,(py,px,c)] = x[n,2i+py,2j+px,c] the
-// stride-2 gather becomes a unit-stride 2x2-tap convolution over 4C channels, which the tcgen05 stride-1 kernels run as a
+// stride-2 gather becomes a unit-stride 2x2-tap convolution over 4C channels, which the wgmma stride-1 kernels run as a
 // 3x3 convolution whose other five taps are zero:  y[o] = sum_{a,b in {0,1}} X4[o+(a,b)] . W9[(a+1,b+1)],
 // W9[(a+1,b+1)][(py,px,c)] = W[2a+py][2b+px][c] (0 where 2a+py or 2b+px exceeds 2).  Zero padding beyond the last X4
 // row/column is exactly the reference's bottom/right pad.
@@ -353,7 +353,7 @@ extern "C" {
 int mas_space_to_depth(const float* x, float* y, int N, int H, int W, int C, void* stream) {
   if (C % 4 || H % 2 || W % 2) return fail(MAS_ERR_UNSUPPORTED, "space_to_depth: needs C %% 4 == 0 and even H, W");
   int64_t total4 = (int64_t)N * H * W * (C / 4);
-  int grid = (int)(cdiv(total4, 256) < 148 * 16 ? cdiv(total4, 256) : 148 * 16);
+  int grid = (int)(cdiv(total4, 256) < NUM_SMS * 16 ? cdiv(total4, 256) : NUM_SMS * 16);
   space_to_depth_kernel<<<grid, 256, 0, S(stream)>>>(x, y, H, W, C / 4, total4);
   return launched("space_to_depth");
 }

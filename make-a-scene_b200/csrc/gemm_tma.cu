@@ -1,4 +1,4 @@
-// Row GEMM  y[M, N] = alpha * x[M, K] . W[N, K]^T (+ bias, + residual)  as a pure TMA + tcgen05 kernel on fp16 operands: the
+// Row GEMM  y[M, N] = alpha * x[M, K] . W[N, K]^T (+ bias, + residual)  as a pure TMA + wgmma kernel on fp16 operands: the
 // Linear layers of the token transformer (transformer.py:17-56, forward and data gradient) and, in general, any 1x1
 // convolution whose input exists as a dense fp16 [M, K] matrix.  It is shift_gemm_t16 (conv_tma.cu) with one tap:
 //   * A side of the problem (activations): ONE 2-D tensor-map copy per 64-channel chunk, box 64 halves x 256 rows under the
@@ -6,18 +6,19 @@
 //     M are zero-filled by the copy engine;
 //   * weights: mas_pack_gemm_tc16 image [n_tile][k/16][k/8 % 2][128][8 halves] (no swizzle): the four K = 16 steps of a chunk are
 //     16 KB contiguous -> one cp.async.bulk per chunk, into the same ring stage as the activation tile (one barrier pair);
-//   * operand roles swapped (D^T = W x X^T: weights on the M side, 256 rows on the N side of ONE M128 x N256 x K16 MMA): a TMEM
-//     lane is an output feature, a column a row of x - the epilogue's 32 lanes store 32 consecutive floats of one output row
-//     (a full 128-byte line per instruction, no shared-memory transpose), bias is a per-thread scalar;
+//   * operand roles swapped (D^T = W x X^T: weights on the M side, 256 rows on the N side of wgmma.m64n256k16): warpgroup g
+//     owns output features 64 g .. 64 g + 63 of the 128-feature tile, bias is a per-row scalar of the fragment;
 //   * one persistent CTA per SM over (256-row tile x 128-feature tile) items, feature tile fastest (the row tile is re-read
-//     from L2), 4-stage ring of 48 KB, two 256-column accumulator sets: 8 epilogue warps drain one while the MMAs fill the other;
-//   * warps 0-7 epilogue, warp 8 MMA issuer (warp-uniform loop, elected lane), warp 9 copy issuer: no thread touches an operand.
+//     from L2), 4-stage ring of 48 KB that keeps running across items while the warpgroups store the previous item;
+//   * warps 0-7 MMA + epilogue (two warpgroups), warp 8 copy issuer (its warpgroup hands its registers to the MMA ones):
+//     no thread touches an operand.
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <cuda_fp16.h>
 
 #include "mas_common.cuh"
 #include "tc_ptx.cuh"
+#include "wgmma.cuh"
 
 namespace mas {
 
@@ -25,8 +26,8 @@ PFN_cuTensorMapEncodeTiled tensor_map_encoder();   // contract_tc.cu
 
 namespace tc {
 
-constexpr int G_EPI_WARPS = 8;
-constexpr int G_THREADS = (G_EPI_WARPS + 2) * 32;
+constexpr int G_MMA_WARPS = 8;
+constexpr int G_THREADS = (G_MMA_WARPS + 4) * 32;   // + the copy-issuing warpgroup
 constexpr int G_STAGES = 4;
 constexpr int G_ROWS = 256;                        // rows of x per work item (N of the MMA)
 constexpr int G_A = G_ROWS * 128;                  // 256 rows x 64 halves
@@ -46,23 +47,15 @@ struct GParams {
   float alpha;
 };
 
-__device__ __forceinline__ uint64_t make_desc_sw128g(uint32_t saddr, uint32_t sbo_bytes) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) | (1ull << 46) | (2ull << 61);
-}
-
 __global__ void __launch_bounds__(G_THREADS, 1) rows_gemm_t16(const GParams p, const __grid_constant__ CUtensorMap x_map) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
   const uint32_t smem_base = (raw_base + 1023u) & ~1023u;           // swizzle atoms are 1024-byte aligned
   uint8_t* smem = smem_raw + (smem_base - raw_base);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)G_STAGES * G_STAGE);
-  constexpr int NBARS = 2 * G_STAGES + 4;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + NBARS);
   const uint32_t bar_base = smem_u32(bars);
   auto full = [&](int s) { return bar_base + 8u * s; };
   auto empty = [&](int s) { return bar_base + 8u * (G_STAGES + s); };
-  auto accf = [&](int b) { return bar_base + 8u * (2 * G_STAGES + b); };
-  auto acce = [&](int b) { return bar_base + 8u * (2 * G_STAGES + 2 + b); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int chunks = p.K / 64;
@@ -70,90 +63,68 @@ __global__ void __launch_bounds__(G_THREADS, 1) rows_gemm_t16(const GParams p, c
   const int64_t nitems = p.units * n_tiles;
 
   if (tid == 0) {
-    for (int s = 0; s < G_STAGES; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(accf(b), 1); mbar_init(acce(b), G_EPI_WARPS * 32); }
+    for (int s = 0; s < G_STAGES; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), G_MMA_WARPS * 32); }
     fence_barrier_init();
   }
-  if (warp == G_EPI_WARPS) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp < G_EPI_WARPS) {
-    // ===================== epilogue warps: lane = output feature, column = row of x =====================
+  if (warp < G_MMA_WARPS) {
+    // ===================== MMA warpgroups: fragment row = output feature, column = row of x =====================
+    wg::regs_inc<wg::MMA_REGS>();
     float inv_scale = 1.f;
     operand_scale(p.x_amax, &inv_scale);
     const float alpha = inv_scale * p.alpha;
-    const int quarter = warp & 3, hf = warp >> 2;
-    int buf = 0;
-    uint32_t ph[2] = {0u, 0u};
+    const int wgi = warp >> 2;
+    const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+    int s = 0, prev = 0;
+    uint32_t sph = 0;
+    float acc[G_ROWS / 2];
     for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-      const int64_t unit = item / n_tiles;
-      const int ch = (int)(item % n_tiles) * BN + quarter * 32 + lane;
-      const bool st_ok = ch < p.Nstore;
-      const float bv = (p.bias && st_ok) ? __ldg(p.bias + ch) : 0.f;
-      const int64_t row0 = unit * G_ROWS + hf * 128;
-      mbar_wait(accf(buf), ph[buf]);
-      ph[buf] ^= 1u;
-      tc_fence_after();
-#pragma unroll 1
-      for (int cb = 0; cb < 4; ++cb) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(quarter * 32) << 16) + (uint32_t)(buf * 256 + hf * 128 + cb * 32), v);
-        if (cb == 3) {
-          tc_fence_before();
-          mbar_arrive(acce(buf));     // this warp's share of the accumulator set is in registers
-        }
-        const int64_t r0 = row0 + cb * 32;
-        if (st_ok) {
-          float* yp = p.y + r0 * p.ldy + ch;
-          const float* rp = p.res ? p.res + r0 * p.ldy + ch : nullptr;
+      for (int c = 0; c < chunks; ++c) {
+        mbar_wait(full(s), sph);
+        const uint32_t st = smem_base + (uint32_t)s * G_STAGE;
+        const uint64_t xd0 = wg::desc(st, 16, 1024, wg::SW_128);
+        const uint64_t wd0 = wg::desc(st + G_A + (uint32_t)(wgi * 1024), BN * 16, 128);
+        wg::fence();
 #pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            if (r0 + j < p.M) {
-              float o = fmaf(v[j], alpha, bv);
-              if (rp) o += __ldg(rp + (int64_t)j * p.ldy);
-              yp[(int64_t)j * p.ldy] = o;
+        for (int sub = 0; sub < 4; ++sub)   // D^T = W x X^T: weights on the M side, the 256 rows on the N side
+          wg::wgmma_f16_ss_n256<0, 0>(acc, wd0 + (uint64_t)((sub * G_BSUB) >> 4), xd0 + (uint64_t)((sub * 32) >> 4),
+                                      (c > 0 || sub > 0) ? 1u : 0u);
+        wg::commit();
+        wg::wait<1>();
+        if (c > 0) mbar_arrive(empty(prev));   // the previous chunk's MMAs have read their stage
+        prev = s;
+        if (++s == G_STAGES) { s = 0; sph ^= 1; }
+      }
+      wg::wait<0>();
+      wg::fence_regs<G_ROWS / 2>(acc);
+      mbar_arrive(empty(prev));
+      const int64_t unit = item / n_tiles;
+      const int64_t row0 = unit * G_ROWS + fcol;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int ch = (int)(item % n_tiles) * BN + frow + 8 * i;
+        if (ch < p.Nstore) {
+          const float bv = p.bias ? __ldg(p.bias + ch) : 0.f;
+#pragma unroll
+          for (int j = 0; j < G_ROWS / 8; ++j) {
+#pragma unroll
+            for (int cc = 0; cc < 2; ++cc) {
+              const int64_t r = row0 + 8 * j + cc;
+              if (r < p.M) {
+                float o = fmaf(acc[4 * j + 2 * i + cc], alpha, bv);
+                if (p.res) o += __ldg(p.res + r * p.ldy + ch);
+                p.y[r * p.ldy + ch] = o;
+              }
             }
           }
         }
       }
-      buf ^= 1;
-    }
-  } else if (warp == G_EPI_WARPS) {
-    // ===================== MMA issuer =====================
-    constexpr uint32_t idesc = make_idesc_f16(G_ROWS);
-    int s = 0, buf = 0;
-    uint32_t sph = 0, eph[2] = {0u, 0u};
-    for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-      mbar_wait(acce(buf), eph[buf] ^ 1);     // the epilogue warps have read this accumulator set (first use: passes)
-      eph[buf] ^= 1u;
-      tc_fence_after();
-      const uint32_t acc = tmem_base + (uint32_t)(buf * 256);
-      for (int c = 0; c < chunks; ++c) {
-        mbar_wait(full(s), sph);
-        tc_fence_after();
-        const uint32_t st = smem_base + (uint32_t)s * G_STAGE;
-        const uint64_t xd0 = make_desc_sw128g(st, 1024);
-        const uint64_t wd0 = make_desc(st + G_A, BN * 16, 128);
-        if (elect_one()) {
-#pragma unroll
-          for (int sub = 0; sub < 4; ++sub) {
-            // D^T = W x X^T: weights on the M side, the 256 rows on the N side
-            mma_f16_ss(acc, wd0 + (uint64_t)((sub * G_BSUB) >> 4), xd0 + (uint64_t)((sub * 32) >> 4), idesc, (c > 0 || sub > 0) ? 1u : 0u);
-          }
-          mma_commit(empty(s));
-          if (c == chunks - 1) mma_commit(accf(buf));
-        }
-        __syncwarp();
-        if (++s == G_STAGES) { s = 0; sph ^= 1; }
-      }
-      buf ^= 1;
     }
   } else {
     // ===================== copy issuer (one thread) =====================
-    if (lane == 0) {
+    wg::regs_dec<wg::COPY_REGS>();
+    if (warp == G_MMA_WARPS && lane == 0) {
       int s = 0;
       uint32_t sph = 0;
       const int ksteps = p.K / 16;
@@ -172,30 +143,25 @@ __global__ void __launch_bounds__(G_THREADS, 1) rows_gemm_t16(const GParams p, c
     }
     __syncwarp();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == G_EPI_WARPS) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
-constexpr size_t g16_smem_bytes() { return 1024 + (size_t)G_STAGES * G_STAGE + (2 * G_STAGES + 4) * 8 + 16; }
+constexpr size_t g16_smem_bytes() { return 1024 + (size_t)G_STAGES * G_STAGE + 2 * G_STAGES * 8 + 16; }
 
 // ------------------------------------------------------------------------------------------------------------
 // Weight gradient of a Linear layer from the two fp16 copies (activation x16 [M,K], output gradient dy16 [M,N], both scaled by
 // their power-of-two operand scales): dW[n][k] = sum_m dy[m][n] * x[m][k].  The reduction runs over ROWS, so both operands are
 // "MN-major" in memory (features contiguous, rows strided) - the one-tap form of wgrad_t16 (conv_tma.cu):
-//   * A = dy^T in tensor memory (TS mode): the dy tile of a unit (64 rows x 128 features, one 2-D tensor-map copy, no swizzle)
-//     is moved shared -> registers -> TMEM by four loader warps, two rows per 32-bit column, lane = output feature;
+//   * A = dy^T: the dy tile of a unit (64 rows x 128 features) lands as two 64-feature tensor-map boxes under the 128-byte
+//     swizzle, an MN-major operand; warpgroup g multiplies features 64 g .. 64 g + 63;
 //   * B = x tiles exactly as the copy engine lands them under the 128-byte swizzle: [64 rows][64 features] atoms read as an
 //     MN-major operand (K groups = 8 rows, SBO = 1024 B), N = 64 MMAs, K = 16 rows per MMA;
-//   * a CTA owns a 128 x NCI block of dW (NCI accumulator columns); split-K over the 64-row units; partial sums (and the bias
-//     gradient from the dy loaders) go to the caller's workspace in the layout conv_wgrad_reduce expects (one tap).
+//   * a CTA owns a 128 x NCI block of dW (NCI / 64 accumulator fragments per warpgroup); split-K over the 64-row units; partial
+//     sums (and the bias gradient, summed from the staged dy tile) go to the caller's workspace in the layout conv_wgrad_reduce
+//     expects (one tap).
 constexpr int RW_STAGES = 4;
 constexpr int RW_XATOM = 64 * 128;          // 64 rows x 64 features (halves)
-constexpr int RW_DY = 64 * 128 * 2;         // 64 rows x 128 features (halves)
-constexpr int RW_THREADS = 6 * 32;
+constexpr int RW_DY = 2 * RW_XATOM;         // 64 rows x 128 features (halves), two swizzle atoms
+constexpr int RW_THREADS = 12 * 32;
 
 struct RWParams {
   float* part;      // [splits][N][K]
@@ -210,22 +176,16 @@ template <int NCI>
 __global__ void __launch_bounds__(RW_THREADS, 1) rows_wgrad_t16(const RWParams p, const __grid_constant__ CUtensorMap x_map,
                                                                const __grid_constant__ CUtensorMap dy_map) {
   constexpr int XB = (NCI / 64) * RW_XATOM, STAGE = XB + RW_DY;
-  constexpr uint32_t ACC_COLS = NCI, A_COLS = 32;
-  static_assert(ACC_COLS + RW_STAGES * A_COLS <= 512, "tensor memory budget");
   static_assert(STAGE % 1024 == 0, "stages must keep the swizzle atoms 1024-byte aligned");
-  constexpr uint32_t idesc = make_idesc_f16(64) | (1u << 16);   // B operand MN-major
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
   const uint32_t smem_base = (raw_base + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (smem_base - raw_base);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)RW_STAGES * STAGE);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 3 * RW_STAGES + 1);
   const uint32_t bar_base = smem_u32(bars);
   auto fullD = [&](int s) { return bar_base + 8u * s; };                      // copies of the stage have landed
-  auto fullA = [&](int s) { return bar_base + 8u * (RW_STAGES + s); };        // dy^T of the stage is in tensor memory
-  auto empty = [&](int s) { return bar_base + 8u * (2 * RW_STAGES + s); };    // the MMAs of the stage have completed
-  const uint32_t accum_bar = bar_base + 8u * (3 * RW_STAGES);
+  auto empty = [&](int s) { return bar_base + 8u * (RW_STAGES + s); };        // the MMAs of the stage have completed
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int ci0 = blockIdx.x * NCI, co0 = blockIdx.y * BM, split = blockIdx.z;
@@ -233,89 +193,76 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_wgrad_t16(const RWParams p
   const int64_t u1 = min(p.total_units, u0 + p.units_per_split);
 
   if (tid == 0) {
-    for (int s = 0; s < RW_STAGES; ++s) { mbar_init(fullD(s), 1); mbar_init(fullA(s), 128); mbar_init(empty(s), 1); }
-    mbar_init(accum_bar, 1);
+    for (int s = 0; s < RW_STAGES; ++s) { mbar_init(fullD(s), 1); mbar_init(empty(s), 256); }
     fence_barrier_init();
   }
-  if (warp == 4) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  if (warp < 4) {
-    // ============ dy loaders, then epilogue ============
-    const int cl = warp * 32 + lane;          // feature within the tile = TMEM lane
+  if (warp < 8) {
+    // ============ MMA warpgroups (bias-gradient sums by warpgroup 0), then epilogue ============
+    wg::regs_inc<wg::MMA_REGS>();
+    const int wgi = warp >> 2;
     float dy_inv, x_inv;
     operand_scale(p.dy_amax, &dy_inv);
     operand_scale(p.x_amax, &x_inv);
     float bsum = 0.f;
-    const bool want_bias = p.bpart != nullptr && blockIdx.x == 0;
-    int stage = 0;
+    const bool want_bias = p.bpart != nullptr && blockIdx.x == 0 && tid < 128;
+    float acc[NCI / 64][32];
+#pragma unroll
+    for (int h = 0; h < NCI / 64; ++h)
+#pragma unroll
+      for (int i = 0; i < 32; ++i) acc[h][i] = 0.f;
+    int stage = 0, prev = 0;
     uint32_t phase = 0;
     for (int64_t u = u0; u < u1; ++u) {
       mbar_wait(fullD(stage), phase);
-      const unsigned short* dh = reinterpret_cast<const unsigned short*>(smem + (size_t)stage * STAGE + XB) + cl;
-      float w[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        const uint32_t lo = dh[(2 * j) * 128], hi = dh[(2 * j + 1) * 128];
-        w[j] = __uint_as_float(lo | (hi << 16));
-        if (want_bias) bsum += __half2float(__ushort_as_half((unsigned short)lo)) + __half2float(__ushort_as_half((unsigned short)hi));
-      }
-      tc_fence_after();
-      tmem_st32(tmem_base + ((uint32_t)(warp * 32) << 16) + ACC_COLS + (uint32_t)(stage * A_COLS), w);
-      tmem_st_wait();
-      tc_fence_before();
-      mbar_arrive(fullA(stage));
-      if (++stage == RW_STAGES) { stage = 0; phase ^= 1; }
-    }
-    if (want_bias) p.bpart[(size_t)split * p.N + co0 + cl] = bsum * dy_inv;
-    mbar_wait(accum_bar, 0);
-    tc_fence_after();
-    const float a_inv = dy_inv * x_inv;
-    float* o = p.part + ((size_t)split * p.N + co0 + cl) * p.K + ci0;
-#pragma unroll 1
-    for (int cb = 0; cb < NCI / 32; ++cb) {
-      float v[32];
-      tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(cb * 32), v);
-#pragma unroll
-      for (int q = 0; q < 8; ++q)
-        *reinterpret_cast<float4*>(o + cb * 32 + q * 4) = make_float4(v[4 * q] * a_inv, v[4 * q + 1] * a_inv, v[4 * q + 2] * a_inv, v[4 * q + 3] * a_inv);
-    }
-    tc_fence_before();
-  } else if (warp == 4) {
-    // ============ MMA issuer (warp-uniform loop, one elected lane issues) ============
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int64_t u = u0; u < u1; ++u) {
-      mbar_wait(fullA(stage), phase);     // implies fullD: the x tiles of the stage have landed too
-      tc_fence_after();
       const uint32_t xs = smem_base + (uint32_t)stage * STAGE;
-      const uint32_t a_t = tmem_base + ACC_COLS + (uint32_t)(stage * A_COLS);
       // MN-major, 128-byte swizzle: K groups (8 rows of 128 bytes) are SBO = 1024 B apart
-      const uint64_t xd0 = (uint64_t)((xs >> 4) & 0x3FFF) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-      const uint32_t acc0 = (u > u0) ? 1u : 0u;
-      if (elect_one()) {
+      const uint64_t xd0 = wg::desc(xs, 16, 1024, wg::SW_128);
+      const uint64_t ad0 = wg::desc(xs + XB + (uint32_t)(wgi * RW_XATOM), 16, 1024, wg::SW_128);
+      wg::fence();
 #pragma unroll
-        for (int r = 0; r < 4; ++r) {             // K = 16 rows per MMA: rows 16 r .. 16 r + 15 of the unit
+      for (int r = 0; r < 4; ++r) {             // K = 16 rows per MMA: rows 16 r .. 16 r + 15 of the unit
 #pragma unroll
-          for (int hf = 0; hf < NCI / 64; ++hf) {
-            const uint64_t xd = xd0 + (uint64_t)((hf * RW_XATOM + r * 2048) >> 4);
-            mma_f16_ts(tmem_base + (uint32_t)(hf * 64), a_t + (uint32_t)(r * 8), xd, idesc, r > 0 ? 1u : acc0);
-          }
-        }
-        mma_commit(empty(stage));
-        if (u + 1 == u1) mma_commit(accum_bar);
+        for (int hf = 0; hf < NCI / 64; ++hf)
+          wg::wgmma_f16_ss_n64<1, 1>(acc[hf], ad0 + (uint64_t)((r * 2048) >> 4), xd0 + (uint64_t)((hf * RW_XATOM + r * 2048) >> 4), 1u);
       }
-      __syncwarp();
+      wg::commit();
+      if (want_bias) {
+        // column tid of the staged dy tile (swizzled: 16-byte chunk index XOR row % 8), rows in pairs
+        const uint8_t* dyt = smem + (size_t)stage * STAGE + XB + (tid >> 6) * RW_XATOM;
+        const int ch = (tid & 63) >> 3, e = tid & 7;
+#pragma unroll 4
+        for (int m = 0; m < 64; m += 2) {
+          const __half lo = *reinterpret_cast<const __half*>(dyt + m * 128 + ((ch ^ (m & 7)) << 4) + e * 2);
+          const __half hi = *reinterpret_cast<const __half*>(dyt + (m + 1) * 128 + ((ch ^ ((m + 1) & 7)) << 4) + e * 2);
+          bsum += __half2float(lo) + __half2float(hi);
+        }
+      }
+      wg::wait<1>();
+      if (u > u0) mbar_arrive(empty(prev));
+      prev = stage;
       if (++stage == RW_STAGES) { stage = 0; phase ^= 1; }
     }
-    if (u0 >= u1 && elect_one()) mma_commit(accum_bar);
-    __syncwarp();
+    wg::wait<0>();
+#pragma unroll
+    for (int h = 0; h < NCI / 64; ++h) wg::fence_regs<32>(acc[h]);
+    if (want_bias) p.bpart[(size_t)split * p.N + co0 + tid] = bsum * dy_inv;
+    const float a_inv = dy_inv * x_inv;
+    const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      float* o = p.part + ((size_t)split * p.N + co0 + frow + 8 * i) * p.K + ci0 + fcol;
+#pragma unroll
+      for (int hf = 0; hf < NCI / 64; ++hf)
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+          *reinterpret_cast<float2*>(o + hf * 64 + 8 * j) = make_float2(acc[hf][4 * j + 2 * i] * a_inv, acc[hf][4 * j + 2 * i + 1] * a_inv);
+    }
   } else {
     // ============ copy issuer (one thread): dy tile + x tiles of the unit ============
-    if (lane == 0) {
+    wg::regs_dec<wg::COPY_REGS>();
+    if (warp == 8 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       for (int64_t u = u0; u < u1; ++u) {
@@ -324,22 +271,18 @@ __global__ void __launch_bounds__(RW_THREADS, 1) rows_wgrad_t16(const RWParams p
         mbar_expect_tx(fullD(stage), STAGE);
 #pragma unroll
         for (int hf = 0; hf < NCI / 64; ++hf) tma_load_2d(dst + (uint32_t)(hf * RW_XATOM), &x_map, ci0 + hf * 64, (int)(u * 64), fullD(stage));
-        tma_load_2d(dst + XB, &dy_map, co0, (int)(u * 64), fullD(stage));
+#pragma unroll
+        for (int hf = 0; hf < 2; ++hf) tma_load_2d(dst + XB + (uint32_t)(hf * RW_XATOM), &dy_map, co0 + hf * 64, (int)(u * 64), fullD(stage));
         if (++stage == RW_STAGES) { stage = 0; phase ^= 1; }
       }
     }
     __syncwarp();
   }
-  __syncthreads();
-  if (warp == 4) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
 }
 
 template <int NCI>
 constexpr size_t rw_smem_bytes() {
-  return 1024 + (size_t)RW_STAGES * ((NCI / 64) * RW_XATOM + RW_DY) + (3 * RW_STAGES + 1) * 8 + 16;
+  return 1024 + (size_t)RW_STAGES * ((NCI / 64) * RW_XATOM + RW_DY) + 2 * RW_STAGES * 8 + 16;
 }
 
 }  // namespace tc
@@ -368,7 +311,7 @@ int gemm_rows_f16_launch(const void* x16, int64_t M, int K, const void* w_tc16, 
 
   constexpr size_t smem = tc::g16_smem_bytes();
   static std::atomic<uint64_t> configured{0};
-  static int sm_count = 148;
+  static int sm_count = 132;
   if (first_on_device(configured)) {
     cudaError_t e = cudaFuncSetAttribute(tc::rows_gemm_t16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e));
@@ -390,13 +333,13 @@ void conv_wgrad_reduce_launch(const float* part, int splits, int ntap, int Cout,
 bool wgrad_rows_f16_ok(int64_t M, int N, int K) { return M > 0 && N % 128 == 0 && K % 128 == 0 && N > 0 && K > 0 && M < (1ll << 31) - 64; }
 static int rw_nci(int K) { return K % 256 == 0 ? 256 : 128; }
 static int rw_splits(int64_t M, int N, int K) {
-  // split-K factor: fill whole waves of the 148 SMs (the partial sums cost a reduction pass, so fewer splits win ties)
+  // split-K factor: fill whole waves of the 132 SMs (the partial sums cost a reduction pass, so fewer splits win ties)
   const int64_t ctas = (int64_t)(N / 128) * (K / rw_nci(K)), units = cdiv(M, 64);
   int best = 1;
   double best_score = -1.0;
   for (int s = 1; s <= 16 && s <= units; ++s) {
     const int64_t g = ctas * s;
-    const double eff = (double)g / (double)(cdiv(g, 148) * 148) - 0.02 * s;
+    const double eff = (double)g / (double)(cdiv(g, 132) * 132) - 0.02 * s;
     if (eff > best_score + 1e-9) { best_score = eff; best = s; }
   }
   const int64_t ups = cdiv(units, best);
@@ -434,9 +377,9 @@ int wgrad_rows_f16_launch(const void* x16, const void* dy16, int64_t M, int N, i
   {
     cuuint64_t dims[2] = {(cuuint64_t)N, (cuuint64_t)M};
     cuuint64_t strides[1] = {(cuuint64_t)N * 2};
-    cuuint32_t box[2] = {128, 64}, es[2] = {1, 1};
+    cuuint32_t box[2] = {64, 64}, es[2] = {1, 1};
     CUresult r = enc(&dmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(dy16), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (row wgrad dy map) failed (%d)", (int)r);
   }
   static std::atomic<uint64_t> configured{0};

@@ -1,4 +1,4 @@
-// Shared helpers for libmas_b200.so (sm_100a only).
+// Shared helpers for libmas_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -9,6 +9,9 @@
 
 namespace mas {
 
+// streaming multiprocessors of the H100 SXM: grid-size heuristics (the persistent kernels query the device instead)
+constexpr int NUM_SMS = 132;
+
 extern thread_local char g_err[512];
 extern std::atomic<int64_t> g_launches;
 extern std::atomic<int64_t> g_tc_launches;
@@ -16,7 +19,7 @@ extern std::atomic<int64_t> g_tc_launches;
 int fail(int code, const char* fmt, ...);
 // Checks the launch that was just enqueued (no synchronisation) and counts it.
 int launched(const char* what);
-// Same, for a kernel that issues tcgen05 MMAs (counted separately: mas_tc_launch_count).
+// Same, for a kernel that issues tensor-core (wgmma) MMAs (counted separately: mas_tc_launch_count).
 int launched_tc(const char* what);
 
 // cudaFuncSetAttribute is per device: true the first time a call site runs on the CURRENT device (bit d of `mask`).

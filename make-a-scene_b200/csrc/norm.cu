@@ -790,7 +790,7 @@ __global__ void sum_final_kernel(const double* __restrict__ part, int n, double 
 
 static inline int ew_grid(int64_t n, int threads = 256) {
   int64_t b = cdiv(n, threads);
-  return (int)(b < 148 * 16 ? (b < 1 ? 1 : b) : 148 * 16);
+  return (int)(b < NUM_SMS * 16 ? (b < 1 ? 1 : b) : NUM_SMS * 16);
 }
 
 }  // namespace mas
@@ -814,7 +814,7 @@ static int gn_check(int N, int HW, int C, int G) {
 static int gn_chunks(int N, int HW, int C) {
   const int lanes = GN_THREADS / (C / 4);
   int pix = GN_PIX;
-  while (pix > 4 * lanes && pix > 8 && (int64_t)N * cdiv(HW, pix) < 4 * 148) pix >>= 1;
+  while (pix > 4 * lanes && pix > 8 && (int64_t)N * cdiv(HW, pix) < 4 * NUM_SMS) pix >>= 1;
   return (int)cdiv(HW, pix);
 }
 
@@ -940,7 +940,7 @@ int mas_amax(const float* x, int64_t n, float* out, void* stream) {
   if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "amax: memset: %s", cudaGetErrorString(e));
   const int64_t n4 = n / 4;
   const int64_t blocks = cdiv(n4 > 0 ? n4 : 1, 256 * 8);
-  amax_kernel<<<(int)(blocks < 148 * 8 ? blocks : 148 * 8), 256, 0, S(stream)>>>(reinterpret_cast<const float4*>(x), n4, x + n4 * 4,
+  amax_kernel<<<(int)(blocks < NUM_SMS * 8 ? blocks : NUM_SMS * 8), 256, 0, S(stream)>>>(reinterpret_cast<const float4*>(x), n4, x + n4 * 4,
                                                                                  (int)(n - n4 * 4), reinterpret_cast<unsigned int*>(out));
   return launched("amax");
 }

@@ -27,7 +27,7 @@ extern "C" {
 // Launches the probe; *flops_out (host) receives the FLOPs one launch executes (2 per FMA).
 int mas_ffma_probe(float* scratch, int iters, double* flops_out_host, void* stream) {
   MAS_REQUIRE(scratch && iters > 0, "ffma_probe: bad arguments");
-  const int blocks = 148 * 4, threads = 512;
+  const int blocks = NUM_SMS * 4, threads = 512;
   ffma_probe_kernel<<<blocks, threads, 0, S(stream)>>>(scratch, iters, 0.999f, 0.001f);
   if (flops_out_host) *flops_out_host = 2.0 * 16 * 8 * (double)iters * blocks * threads;
   return launched("ffma_probe");

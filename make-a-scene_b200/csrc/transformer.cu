@@ -251,7 +251,7 @@ __global__ void __launch_bounds__(256) layernorm_bwd_dx_block_kernel(const float
 }
 
 // column sums for dgamma / dbeta: block (32,8) per 32-column tile and row chunk; deterministic two-stage
-constexpr int LN_ROWS = 128;    // rows per partial block: 5120 rows x 1024 columns -> 32 x 40 blocks (1024 rows per block left 160 blocks for 148 SMs)
+constexpr int LN_ROWS = 128;    // rows per partial block: 5120 rows x 1024 columns -> 32 x 40 blocks (1024 rows per block left 160 blocks for 132 SMs)
 __global__ void layernorm_bwd_param_partial(const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ mean,
                                             const float* __restrict__ rstd, int64_t R, int H, double* __restrict__ part) {
   __shared__ double sh[8][32][2];
@@ -449,7 +449,7 @@ __global__ void __launch_bounds__(256) ce_bwd_kernel(const float* __restrict__ l
 
 static inline int ew_grid2(int64_t n) {
   int64_t b = cdiv(n, 256);
-  return (int)(b < 148 * 16 ? (b < 1 ? 1 : b) : 148 * 16);
+  return (int)(b < NUM_SMS * 16 ? (b < 1 ? 1 : b) : NUM_SMS * 16);
 }
 
 }  // namespace mas

@@ -232,7 +232,7 @@ __global__ void __launch_bounds__(256) vq_merge_kernel(const float* __restrict__
 // Error model behind the margin.  For a pair (row r, code k) let P = |z_r| * max_k |e_k| >= sum_i |z_i e_i|.
 //   * operand split: each operand keeps >= 22 significant bits and the product of the two low parts is dropped:
 //       |error| <= (2^-21 + 2^-22) P;
-//   * fp32 accumulation in tensor memory: at most 3 * D/16 + 16 * 3 additions per dot product in whatever order and
+//   * fp32 accumulation in the tensor cores: at most 3 * D/16 + 16 * 3 additions per dot product in whatever order and
 //     rounding mode (truncation assumed): <= (3*D/16 + 48) * 2^-23 * 3 P   (the factor 3: three partial products of size <= P);
 //   * the exact path itself (the FFMA kernel, and equally the reference's sgemm in any summation order):
 //       <= (D + 2) * 2^-24 * P  for the dot product, + 3 * 2^-24 * (|z|^2 + |e|^2) for the two roundings of the formula.
@@ -458,7 +458,7 @@ using namespace mas;
 
 extern "C" {
 
-static int vq_splits(int64_t R) { return cdiv(R, VQ_BM) < 148 * 2 ? 2 : 1; }
+static int vq_splits(int64_t R) { return cdiv(R, VQ_BM) < NUM_SMS * 2 ? 2 : 1; }
 static size_t a256(size_t v) { return (v + 255) / 256 * 256; }
 static std::atomic<int> g_vq_tc{-1};   // -1: unset (MAS_VQ_TC=0 in the environment disables), 0 / 1: mas_vq_select_path
 static bool vq_use_tc(int64_t R, int K, int D) {
@@ -585,10 +585,10 @@ int mas_kmeans_update(const float* x, const int64_t* idx, int64_t n, int K, int 
   cudaError_t e = cudaMemsetAsync(ws, 0, mas_kmeans_ws_bytes(K, D), S(stream));
   if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "kmeans_update: memset: %s", cudaGetErrorString(e));
   const int64_t items = n * (D / 4);
-  kmeans_accumulate_kernel<<<(int)(cdiv(items, 256) < 148 * 16 ? cdiv(items, 256) : 148 * 16), 256, 0, S(stream)>>>(x, idx, n, D, sums, cnt);
+  kmeans_accumulate_kernel<<<(int)(cdiv(items, 256) < NUM_SMS * 16 ? cdiv(items, 256) : NUM_SMS * 16), 256, 0, S(stream)>>>(x, idx, n, D, sums, cnt);
   if (int er = launched("kmeans_accumulate")) return er;
   const int64_t tot = (int64_t)K * D;
-  kmeans_finalize_kernel<<<(int)(cdiv(tot, 256) < 148 * 8 ? cdiv(tot, 256) : 148 * 8), 256, 0, S(stream)>>>(sums, cnt, centres_old, centres_new,
+  kmeans_finalize_kernel<<<(int)(cdiv(tot, 256) < NUM_SMS * 8 ? cdiv(tot, 256) : NUM_SMS * 8), 256, 0, S(stream)>>>(sums, cnt, centres_old, centres_new,
                                                                                                        K, D, shift2);
   if (int er = launched("kmeans_finalize")) return er;
   if (shift_out) {
@@ -603,7 +603,7 @@ int mas_vq_backward(const float* g_zq, const float* g_loss, const float* z, cons
   (void)K;
   MAS_REQUIRE(R > 0 && D > 0 && D % 4 == 0, "vq_backward: bad shape");
   int64_t n = R * (D / 4);
-  int grid = (int)(cdiv(n, 256) < 148 * 16 ? cdiv(n, 256) : 148 * 16);
+  int grid = (int)(cdiv(n, 256) < NUM_SMS * 16 ? cdiv(n, 256) : NUM_SMS * 16);
   vq_backward_kernel<<<grid, 256, 0, S(stream)>>>(g_zq, g_loss, z, E, idx, R, D, beta, grad_z, grad_E);
   return launched("vq_backward");
 }
@@ -611,7 +611,7 @@ int mas_vq_backward(const float* g_zq, const float* g_loss, const float* z, cons
 int mas_vq_gather(const float* E, const int64_t* idx, int64_t R, int K, int D, float* out, void* stream) {
   MAS_REQUIRE(R > 0 && D > 0 && D % 4 == 0, "vq_gather: bad shape");
   int64_t n = R * (D / 4);
-  int grid = (int)(cdiv(n, 256) < 148 * 16 ? cdiv(n, 256) : 148 * 16);
+  int grid = (int)(cdiv(n, 256) < NUM_SMS * 16 ? cdiv(n, 256) : NUM_SMS * 16);
   vq_gather_kernel<<<grid, 256, 0, S(stream)>>>(E, idx, R, K, D, out);
   return launched("vq_gather");
 }

@@ -11,35 +11,37 @@
 // The indices are therefore those of the exact kernel, bit for bit, at tensor-core speed for ordinary data.
 //
 // Arithmetic: operand splitting into two fp16 numbers, x*s = h + l (h = fp16(x*s), l = fp16(x*s - h): 22 significant
-// bits; s a power of two from the tensor's largest magnitude), and three kind::f16 MMAs per K step,
+// bits; s a power of two from the tensor's largest magnitude), and three fp16 wgmma per K step,
 //   z.e ~= (zh.eh + zl.eh + zh.el) / (s_z s_e),   dropped term zl.el ~ 2^-22 relative,
-// accumulated in fp32 in tensor memory.
+// accumulated in fp32.
 //
 // Structure (one CTA = 128 latent rows x a contiguous range of 128-code tiles):
-//   * A (the 128 x D latent tile, both halves) is converted once and stays in TENSOR MEMORY for the whole sweep (lane = row,
-//     two fp16 per column: 2 x D/2 columns), which leaves shared memory to a 12-stage ring of code stages - the first version
-//     kept A in shared memory, had room for 2 stages and was bound by the latency of the bulk copies (ncu: 14 % tensor pipe);
+//   * A (the 128 x D latent tile, both halves) is converted once and stays in SHARED MEMORY for the whole sweep (K-major
+//     no-swizzle planes [hi|lo][d/8][row][8 halves], 130 KB for D = 256), the rest of shared memory is a 5-stage ring of
+//     code stages;
 //   * B (codes): split ONCE per launch by vq_pack_codes into the exact shared-memory image of a pipeline stage
-//     ([tile][32-dim chunk][hi|lo][k/8][code][8 halves], K-major no-swizzle UMMA layout), so one thread feeds the ring with
+//     ([tile][32-dim chunk][hi|lo][k/8][code][8 halves], K-major no-swizzle layout), so one thread feeds the ring with
 //     a single cp.async.bulk (16.6 KB, mbarrier complete_tx) per stage;
-//   * one thread issues the MMAs (A from tensor memory, M 128, N 128, K 16; 3 per K step) into one of TWO 128-column accumulators;
-//   * 4 epilogue warps (thread = latent row) drain the other accumulator meanwhile: tcgen05.ld, d~ = |e|^2 - 2 dot, sorted
-//     insertion into the row's five smallest values (four of them with their code index).
+//   * two warpgroups issue the wgmma.m64n128k16 of latent rows 64 g .. 64 g + 63 (3 per K step) and keep, per fragment row,
+//     the five smallest values (four of them with their code index) in a sorted insertion list; the four lanes that share
+//     a row merge their lists at the end.
 #include <cuda_fp16.h>
 
 #include "mas_common.cuh"
+#include "wgmma.cuh"
 
 namespace mas {
 namespace vqtc {
 
-constexpr int BM = 128, BN = 128, KC = 32, STAGES = 12;
-constexpr int NEPI = 128, NTHREADS = NEPI + 64;   // warps 0-3: A staging then epilogue; warp 4: code-stage feeder; warp 5: MMA issuer
+constexpr int BM = 128, BN = 128, KC = 32, STAGES = 5;
+constexpr int NMMA = 256, NTHREADS = NMMA + 128;   // warps 0-7: A staging, MMA and candidate lists; warp 8: code-stage feeder
 constexpr int PITCH_B = BN * 16 + 32;   // bytes between 8-dimension planes of a B stage half
 constexpr int B_HALF = (KC / 8) * PITCH_B;
 constexpr int B_STAGE = 2 * B_HALF;     // hi planes then lo planes (16.6 KB)
 constexpr int NCAND = 4;                // candidates kept with their index (+ one more value)
 constexpr int REC = 12;                 // floats per (row, split) record: b[5], i[4] (as int bits), pad
-constexpr int A_COLS = 256;             // tensor-memory columns of the latent tile: D/2 for each half (D <= 256)
+constexpr int D_MAX = 256;              // latent dimensions the shared-memory A tile holds
+constexpr int PITCH_A = BM * 16 + 32;   // bytes between 8-dimension planes of the A tile
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
@@ -70,75 +72,6 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
 }
 __device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void mma_f16_ss(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void mma_f16_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(d_tmem), "r"(a_tmem), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,"
-      "%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// one lane of the (converged) warp: true for exactly one thread.  The MMA-issuing warps run their loops warp-uniformly (operand
-// descriptors stay in uniform registers) and only the issue itself is predicated on this.
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
-}
-__device__ __forceinline__ void mma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,"
-      "%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]),
-        "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]),
-        "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-// shared-memory matrix descriptor, K-major, no swizzle, sm_100 version field = 1 (as in contract_tc.cu)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  return (uint64_t)((saddr >> 4) & 0x3FFF) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16) | ((uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32) |
-         (1ull << 46);
-}
-// instruction descriptor: D = f32, A = B = f16, both K-major, M = 128, N = 256
-constexpr uint32_t IDESC = (1u << 4) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(BM >> 4) << 24);
 
 // power-of-two scale putting the tensor's largest magnitude into [2^14, 2^15) (fp16 tops out at 65504); *inv = 1/s, exact
 __device__ __forceinline__ float split_scale(const float* amax, float* inv) {
@@ -164,6 +97,25 @@ __device__ __forceinline__ void split2(float a, float b, float s, uint32_t* hi, 
   *lo = *reinterpret_cast<const uint32_t*>(&l);
 }
 
+// sorted insertion (ascending by value, then by code) into a five-entry list
+__device__ __forceinline__ void cand_insert(float* b, int* ci, float d, int code) {
+  auto lt = [&](int k) { return d < b[k] || (d == b[k] && code < ci[k]); };
+  if (d == INFINITY || !lt(4)) return;   // +inf: a code beyond K (or an empty slot of another list) is never a candidate
+  if (lt(3)) {
+    b[4] = b[3]; ci[4] = ci[3];
+    if (lt(2)) {
+      b[3] = b[2]; ci[3] = ci[2];
+      if (lt(1)) {
+        b[2] = b[1]; ci[2] = ci[1];
+        if (lt(0)) { b[1] = b[0]; ci[1] = ci[0]; b[0] = d; ci[0] = code; }
+        else { b[1] = d; ci[1] = code; }
+      } else { b[2] = d; ci[2] = code; }
+    } else { b[3] = d; ci[3] = code; }
+  } else {
+    b[4] = d; ci[4] = code;
+  }
+}
+
 struct Params {
   const float* z;      // [R, D]
   const uint8_t* Epk;  // packed split codes: [ntile][D/32][B_STAGE bytes] (vq_pack_codes)
@@ -177,129 +129,137 @@ struct Params {
 
 __global__ void __launch_bounds__(NTHREADS, 1) vq_filter_tc(const Params p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* b_smem = smem;
-  float* ee_s = reinterpret_cast<float*>(b_smem + (size_t)STAGES * B_STAGE);     // [2][BN]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ee_s + 2 * BN);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 2 * STAGES + 4);
-  const uint32_t smem_base = smem_u32(smem), bar_base = smem_u32(bars);
+  const int a_half = (p.D / 8) * PITCH_A;
+  uint8_t* a_smem = smem;                                  // [hi|lo][d/8][row][8 halves]
+  uint8_t* b_smem = smem + 2 * a_half;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(b_smem + (size_t)STAGES * B_STAGE);
+  const uint32_t a_base = smem_u32(a_smem), b_base = smem_u32(b_smem), bar_base = smem_u32(bars);
   auto full_bar = [&](int s) { return bar_base + 8u * s; };
   auto empty_bar = [&](int s) { return bar_base + 8u * (STAGES + s); };
-  auto accf_bar = [&](int b) { return bar_base + 8u * (2 * STAGES + b); };
-  auto acce_bar = [&](int b) { return bar_base + 8u * (2 * STAGES + 2 + b); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int64_t row0 = (int64_t)blockIdx.x * BM;
   const int ntile_all = (p.K + BN - 1) / BN;
   const int tile_lo = blockIdx.y * p.tiles_per_split, tile_hi = min(ntile_all, tile_lo + p.tiles_per_split);
   const int nchunk = p.D / KC;
-  const int half_cols = p.D >> 1;                    // tensor-memory columns of one half of A (two fp16 per column)
 
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full_bar(s), 1);
-      mbar_init(empty_bar(s), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(accf_bar(b), 1);
-      mbar_init(acce_bar(b), NEPI);
+      mbar_init(empty_bar(s), NMMA);
     }
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc(smem_u32(tmem_slot), 512);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
   float inv_z, inv_e;
   const float s_z = split_scale(p.z_amax, &inv_z);
   split_scale(p.e_amax, &inv_e);
 
-  // ---- A: thread = latent row (TMEM lane); 64 dimensions at a time -> 32 packed hi words + 32 packed lo words ----
-  if (warp < 4) {
-    const int64_t row = row0 + warp * 32 + lane;
+  // ---- A: thread = (latent row, half of the dimensions); 8 dimensions at a time -> one 16-byte hi and one lo store ----
+  if (warp < 8) {
+    const int r = tid & (BM - 1);
+    const int64_t row = row0 + r;
     const float4* src = reinterpret_cast<const float4*>(p.z + (size_t)(row < p.R ? row : 0) * p.D);
-    for (int d0 = 0; d0 < p.D; d0 += 64) {
-      uint32_t hi[32], lo[32];
-#pragma unroll
-      for (int q = 0; q < 16; ++q) {
-        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (row < p.R) v = __ldg(src + (d0 >> 2) + q);
-        split2(v.x, v.y, s_z, &hi[2 * q], &lo[2 * q]);
-        split2(v.z, v.w, s_z, &hi[2 * q + 1], &lo[2 * q + 1]);
-      }
-      const uint32_t ta = tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(d0 >> 1);
-      tmem_st32(ta, hi);
-      tmem_st32(ta + (uint32_t)half_cols, lo);
+    const int octs = p.D / 8;
+    for (int oc = (tid >> 7) * (octs / 2); oc < ((tid >> 7) + 1) * (octs / 2); ++oc) {
+      float4 v0 = make_float4(0.f, 0.f, 0.f, 0.f), v1 = v0;
+      if (row < p.R) { v0 = __ldg(src + 2 * oc); v1 = __ldg(src + 2 * oc + 1); }
+      uint4 h, l;
+      split2(v0.x, v0.y, s_z, &h.x, &l.x);
+      split2(v0.z, v0.w, s_z, &h.y, &l.y);
+      split2(v1.x, v1.y, s_z, &h.z, &l.z);
+      split2(v1.z, v1.w, s_z, &h.w, &l.w);
+      uint8_t* dst = a_smem + (size_t)oc * PITCH_A + r * 16;
+      *reinterpret_cast<uint4*>(dst) = h;
+      *reinterpret_cast<uint4*>(dst + a_half) = l;
     }
-    tmem_st_wait();
+    fence_proxy_async();
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
 
-  if (warp < 4) {
-    // ===================== epilogue: running five smallest approximate distances per row =====================
-    float b[NCAND + 1];
-    int ci[NCAND];
+  if (warp < 8) {
+    // ===================== MMA warpgroups: running five smallest approximate distances per fragment row =====================
+    wg::regs_inc<wg::MMA_REGS>();
+    const int wgi = warp >> 2, fk = lane & 3;
+    float b[2][NCAND + 1];
+    int ci[2][NCAND + 1];
 #pragma unroll
-    for (int j = 0; j <= NCAND; ++j) b[j] = INFINITY;
+    for (int i = 0; i < 2; ++i)
 #pragma unroll
-    for (int j = 0; j < NCAND; ++j) ci[j] = 0;
+      for (int j = 0; j <= NCAND; ++j) { b[i][j] = INFINITY; ci[i][j] = 0; }
     const float m2 = -2.0f * inv_z * inv_e;          // dot (scaled) -> -2 z.e
-    int buf = 0;
-    uint32_t ph[2] = {0u, 0u};
+    int stage = 0, prev = 0;
+    uint32_t phase = 0;
+    float acc[BN / 2];
+    const uint32_t a_rows = a_base + (uint32_t)(wgi * 64 * 16);
     for (int t = tile_lo; t < tile_hi; ++t) {
-      float* es = ee_s + buf * BN;
-      {
-        const int code = t * BN + tid;
-        es[tid] = code < p.K ? __ldg(p.ee + code) : INFINITY;
-      }
-      asm volatile("bar.sync 1, 128;" ::: "memory");
-      mbar_wait(accf_bar(buf), ph[buf]);
-      ph[buf] ^= 1u;
-      tc_fence_after();
-#pragma unroll 1
-      for (int cb = 0; cb < BN / 32; ++cb) {
-        float v[32];
-        tmem_ld32(tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(A_COLS + buf * BN + cb * 32), v);
+      for (int c = 0; c < nchunk; ++c) {
+        mbar_wait(full_bar(stage), phase);
+        const uint32_t bst = b_base + (uint32_t)stage * B_STAGE;
+        wg::fence();
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float d = fmaf(v[j], m2, es[cb * 32 + j]);     // INFINITY for codes beyond K: never inserted
-          if (d < b[NCAND]) {
-            const int code = t * BN + cb * 32 + j;
-            // sorted insertion (ascending); equal values keep the earlier code first
-            if (d < b[3]) {
-              b[4] = b[3];
-              if (d < b[2]) {
-                b[3] = b[2]; ci[3] = ci[2];
-                if (d < b[1]) {
-                  b[2] = b[1]; ci[2] = ci[1];
-                  if (d < b[0]) { b[1] = b[0]; ci[1] = ci[0]; b[0] = d; ci[0] = code; }
-                  else { b[1] = d; ci[1] = code; }
-                } else { b[2] = d; ci[2] = code; }
-              } else { b[3] = d; ci[3] = code; }
-            } else {
-              b[4] = d;
-            }
-          }
+        for (int k16 = 0; k16 < KC / 16; ++k16) {
+          const uint32_t aoff = (uint32_t)((c * KC / 8 + k16 * 2) * PITCH_A);
+          const uint64_t ah = wg::desc(a_rows + aoff, PITCH_A, 128), al = wg::desc(a_rows + (uint32_t)a_half + aoff, PITCH_A, 128);
+          const uint64_t bh = wg::desc(bst + (uint32_t)(k16 * 2 * PITCH_B), PITCH_B, 128);
+          const uint64_t bl = wg::desc(bst + (uint32_t)(B_HALF + k16 * 2 * PITCH_B), PITCH_B, 128);
+          wg::wgmma_f16_ss_n128<0, 0>(acc, ah, bh, (c > 0 || k16 > 0) ? 1u : 0u);   // zh . eh
+          wg::wgmma_f16_ss_n128<0, 0>(acc, al, bh, 1u);                           // zl . eh
+          wg::wgmma_f16_ss_n128<0, 0>(acc, ah, bl, 1u);                           // zh . el
+        }
+        wg::commit();
+        wg::wait<1>();
+        if (t > tile_lo || c > 0) mbar_arrive(empty_bar(prev));
+        prev = stage;
+        if (++stage == STAGES) { stage = 0; phase ^= 1; }
+      }
+      wg::wait<0>();
+      wg::fence_regs<BN / 2>(acc);
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+        for (int cc = 0; cc < 2; ++cc) {
+          const int code = t * BN + 8 * j + 2 * fk + cc;
+          const float e2 = code < p.K ? __ldg(p.ee + code) : INFINITY;     // INFINITY for codes beyond K: never inserted
+#pragma unroll
+          for (int i = 0; i < 2; ++i) cand_insert(b[i], ci[i], fmaf(acc[4 * j + 2 * i + cc], m2, e2), code);
         }
       }
-      tc_fence_before();
-      mbar_arrive(acce_bar(buf));
-      buf ^= 1;
     }
-    const int64_t row = row0 + warp * 32 + lane;
-    if (row < p.R) {
-      float* o = p.cand + ((size_t)row * gridDim.y + blockIdx.y) * REC;
+    if (tile_hi > tile_lo) mbar_arrive(empty_bar(prev));
+    // the four lanes of a fragment row hold disjoint code subsets: merge their lists
 #pragma unroll
-      for (int j = 0; j <= NCAND; ++j) o[j] = b[j];
+    for (int x = 1; x <= 2; x <<= 1) {
 #pragma unroll
-      for (int j = 0; j < NCAND; ++j) o[5 + j] = __int_as_float(ci[j]);
+      for (int i = 0; i < 2; ++i) {
+        float ob[NCAND + 1];
+        int oc[NCAND + 1];
+#pragma unroll
+        for (int j = 0; j <= NCAND; ++j) {
+          ob[j] = __shfl_xor_sync(0xffffffffu, b[i][j], x);
+          oc[j] = __shfl_xor_sync(0xffffffffu, ci[i][j], x);
+        }
+#pragma unroll
+        for (int j = 0; j <= NCAND; ++j) cand_insert(b[i], ci[i], ob[j], oc[j]);
+      }
     }
-  } else if (warp == 4) {
+    if (fk == 0) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int64_t row = row0 + wgi * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+        if (row < p.R) {
+          float* o = p.cand + ((size_t)row * gridDim.y + blockIdx.y) * REC;
+#pragma unroll
+          for (int j = 0; j <= NCAND; ++j) o[j] = b[i][j];
+#pragma unroll
+          for (int j = 0; j < NCAND; ++j) o[5 + j] = __int_as_float(ci[i][j]);
+        }
+      }
+    }
+  } else {
     // ===================== code-stage feeder (one thread): one bulk copy per stage =====================
-    if (lane == 0) {
+    wg::regs_dec<wg::COPY_REGS>();
+    if (warp == 8 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
       const int nsteps = (tile_hi - tile_lo) * nchunk;
@@ -307,57 +267,15 @@ __global__ void __launch_bounds__(NTHREADS, 1) vq_filter_tc(const Params p) {
       for (int step = 0; step < nsteps; ++step) {
         mbar_wait(empty_bar(stage), phase ^ 1);
         mbar_expect_tx(full_bar(stage), B_STAGE);
-        bulk_g2s(smem_base + (uint32_t)stage * B_STAGE, src + (size_t)step * B_STAGE, B_STAGE, full_bar(stage));
+        bulk_g2s(b_base + (uint32_t)stage * B_STAGE, src + (size_t)step * B_STAGE, B_STAGE, full_bar(stage));
         if (++stage == STAGES) { stage = 0; phase ^= 1; }
       }
     }
     __syncwarp();
-  } else {
-    // ===================== MMA issuer (warp-uniform loop, one elected lane issues) =====================
-    {
-      int stage = 0, buf = 0;
-      uint32_t phase = 0, eph[2] = {0u, 0u};
-      for (int t = tile_lo; t < tile_hi; ++t) {
-        mbar_wait(acce_bar(buf), eph[buf] ^ 1);       // the epilogue has drained this accumulator (first use: passes)
-        eph[buf] ^= 1u;
-        tc_fence_after();
-        const uint32_t acc = tmem_base + (uint32_t)(A_COLS + buf * BN);
-        for (int c = 0; c < nchunk; ++c) {
-          mbar_wait(full_bar(stage), phase);
-          tc_fence_after();
-          const uint32_t bst = smem_base + (uint32_t)stage * B_STAGE;
-          if (elect_one()) {
-#pragma unroll
-            for (int k16 = 0; k16 < KC / 16; ++k16) {
-              const uint32_t acol = (uint32_t)((c * KC + k16 * 16) >> 1);          // 16 dimensions = 8 columns
-              const uint64_t bh = make_desc(bst + (uint32_t)(k16 * 2 * PITCH_B), PITCH_B, 128);
-              const uint64_t bl = make_desc(bst + (uint32_t)(B_HALF + k16 * 2 * PITCH_B), PITCH_B, 128);
-              mma_f16_ts(acc, tmem_base + acol, bh, IDESC, (c > 0 || k16 > 0) ? 1u : 0u);                    // zh . eh
-              mma_f16_ts(acc, tmem_base + (uint32_t)half_cols + acol, bh, IDESC, 1u);                     // zl . eh
-              mma_f16_ts(acc, tmem_base + acol, bl, IDESC, 1u);                                          // zh . el
-            }
-            mma_commit(empty_bar(stage));
-            if (c == nchunk - 1) mma_commit(accf_bar(buf));
-          }
-          __syncwarp();
-          if (++stage == STAGES) { stage = 0; phase ^= 1; }
-        }
-        buf ^= 1;
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
-size_t filter_smem_bytes(int D) {
-  (void)D;
-  return (size_t)STAGES * B_STAGE + 2 * BN * sizeof(float) + (2 * STAGES + 4) * 8 + 16;
-}
+size_t filter_smem_bytes(int D) { return (size_t)2 * (D / 8) * PITCH_A + (size_t)STAGES * B_STAGE + 2 * STAGES * 8; }
 
 }  // namespace vqtc
 
@@ -390,12 +308,12 @@ __global__ void vq_pack_codes(const float* __restrict__ E, const float* __restri
 
 // Host side: eligibility and launch (called from mas_vq_forward in vq.cu).
 bool vq_filter_tc_ok(int64_t R, int K, int D) {
-  return D % 64 == 0 && D >= 64 && D <= 2 * vqtc::A_COLS && K >= 8 && R > 0;   // latent tile: two fp16 halves in 256 TMEM columns
+  return D % 64 == 0 && D >= 64 && D <= vqtc::D_MAX && K >= 8 && R > 0;   // latent tile: two fp16 halves in shared memory
 }
 int vq_filter_splits(int64_t R, int K) {
   const int64_t row_blocks = cdiv(R, vqtc::BM);
   const int ntile = (int)cdiv(K, vqtc::BN);
-  int s = (int)(148 / row_blocks);
+  int s = (int)(132 / row_blocks);
   if (s < 1) s = 1;
   if (s > ntile) s = ntile;
   if (s > 4) s = 4;

@@ -143,7 +143,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(
             f"libmas_b200.so not found at {LIB_PATH}: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). There is no CPU/PyTorch fallback for this path.")
+            "(nvcc, sm_90a). There is no CPU/PyTorch fallback for this path.")
     lib = ctypes.CDLL(LIB_PATH)
     for name, (res, args) in _SPEC.items():
         fn = getattr(lib, name)  # AttributeError here = header/library drift, which must be loud
@@ -231,7 +231,7 @@ def launch_count() -> int:
 
 
 def tc_launch_count() -> int:
-    """Launches of kernels that issue tcgen05 MMAs (subset of launch_count)."""
+    """Launches of kernels that issue tensor-core (wgmma) MMAs (subset of launch_count)."""
     return int(load().mas_tc_launch_count())
 
 

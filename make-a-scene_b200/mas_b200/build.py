@@ -1,4 +1,4 @@
-"""Builds libmas_b200.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo snapshot)."""
+"""Builds libmas_b200.so in-tree with nvcc for sm_90a (H100). No JIT cache: the library lives next to the package."""
 import os
 import subprocess
 import sys
@@ -11,7 +11,7 @@ CSRC = os.path.join(PKG, "csrc")
 OBJ = os.path.join(PKG, "build")
 LIB = os.path.join(PKG, "lib", "libmas_b200.so")
 SOURCES = ["norm.cu", "vq.cu", "vq_tc.cu", "contract_simt.cu", "contract_tc.cu", "conv_tma.cu", "gemm_tma.cu", "contract_tc3.cu", "edge.cu", "edge_quad.cu", "transformer.cu", "decode.cu", "attn.cu", "attn_fused.cu", "attn_causal.cu", "probe.cu", "capi.cu"]
-NVCC_FLAGS = ["-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
               "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 
 

@@ -51,7 +51,7 @@ def get_impl() -> int:
 
 def _need_cuda(x):
     if not x.is_cuda:
-        raise RuntimeError("make-a-scene_b200 kernels run on CUDA (sm_100a) only; got a %s tensor — there is no CPU path"
+        raise RuntimeError("make-a-scene_b200 kernels run on CUDA (sm_90a) only; got a %s tensor — there is no CPU path"
                            % x.device.type)
     if x.dtype != torch.float32:
         raise RuntimeError("make-a-scene_b200 kernels take float32 tensors, got %s" % x.dtype)
@@ -164,7 +164,7 @@ def _tc_on():
 
 
 def conv_tc_eligible(x, cout, mode):
-    """True when conv3x3 of dense-NHWC x with `cout` output channels runs on the tcgen05 kernel."""
+    """True when conv3x3 of dense-NHWC x with `cout` output channels runs on the tensor-core kernel."""
     if not _tc_on() or not _is_dense_nhwc(x):
         return False
     n, _, h, w = x.shape
@@ -191,7 +191,7 @@ def conv3x3_raw(x, weight, bias, residual, mode, out_nchw=False, transpose=False
                 prepack=False, x_amax=None):
     """y = conv3x3(x; weight) (+bias, +residual). transpose=True applies the data-gradient operand
     (taps flipped, Cin<->Cout). Dense NHWC shapes with Cin%8==0, Cout%128==0, Hout%16==0, Wout%8==0 run on the
-    tcgen05 kernel; everything else (edge layers, NCHW views, small images) on the fp32 SIMT kernel.
+    tensor-core kernel; everything else (edge layers, NCHW views, small images) on the fp32 SIMT kernel.
     table: fused GroupNorm(+SiLU) prologue (tensor path only); want_stats: also return the output's GroupNorm
     (mean, rstd) from the fused epilogue (None when the tensor path does not apply)."""
     n, _, h, w = x.shape
@@ -225,7 +225,7 @@ def conv3x3_raw(x, weight, bias, residual, mode, out_nchw=False, transpose=False
         if table is not None:
             raise RuntimeError("fused GroupNorm prologue requested for a shape that is not tensor-path eligible")
         if _cfg["impl"] == L.IMPL_TC:
-            raise RuntimeError("IMPL_TC requested but the conv shape is not eligible for the tcgen05 kernel")
+            raise RuntimeError("IMPL_TC requested but the conv shape is not eligible for the tensor-core kernel")
         wp = torch.empty(9 * cout * cin, dtype=torch.float32, device=x.device)
         L.call("mas_pack_conv3x3", wc, wp, weight.shape[0], weight.shape[1], int(transpose), 0)
         L.call("mas_conv3x3_fprop", x, xs, wp, bias, residual, y, ys, mode, L.IMPL_SIMT)
@@ -261,7 +261,7 @@ def gn_apply_f16(x, mean, rstd, gamma, beta, silu):
 
 
 def conv3x3_h_raw(x16, weight, bias, residual, transpose=False, want_stats=False, prepack=False, x_amax=None):
-    """Stride-1 conv3x3 of an fp16 channels-last shadow on the TMA-fed tcgen05 kernel (fp32 output, same epilogues as
+    """Stride-1 conv3x3 of an fp16 channels-last shadow on the TMA-fed tensor-core kernel (fp32 output, same epilogues as
     conv3x3_raw). x_amax: the device scalar the shadow was scaled with (None: unscaled)."""
     n, _, h, w = x16.shape
     cout = weight.shape[1] if transpose else weight.shape[0]
@@ -505,7 +505,7 @@ def _is_dense_nhwc(t):
 class Conv3x3Fn(torch.autograd.Function):
     """nn.Conv2d 3x3 / Downsample / Upsample (modules.py:44-81,93-104) with optional fused residual add.
     3-channel edge layers (conv_in reading the NCHW image, conv_out writing the NCHW reconstruction) use the
-    direct fp32 edge kernels; everything else goes through conv3x3_raw (tcgen05 or SIMT)."""
+    direct fp32 edge kernels; everything else goes through conv3x3_raw (wgmma or SIMT)."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, residual, mode, out_nchw):
@@ -1227,7 +1227,7 @@ def gemm2(A, B, C, M, N, K, outer, batch, lda, ldb, ldc, osa, osb, osc, sa, sb, 
 
 
 def attn_causal_fused_on(S_, hd):
-    """The fused tcgen05 forward core (csrc/attn_causal.cu): head dim 64, S % 128 == 0, tensor path enabled.
+    """The fused wgmma forward core (csrc/attn_causal.cu): head dim 64, S % 128 == 0, tensor path enabled.
     MAS_ATTN_FUSED=0 selects the GEMM / softmax / GEMM sequence instead."""
     return _tc_on() and hd == 64 and S_ % 128 == 0 and S_ >= 128 and os.environ.get("MAS_ATTN_FUSED", "1") != "0"
 

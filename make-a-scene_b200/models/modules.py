@@ -1,4 +1,4 @@
-"""Drop-in for reference models/modules.py (Encoder/Decoder/ResnetBlock/AttnBlock/Codebook ...) on sm_100a kernels.
+"""Drop-in for reference models/modules.py (Encoder/Decoder/ResnetBlock/AttnBlock/Codebook ...) on sm_90a kernels.
 
 Every class keeps the reference's name, constructor signature, attribute names and parameter shapes
 (modules.py:35-240,337-369,451-528); forward passes run exclusively through libmas_b200.so

@@ -1,4 +1,4 @@
-"""Drop-in for reference models/transformer.py (MakeAScene token transformer, tier 2) on the sm_100a kernels.
+"""Drop-in for reference models/transformer.py (MakeAScene token transformer, tier 2) on the sm_90a kernels.
 
 Same class names, constructor signatures, attribute names and state_dict keys (including the `transformer.mask`
 buffer). Supported configuration = the reference's defaults: cogview_pb_relax=True (a softmax-invariant shift),

@@ -1,4 +1,4 @@
-"""VQBASE — drop-in for reference models/vqvae.py:8-39 over the sm_100a kernels in libmas_b200.so.
+"""VQBASE — drop-in for reference models/vqvae.py:8-39 over the sm_90a kernels in libmas_b200.so.
 
 Same constructor/forward signatures and state_dict keys (348 entries for conf/img_config.yaml); parameters are
 held by stock torch.nn holders created in the reference's order, so `torch.manual_seed(s)` gives identical

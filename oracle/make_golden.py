@@ -5,6 +5,8 @@ Run in the authoring container only (the GPU box has no /root/reference):
 Writes small ``.pt`` fixtures to tests/golden/. The oracle (oracle/vqgan_oracle.py) and the CUDA
 product are both checked against these files. TEST INFRASTRUCTURE — never imported by the product.
 """
+import hashlib
+import json
 import os
 import sys
 import types
@@ -58,6 +60,8 @@ def main():
         tensor_path_block_fixtures(M)
     if only is None or "img256" in only:
         img256_fixture(ref_models)
+    if only is None or "schedule" in only:
+        codebook_schedule_fixture(M)
 
 
 def base_fixtures(ref_models, M, V, L, T):
@@ -232,7 +236,7 @@ def base_fixtures(ref_models, M, V, L, T):
 
 
 def tensor_path_block_fixtures(M):
-    """G7: blocks at widths / extents that the tcgen05 kernels take (Cout % 128 == 0, H % 16 == 0, W % 8 == 0), run on the
+    """G7: blocks at widths / extents that the tensor-core kernels take (Cout % 128 == 0, H % 16 == 0, W % 8 == 0), run on the
     REAL reference modules. Weights and inputs are regenerated from seeds on both sides (oracle/seeded.py)."""
     import torch.nn as nn
     sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
@@ -308,6 +312,37 @@ def img256_fixture(ref_models):
                     grad_norms={k: float(p.grad.double().norm()) for k, p in named.items()}, grad_samples=grad_samples),
                os.path.join(OUT, "vqbase_img_256.pt"))
     print("img 256 done: loss", float(loss))
+
+
+def tensor_digest(t):
+    """Shape, dtype and SHA-256 of the bytes: equal digests <=> torch.equal."""
+    t = t.detach().contiguous().cpu()
+    return "%s %s %s" % (tuple(t.shape), t.dtype, hashlib.sha256(t.numpy().tobytes()).hexdigest())
+
+
+def codebook_schedule_fixture(M):
+    """G8: digests of the reference Codebook's initial weights and of its output and reservoir after each of steps 1 .. 11
+    under fixed seeds (modules.py:474-499: step counter, reservoir sampling, warm-up bypass)."""
+    K, D, init_steps = 16, 8, 4
+    torch.manual_seed(3)
+    first = M.Codebook(K, D, 0.25, init_steps, 60)     # the drop-in is constructed first in the test (same init order)
+    ref = M.Codebook(K, D, 0.25, init_steps, 60)
+    ref.load_state_dict(first.state_dict())
+    ref.train()
+    gz = torch.Generator().manual_seed(11)
+    zs = [torch.randn(3, D, 4, 4, generator=gz) for _ in range(16)]
+    outs, res, cnt = [], [], []
+    for step, z in enumerate(zs[:11], start=1):
+        torch.manual_seed(100 + step)
+        zq, loss, idx = ref(z)
+        assert idx is None and float(loss) == 0.0
+        outs.append(tensor_digest(zq))
+        res.append(None if ref.reservoir is None else tensor_digest(ref.reservoir))
+        cnt.append(int(ref.q_counter))
+    with open(os.path.join(OUT, "codebook_schedule.json"), "w") as f:
+        json.dump(dict(init={k: tensor_digest(v) for k, v in first.state_dict().items()}, out=outs, reservoir=res,
+                       q_counter=cnt), f, indent=0)
+        f.write("\n")
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""csrc/contract_tc3.cu: fp32-accurate 3xTF32 operand-split batched GEMM on tcgen05 (mas_gemm(impl=MAS_IMPL_TC3); the
+"""csrc/contract_tc3.cu: fp32-accurate 3xTF32 operand-split batched GEMM on wgmma (mas_gemm(impl=MAS_IMPL_TC3); the
 AttnBlock's QK^T / PV and their four gradients run on it) against fp64."""
 import os
 

@@ -1,4 +1,4 @@
-"""GPU parity tests (run on the B200 box): every call goes through the C-ABI (ctypes -> libmas_b200.so) and is
+"""GPU parity tests (run on an H100): every call goes through the C-ABI (ctypes -> libmas_b200.so) and is
 compared with (a) fixtures generated from the REAL reference and (b) the CPU oracle on seeded inputs.
 
 Tolerances: VQ indices bit-exact (or fp64-tie-explained on the tie-heavy sets); floating point within 1e-3
@@ -391,7 +391,7 @@ TC_BLOCKS = ["res_128_128", "res_128_256", "res_512_512", "attn_512", "attn_res_
 
 @pytest.mark.parametrize("name", TC_BLOCKS)
 def test_tensor_path_blocks_vs_reference(name):
-    """Blocks at widths / extents the tcgen05 kernels take (fused GroupNorm prologue, statistics epilogue and its
+    """Blocks at widths / extents the tensor-core kernels take (fused GroupNorm prologue, statistics epilogue and its
     take_stats hand-off between modules, AttnBlock at C=512 / HW=256, Up/Downsample on the tensor kernels) against
     outputs and gradients of the REAL reference (tests/golden/blocks_tc.pt; weights / inputs regenerated from seeds)."""
     from mas_b200 import _lib as L
@@ -669,7 +669,7 @@ def test_conv1x1_vs_oracle(cin, cout, hw, n, impl):
 
 
 def test_tensor_path_full_resolution_linearity():
-    """BASELINE-size conv (128->128 @256x256, batch 4 here) on the tcgen05 kernel: compared with the exact-fp32 SIMT
+    """BASELINE-size conv (128->128 @256x256, batch 4 here) on the tensor-core kernel: compared with the exact-fp32 SIMT
     kernel on the same inputs, plus linearity conv(a*x1 + x2) = a*conv(x1) + conv(x2) (bias-free)."""
     from mas_b200 import _lib as L, ops
     dev = _dev()
@@ -737,7 +737,7 @@ def test_seg_loss_vs_reference():
 @pytest.mark.parametrize("cin,cout,h,w", [(159, 128, 32, 32), (128, 159, 32, 64), (100, 256, 16, 16), (64, 200, 16, 24)])
 def test_conv3x3_padded_channel_counts_vs_oracle(cin, cout, h, w):
     """Channel counts off the tensor tiles (VQ-SEG's 159-channel input / output layers): zero-padded to the 16-wide K step /
-    the 128-wide output tile inside Conv3x3Fn, run on the fp16 tcgen05 kernels; the 159-wide output comes back as a
+    the 128-wide output tile inside Conv3x3Fn, run on the fp16 tensor-core kernels; the 159-wide output comes back as a
     channels-last view. Forward and all gradients against F.conv2d (fp32, CPU)."""
     import torch.nn.functional as F
     from mas_b200 import _lib as L, ops

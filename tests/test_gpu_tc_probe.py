@@ -1,4 +1,6 @@
-"""GPU: pins the tcgen05 operand conventions (shared-memory descriptor majorness, A-from-TMEM) with a one-MMA probe."""
+"""GPU: pins the wgmma operand conventions (shared-memory descriptor majorness, A from registers) with a one-MMA probe.
+Descriptors are built in the sm_100 encoding: the probe drops its version bits; the swizzle codes 2 / 4 / 6 at bit 61 are the
+sm_90 128 / 64 / 32-byte codes at bit 62, and bit 16 of the instruction descriptor selects an MN-major (transposed) B."""
 import pytest
 import torch
 
@@ -18,10 +20,10 @@ def test_single_mma_conventions(a_src, b_layout):
     err = float((D.double() - ref).norm() / ref.norm())
     print(f"probe a_src={a_src} b_layout={b_layout}: rel err {err:.3e} D[0,:4]={D[0,:4].tolist()} ref={ref[0,:4].tolist()}")
     if b_layout == 0:
-        assert err < 2e-3, (a_src, b_layout, err)   # K-major B; A from smem (SS) and from tensor memory (TS) both work
+        assert err < 2e-3, (a_src, b_layout, err)   # K-major B; A from smem (SS) and from registers (RS) both work
     else:
-        # MN-major TF32 shared-memory operands return zeros on this part (any LBO/SBO order, any swizzle): the
-        # production kernels therefore keep every smem operand K-major (see wgrad_tc's transposed halo copies)
+        # wgmma transposes 16-bit operands only: an MN-major TF32 image is read as K-major and the product is wrong, so the
+        # production kernels keep every TF32 smem operand K-major (see wgrad_tc's transposed halo copies)
         assert err > 0.5
 
 
@@ -102,7 +104,7 @@ RAW16 = [  # name, lbo, sbo, layout_type, b_mn, start_off
 
 @pytest.mark.parametrize("case", RAW16, ids=[c[0] for c in RAW16])
 def test_reveal_raw_f16(case):
-    """kind::f16 shared-memory operand addressing under MN-major / K-major descriptors (prints the half index read for each
+    """fp16 wgmma shared-memory operand addressing under MN-major / K-major descriptors (prints the half index read for each
     (n, k)); the K-major control must reproduce the layout the production kernels rely on: index = (k/8)*LBO/2 + n*8 + k%8."""
     from mas_b200 import _lib as L
     name, lbo, sbo, lt, b_mn, off = case

@@ -187,7 +187,7 @@ def test_layernorm_pair_vs_torch(R, H, res):
 
 def test_causal_attention_on_tensor_cores_matches_fp32_kernels(monkeypatch):
     """transformer.py:77-103 at the paper's extents (640 tokens, 16 heads of 64): QK^T / PV and their four gradients on the
-    3xTF32 tcgen05 GEMM against the exact-fp32 FFMA kernels (which the reference fixtures pin at small extents)."""
+    3xTF32 wgmma GEMM against the exact-fp32 FFMA kernels (which the reference fixtures pin at small extents)."""
     from mas_b200 import _lib as L, ops
     dev = torch.device("cuda:0")
     g = torch.Generator().manual_seed(3)
@@ -285,7 +285,7 @@ def test_sample_topk_kernel():
 
 @pytest.mark.parametrize("B,S,heads", [(1, 128, 1), (2, 640, 16), (3, 256, 2)])
 def test_fused_causal_attention_core_matches_fp32_kernels(B, S, heads, monkeypatch):
-    """csrc/attn_causal.cu (scores -> causal softmax -> P v in one tcgen05 kernel, 2 x fp16 operand split) against the
+    """csrc/attn_causal.cu (scores -> causal softmax -> P v in one tensor-core kernel, 2 x fp16 operand split) against the
     exact-fp32 FFMA sequence: ctx, the saved probabilities (incl. the zeros above the diagonal) and the gradients."""
     from mas_b200 import _lib as L, ops
     dev = torch.device("cuda:0")

@@ -111,7 +111,7 @@ def _oracle_tc_block(name, x, sd):
 
 
 def test_tensor_path_blocks_oracle_matches_reference():
-    """blocks_tc.pt (wide blocks the tcgen05 kernels take; weights regenerated from seeds, oracle/seeded.py): the
+    """blocks_tc.pt (wide blocks the tensor-core kernels take; weights regenerated from seeds, oracle/seeded.py): the
     restatement agrees with the REAL reference's outputs and gradients. The drop-in modules are used on the CPU as
     parameter holders only (no kernel runs): their parameter names / shapes are the reference's."""
     from models import modules as M

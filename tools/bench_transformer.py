@@ -71,7 +71,7 @@ att = 2 * 2 * S * S * H * L                                # QK^T and PV over th
 print(json.dumps({"metric": "token transformer training step (fwd + cross-entropy + bwd), sequence tokens/s", "value": B * S / sec,
                   "unit": "tokens/s", "batch": B, "seq_len": S, "ms_per_step": sec * 1e3, "loss": float(loss),
                   "model_tflops": 3 * (lin + att) * B / sec / 1e12, "gpu_launches_per_step": (_lib.launch_count() - l0) // args.steps,
-                  "tcgen05_launches_per_step": (_lib.tc_launch_count() - t0) // args.steps,
+                  "tensor_core_launches_per_step": (_lib.tc_launch_count() - t0) // args.steps,
                   "peak_mem_gb": torch.cuda.max_memory_allocated() / 1e9,
                   "attention": "fused core (attn_causal_fwd)" if os.environ.get("MAS_ATTN_FUSED", "1") != "0" else "GEMM / softmax / GEMM",
                   "loss_entry": "F.cross_entropy (torch)" if args.torch_ce else "MakeAScene.loss (mas_ce_*)", "config": cfg}))
