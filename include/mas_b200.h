@@ -181,8 +181,9 @@ int mas_wgrad_rows_f16(const void* x_f16, const void* dy_f16, int64_t M, int N, 
  * start offset are taken verbatim from raw_* and the B region holds its own word indices (address reveal). */
 int mas_tc_probe(const float* A, const float* B, float* D, int a_src, int b_layout, uint64_t raw_desc,
                  uint32_t raw_idesc, int raw_off, void* stream);
-/* fp16 address-reveal form: D[k][n] (k < 16, n < 32; D is [128][32]) = index of the half the tensor core reads for element
- * (n, k) of a B operand described by the raw descriptor (MN-major when bit 16 of raw_idesc is set), from a region filled with 0..2047. */
+/* fp16 address-reveal form: D[k][n] (k < 16, n < N; D is [128][N]) = index of the half the tensor core reads for element
+ * (n, k) of a B operand described by the raw descriptor (MN-major when bit 16 of raw_idesc is set, N = 8 x bits 17-22 of
+ * raw_idesc, 32 or 128), from a region filled with 0..2047. */
 int mas_tc_probe16(float* D, uint64_t raw_desc, uint32_t raw_idesc, int raw_off, void* stream);
 /* Weight gradient, written in the reference's [Cout,Cin,3,3] layout; dbias [Cout] may be NULL.
  * x is the convolution's (already normalised+activated) input, dy the output gradient. */

@@ -913,7 +913,7 @@ __global__ void __launch_bounds__(128, 1) mma_probe(const float* __restrict__ A,
 // fp16 address-reveal probe: A (shared memory, K-major) selects k = m % 16 in row m; the B region holds its own half index
 // (0 .. 2047); D[k][n] is therefore the index of the half the tensor core reads for element (n, k) of B under the raw shared-
 // memory descriptor supplied by the host, read MN-major when b_mn is set (tests/test_gpu_tc_probe.py).
-__global__ void __launch_bounds__(128, 1) mma_probe16(float* __restrict__ D, unsigned long long raw_desc, int b_mn, int raw_off) {
+__global__ void __launch_bounds__(128, 1) mma_probe16(float* __restrict__ D, unsigned long long raw_desc, int b_mn, int n, int raw_off) {
   __shared__ __align__(1024) uint8_t sm[16384];
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   __half* sa = reinterpret_cast<__half*>(sm);          // A: 128 x 16 halves, K-major [k/8][m][8]: LBO 2048, SBO 128
@@ -926,21 +926,28 @@ __global__ void __launch_bounds__(128, 1) mma_probe16(float* __restrict__ D, uns
   fence_proxy_async();
   __syncthreads();
   const uint64_t bd = (raw_desc & ~(0x3FFFull | (7ull << 46))) | (uint64_t)(((smem_u32(sb) + (uint32_t)raw_off) >> 4) & 0x3FFF);
-  float acc[2][16];
+  float acc[2][64];   // D = 128 x n (n = 32 or 128)
   wg::fence();
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    if (b_mn) wg::wgmma_f16_ss_n32<0, 1>(acc[h], wg::desc(smem_u32(sa) + h * 1024, 2048, 128), bd, 0u);
-    else wg::wgmma_f16_ss_n32<0, 0>(acc[h], wg::desc(smem_u32(sa) + h * 1024, 2048, 128), bd, 0u);
+    const uint64_t ad = wg::desc(smem_u32(sa) + h * 1024, 2048, 128);
+    if (n == 128) {
+      if (b_mn) wg::wgmma_f16_ss_n128<0, 1>(acc[h], ad, bd, 0u);
+      else wg::wgmma_f16_ss_n128<0, 0>(acc[h], ad, bd, 0u);
+    } else {
+      if (b_mn) wg::wgmma_f16_ss_n32<0, 1>(acc[h], ad, bd, 0u);
+      else wg::wgmma_f16_ss_n32<0, 0>(acc[h], ad, bd, 0u);
+    }
   }
   wg::commit();
   wg::wait<0>();
   const int r = (warp & 3) * 16 + (lane >> 2), c = lane & 3;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
-    wg::fence_regs<16>(acc[h]);
+    wg::fence_regs<64>(acc[h]);
 #pragma unroll
-    for (int j = 0; j < 16; ++j) D[(h * 64 + r + 8 * ((j >> 1) & 1)) * 32 + 8 * (j >> 2) + 2 * c + (j & 1)] = acc[h][j];
+    for (int j = 0; j < 64; ++j)
+      if (j < n / 2) D[(h * 64 + r + 8 * ((j >> 1) & 1)) * n + 8 * (j >> 2) + 2 * c + (j & 1)] = acc[h][j];
   }
 }
 
@@ -1245,7 +1252,10 @@ int mas_tc_probe(const float* A, const float* B, float* D, int a_src, int b_layo
 }
 
 int mas_tc_probe16(float* D, uint64_t raw_desc, uint32_t raw_idesc, int raw_off, void* stream) {
-  tc::mma_probe16<<<1, 128, 0, S(stream)>>>(D, (unsigned long long)raw_desc, (int)((raw_idesc >> 16) & 1), raw_off);
+  // raw_idesc: bit 16 = MN-major B, bits 17-22 = N / 8 (32 or 128; D is 128 x N)
+  const int n = (int)((raw_idesc >> 17) & 0x3F) * 8;
+  if (n != 32 && n != 128) return fail(MAS_ERR_INVALID_ARG, "tc_probe16: N must be 32 or 128 (got %d)", n);
+  tc::mma_probe16<<<1, 128, 0, S(stream)>>>(D, (unsigned long long)raw_desc, (int)((raw_idesc >> 16) & 1), n, raw_off);
   return launched_tc("mma_probe16");
 }
 

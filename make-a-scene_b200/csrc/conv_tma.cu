@@ -249,23 +249,32 @@ constexpr size_t t16_smem_bytes() {
 // Weight gradient of the 3x3 stride-1 convolution from the two fp16 shadows (activation x16, output gradient dy16 - already
 // scaled), dW[tap][co][ci] = sum_pixels dy[p][co] * x[p + tap][ci]; the reduction runs over PIXELS, so both operands are
 // "MN-major" in memory (channels contiguous, pixels strided):
-//   * A = dy^T: the dy tile of a unit (8 x 8 pixels x 128 co) lands as two 64-channel tensor-map boxes under the 128-byte
-//     swizzle, an MN-major operand (K groups = image rows of 8 pixels, SBO = 1024 B); warpgroup g multiplies co 64 g .. 64 g + 63;
-//   * B = the activation halo exactly as the copy engine lands it under the 128-byte swizzle: [row][pixel][64 ci] with 128-byte
-//     pixel rows, read as an MN-major operand (K groups = image rows of 8 pixels, SBO = the 1280-byte halo row).  A tap is a
-//     descriptor start shift (dx * 128 B); no producer warps, no dx copies;
-//   * a CTA owns one kernel ROW (3 horizontal taps) of a 128 co x 64 ci block: three m64n64 accumulators per warpgroup,
-//     K = 16 pixels = two image rows of the unit per MMA;
-//   * split-K over the units; partial sums (and the bias gradient, summed from the staged dy tile) go to the caller's
-//     workspace in the layout conv_wgrad_reduce expects.
-constexpr int WT_STAGES = 4;
-constexpr int WT_NCI = 64;                  // input channels per CTA (one swizzle atom of the halo)
-constexpr int WT_XATOM = 8 * 10 * 128;      // 8 halo rows x 10 pixels x 128 B (64 channels)
+//   * a CTA owns one kernel ROW (3 horizontal taps) of a 128 co x NCI ci block (NCI = 128, or 64 when Cin % 128 != 0) and
+//     walks its split's work units (8 x 8 output pixels); warpgroup g multiplies co 64 g .. 64 g + 63 into three m64nNCI
+//     accumulators (one per horizontal tap, 3 x 64 fp32 registers per thread at NCI = 128), K = 16 pixels = two image rows;
+//   * A = dy^T from REGISTERS: the dy tile of a unit (64 pixels x 128 co) lands as two 64-channel tensor-map boxes under the
+//     128-byte swizzle; per K step each warp reads its 16 co x 16 pixel fragment once with ldmatrix.x4.trans and the three
+//     tap MMAs use it (RS wgmma), so shared memory feeds the tensor cores the B operand only;
+//   * B = the activation halo exactly as the copy engine lands it: NCI / 64 boxes of [8 rows][10 pixels][64 ci] with 128-byte
+//     pixel rows, read as ONE MN-major operand (K groups = image rows of 8 pixels, SBO = the 1280-byte halo row; the 64-channel
+//     swizzle atoms are the boxes, LBO = the box stride). A tap is a descriptor start shift (dx * 128 B);
+//   * one commit group per K step, two register sets for A: a step's fragment is reloaded only after the group that read it
+//     has retired, while the next group keeps the tensor cores busy;
+//   * split-K over the units; partial sums go to the caller's workspace in the layout conv_wgrad_reduce expects. The bias
+//     gradient comes from the same A fragments (fp32 sums per thread, reduced over the four lanes of a row) in the CTAs of
+//     kernel row 0 / ci block 0, so the bias adds no shared-memory pass and no CTA does more than the others.
+constexpr int WT_STAGES = 5;
+constexpr int WT_XATOM = 8 * 10 * 128;      // one 64-channel halo box: 8 halo rows x 10 pixels x 128 B
 constexpr int WT_DYATOM = 64 * 128;         // 64 pixels x 64 co halves
 constexpr int WT_DY = 2 * WT_DYATOM;        // 64 pixels x 128 co halves
 constexpr int WT_THREADS = 12 * 32;
-constexpr int WT_STAGE = WT_XATOM + WT_DY;
-static_assert(WT_STAGE % 1024 == 0 && WT_XATOM % 1024 == 0, "stages must keep the swizzle atoms 1024-byte aligned");
+template <int NCI>
+__host__ __device__ constexpr int wt_stage() { return (NCI / 64) * WT_XATOM + WT_DY; }
+static_assert(wt_stage<64>() % 1024 == 0 && wt_stage<128>() % 1024 == 0 && WT_XATOM % 1024 == 0,
+              "stages must keep the swizzle atoms 1024-byte aligned");
+template <int NCI>
+constexpr size_t wt_smem_bytes() { return 1024 + (size_t)WT_STAGES * wt_stage<NCI>() + 2 * WT_STAGES * 8 + 16; }
+static inline int wt_nci(int64_t cin) { return cin % 128 == 0 ? 128 : 64; }
 
 struct WTParams {
   float* part;      // [splits][9][Cout][Cin]
@@ -276,19 +285,29 @@ struct WTParams {
   const float* dy_amax;   // the magnitude dy16's power-of-two scale was derived from
 };
 
+template <int NCI>
+__device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t bdesc) {
+  if (NCI == 128) wg::wgmma_f16_rs_n128<1>(d, a, bdesc, 1u);
+  else wg::wgmma_f16_rs_n64<1>(d, a, bdesc, 1u);
+}
+
+template <int NCI>
 __global__ void __launch_bounds__(WT_THREADS, 1) wgrad_t16(const WTParams p, const __grid_constant__ CUtensorMap x_map,
                                                           const __grid_constant__ CUtensorMap dy_map) {
+  constexpr int XBOX = NCI / 64;               // 64-channel halo boxes per stage
+  constexpr int STAGE = wt_stage<NCI>();
+  constexpr int NR = NCI / 2;                  // accumulator registers per tap
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
   const uint32_t smem_base = (raw_base + 1023u) & ~1023u;
   uint8_t* smem = smem_raw + (smem_base - raw_base);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)WT_STAGES * WT_STAGE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)WT_STAGES * STAGE);
   const uint32_t bar_base = smem_u32(bars);
   auto fullD = [&](int s) { return bar_base + 8u * s; };                      // copies of the stage have landed
   auto empty = [&](int s) { return bar_base + 8u * (WT_STAGES + s); };        // the MMAs of the stage have completed
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int dyy = blockIdx.x % 3, ci0 = (blockIdx.x / 3) * WT_NCI, co0 = blockIdx.y * BM, split = blockIdx.z;
+  const int dyy = blockIdx.x % 3, ci0 = (blockIdx.x / 3) * NCI, co0 = blockIdx.y * BM, split = blockIdx.z;
   const int64_t u0 = (int64_t)split * p.units_per_split;
   const int64_t u1 = min(p.total_units, u0 + p.units_per_split);
 
@@ -299,62 +318,73 @@ __global__ void __launch_bounds__(WT_THREADS, 1) wgrad_t16(const WTParams p, con
   __syncthreads();
 
   if (warp < 8) {
-    // ============ MMA warpgroups (bias-gradient sums by warpgroup 0), then epilogue ============
+    // ============ MMA warpgroups, then epilogue ============
     wg::regs_inc<wg::MMA_REGS>();
     const int wgi = warp >> 2;
     float a_inv;
     operand_scale(p.dy_amax, &a_inv);
-    float bsum = 0.f;
-    const bool want_bias = p.bpart != nullptr && blockIdx.x == 0 && tid < 128;
-    float acc[3][32];
+    const bool want_bias = p.bpart != nullptr && blockIdx.x == 0;
+    float bsum[2] = {0.f, 0.f};                // co rows lane / 4 and lane / 4 + 8 of the warp
+    float acc[3][NR];
 #pragma unroll
     for (int dx = 0; dx < 3; ++dx)
 #pragma unroll
-      for (int i = 0; i < 32; ++i) acc[dx][i] = 0.f;
-    int stage = 0, prev = 0;
+      for (int i = 0; i < NR; ++i) acc[dx][i] = 0.f;
+    // ldmatrix.x4.trans: lane l addresses pixel 8 (l / 16) + l % 8 of the K step, co chunk 2 (warp % 4) + (l / 8) % 2 of the
+    // warpgroup's 64; matrices (co +0 / +8) x (pixels +0 / +8) give the wgmma A fragment registers 0..3 in order. The
+    // 128-byte swizzle XORs the 16-byte chunk with the pixel's row in the atom, which is l % 8 for every K step.
+    const int lpix = ((lane >> 4) << 3) + (lane & 7);
+    const uint32_t a_lane = (uint32_t)(lpix * 128 + (((((warp & 3) << 1) | ((lane >> 3) & 1)) ^ (lane & 7)) << 4));
+    uint32_t a[2][4] = {{0u, 0u, 0u, 0u}, {0u, 0u, 0u, 0u}};
+    int stage = 0, prev = -1;
     uint32_t phase = 0;
     for (int64_t u = u0; u < u1; ++u) {
       mbar_wait(fullD(stage), phase);
-      const uint32_t xs = smem_base + (uint32_t)stage * WT_STAGE;
-      // MN-major, 128-byte swizzle: K groups (8 pixels = one image row of the unit) are 1280 B (halo) / 1024 B (dy) apart
-      const uint64_t xd0 = wg::desc(xs, 16, 1280, wg::SW_128);
-      const uint64_t ad0 = wg::desc(xs + WT_XATOM + (uint32_t)(wgi * WT_DYATOM), 16, 1024, wg::SW_128);
-      wg::fence();
+      const uint32_t xs = smem_base + (uint32_t)stage * STAGE;
+      const uint64_t xd0 = wg::desc(xs, WT_XATOM, 1280, wg::SW_128);
+      const uint32_t arow = xs + XBOX * WT_XATOM + (uint32_t)(wgi * WT_DYATOM) + a_lane;
 #pragma unroll
-      for (int r = 0; r < 8; r += 2) {          // K = 16 pixels: image rows r, r + 1 of the unit
+      for (int s = 0; s < 4; ++s) {             // K step s: image rows 2 s, 2 s + 1 of the unit
+        uint32_t* af = a[s & 1];
+        wg::wait<1>();                          // the group that last read af (two steps back) has retired
 #pragma unroll
-        for (int dx = 0; dx < 3; ++dx)
-          wg::wgmma_f16_ss_n64<1, 1>(acc[dx], ad0 + (uint64_t)((r * 1024) >> 4), xd0 + (uint64_t)((r * 1280 + dx * 128) >> 4), 1u);
-      }
-      wg::commit();
-      if (want_bias) {
-        // channel tid of the staged dy tile (swizzled: 16-byte chunk index XOR pixel % 8), pixels in pairs
-        const uint8_t* dyt = smem + (size_t)stage * WT_STAGE + WT_XATOM + (tid >> 6) * WT_DYATOM;
-        const int chk = (tid & 63) >> 3, e = tid & 7;
-#pragma unroll 4
-        for (int m = 0; m < 64; m += 2) {
-          const __half lo = *reinterpret_cast<const __half*>(dyt + m * 128 + ((chk ^ (m & 7)) << 4) + e * 2);
-          const __half hi = *reinterpret_cast<const __half*>(dyt + (m + 1) * 128 + ((chk ^ ((m + 1) & 7)) << 4) + e * 2);
-          bsum += __half2float(lo) + __half2float(hi);
+        for (int i = 0; i < 4; ++i) asm volatile("" : "+r"(af[i]));   // ... so af stays untouched until here
+        if (s == 1 && prev >= 0) mbar_arrive(empty(prev));             // the previous unit's last group has retired too
+        ldsm_x4_trans(arow + (uint32_t)(s * 16 * 128), af);
+        if (want_bias) {
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&af[i]));
+            bsum[i & 1] += f.x + f.y;
+          }
         }
+        wg::fence();
+#pragma unroll
+        for (int dx = 0; dx < 3; ++dx) wgmma_rs<NCI>(acc[dx], af, xd0 + (uint64_t)((s * 2 * 1280 + dx * 128) >> 4));
+        wg::commit();
       }
-      wg::wait<1>();
-      if (u > u0) mbar_arrive(empty(prev));
       prev = stage;
       if (++stage == WT_STAGES) { stage = 0; phase ^= 1; }
     }
     wg::wait<0>();
 #pragma unroll
-    for (int dx = 0; dx < 3; ++dx) wg::fence_regs<32>(acc[dx]);
-    if (want_bias) p.bpart[(size_t)split * p.Cout + co0 + tid] = bsum * a_inv;
+    for (int dx = 0; dx < 3; ++dx) wg::fence_regs<NR>(acc[dx]);
     const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+    if (want_bias) {
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        bsum[i] += __shfl_xor_sync(0xffffffffu, bsum[i], 1);
+        bsum[i] += __shfl_xor_sync(0xffffffffu, bsum[i], 2);
+        if ((lane & 3) == 0) p.bpart[(size_t)split * p.Cout + co0 + frow + 8 * i] = bsum[i] * a_inv;
+      }
+    }
 #pragma unroll
     for (int dx = 0; dx < 3; ++dx) {
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         float* o = p.part + (((size_t)split * 9 + dyy * 3 + dx) * p.Cout + co0 + frow + 8 * i) * p.Cin + ci0 + fcol;
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
+        for (int j = 0; j < NCI / 8; ++j)
           *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[dx][4 * j + 2 * i] * a_inv, acc[dx][4 * j + 2 * i + 1] * a_inv);
       }
     }
@@ -367,21 +397,21 @@ __global__ void __launch_bounds__(WT_THREADS, 1) wgrad_t16(const WTParams p, con
       for (int64_t u = u0; u < u1; ++u) {
         const int ux = (int)(u % p.units_x), uy = (int)((u / p.units_x) % p.units_y);
         const int n = (int)(u / ((int64_t)p.units_x * p.units_y));
-        const uint32_t dst = smem_base + (uint32_t)stage * WT_STAGE;
+        const uint32_t dst = smem_base + (uint32_t)stage * STAGE;
         mbar_wait(empty(stage), phase ^ 1);
-        mbar_expect_tx(fullD(stage), WT_STAGE);
-        tma_load_4d(dst, &x_map, ci0, ux * 8 - 1, uy * 8 + dyy - 1, n, fullD(stage));
+        mbar_expect_tx(fullD(stage), STAGE);
+#pragma unroll
+        for (int b = 0; b < XBOX; ++b)
+          tma_load_4d(dst + (uint32_t)(b * WT_XATOM), &x_map, ci0 + b * 64, ux * 8 - 1, uy * 8 + dyy - 1, n, fullD(stage));
 #pragma unroll
         for (int hf = 0; hf < 2; ++hf)
-          tma_load_4d(dst + WT_XATOM + (uint32_t)(hf * WT_DYATOM), &dy_map, co0 + hf * 64, ux * 8, uy * 8, n, fullD(stage));
+          tma_load_4d(dst + (uint32_t)(XBOX * WT_XATOM + hf * WT_DYATOM), &dy_map, co0 + hf * 64, ux * 8, uy * 8, n, fullD(stage));
         if (++stage == WT_STAGES) { stage = 0; phase ^= 1; }
       }
     }
     __syncwarp();
   }
 }
-
-constexpr size_t wt_smem_bytes() { return 1024 + (size_t)WT_STAGES * WT_STAGE + 2 * WT_STAGES * 8 + 16; }
 
 // fp32 -> fp16 shadow (optionally scaled by the power-of-two operand scale of *amax): plain vectorised copy
 __global__ void to_half_kernel(const float4* __restrict__ x, uint2* __restrict__ y, int64_t n4, const float* __restrict__ amax) {
@@ -455,6 +485,8 @@ int conv3x3_fprop_tma16_launch(const void* x16, mas_tensor4 xs, const void* w_tc
 void conv_wgrad_reduce_launch(const float* part, int splits, int ntap, int Cout, int Cin, float* dw, const float* bpart, float* dbias,
                               cudaStream_t st);   // contract_simt.cu
 
+// splits of the pixel reduction: as many as keep all CTAs (cps per split) in one wave of the 132 SMs - more waves would add
+// partial-sum traffic for the reduction and, for the small deep layers, leave CTAs with too few units to hide the epilogue
 static int wt_splits(int64_t cps, int64_t units) {
   int64_t s = 132 / cps;
   if (s < 1) s = 1;
@@ -469,7 +501,7 @@ bool conv_wgrad_t16_ok(mas_tensor4 xs, mas_tensor4 dys) {
 size_t conv_wgrad_t16_ws(mas_tensor4 xs, mas_tensor4 dys) {
   if (!conv_wgrad_t16_ok(xs, dys)) return 0;
   const int64_t coutk = cdiv(dys.c, tc::BM) * tc::BM;
-  const size_t splits = wt_splits((coutk / tc::BM) * (xs.c / tc::WT_NCI) * 3, dys.n * (dys.h / 8) * (dys.w / 8));
+  const size_t splits = wt_splits((coutk / tc::BM) * (xs.c / tc::wt_nci(xs.c)) * 3, dys.n * (dys.h / 8) * (dys.w / 8));
   return splits * 9 * (size_t)coutk * xs.c * sizeof(float) + splits * (size_t)coutk * sizeof(float) + 256;
 }
 // x16: fp16 activation shadow; dy16: fp16 output-gradient shadow scaled by operand_scale(*dy_amax); dw/dbias sized for
@@ -483,7 +515,8 @@ int conv_wgrad_t16_launch(const void* x16, mas_tensor4 xs, const void* dy16, mas
   p.units_x = (int)(dys.w / 8); p.units_y = (int)(dys.h / 8);
   p.total_units = (int64_t)p.N * p.units_x * p.units_y;
   p.dy_amax = dy_amax;
-  const int splits = wt_splits((int64_t)(p.Cout / tc::BM) * (p.Cin / tc::WT_NCI) * 3, p.total_units);
+  const int nci = tc::wt_nci(p.Cin);
+  const int splits = wt_splits((int64_t)(p.Cout / tc::BM) * (p.Cin / nci) * 3, p.total_units);
   p.units_per_split = cdiv(p.total_units, splits);
   p.part = (float*)ws;
   p.bpart = dbias ? (float*)ws + (size_t)splits * 9 * p.Cout * p.Cin : nullptr;
@@ -509,13 +542,16 @@ int conv_wgrad_t16_launch(const void* x16, mas_tensor4 xs, const void* dy16, mas
   }
   static std::atomic<uint64_t> configured{0};
   if (first_on_device(configured)) {
-    cudaError_t e = cudaFuncSetAttribute(tc::wgrad_t16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::wt_smem_bytes());
+    cudaError_t e = cudaFuncSetAttribute(tc::wgrad_t16<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::wt_smem_bytes<128>());
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(tc::wgrad_t16<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::wt_smem_bytes<64>());
     if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(wgrad_t16): %s", cudaGetErrorString(e));
     mark_device(configured);
   }
-  dim3 grid((unsigned)((p.Cin / tc::WT_NCI) * 3), (unsigned)(p.Cout / tc::BM), (unsigned)splits);
-  tc::wgrad_t16<<<grid, tc::WT_THREADS, tc::wt_smem_bytes(), st>>>(p, xmap, dmap);
-  if (int e = launched_tc("wgrad_t16")) return e;
+  dim3 grid((unsigned)((p.Cin / nci) * 3), (unsigned)(p.Cout / tc::BM), (unsigned)splits);
+  if (nci == 128) tc::wgrad_t16<128><<<grid, tc::WT_THREADS, tc::wt_smem_bytes<128>(), st>>>(p, xmap, dmap);
+  else tc::wgrad_t16<64><<<grid, tc::WT_THREADS, tc::wt_smem_bytes<64>(), st>>>(p, xmap, dmap);
+  if (int e = launched_tc(nci == 128 ? "wgrad_t16<128>" : "wgrad_t16<64>")) return e;
   conv_wgrad_reduce_launch((const float*)ws, splits, 9, p.Cout, p.Cin, dw, p.bpart, dbias, st);
   return launched("conv_wgrad_reduce");
 }

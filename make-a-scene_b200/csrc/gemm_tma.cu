@@ -150,7 +150,7 @@ constexpr size_t g16_smem_bytes() { return 1024 + (size_t)G_STAGES * G_STAGE + 2
 // ------------------------------------------------------------------------------------------------------------
 // Weight gradient of a Linear layer from the two fp16 copies (activation x16 [M,K], output gradient dy16 [M,N], both scaled by
 // their power-of-two operand scales): dW[n][k] = sum_m dy[m][n] * x[m][k].  The reduction runs over ROWS, so both operands are
-// "MN-major" in memory (features contiguous, rows strided) - the one-tap form of wgrad_t16 (conv_tma.cu):
+// "MN-major" in memory (features contiguous, rows strided) - a one-tap relative of wgrad_t16 (conv_tma.cu), both operands in shared memory:
 //   * A = dy^T: the dy tile of a unit (64 rows x 128 features) lands as two 64-feature tensor-map boxes under the 128-byte
 //     swizzle, an MN-major operand; warpgroup g multiplies features 64 g .. 64 g + 63;
 //   * B = x tiles exactly as the copy engine lands them under the 128-byte swizzle: [64 rows][64 features] atoms read as an

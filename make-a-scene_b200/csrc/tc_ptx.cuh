@@ -51,6 +51,14 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
                ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
                : "memory");
 }
+// four 8 x 8 fp16 matrices, transposed on the way: lanes 8 i .. 8 i + 7 address the eight 16-byte rows of matrix i, and
+// r[i] receives the wgmma / mma A-fragment register of that matrix
+__device__ __forceinline__ void ldsm_x4_trans(uint32_t addr, uint32_t* r) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0,%1,%2,%3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
+}
 // two floats -> packed half2 (lo = a, hi = b), round-to-nearest-even, saturating to +-65504 instead of inf
 __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
   uint32_t r;

@@ -92,6 +92,16 @@ __device__ __forceinline__ void wgmma_f16_ss_n256(float* d, uint64_t adesc, uint
                : WG_D128 : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
 }
 template <int TB>
+__device__ __forceinline__ void wgmma_f16_rs_n64(float* d, const uint32_t* a, uint64_t bdesc, uint32_t acc) {
+  asm volatile(WG_PRED(37) "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " WG_V32 ", {%32,%33,%34,%35}, %36, p, 1, 1, %38;\n\t}"
+               : WG_D32 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc), "n"(TB));
+}
+template <int TB>
+__device__ __forceinline__ void wgmma_f16_rs_n128(float* d, const uint32_t* a, uint64_t bdesc, uint32_t acc) {
+  asm volatile(WG_PRED(69) "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " WG_V64 ", {%64,%65,%66,%67}, %68, p, 1, 1, %70;\n\t}"
+               : WG_D64 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc), "n"(TB));
+}
+template <int TB>
 __device__ __forceinline__ void wgmma_f16_rs_n96(float* d, const uint32_t* a, uint64_t bdesc, uint32_t acc) {
   asm volatile(WG_PRED(53) "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 " WG_V48 ", {%48,%49,%50,%51}, %52, p, 1, 1, %54;\n\t}"
                : WG_D48 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc), "n"(TB));
