@@ -36,6 +36,10 @@ extern "C" {
 #define MAS_CONV_S2 1 /* pad (0,1,0,1) + stride 2, pad 0       — Downsample.forward, modules.py:74-78      */
 #define MAS_CONV_UP 2 /* nearest x2 upsample then stride 1 p1  — Upsample.forward, modules.py:55-59        */
 #define MAS_CONV_ZS 3 /* zero-stuffed x2 input (data gradient of MAS_CONV_S2), stride 1 pad 1             */
+/* Phase-decomposed forms of MAS_CONV_UP / MAS_CONV_S2 (mas_conv3x3_phase_tc16h); mas_conv3x3_tc_eligible(xs, ys, mode) with
+ * the layer's input / output shapes answers whether both the forward and the data gradient can take them. */
+#define MAS_CONV_UP_PHASE 4
+#define MAS_CONV_S2_PHASE 5
 
 /* Implementation selector for the contraction kernels. */
 #define MAS_IMPL_AUTO 0  /* wgmma (TF32 operands, fp32 accumulate) when the shape is eligible, else SIMT */
@@ -147,6 +151,16 @@ int mas_conv3x3_fprop_tc16h(const void* x_f16, mas_tensor4 xs, const void* w_tc1
                             const float* residual, float* y, mas_tensor4 ys, float* stats_part,
                             const float* x_amax, void* stream);
 int mas_to_half(const float* x, void* y_f16, int64_t n, const float* amax, void* stream);
+/* Upsample / Downsample convolution (mode MAS_CONV_UP_PHASE / MAS_CONV_S2_PHASE) in phase-decomposed form on the same TMA-fed
+ * kernel: the Upsample is four 2x2 convolutions of the low-resolution input (taps summed per output phase), the Downsample
+ * reads the four phase planes of its input with 4 / 2 / 2 / 1 of the nine taps each.  transpose = 0: forward (x_f16 the
+ * layer input, y its output, bias optional); transpose = 1: data gradient (x_f16 the output-gradient shadow, y = dx, no
+ * bias).  Phase planes are read through tensor-map strides: no copy of any of them is made.  Weights: the
+ * mas_pack_conv3x3_phase16 image of the same mode and transpose (Upsample 16 Cout Cin halves, Downsample 9 Cout Cin);
+ * combined taps are summed in fp32 and rounded to fp16 once.  Eligible: see MAS_CONV_UP_PHASE. */
+int mas_pack_conv3x3_phase16(const float* w_oihw, void* w_ph16, int Cout, int Cin, int mode, int transpose, void* stream);
+int mas_conv3x3_phase_tc16h(const void* x_f16, mas_tensor4 xs, const void* w_ph16, const float* bias, float* y,
+                            mas_tensor4 ys, int mode, int transpose, const float* x_amax, void* stream);
 /* Both packings of one weight (transpose = 0 and 1 of mas_pack_conv3x3_tc) in a single pass; Cout % 128 == Cin % 128 == 0. */
 int mas_pack_conv3x3_tc_pair(const float* w_oihw, float* w_tc_fwd, float* w_tc_dgrad, int Cout, int Cin, void* stream);
 int mas_gn_finalize_partials(const float* part, int tiles_per_image, int N, int C, int G, int64_t hw, float eps,

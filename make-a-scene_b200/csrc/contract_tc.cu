@@ -1064,6 +1064,7 @@ static int wgrad_tc_splits(int64_t cps, int64_t units) {
 }
 size_t conv_wgrad_t16_ws(mas_tensor4 xs, mas_tensor4 dys);   // conv_tma.cu: the shadow-fed kernel splits differently
 bool conv_wgrad_t16_ok(mas_tensor4 xs, mas_tensor4 dys);
+bool conv3x3_phase_ok(mas_tensor4 xs, mas_tensor4 ys, bool up);   // conv_tma.cu
 int conv_wgrad_t16_launch(const void* x16, mas_tensor4 xs, const void* dy16, mas_tensor4 dys, float* dw, float* dbias,
                           const float* dy_amax, void* ws, size_t ws_bytes, cudaStream_t st);
 size_t conv_wgrad_tc_ws(mas_tensor4 xs, mas_tensor4 dys, int mode) {
@@ -1261,6 +1262,7 @@ int mas_tc_probe16(float* D, uint64_t raw_desc, uint32_t raw_idesc, int raw_off,
 
 int mas_conv3x3_tc_eligible(mas_tensor4 xs, mas_tensor4 ys, int mode) {
   const int Cin = (int)xs.c, Cout = (int)ys.c;
+  if (mode == MAS_CONV_UP_PHASE || mode == MAS_CONV_S2_PHASE) return conv3x3_phase_ok(xs, ys, mode == MAS_CONV_UP_PHASE) ? 1 : 0;
   if (!(mode == MAS_CONV_S1 || mode == MAS_CONV_UP || mode == MAS_CONV_ZS)) return 0;
   // (the launch itself also takes Cout % 4 == 0 with weights / bias padded to the next multiple of 128: an explicit path of
   //  the caller, see mas_conv3x3_fprop_tc16; "eligible" means no padding is needed)

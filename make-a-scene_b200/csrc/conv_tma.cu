@@ -17,6 +17,18 @@
 //     thread of the CTA touches the operands; the copy issuer fills the rings of the next item while the warpgroups store the current one.
 //
 // Reference call sites replaced: nn.Conv2d 3x3 stride 1 (modules.py:93-104) forward and its data gradient.
+//
+// Phase-decomposed form (PH != 0) of the resampling convolutions, on the same kernel with a per-launch tap table:
+//   * Upsample (nearest x2, then 3x3): output phase (py, px) is a 2 x 2 convolution of the LOW-resolution input with the taps
+//     summed per phase (per dimension, phase 0 reads offsets {-1: w0, 0: w1 + w2}, phase 1 {0: w0 + w1, +1: w2}): 4 taps per
+//     output pixel instead of 9;
+//   * Downsample ((0,1,0,1) pad, 3x3 stride 2): input phase plane (py, px) = x[2 i + py][2 j + px] holds 4 / 2 / 2 / 1 of the
+//     nine taps, each at offset (ty >> 1, tx >> 1): 9 taps per output pixel instead of 36 on a space-to-depth map;
+//   * PH 1 "phase-out": one dense source, the item's output phase selects the taps, the epilogue writes that phase plane of
+//     the 2x output (Upsample forward, Downsample data gradient); PH 2 "phase-in": the K loop runs over the four phase planes
+//     of a 2x source (a 5-D tensor map with doubled pixel / row strides: nothing is materialised; out-of-image zero fill gives
+//     the borders and the Downsample pad) and each plane's taps, into a dense output (Downsample forward, Upsample data
+//     gradient).
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <cuda_fp16.h>
@@ -50,6 +62,11 @@ struct HParams {
   int64_t units;          // work units of 256 pixels: 32 x 8 tiles (TALL) or pairs of consecutive 16 x 8 tiles
   float* stats_part;   // GroupNorm-statistics epilogue (see shift_gemm_tc), or null
   const float* x_amax; // amax the shadow's power-of-two scale was derived from (null: unscaled shadow)
+  int64_t ysn, ysh, ysw;    // element strides of y per image / tile-grid row / tile-grid column
+  // phase forms only: per tap group (output phase for PH 1, source plane for PH 2) the staged-halo offsets (ty * 10 + tx)
+  // of its four taps and (PH 1) the element offset of its output plane
+  int ph_hoff[4][4];
+  int64_t ph_yoff[4];
 };
 
 // 16 x 8 tile (n, ty, tx) of half `hf` of work unit `u`; false when the unit's second tile does not exist (odd tile count)
@@ -74,9 +91,12 @@ __device__ __forceinline__ bool unit_tile(const HParams& p, int64_t u, int hf, i
 
 // TALL: the unit is one 32 x 8 tile whose staged halo (34 x 10 pixels, uniform 1280-byte row pitch) is ONE N = 256 operand:
 // per K = 16 step and tap a single m64n256 MMA per warpgroup instead of two m64n128 ones over the two halos of a pair.
-template <bool TALL>
+// PH: 0 the nine taps of a stride-1 3x3 convolution, 1 phase-out, 2 phase-in (see the top of the file).
+template <bool TALL, int PH = 0>
 __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, const __grid_constant__ CUtensorMap x_map) {
-  constexpr int TAPS = 9;
+  constexpr int TAPS = PH == 0 ? 9 : 4;              // phase forms: groups with fewer taps carry zero weights
+  constexpr int GOUT = PH == 1 ? 4 : 1;              // output phases per work unit
+  constexpr int KPL = PH == 2 ? 4 : 1;               // source planes per K loop
   constexpr int LBO_B = BN * 16, B_TAP = 2 * LBO_B;
   constexpr int A_BYTES = TALL ? 34 * 10 * 128 : 2 * 18 * 10 * 128;
 
@@ -95,8 +115,9 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int achunks = p.Cin / 64;
+  const int kiters = KPL * achunks;
   const int n_tiles = p.Cout / BN;
-  const int64_t nitems = p.units * n_tiles;       // channel tile fastest: the halo of a unit is re-read from L2
+  const int64_t nitems = p.units * n_tiles * GOUT;   // channel tile (then output phase) fastest: a unit's halo is re-read from L2
 
   if (tid == 0) {
     for (int s = 0; s < T_ASTAGES; ++s) { mbar_init(afull(s), 1); mbar_init(aempty(s), T_MMA_WARPS * 32); }
@@ -118,7 +139,9 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
     uint32_t aph = 0, bph = 0;
     float acc[128];
     for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-      for (int c = 0; c < achunks; ++c) {
+      const int gout = PH == 1 ? (int)((item / n_tiles) % GOUT) : 0;
+      for (int kk = 0; kk < kiters; ++kk) {
+        const int grp = PH == 2 ? kk / achunks : gout;
         mbar_wait(afull(as), aph);
         const uint64_t xd0 = wg::desc(a_base + (uint32_t)as * T_ASTAGE, 16, 1280, wg::SW_128);
 #pragma unroll 1
@@ -126,11 +149,11 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
           mbar_wait(bfull(bs), bph);
           const uint64_t wd0 = wg::desc(b_base + (uint32_t)bs * T_BSTAGE + (uint32_t)(wgi * 1024), LBO_B, 128);
           const uint64_t xds = xd0 + (uint64_t)((sub * 32) >> 4);
-          const uint32_t acc0 = (c > 0 || sub > 0) ? 1u : 0u;
+          const uint32_t acc0 = (kk > 0 || sub > 0) ? 1u : 0u;
           wg::fence();
 #pragma unroll
           for (int t = 0; t < TAPS; ++t) {
-            const uint32_t tapoff = (uint32_t)(((t / 3) * 10 + (t % 3)) * 128);
+            const uint32_t tapoff = (uint32_t)((PH == 0 ? (t / 3) * 10 + (t % 3) : p.ph_hoff[grp][t]) * 128);
             const uint64_t wd = wd0 + (uint64_t)((t * B_TAP) >> 4);
             const uint64_t xd = xds + (uint64_t)(tapoff >> 4);
             // D^T = W x X^T: weights on the M side, pixels on the N side
@@ -144,7 +167,7 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
           wg::commit();
           // the previous step's MMAs have read their weight stage (and, after a chunk's last step, its halo stage)
           wg::wait<1>();
-          if (c > 0 || sub > 0) {
+          if (kk > 0 || sub > 0) {
             mbar_arrive(bempty(prev_b));
             if (prev_a >= 0) mbar_arrive(aempty(prev_a));
           }
@@ -163,9 +186,11 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         int n_img, ty_, tx_;
-        const bool live = unit_tile<TALL>(p, item / n_tiles, h, n_img, ty_, tx_);   // block-uniform
+        const bool live = unit_tile<TALL>(p, item / (n_tiles * GOUT), h, n_img, ty_, tx_);   // block-uniform
         if (!live) continue;
         const int64_t pix0 = ((int64_t)n_img * p.H + ty_ * 16) * p.W + tx_ * 8;
+        const int64_t cstep = PH == 0 ? p.ldy : p.ysw;
+        const int64_t ybase = PH == 0 ? 0 : n_img * p.ysn + (ty_ * 16) * p.ysh + (tx_ * 8) * p.ysw + (PH == 1 ? p.ph_yoff[gout] : 0);
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
           const int ch = ch_tile + frow + 8 * i;
@@ -177,13 +202,13 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
 #pragma unroll
             for (int jj = 0; jj < 4; ++jj) {
               const int j = cb * 4 + jj;           // pixel row j of the tile, columns fcol, fcol + 1
-              const int64_t off = (pix0 + (int64_t)j * p.W + fcol) * p.ldy + ch;
+              const int64_t off = PH == 0 ? (pix0 + (int64_t)j * p.W + fcol) * p.ldy + ch : ybase + j * p.ysh + fcol * p.ysw + ch;
 #pragma unroll
               for (int cc = 0; cc < 2; ++cc) {
                 float o = fmaf(acc[64 * h + 4 * j + 2 * i + cc], alpha, bv);
                 if (st_ok) {
-                  if (p.res) o += __ldg(p.res + off + cc * p.ldy);
-                  p.y[off + cc * p.ldy] = o;
+                  if (p.res) o += __ldg(p.res + off + cc * cstep);
+                  p.y[off + cc * cstep] = o;
                   st_s += o;
                   st_q = fmaf(o, o, st_q);
                 }
@@ -217,21 +242,31 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
       uint32_t aph = 0, bph = 0;
       const int kchunks = p.Cin / 16;
       for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-        const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)(item % n_tiles) * kchunks * T_BSTAGE;
-        for (int c = 0; c < achunks; ++c) {
+        const int gout = PH == 1 ? (int)((item / n_tiles) % GOUT) : 0;
+        const int64_t unit = item / (n_tiles * GOUT);
+        constexpr uint32_t bstage = TAPS * B_TAP;
+        const uint8_t* wsrc0 = reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)(item % n_tiles) * kchunks * bstage;
+        for (int kk = 0; kk < kiters; ++kk) {
+          const int grp = PH == 2 ? kk / achunks : gout, c = kk % achunks;
+          // phase forms: one weight image per tap group, [group][n_tile][16-channel K step][4 taps][k / 8][128][8 halves]
+          const uint8_t* wsrc = PH == 0 ? wsrc0 : wsrc0 + (size_t)grp * (p.Cout / BN) * kchunks * bstage;
           mbar_wait(aempty(as), aph ^ 1);
           mbar_expect_tx(afull(as), A_BYTES);
 #pragma unroll
           for (int hf = 0; hf < (TALL ? 1 : 2); ++hf) {
             int n, ty_, tx_;
-            unit_tile<TALL>(p, item / n_tiles, hf, n, ty_, tx_);   // a missing second tile re-reads the last one (never stored)
-            tma_load_4d(a_base + (uint32_t)(as * T_ASTAGE + hf * T_ATILE), &x_map, c * 64, tx_ * 8 - 1, ty_ * 16 - 1, n, afull(as));
+            unit_tile<TALL>(p, unit, hf, n, ty_, tx_);   // a missing second tile re-reads the last one (never stored)
+            const uint32_t dst = a_base + (uint32_t)(as * T_ASTAGE + hf * T_ATILE);
+            if (PH == 2)   // plane (py, px) = grp: channel half px of the pixel pair, row parity py
+              tma_load_5d(dst, &x_map, (grp & 1) * p.Cin + c * 64, tx_ * 8 - 1, grp >> 1, ty_ * 16 - 1, n, afull(as));
+            else
+              tma_load_4d(dst, &x_map, c * 64, tx_ * 8 - 1, ty_ * 16 - 1, n, afull(as));
           }
           if (++as == T_ASTAGES) { as = 0; aph ^= 1; }
           for (int sub = 0; sub < 4; ++sub) {
             mbar_wait(bempty(bs), bph ^ 1);
-            mbar_expect_tx(bfull(bs), T_BSTAGE);
-            bulk_g2s(b_base + (uint32_t)bs * T_BSTAGE, wsrc + (size_t)(c * 4 + sub) * T_BSTAGE, T_BSTAGE, bfull(bs));
+            mbar_expect_tx(bfull(bs), bstage);
+            bulk_g2s(b_base + (uint32_t)bs * T_BSTAGE, wsrc + (size_t)(c * 4 + sub) * bstage, bstage, bfull(bs));
             if (++bs == T_BSTAGES) { bs = 0; bph ^= 1; }
           }
         }
@@ -423,7 +458,78 @@ __global__ void to_half_kernel(const float4* __restrict__ x, uint2* __restrict__
   }
 }
 
+// Tap table of a phase-decomposed resampling convolution: per tap group (output phase / source plane, index 2 py + px) the
+// staged-halo offset of each of its four taps and the set of the nine weight taps (bit ty * 3 + tx) summed into it. The
+// Downsample's groups hold 4 / 2 / 2 / 1 taps; the others are padded with empty sets (zero weights), so that every group
+// runs the same four MMAs per K step: a tap count that varies inside the kernel would serialise the asynchronous MMAs.
+struct PhaseTable {
+  int hoff[4][4];
+  int mask[4][4];
+};
+
+// fp16 weight images of the four tap groups, [group][n_tile][K / 16][4 taps][k / 8][128][8 halves] (each group like
+// pack_weights_tc16); a combined tap is summed in fp32 and rounded once. transpose: N = Cin, K = Cout (data gradient; the
+// table already holds the mirrored geometry, so taps are not flipped here).
+__global__ void pack_phase16(const float* __restrict__ w, __half* __restrict__ out, int Cout, int Cin, int transpose, PhaseTable tb,
+                             int64_t total) {
+  const int N = transpose ? Cin : Cout, K = transpose ? Cout : Cin;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    int64_t r = i;
+    const int k8 = (int)(r % 8); r /= 8;
+    const int nn = (int)(r % BN); r /= BN;
+    const int oct = (int)(r % 2); r /= 2;
+    const int j = (int)(r % 4); r /= 4;
+    const int kc = (int)(r % (K / 16)); r /= K / 16;
+    const int nt_ = (int)(r % (N / BN)), g = (int)(r / (N / BN));
+    const int n = nt_ * BN + nn, k = kc * 16 + oct * 8 + k8;
+    const int co = transpose ? k : n, ci = transpose ? n : k;
+    const float* src = w + ((size_t)co * Cin + ci) * 9;
+    float s = 0.f;
+    for (int t = 0; t < 9; ++t)
+      if ((tb.mask[g][j] >> t) & 1) s += src[t];
+    out[i] = __float2half_rn(s);
+  }
+}
+
 }  // namespace tc
+
+// up: Upsample (else Downsample); transpose: the data gradient. Staged halos start one pixel up / left of the tile, so a
+// tap at source offset (oy, ox) sits at halo offset (oy + 1) * 10 + ox + 1.
+static tc::PhaseTable phase_table(bool up, bool transpose) {
+  tc::PhaseTable tb{};
+  for (int g = 0; g < 4; ++g) {
+    const int py = g >> 1, px = g & 1;
+    if (up) {
+      // phase p, tap a of a dimension: offset p - 1 + a, original taps {0} / {1, 2} (p = 0) or {0, 1} / {2} (p = 1)
+      auto set = [](int ph, int a) { return ph == 0 ? (a == 0 ? 1 : 6) : (a == 0 ? 3 : 4); };
+      for (int a = 0; a < 2; ++a)
+        for (int b = 0; b < 2; ++b) {
+          const int oy = py - 1 + a, ox = px - 1 + b, j = a * 2 + b;
+          // forward: output phase g reads x[i + o]; data gradient: source plane g of dy contributes to dx[i] from dy[i - o]
+          tb.hoff[g][j] = transpose ? (1 - oy) * 10 + (1 - ox) : (oy + 1) * 10 + (ox + 1);
+          int m = 0;
+          for (int ty = 0; ty < 3; ++ty)
+            for (int tx = 0; tx < 3; ++tx)
+              if (((set(py, a) >> ty) & 1) && ((set(px, b) >> tx) & 1)) m |= 1 << (ty * 3 + tx);
+          tb.mask[g][j] = m;
+        }
+    } else {
+      // plane (py, px) holds the taps with ty % 2 == py, tx % 2 == px, at plane offset (ty / 2, tx / 2)
+      int j = 0;
+      for (int ty = py; ty < 3; ty += 2)
+        for (int tx = px; tx < 3; tx += 2, ++j) {
+          const int oy = ty >> 1, ox = tx >> 1;
+          tb.hoff[g][j] = transpose ? (1 - oy) * 10 + (1 - ox) : (oy + 1) * 10 + (ox + 1);
+          tb.mask[g][j] = 1 << (ty * 3 + tx);
+        }
+      for (; j < 4; ++j) {   // padding taps: empty weight set, any in-halo offset
+        tb.hoff[g][j] = 11;
+        tb.mask[g][j] = 0;
+      }
+    }
+  }
+  return tb;
+}
 
 static bool dense_nhwc4(const mas_tensor4& t) {
   return t.sc == 1 && t.sw == t.c && t.sh == t.w * t.c && t.sn == t.h * t.w * t.c;
@@ -480,6 +586,99 @@ int conv3x3_fprop_tma16_launch(const void* x16, mas_tensor4 xs, const void* w_tc
   if (tall) tc::shift_gemm_t16<true><<<g, tc::T_THREADS, smem, st>>>(p, map);
   else tc::shift_gemm_t16<false><<<g, tc::T_THREADS, smem, st>>>(p, map);
   return launched_tc(tall ? "shift_gemm_t16<tall>" : "shift_gemm_t16<pair>");
+}
+
+// Phase-decomposed Upsample / Downsample convolution, xs / ys the shapes of the layer's input and output (forward).
+bool conv3x3_phase_ok(mas_tensor4 xs, mas_tensor4 ys, bool up) {
+  const mas_tensor4& lo = up ? xs : ys;   // the low-resolution side: the phase planes' extent
+  const mas_tensor4& hi = up ? ys : xs;
+  return dense_nhwc4(xs) && dense_nhwc4(ys) && xs.c % 128 == 0 && ys.c % 128 == 0 && xs.n == ys.n && hi.h == 2 * lo.h &&
+         hi.w == 2 * lo.w && lo.h % 16 == 0 && lo.w % 8 == 0;
+}
+
+int pack_phase16_launch(const float* w, void* out, int Cout, int Cin, bool up, bool transpose, cudaStream_t st) {
+  if (Cout % tc::BN || Cin % tc::BN) return fail(MAS_ERR_UNSUPPORTED, "pack_conv3x3_phase16: Cout=%d and Cin=%d must be multiples of 128", Cout, Cin);
+  const tc::PhaseTable tb = phase_table(up, transpose);
+  const int64_t total = (int64_t)16 * Cout * Cin;
+  tc::pack_phase16<<<(unsigned)(cdiv(total, 256) < 2368 ? cdiv(total, 256) : 2368), 256, 0, st>>>(w, (__half*)out, Cout, Cin, transpose ? 1 : 0,
+                                                                                              tb, total);
+  return launched("pack_phase16");
+}
+
+// x16: fp16 NHWC shadow of the convolution's source (the layer input, or for the data gradient the output gradient, scaled
+// by operand_scale(*x_amax) when x_amax is given); xs / ys: source and destination of THIS pass; w_ph16: pack_phase16 image
+// of the same (up, transpose).
+int conv3x3_phase_tma16_launch(const void* x16, mas_tensor4 xs, const void* wpk, const float* bias, float* y, mas_tensor4 ys, bool up,
+                               bool transpose, const float* x_amax, cudaStream_t st) {
+  const bool phase_out = up != transpose;   // Upsample forward / Downsample data gradient: the destination is the 2x side
+  if (!conv3x3_phase_ok(phase_out ? xs : ys, phase_out ? ys : xs, true))
+    return fail(MAS_ERR_UNSUPPORTED, "phase conv: shape/layout not eligible (Cin=%lld Cout=%lld H=%lld W=%lld)", (long long)xs.c,
+                (long long)ys.c, (long long)xs.h, (long long)xs.w);
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  if (!al16(x16) || !al16(y) || !al16(wpk) || (bias && !al16(bias))) return fail(MAS_ERR_INVALID_ARG, "phase conv: pointers must be 16-byte aligned");
+  const tc::PhaseTable tb = phase_table(up, transpose);
+  const mas_tensor4& lo = phase_out ? xs : ys;
+  tc::HParams p{};
+  p.wpk = wpk; p.bias = bias; p.res = nullptr; p.y = y;
+  p.N = (int)xs.n; p.H = (int)lo.h; p.W = (int)lo.w; p.Cin = (int)xs.c; p.Cout = (int)ys.c; p.Cstore = (int)ys.c; p.ldy = ys.c;
+  p.tiles_x = (int)(lo.w / 8); p.tiles_y = (int)(lo.h / 16);
+  p.stats_part = nullptr; p.x_amax = x_amax;
+  const bool tall = lo.h % 32 == 0;
+  const int64_t tiles = (int64_t)p.N * p.tiles_x * p.tiles_y;
+  p.units = tall ? tiles / 2 : cdiv(tiles, 2);
+  p.ysn = ys.sn;
+  p.ysh = phase_out ? 2 * ys.sh : ys.sh;
+  p.ysw = phase_out ? 2 * ys.sw : ys.sw;
+  for (int g = 0; g < 4; ++g) {
+    for (int j = 0; j < 4; ++j) p.ph_hoff[g][j] = tb.hoff[g][j];
+    p.ph_yoff[g] = phase_out ? (g >> 1) * ys.sh + (g & 1) * ys.sw : 0;
+  }
+
+  PFN_cuTensorMapEncodeTiled enc = tensor_map_encoder();
+  if (!enc) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled entry point not available");
+  CUtensorMap map;
+  CUresult r;
+  const cuuint32_t hbox = tall ? 34u : 18u;
+  if (phase_out) {
+    cuuint64_t dims[4] = {(cuuint64_t)xs.c, (cuuint64_t)xs.w, (cuuint64_t)xs.h, (cuuint64_t)xs.n};
+    cuuint64_t strides[3] = {(cuuint64_t)xs.c * 2, (cuuint64_t)xs.w * xs.c * 2, (cuuint64_t)xs.h * xs.w * xs.c * 2};
+    cuuint32_t box[4] = {64, 10, hbox, 1}, es[4] = {1, 1, 1, 1};
+    r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(x16), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  } else {
+    // the four phase planes of the 2x source: [n][row pair][row parity py][pixel pair][px * C + c]
+    cuuint64_t dims[5] = {(cuuint64_t)xs.c * 2, (cuuint64_t)xs.w / 2, 2, (cuuint64_t)xs.h / 2, (cuuint64_t)xs.n};
+    cuuint64_t strides[4] = {(cuuint64_t)xs.c * 4, (cuuint64_t)xs.w * xs.c * 2, (cuuint64_t)xs.w * xs.c * 4, (cuuint64_t)xs.h * xs.w * xs.c * 2};
+    cuuint32_t box[5] = {64, 10, 1, hbox, 1}, es[5] = {1, 1, 1, 1, 1};
+    r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(x16), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  }
+  if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (phase conv map) failed (%d)", (int)r);
+
+  constexpr size_t smem = tc::t16_smem_bytes();
+  static std::atomic<uint64_t> configured{0};
+  static int sm_count = 132;
+  if (first_on_device(configured)) {
+    cudaError_t e = cudaFuncSetAttribute(tc::shift_gemm_t16<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::shift_gemm_t16<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::shift_gemm_t16<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::shift_gemm_t16<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e));
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
+    mark_device(configured);
+  }
+  const int64_t nitems = p.units * (p.Cout / tc::BN) * (phase_out ? 4 : 1);
+  const unsigned g = (unsigned)(nitems < sm_count ? nitems : sm_count);
+  if (phase_out) {
+    if (tall) tc::shift_gemm_t16<true, 1><<<g, tc::T_THREADS, smem, st>>>(p, map);
+    else tc::shift_gemm_t16<false, 1><<<g, tc::T_THREADS, smem, st>>>(p, map);
+    return launched_tc(tall ? "shift_gemm_t16<tall, phase-out>" : "shift_gemm_t16<pair, phase-out>");
+  }
+  if (tall) tc::shift_gemm_t16<true, 2><<<g, tc::T_THREADS, smem, st>>>(p, map);
+  else tc::shift_gemm_t16<false, 2><<<g, tc::T_THREADS, smem, st>>>(p, map);
+  return launched_tc(tall ? "shift_gemm_t16<tall, phase-in>" : "shift_gemm_t16<pair, phase-in>");
 }
 
 void conv_wgrad_reduce_launch(const float* part, int splits, int ntap, int Cout, int Cin, float* dw, const float* bpart, float* dbias,
@@ -581,6 +780,20 @@ int mas_conv3x3_fprop_tc16h(const void* x_f16, mas_tensor4 xs, const void* w_tc1
 int mas_to_half(const float* x, void* y_f16, int64_t n, const float* amax, void* stream) {
   MAS_REQUIRE(x && y_f16 && n > 0, "to_half: bad arguments");
   return mas::to_half_launch(x, y_f16, n, amax, mas::S(stream));
+}
+
+int mas_pack_conv3x3_phase16(const float* w_oihw, void* w_ph16, int Cout, int Cin, int mode, int transpose, void* stream) {
+  MAS_REQUIRE(w_oihw && w_ph16, "pack_conv3x3_phase16: null pointer");
+  MAS_REQUIRE(mode == MAS_CONV_UP_PHASE || mode == MAS_CONV_S2_PHASE, "pack_conv3x3_phase16: mode %d", mode);
+  return mas::pack_phase16_launch(w_oihw, w_ph16, Cout, Cin, mode == MAS_CONV_UP_PHASE, transpose != 0, mas::S(stream));
+}
+
+int mas_conv3x3_phase_tc16h(const void* x_f16, mas_tensor4 xs, const void* w_ph16, const float* bias, float* y, mas_tensor4 ys,
+                            int mode, int transpose, const float* x_amax, void* stream) {
+  MAS_REQUIRE(x_f16 && w_ph16 && y, "conv3x3_phase_tc16h: null pointer");
+  MAS_REQUIRE(mode == MAS_CONV_UP_PHASE || mode == MAS_CONV_S2_PHASE, "conv3x3_phase_tc16h: mode %d", mode);
+  return mas::conv3x3_phase_tma16_launch(x_f16, xs, w_ph16, bias, y, ys, mode == MAS_CONV_UP_PHASE, transpose != 0, x_amax,
+                                         mas::S(stream));
 }
 
 }  // extern "C"

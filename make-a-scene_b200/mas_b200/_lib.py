@@ -16,6 +16,7 @@ LIB_PATH = os.path.join(os.path.dirname(_HERE), "lib", "libmas_b200.so")
 
 IMPL_AUTO, IMPL_SIMT, IMPL_TC, IMPL_TC3 = 0, 1, 2, 3
 CONV_S1, CONV_S2, CONV_UP, CONV_ZS = 0, 1, 2, 3
+CONV_UP_PHASE, CONV_S2_PHASE = 4, 5   # phase-decomposed Upsample / Downsample (mas_conv3x3_phase_tc16h)
 
 
 class Tensor4(ctypes.Structure):
@@ -56,6 +57,8 @@ _SPEC = {
     "mas_conv3x3_tc16h_eligible": (_I, [_T, _T]),
     "mas_conv3x3_fprop_tc16h": (_I, [_P, _T, _P, _P, _P, _P, _T, _P, _P, _P]),
     "mas_to_half": (_I, [_P, _P, _L, _P, _P]),
+    "mas_pack_conv3x3_phase16": (_I, [_P, _P, _I, _I, _I, _I, _P]),
+    "mas_conv3x3_phase_tc16h": (_I, [_P, _T, _P, _P, _P, _T, _I, _I, _P, _P]),
     "mas_gn_finalize_partials": (_I, [_P, _I, _I, _I, _I, _L, _F, _P, _P, _P]),
     "mas_gn_table": (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P]),
     "mas_pack_gemm_tc": (_I, [_P, _P, _I, _I, _I, _P]),

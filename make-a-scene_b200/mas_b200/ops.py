@@ -320,6 +320,38 @@ def _packed_conv_weight(wc, weight, cout, cin, transpose, dev, prepack=False, f1
     return wt
 
 
+def phase_mode(x, cout, mode):
+    """CONV_UP_PHASE / CONV_S2_PHASE when the Upsample / Downsample convolution of dense-NHWC x runs phase-decomposed on the
+    TMA-fed kernel (forward and data gradient), else None. MAS_CONV_PHASE=0 keeps the register-staged route for A/B runs."""
+    if mode not in (L.CONV_UP, L.CONV_S2) or not conv_tma_on() or os.environ.get("MAS_CONV_PHASE", "1") == "0":
+        return None
+    if not _is_dense_nhwc(x):
+        return None
+    n, _, h, w = x.shape
+    ho, wo = _conv_out_hw(h, w, mode)
+    ys = L.Tensor4(n, ho, wo, cout, ho * wo * cout, wo * cout, cout, 1)
+    pm = L.CONV_UP_PHASE if mode == L.CONV_UP else L.CONV_S2_PHASE
+    return pm if L.query("mas_conv3x3_tc_eligible", L.t4(x), ys, pm) else None
+
+
+def conv3x3_phase_raw(x16, weight, bias, pmode, transpose=False, x_amax=None):
+    """Phase-decomposed Upsample / Downsample convolution (forward, or its data gradient with transpose=True) of an fp16
+    channels-last shadow x16, scaled by the power-of-two operand scale of *x_amax."""
+    n, c, h, w = x16.shape
+    cout = weight.shape[1] if transpose else weight.shape[0]
+    up_side = (pmode == L.CONV_UP_PHASE) != transpose   # the destination is the 2x side
+    y = empty_nhwc(n, cout, 2 * h if up_side else h // 2, 2 * w if up_side else w // 2, x16)
+    ent = _pack_entry(weight)
+    key = ("phase", pmode, transpose)
+    wt = ent.get(key)
+    if wt is None or wt.device != x16.device:
+        wt = torch.empty(16 * weight.shape[0] * weight.shape[1], dtype=torch.float16, device=x16.device)
+        L.call("mas_pack_conv3x3_phase16", weight.contiguous(), wt, weight.shape[0], weight.shape[1], pmode, int(transpose))
+        ent[key] = wt
+    L.call("mas_conv3x3_phase_tc16h", x16, L.t4(x16), wt, bias, y, L.t4(y), pmode, int(transpose), x_amax)
+    return y
+
+
 def conv3x3_wgrad_raw(x, dy, cout, cin, mode, want_bias=True, table=None, silu=True, dy_amax=None):
     """table: x is the PRE-normalisation tensor and act(GroupNorm(x)) is recomputed while staging (tensor path only)."""
     dw = torch.empty((cout, cin, 3, 3), dtype=torch.float32, device=x.device)
@@ -553,6 +585,14 @@ class Conv3x3Fn(torch.autograd.Function):
             full = torch.empty((n, h, w, cpo), dtype=torch.float32, device=x.device).permute(0, 3, 1, 2)
             L.call("mas_conv3x3_fprop_tc16", x, L.t4(x), wt, bk, None, full, L.t4(full), L.CONV_S1, None, 0, None, amax_of(x))
             y = full[:, :cout]
+        elif residual is None and not out_nchw and phase_mode(x, cout, mode) is not None:
+            # Upsample / Downsample as four small convolutions over phase planes read straight from an fp16 shadow of x
+            edge = 6
+            am = amax_of(x)
+            y = conv3x3_phase_raw(to_half(x, am), weight, bias, phase_mode(x, cout, mode), x_amax=am)
+            if mode == L.CONV_UP:
+                # a following ResnetBlock without shortcut writes its input gradient's fp16 shadow: the data gradient here reads it
+                y._mas_res_out = True
         elif (mode == L.CONV_S2 and _tc_on() and residual is None and not out_nchw and _is_dense_nhwc(x) and cin % 8 == 0
               and cout % 128 == 0 and h % 32 == 0 and w % 16 == 0):
             edge = 3  # stride-2 conv on the stride-1 tensor kernels through space-to-depth
@@ -619,6 +659,24 @@ class Conv3x3Fn(torch.autograd.Function):
             if want_w:
                 dwk, dbk = conv3x3_wgrad_raw(x, full, ck, cin, L.CONV_S1, True, dy_amax=am)
                 dw, db = dwk[:cout].contiguous(), dbk[:cout].contiguous()
+        elif ctx.edge == 6:
+            dy = nhwc(dy)
+            am = amax_of(dy)
+            if ctx.needs_input_grad[0]:
+                sh = shadow_of(dy)
+                if sh is None:
+                    sh = (to_half(dy, am), am)
+                dx = conv3x3_phase_raw(sh[0], weight, None, phase_mode(x, cout, ctx.mode), transpose=True, x_amax=sh[1])
+            if want_w:
+                if ctx.mode == L.CONV_UP:
+                    dw, db = conv3x3_wgrad_raw(x, dy, cout, cin, ctx.mode, ctx.has_bias, dy_amax=am)
+                else:   # the register-staged weight gradient over the space-to-depth map
+                    n, _, h, w = x.shape
+                    x4 = empty_nhwc(n, 4 * cin, h // 2, w // 2, x)
+                    L.call("mas_space_to_depth", x, x4, n, h, w, cin)
+                    dw9, db = conv3x3_wgrad_raw(x4, dy, cout, 4 * cin, L.CONV_S1, ctx.has_bias, dy_amax=am)
+                    dw = torch.empty_like(weight)
+                    L.call("mas_s2d_unpack_wgrad", dw9, dw, cout, cin)
         elif ctx.edge == 3:
             if ctx.needs_input_grad[0]:
                 dx = conv3x3_dgrad_raw(nhwc(dy), weight, ctx.mode)       # zero-stuffed map on the tensor kernel
