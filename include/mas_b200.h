@@ -319,6 +319,55 @@ int mas_bn_backward_apply(const float* dy, const float* x, const float* mean, co
                           double inv_count, float* dx, float* dgamma, float* dbeta, int64_t R, int C,
                           void* stream);
 
+/* ---- PatchGAN discriminator — losses/discriminator.py:21-35 ---------------------------------------------
+ * nn.Conv2d(k=4, s in {1, 2}, p=1) (+ LeakyReLU(0.2) after the first one), nn.BatchNorm2d + LeakyReLU(0.2) (plain, per-call
+ * batch statistics), csrc/conv4x4.cu and csrc/norm.cu.  The convolutions are exact-fp32 SIMT implicit GEMMs over explicit
+ * strides and any channel counts (the first reads the caller's NCHW image, the last has Cout = 1).
+ * mas_pack_conv4x4: [Cout,Cin,4,4] -> transpose 0: [(4kh+kw)*Cin + ci][co] (forward operand); transpose 1:
+ * [(4kh+kw)*Cout + co][ci] (data-gradient operand).
+ * mas_conv4x4: y = conv(x) (+bias[co] when bias != NULL), then LeakyReLU(act_slope) when act != 0.  ys.h = (xs.h - 2) / stride + 1.
+ * mas_conv4x4_dgrad: dx of that convolution from dy (any strides: an expanded loss gradient with zero strides is fine).
+ * mas_conv4x4_wgrad: dw [Cout,Cin,4,4] (OIHW), deterministic (split over pixels, ordered reduction); bias gradients are
+ * mas_colsum(dy).  Workspace: mas_conv4x4_wgrad_ws_bytes.
+ * mas_lrelu_backward: dx = dy * (y > 0 ? 1 : slope) with y the LeakyReLU output (dense, n elements).
+ * BatchNorm2d + LeakyReLU: mas_bn_stats, then mas_bn_finalize(count = 0) (momentum, eps, unbiased running variance as
+ * nn.BatchNorm2d), then mas_bn_apply_lrelu: y = LeakyReLU(slope)(BN(x)).  Backward from dy = dL/dy, y the forward output:
+ * mas_bn_backward_reduce_lrelu writes [sum_dz(C), sum_dz_xhat(C), R] of dz = dy * LeakyReLU'(y) (row chunks, then an ordered
+ * sum: deterministic; workspace mas_bn_backward_reduce_lrelu_ws_bytes), and
+ * mas_bn_backward_apply_lrelu writes dx and (when dgamma != NULL) dgamma / dbeta from those sums.  Eval mode: mas_bn_invstd
+ * of the running variance with the running mean in mas_bn_apply_lrelu. */
+int mas_pack_conv4x4(const float* w_oihw, float* w_packed, int Cout, int Cin, int transpose, void* stream);
+int mas_conv4x4(const float* x, mas_tensor4 xs, const float* w_packed, const float* bias, float* y, mas_tensor4 ys, int stride,
+                float act_slope, int act, void* stream);
+int mas_conv4x4_dgrad(const float* dy, mas_tensor4 dys, const float* w_packed_t, float* dx, mas_tensor4 dxs, int stride,
+                      void* stream);
+size_t mas_conv4x4_wgrad_ws_bytes(mas_tensor4 xs, mas_tensor4 dys);
+int mas_conv4x4_wgrad(const float* x, mas_tensor4 xs, const float* dy, mas_tensor4 dys, float* dw_oihw, int stride, void* ws,
+                      size_t ws_bytes, void* stream);
+int mas_lrelu_backward(const float* dy, const float* y, float slope, float* dx, int64_t n, void* stream);
+/* Tensor-core route of the 4x4 convolution (dense NHWC, Cout % 128 == 0, stride 2 with even extents): it is the 3x3 stride-1
+ * pad-1 convolution of the 4*Cin-channel shift map X'(i, j, (2p + q)*Cin + c) = x(s*i + p, s*j + q, c) (0 outside x;
+ * X' is H/s x W/s) with the remapped weight W3 [Cout, 4*Cin, 3, 3]: 4x4 tap kh is the 3x3 tap a of plane p with
+ * kh = 2a - 1 + p at stride 2 (16 of the 36 taps), kh = a (p = 0) for kh < 3 and (a, p) = (2, 1) for kh = 3 at stride 1.
+ * So the forward, data gradient and weight gradient run on mas_conv3x3_fprop_tc16 / mas_conv3x3_wgrad_tc16 (fp16 operands,
+ * power-of-two scales from device-side amax, fp32 accumulate).  At stride 1 the 3x3 output is H x W: its last row and column
+ * are dropped (the layer's output is the H-1 x W-1 view), and the output gradient handed to the data / weight gradient must be
+ * zero there.  mas_conv4x4_shift_map writes X' (dense); mas_conv4x4_shift_map_adjoint writes dx from dX' (sum over the up to
+ * four X' positions that read each x element); mas_conv4x4_remap_weight: to3x3 = 1 writes W3 from w [Cout,Cin,4,4],
+ * to3x3 = 0 writes dw [Cout,Cin,4,4] from dW3. */
+int mas_conv4x4_shift_map(const float* x, mas_tensor4 xs, float* y, int stride, void* stream);
+int mas_conv4x4_shift_map_adjoint(const float* dmap, float* dx, mas_tensor4 dxs, int stride, void* stream);
+int mas_conv4x4_remap_weight(const float* src, float* dst, int Cout, int Cin, int stride, int to3x3, void* stream);
+int mas_bn_apply_lrelu(const float* x, const float* mean, const float* invstd, const float* gamma, const float* beta, float slope,
+                       float* y, int64_t R, int C, void* stream);
+size_t mas_bn_backward_reduce_lrelu_ws_bytes(int64_t R, int C);
+int mas_bn_backward_reduce_lrelu(const float* dy, const float* y, float slope, const float* x, const float* mean,
+                                 const float* invstd, int64_t R, int C, double* sums_out, void* ws, size_t ws_bytes,
+                                 void* stream);
+int mas_bn_backward_apply_lrelu(const float* dy, const float* y, float slope, const float* x, const float* mean,
+                                const float* invstd, const float* gamma, const double* sums, float* dx, float* dgamma,
+                                float* dbeta, int64_t R, int C, void* stream);
+
 /* ---- Codebook (vector quantiser) — modules.py:470-473,501-517 ---------------------------------------
  * z: [R, D] latent rows (NHWC order, R = B*h*w), E: [K, D] codebook.
  * idx_out[r] = argmin_k ( (|z_r|^2 + |e_k|^2) - 2 z_r.e_k ), fp32, the reference's association and

@@ -574,10 +574,12 @@ __global__ void bn_invstd_kernel(const float* __restrict__ var, float eps, float
 }
 __global__ void bn_apply_kernel(const float* __restrict__ x, const float* __restrict__ mean, const float* __restrict__ invstd,
                                 const float* __restrict__ gamma, const float* __restrict__ beta, float* __restrict__ y,
-                                int64_t total, int C) {
+                                int64_t total, int C, float slope) {
+  // slope: LeakyReLU on the output (1 = none: v * 1 is exact)
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     int c = (int)(i % C);
-    y[i] = (x[i] - mean[c]) * invstd[c] * gamma[c] + beta[c];
+    float v = (x[i] - mean[c]) * invstd[c] * gamma[c] + beta[c];
+    y[i] = v > 0.f ? v : v * slope;
   }
 }
 __global__ void bn_bwd_reduce_kernel(const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ mean,
@@ -606,17 +608,60 @@ __global__ void bn_bwd_reduce_kernel(const float* __restrict__ dy, const float* 
     if (c == 0) out[2 * C] = (double)R;
   }
 }
+// BatchNorm+LeakyReLU backward sums over row chunks of BN_RB rows (grid: C/32 x chunks), then an ordered sum of the chunks:
+// deterministic, and enough blocks to fill the GPU at the discriminator's R = N*H*W of 10^4..10^5 rows
+constexpr int BN_RB = 1024;
+__global__ void bn_bwd_reduce_lrelu_part(const float* __restrict__ dy, const float* __restrict__ act_y, float slope,
+                                         const float* __restrict__ x, const float* __restrict__ mean, const float* __restrict__ invstd,
+                                         int64_t R, int C, double* __restrict__ part /*[chunks][2C]*/) {
+  __shared__ double sh[8][32][2];
+  const int c = blockIdx.x * 32 + threadIdx.x;
+  const int64_t r0 = (int64_t)blockIdx.y * BN_RB, r1 = min(R, r0 + BN_RB);
+  double a = 0, b = 0;
+  if (c < C) {
+    const float m = mean[c], is = invstd[c];
+    for (int64_t r = r0 + threadIdx.y; r < r1; r += 8) {
+      float d = dy[r * C + c];
+      if (!(act_y[r * C + c] > 0.f)) d *= slope;
+      a += d;
+      b += (double)d * ((x[r * C + c] - m) * is);
+    }
+  }
+  sh[threadIdx.y][threadIdx.x][0] = a;
+  sh[threadIdx.y][threadIdx.x][1] = b;
+  __syncthreads();
+  if (threadIdx.y == 0 && c < C) {
+    for (int k = 1; k < 8; ++k) {
+      a += sh[k][threadIdx.x][0];
+      b += sh[k][threadIdx.x][1];
+    }
+    part[(int64_t)blockIdx.y * 2 * C + c] = a;
+    part[(int64_t)blockIdx.y * 2 * C + C + c] = b;
+  }
+}
+__global__ void bn_bwd_reduce_lrelu_final(const double* __restrict__ part, int chunks, int64_t R, int C, double* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < 2 * C) {
+    double s = 0;
+    for (int k = 0; k < chunks; ++k) s += part[(int64_t)k * 2 * C + i];
+    out[i] = s;
+  }
+  if (i == 0) out[2 * C] = (double)R;
+}
 __global__ void bn_bwd_apply_kernel(const float* __restrict__ dy, const float* __restrict__ x, const float* __restrict__ mean,
                                     const float* __restrict__ invstd, const float* __restrict__ gamma,
                                     const double* __restrict__ sums /*[2C] global sums*/, double inv_count,
                                     float* __restrict__ dx, float* __restrict__ dgamma, float* __restrict__ dbeta,
-                                    const double* __restrict__ local_sums, int64_t total, int C) {
+                                    const double* __restrict__ local_sums, int64_t total, int C,
+                                    const float* __restrict__ act_y, float slope) {
   if (inv_count <= 0) inv_count = 1.0 / sums[2 * C];
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     int c = (int)(i % C);
     float xh = (x[i] - mean[c]) * invstd[c];
     float sd = (float)(sums[c] * inv_count), sdx = (float)(sums[C + c] * inv_count);
-    dx[i] = gamma[c] * invstd[c] * (dy[i] - sd - xh * sdx);
+    float d = dy[i];
+    if (act_y && !(act_y[i] > 0.f)) d *= slope;
+    dx[i] = gamma[c] * invstd[c] * (d - sd - xh * sdx);
     if (i < C && dgamma) {  // parameter grads are LOCAL sums (DDP all-reduces them like any other grad)
       dbeta[c] = (float)local_sums[c];
       dgamma[c] = (float)local_sums[C + c];
@@ -950,20 +995,46 @@ int mas_bn_invstd(const float* running_var, float eps, float* invstd, int C, voi
 }
 int mas_bn_apply(const float* x, const float* mean, const float* invstd, const float* gamma, const float* beta, float* y,
                  int64_t R, int C, void* stream) {
-  bn_apply_kernel<<<ew_grid(R * C), 256, 0, S(stream)>>>(x, mean, invstd, gamma, beta, y, R * C, C);
+  bn_apply_kernel<<<ew_grid(R * C), 256, 0, S(stream)>>>(x, mean, invstd, gamma, beta, y, R * C, C, 1.0f);
   return launched("bn_apply");
+}
+int mas_bn_apply_lrelu(const float* x, const float* mean, const float* invstd, const float* gamma, const float* beta, float slope,
+                       float* y, int64_t R, int C, void* stream) {
+  MAS_REQUIRE(R > 0 && C > 0, "bn_apply_lrelu: bad shape");
+  bn_apply_kernel<<<ew_grid(R * C), 256, 0, S(stream)>>>(x, mean, invstd, gamma, beta, y, R * C, C, slope);
+  return launched("bn_apply_lrelu");
 }
 int mas_bn_backward_reduce(const float* dy, const float* x, const float* mean, const float* invstd, int64_t R, int C,
                            double* sums_out, void* stream) {
   bn_bwd_reduce_kernel<<<(int)cdiv(C, 32), dim3(32, 8), 0, S(stream)>>>(dy, x, mean, invstd, R, C, sums_out);
   return launched("bn_bwd_reduce");
 }
+size_t mas_bn_backward_reduce_lrelu_ws_bytes(int64_t R, int C) { return (size_t)cdiv(R, BN_RB) * 2 * C * sizeof(double) + 64; }
+int mas_bn_backward_reduce_lrelu(const float* dy, const float* y, float slope, const float* x, const float* mean, const float* invstd,
+                                 int64_t R, int C, double* sums_out, void* ws, size_t ws_bytes, void* stream) {
+  MAS_REQUIRE(R > 0 && C > 0 && y, "bn_backward_reduce_lrelu: bad arguments");
+  if (!ws || ws_bytes < mas_bn_backward_reduce_lrelu_ws_bytes(R, C)) return fail(MAS_ERR_WORKSPACE, "bn_backward_reduce_lrelu: workspace too small");
+  const int chunks = (int)cdiv(R, BN_RB);
+  bn_bwd_reduce_lrelu_part<<<dim3((unsigned)cdiv(C, 32), (unsigned)chunks), dim3(32, 8), 0, S(stream)>>>(dy, y, slope, x, mean, invstd,
+                                                                                                           R, C, (double*)ws);
+  if (int e = launched("bn_bwd_reduce_lrelu_part")) return e;
+  bn_bwd_reduce_lrelu_final<<<(int)cdiv(2 * C, 128), 128, 0, S(stream)>>>((const double*)ws, chunks, R, C, sums_out);
+  return launched("bn_bwd_reduce_lrelu_final");
+}
 int mas_bn_backward_apply(const float* dy, const float* x, const float* mean, const float* invstd, const float* gamma,
                           const double* sums_global, const double* sums_local, double inv_count, float* dx, float* dgamma,
                           float* dbeta, int64_t R, int C, void* stream) {
   bn_bwd_apply_kernel<<<ew_grid(R * C), 256, 0, S(stream)>>>(dy, x, mean, invstd, gamma, sums_global, inv_count, dx, dgamma, dbeta,
-                                                             sums_local, R * C, C);
+                                                             sums_local, R * C, C, nullptr, 1.0f);
   return launched("bn_bwd_apply");
+}
+int mas_bn_backward_apply_lrelu(const float* dy, const float* y, float slope, const float* x, const float* mean, const float* invstd,
+                                const float* gamma, const double* sums, float* dx, float* dgamma, float* dbeta, int64_t R, int C,
+                                void* stream) {
+  MAS_REQUIRE(R > 0 && C > 0 && y, "bn_backward_apply_lrelu: bad arguments");
+  bn_bwd_apply_kernel<<<ew_grid(R * C), 256, 0, S(stream)>>>(dy, x, mean, invstd, gamma, sums, 0.0, dx, dgamma, dbeta, sums, R * C, C,
+                                                             y, slope);
+  return launched("bn_bwd_apply_lrelu");
 }
 
 size_t mas_colsum_ws_bytes(mas_tensor4 t) { return (size_t)cdiv(t.n * t.h * t.w, CS_ROWS) * t.c * sizeof(double) + 64; }

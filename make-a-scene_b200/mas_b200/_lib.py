@@ -92,6 +92,19 @@ _SPEC = {
     "mas_bn_apply": (_I, [_P, _P, _P, _P, _P, _P, _L, _I, _P]),
     "mas_bn_backward_reduce": (_I, [_P, _P, _P, _P, _L, _I, _P, _P]),
     "mas_bn_backward_apply": (_I, [_P, _P, _P, _P, _P, _P, _P, _D, _P, _P, _P, _L, _I, _P]),
+    "mas_pack_conv4x4": (_I, [_P, _P, _I, _I, _I, _P]),
+    "mas_conv4x4": (_I, [_P, _T, _P, _P, _P, _T, _I, _F, _I, _P]),
+    "mas_conv4x4_dgrad": (_I, [_P, _T, _P, _P, _T, _I, _P]),
+    "mas_conv4x4_wgrad_ws_bytes": (_Z, [_T, _T]),
+    "mas_conv4x4_wgrad": (_I, [_P, _T, _P, _T, _P, _I, _P, _Z, _P]),
+    "mas_lrelu_backward": (_I, [_P, _P, _F, _P, _L, _P]),
+    "mas_bn_apply_lrelu": (_I, [_P, _P, _P, _P, _P, _F, _P, _L, _I, _P]),
+    "mas_bn_backward_reduce_lrelu_ws_bytes": (_Z, [_L, _I]),
+    "mas_bn_backward_reduce_lrelu": (_I, [_P, _P, _F, _P, _P, _P, _L, _I, _P, _P, _Z, _P]),
+    "mas_conv4x4_shift_map": (_I, [_P, _T, _P, _I, _P]),
+    "mas_conv4x4_shift_map_adjoint": (_I, [_P, _P, _T, _I, _P]),
+    "mas_conv4x4_remap_weight": (_I, [_P, _P, _I, _I, _I, _I, _P]),
+    "mas_bn_backward_apply_lrelu": (_I, [_P, _P, _F, _P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _P]),
     "mas_vq_select_path": (_I, [_I]),
     "mas_vq_ws_bytes": (_Z, [_L, _I, _I]),
     "mas_vq_forward": (_I, [_P, _P, _L, _I, _I, _F, _P, _P, _P, _P, _Z, _P]),

@@ -954,6 +954,184 @@ def batchnorm_eval(x, weight, bias, running_mean, running_var, eps):
     return y
 
 
+# ------------------------------------------------------------------------------------------------ PatchGAN discriminator
+def _packed_conv4x4_weight(weight, transpose):
+    """mas_pack_conv4x4 image of a [Cout,Cin,4,4] weight, cached per parameter version (D's weights change only at its
+    optimizer step, so the three forwards and the backward passes of one training step share one packing)."""
+    ent = _pack_entry(weight)
+    key = ("c4", bool(transpose))
+    hit = ent.get(key)
+    if hit is not None and hit.device == weight.device:
+        return hit
+    cout, cin = weight.shape[:2]
+    wp = torch.empty(16 * cout * cin, dtype=torch.float32, device=weight.device)
+    L.call("mas_pack_conv4x4", weight.detach().contiguous(), wp, cout, cin, int(transpose))
+    ent[key] = wp
+    return wp
+
+
+def conv4x4_out_hw(h, w, stride):
+    return (h - 2) // stride + 1, (w - 2) // stride + 1
+
+
+def conv4x4_tc_route(x, cout, stride):
+    """True when the 4x4 convolution of dense-NHWC x runs as the 3x3 convolution of its shift map on the fp16 tensor-core
+    kernels (include/mas_b200.h, mas_conv4x4_shift_map): model.2 / 5 / 8 of the discriminator at 256^2."""
+    if not f16_operands() or not _is_dense_nhwc(x):
+        return False
+    n, cin, h, w = x.shape
+    if stride == 2 and (h % 2 or w % 2):
+        return False
+    hs, ws, c4 = h // stride, w // stride, 4 * cin
+    xs = L.Tensor4(n, hs, ws, c4, hs * ws * c4, ws * c4, c4, 1)
+    ys = L.Tensor4(n, hs, ws, cout, hs * ws * cout, ws * cout, cout, 1)
+    return cin % 4 == 0 and bool(L.query("mas_conv3x3_tc_eligible", xs, ys, L.CONV_S1))
+
+
+def _conv4x4_as_3x3(weight, stride):
+    """[Cout, 4*Cin, 3, 3] weight of the shift-map route, cached per parameter version (its own packings then stay cached)."""
+    ent = _pack_entry(weight)
+    key = ("c4to3", stride)
+    w3 = ent.get(key)
+    if w3 is None or w3.device != weight.device:
+        cout, cin = weight.shape[:2]
+        w3 = torch.empty((cout, 4 * cin, 3, 3), dtype=torch.float32, device=weight.device)
+        L.call("mas_conv4x4_remap_weight", weight.detach().contiguous(), w3, cout, cin, stride, 1)
+        ent[key] = w3
+    return w3
+
+
+class Conv4x4Fn(torch.autograd.Function):
+    """nn.Conv2d(cin, cout, 4, stride, 1) (losses/discriminator.py:21,27-28,34), optionally followed by LeakyReLU(slope)
+    (discriminator.py:21). x may have any strides (the first layer reads the caller's NCHW image); the output is dense NHWC.
+    The backward computes only what autograd asks for: no weight gradient while D is frozen (the generator step), no data
+    gradient for a leaf image (the discriminator step)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, stride, slope):
+        _need_cuda(x)
+        n, cin, h, w = x.shape
+        cout = weight.shape[0]
+        if tuple(weight.shape) != (cout, cin, 4, 4):
+            raise RuntimeError("Conv4x4Fn: weight %s does not match a 4x4 kernel over %d channels" % (tuple(weight.shape), cin))
+        ho, wo = conv4x4_out_hw(h, w, stride)
+        act = slope is not None
+        ctx.stride, ctx.slope, ctx.has_bias = int(stride), slope, bias is not None
+        ctx.tc = not act and conv4x4_tc_route(x, cout, stride)
+        if ctx.tc:
+            xm = empty_nhwc(n, 4 * cin, h // stride, w // stride, x)
+            L.call("mas_conv4x4_shift_map", x, L.t4(x), xm, int(stride))
+            y = conv3x3_raw(xm, _conv4x4_as_3x3(weight, stride), bias, None, L.CONV_S1)
+            if stride == 1:
+                y = y[:, :, :ho, :wo]          # the 3x3 output has one extra row and column
+            ctx.in_shape = x.shape
+            ctx.save_for_backward(xm, weight, None)
+            return y
+        y = empty_nhwc(n, cout, ho, wo, x)
+        L.call("mas_conv4x4", x, L.t4(x), _packed_conv4x4_weight(weight, False), bias, y, L.t4(y), int(stride),
+               float(slope) if act else 0.0, int(act))
+        ctx.save_for_backward(x, weight, y if act else None)
+        return y
+
+    @staticmethod
+    def _backward_tc(ctx, dy):
+        xm, weight, _ = ctx.saved_tensors
+        n, cin, h, w = ctx.in_shape
+        cout, s = weight.shape[0], ctx.stride
+        if s == 1:
+            # the dropped last row / column of the 3x3 output must carry a zero gradient
+            dyp = empty_nhwc(n, cout, h, w, dy).zero_()
+            inner = dyp[:, :, :h - 1, :w - 1]
+            L.call("mas_copy_strided", dy, L.t4(dy), inner, L.t4(inner))
+        else:
+            dyp = nhwc(dy)
+        w3 = _conv4x4_as_3x3(weight, s)
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dxm = conv3x3_raw(dyp, w3, None, None, L.CONV_S1, transpose=True)
+            dx = empty_nhwc(n, cin, h, w, dyp)
+            L.call("mas_conv4x4_shift_map_adjoint", dxm, dx, L.t4(dx), s)
+        if ctx.needs_input_grad[1] or (ctx.has_bias and ctx.needs_input_grad[2]):
+            dw3, db = conv3x3_wgrad_raw(xm, dyp, cout, 4 * cin, L.CONV_S1, want_bias=ctx.has_bias and ctx.needs_input_grad[2])
+            if ctx.needs_input_grad[1]:
+                dw = torch.empty_like(weight, memory_format=torch.contiguous_format)
+                L.call("mas_conv4x4_remap_weight", dw3, dw, cout, cin, s, 0)
+        return dx, dw, db, None, None
+
+    @staticmethod
+    def backward(ctx, dy):
+        _need_cuda(dy)
+        if ctx.tc:
+            return Conv4x4Fn._backward_tc(ctx, dy)
+        x, weight, y = ctx.saved_tensors
+        if ctx.slope is not None:
+            dy = nhwc(dy)
+            dz = torch.empty_like(y)
+            L.call("mas_lrelu_backward", dy, y, float(ctx.slope), dz, dz.numel())
+            dy = dz
+        dx = dw = db = None
+        if ctx.needs_input_grad[0]:
+            dx = empty_nhwc(*x.shape, like=x)
+            L.call("mas_conv4x4_dgrad", dy, L.t4(dy), _packed_conv4x4_weight(weight, True), dx, L.t4(dx), ctx.stride)
+        if ctx.needs_input_grad[1]:
+            dw = torch.empty_like(weight, memory_format=torch.contiguous_format)
+            nb = L.query("mas_conv4x4_wgrad_ws_bytes", L.t4(x), L.t4(dy))
+            ws = L.workspace(nb, x.device)
+            L.call("mas_conv4x4_wgrad", x, L.t4(x), dy, L.t4(dy), dw, ctx.stride, ws, ws.numel())
+        if ctx.has_bias and ctx.needs_input_grad[2]:
+            db = torch.empty(weight.shape[0], dtype=torch.float32, device=x.device)
+            ws = L.workspace(L.query("mas_colsum_ws_bytes", L.t4(dy)), x.device)
+            L.call("mas_colsum", dy, L.t4(dy), db, ws, ws.numel())
+        return dx, dw, db, None, None
+
+
+class BatchNormLReLUFn(torch.autograd.Function):
+    """nn.BatchNorm2d (training mode: statistics of this call's batch, running statistics updated) followed by
+    LeakyReLU(slope) (losses/discriminator.py:29-30); slope = 1 is the plain BatchNorm2d."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, running_mean, running_var, momentum, eps, slope):
+        x = nhwc(x)
+        n, c, h, w = x.shape
+        R = n * h * w
+        buf = torch.empty(2 * c + 1, dtype=torch.float64, device=x.device)
+        L.call("mas_bn_stats", x, R, c, buf)
+        mean = torch.empty(c, dtype=torch.float32, device=x.device)
+        invstd = torch.empty_like(mean)
+        L.call("mas_bn_finalize", buf, 0.0, c, float(eps), float(momentum), mean, invstd, running_mean, running_var)
+        y = torch.empty_like(x)
+        L.call("mas_bn_apply_lrelu", x, mean, invstd, weight, bias, float(slope), y, R, c)
+        ctx.slope = float(slope)
+        ctx.save_for_backward(x, weight, mean, invstd, y)
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        x, weight, mean, invstd, y = ctx.saved_tensors
+        dy = nhwc(dy)
+        n, c, h, w = x.shape
+        R = n * h * w
+        sums = torch.empty(2 * c + 1, dtype=torch.float64, device=x.device)
+        ws = L.workspace(L.query("mas_bn_backward_reduce_lrelu_ws_bytes", R, c), x.device)
+        L.call("mas_bn_backward_reduce_lrelu", dy, y, ctx.slope, x, mean, invstd, R, c, sums, ws, ws.numel())
+        dx = torch.empty_like(x)
+        dg = db = None
+        if ctx.needs_input_grad[1] or ctx.needs_input_grad[2]:
+            dg, db = torch.empty_like(weight), torch.empty_like(weight)
+        L.call("mas_bn_backward_apply_lrelu", dy, y, ctx.slope, x, mean, invstd, weight, sums, dx, dg, db, R, c)
+        return dx, dg, db, None, None, None, None, None
+
+
+def batchnorm_lrelu_eval(x, weight, bias, running_mean, running_var, eps, slope):
+    x = nhwc(x)
+    n, c, h, w = x.shape
+    invstd = torch.empty_like(running_var)
+    L.call("mas_bn_invstd", running_var, float(eps), invstd, c)
+    y = torch.empty_like(x)
+    L.call("mas_bn_apply_lrelu", x, running_mean, invstd, weight, bias, float(slope), y, n * h * w, c)
+    return y
+
+
 class VQFn(torch.autograd.Function):
     """Codebook distance+argmin+gather+loss+straight-through (modules.py:501-515) in one kernel."""
 
