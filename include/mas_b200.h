@@ -161,6 +161,16 @@ int mas_to_half(const float* x, void* y_f16, int64_t n, const float* amax, void*
 int mas_pack_conv3x3_phase16(const float* w_oihw, void* w_ph16, int Cout, int Cin, int mode, int transpose, void* stream);
 int mas_conv3x3_phase_tc16h(const void* x_f16, mas_tensor4 xs, const void* w_ph16, const float* bias, float* y,
                             mas_tensor4 ys, int mode, int transpose, const float* x_amax, void* stream);
+/* Weight (and bias) gradient of the same layer from two fp16 shadows, phase-decomposed on the TMA-fed weight-gradient
+ * kernel: x_f16 the layer input (xs), scaled by the power-of-two operand scale of *x_amax (NULL: unscaled); dy_f16 the output
+ * gradient (dys), scaled by that of *dy_amax.  The Upsample runs 16 per-phase 2 x 2 correlations of the low-resolution x
+ * and sums them into the nine taps in a fixed order; the Downsample runs each of the nine taps once over a phase plane of
+ * x.  dw_oihw [Cout][Cin][3][3] and dbias [Cout] (or NULL) are overwritten; deterministic (no atomics).  ws: at least
+ * mas_conv3x3_phase_wgrad_tc16_ws_bytes(xs, dys, mode) bytes (0: the shape is not eligible, see MAS_CONV_UP_PHASE). */
+size_t mas_conv3x3_phase_wgrad_tc16_ws_bytes(mas_tensor4 xs, mas_tensor4 dys, int mode);
+int mas_conv3x3_phase_wgrad_tc16(const void* x_f16, mas_tensor4 xs, const float* x_amax, const void* dy_f16,
+                                 mas_tensor4 dys, const float* dy_amax, float* dw_oihw, float* dbias, int mode, void* ws,
+                                 size_t ws_bytes, void* stream);
 /* Both packings of one weight (transpose = 0 and 1 of mas_pack_conv3x3_tc) in a single pass; Cout % 128 == Cin % 128 == 0. */
 int mas_pack_conv3x3_tc_pair(const float* w_oihw, float* w_tc_fwd, float* w_tc_dgrad, int Cout, int Cin, void* stream);
 int mas_gn_finalize_partials(const float* part, int tiles_per_image, int N, int C, int G, int64_t hw, float eps,

@@ -298,6 +298,17 @@ constexpr size_t t16_smem_bytes() {
 //   * split-K over the units; partial sums go to the caller's workspace in the layout conv_wgrad_reduce expects. The bias
 //     gradient comes from the same A fragments (fp32 sums per thread, reduced over the four lanes of a row) in the CTAs of
 //     kernel row 0 / ci block 0, so the bias adds no shared-memory pass and no CTA does more than the others.
+//
+// Phase forms (PH != 0) of the resampling convolutions' weight gradients: a CTA owns one (tap group g = 2 py + px, kernel
+// row a) of the block and keeps TWO accumulators (horizontal taps b = 0, 1), so each dy^T fragment feeds two MMAs:
+//   * PH 1, Upsample (dy the 2x side): unit = 8 x 8 low-resolution pixels of dy's phase plane g, read through a 5-D tensor
+//     map with doubled pixel / row strides; the x halo is the low-resolution shadow from row py - 1 + a, column px - 1. The
+//     16 partial taps (g, a, b) are phase_table(up, forward) sums of the nine: conv_wgrad_fold16 adds each into its taps;
+//   * PH 2, Downsample (x the 2x side): the x halo is phase plane g of x (the same 5-D map, out-of-image zero fill = the
+//     (0, 1, 0, 1) pad) from row a, column 0, and partial tap (g, a, b) IS weight tap (py + 2 a, px + 2 b): only the six
+//     (g, a) with py + 2 a <= 2 are launched and b = 1 of the odd-px planes (tx = 3) is not stored, so every one of the
+//     nine taps has exactly one producer and the partials keep conv_wgrad_reduce's nine-tap layout;
+//   * x is a SCALED shadow there (x_amax): the epilogue multiplies by both inverse power-of-two scales.
 constexpr int WT_STAGES = 5;
 constexpr int WT_XATOM = 8 * 10 * 128;      // one 64-channel halo box: 8 halo rows x 10 pixels x 128 B
 constexpr int WT_DYATOM = 64 * 128;         // 64 pixels x 64 co halves
@@ -312,13 +323,20 @@ constexpr size_t wt_smem_bytes() { return 1024 + (size_t)WT_STAGES * wt_stage<NC
 static inline int wt_nci(int64_t cin) { return cin % 128 == 0 ? 128 : 64; }
 
 struct WTParams {
-  float* part;      // [splits][9][Cout][Cin]
-  float* bpart;     // [splits][Cout] or null
+  float* part;      // [splits][9][Cout][Cin] (PH 1: [splits][16][Cout][Cin])
+  float* bpart;     // [splits][Cout] (PH 1: [splits][4 phases][Cout]) or null
   int N, H, W, Cin, Cout;
   int units_x, units_y;
   int64_t total_units, units_per_split;
   const float* dy_amax;   // the magnitude dy16's power-of-two scale was derived from
+  const float* x_amax;    // ... and x16's (null: unscaled shadow)
 };
+
+// CTA rows per (ci, co) block: kernel rows (PH 0), (tap group, kernel row) pairs (PH 1: 4 x 2; PH 2: the six that hold a tap)
+template <int PH>
+__host__ __device__ constexpr int wt_rows() { return PH == 0 ? 3 : PH == 1 ? 8 : 6; }
+template <int PH>
+__host__ __device__ constexpr int wt_ntap() { return PH == 1 ? 16 : 9; }
 
 template <int NCI>
 __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t bdesc) {
@@ -326,12 +344,14 @@ __device__ __forceinline__ void wgmma_rs(float* d, const uint32_t* a, uint64_t b
   else wg::wgmma_f16_rs_n64<1>(d, a, bdesc, 1u);
 }
 
-template <int NCI>
+template <int NCI, int PH = 0>
 __global__ void __launch_bounds__(WT_THREADS, 1) wgrad_t16(const WTParams p, const __grid_constant__ CUtensorMap x_map,
                                                           const __grid_constant__ CUtensorMap dy_map) {
   constexpr int XBOX = NCI / 64;               // 64-channel halo boxes per stage
   constexpr int STAGE = wt_stage<NCI>();
   constexpr int NR = NCI / 2;                  // accumulator registers per tap
+  constexpr int NT = PH == 0 ? 3 : 2;          // horizontal taps per CTA
+  constexpr int ROWS = wt_rows<PH>();
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
   const uint32_t smem_base = (raw_base + 1023u) & ~1023u;
@@ -342,7 +362,10 @@ __global__ void __launch_bounds__(WT_THREADS, 1) wgrad_t16(const WTParams p, con
   auto empty = [&](int s) { return bar_base + 8u * (WT_STAGES + s); };        // the MMAs of the stage have completed
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int dyy = blockIdx.x % 3, ci0 = (blockIdx.x / 3) * NCI, co0 = blockIdx.y * BM, split = blockIdx.z;
+  const int row = blockIdx.x % ROWS, ci0 = (blockIdx.x / ROWS) * NCI, co0 = blockIdx.y * BM, split = blockIdx.z;
+  // tap group (phase forms) and kernel row of the CTA; PH 2 rows 0-3: groups 0 / 1 with a = 0, 1, rows 4 / 5: groups 2 / 3
+  const int grp = PH == 1 ? row >> 1 : PH == 2 ? (row < 4 ? row >> 1 : row - 2) : 0;
+  const int ka = PH == 0 ? row : PH == 1 ? row & 1 : (row < 4 ? row & 1 : 0);
   const int64_t u0 = (int64_t)split * p.units_per_split;
   const int64_t u1 = min(p.total_units, u0 + p.units_per_split);
 
@@ -356,13 +379,16 @@ __global__ void __launch_bounds__(WT_THREADS, 1) wgrad_t16(const WTParams p, con
     // ============ MMA warpgroups, then epilogue ============
     wg::regs_inc<wg::MMA_REGS>();
     const int wgi = warp >> 2;
-    float a_inv;
+    float a_inv, x_inv;
     operand_scale(p.dy_amax, &a_inv);
-    const bool want_bias = p.bpart != nullptr && blockIdx.x == 0;
+    operand_scale(p.x_amax, &x_inv);
+    const float w_inv = a_inv * x_inv;          // both powers of two: exact
+    // the bias sums dy over one CTA row per ci block 0 (PH 1: one per phase plane of dy)
+    const bool want_bias = p.bpart != nullptr && blockIdx.x < ROWS && ka == 0 && (PH == 1 || grp == 0);
     float bsum[2] = {0.f, 0.f};                // co rows lane / 4 and lane / 4 + 8 of the warp
-    float acc[3][NR];
+    float acc[NT][NR];
 #pragma unroll
-    for (int dx = 0; dx < 3; ++dx)
+    for (int dx = 0; dx < NT; ++dx)
 #pragma unroll
       for (int i = 0; i < NR; ++i) acc[dx][i] = 0.f;
     // ldmatrix.x4.trans: lane l addresses pixel 8 (l / 16) + l % 8 of the K step, co chunk 2 (warp % 4) + (l / 8) % 2 of the
@@ -395,7 +421,7 @@ __global__ void __launch_bounds__(WT_THREADS, 1) wgrad_t16(const WTParams p, con
         }
         wg::fence();
 #pragma unroll
-        for (int dx = 0; dx < 3; ++dx) wgmma_rs<NCI>(acc[dx], af, xd0 + (uint64_t)((s * 2 * 1280 + dx * 128) >> 4));
+        for (int dx = 0; dx < NT; ++dx) wgmma_rs<NCI>(acc[dx], af, xd0 + (uint64_t)((s * 2 * 1280 + dx * 128) >> 4));
         wg::commit();
       }
       prev = stage;
@@ -403,24 +429,31 @@ __global__ void __launch_bounds__(WT_THREADS, 1) wgrad_t16(const WTParams p, con
     }
     wg::wait<0>();
 #pragma unroll
-    for (int dx = 0; dx < 3; ++dx) wg::fence_regs<NR>(acc[dx]);
+    for (int dx = 0; dx < NT; ++dx) wg::fence_regs<NR>(acc[dx]);
     const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
     if (want_bias) {
+      const size_t bslot = PH == 1 ? (size_t)split * 4 + grp : (size_t)split;
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         bsum[i] += __shfl_xor_sync(0xffffffffu, bsum[i], 1);
         bsum[i] += __shfl_xor_sync(0xffffffffu, bsum[i], 2);
-        if ((lane & 3) == 0) p.bpart[(size_t)split * p.Cout + co0 + frow + 8 * i] = bsum[i] * a_inv;
+        if ((lane & 3) == 0) p.bpart[bslot * p.Cout + co0 + frow + 8 * i] = bsum[i] * a_inv;
       }
     }
 #pragma unroll
-    for (int dx = 0; dx < 3; ++dx) {
+    for (int dx = 0; dx < NT; ++dx) {
+      int tap = row * NT + dx;                  // PH 0: ty * 3 + tx; PH 1: partial tap (g, a, b)
+      if (PH == 2) {
+        const int tx = (grp & 1) + 2 * dx;
+        if (tx > 2) continue;                   // tap 3 of an odd-px plane: outside the 3x3 kernel
+        tap = ((grp >> 1) + 2 * ka) * 3 + tx;
+      }
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
-        float* o = p.part + (((size_t)split * 9 + dyy * 3 + dx) * p.Cout + co0 + frow + 8 * i) * p.Cin + ci0 + fcol;
+        float* o = p.part + (((size_t)split * wt_ntap<PH>() + tap) * p.Cout + co0 + frow + 8 * i) * p.Cin + ci0 + fcol;
 #pragma unroll
         for (int j = 0; j < NCI / 8; ++j)
-          *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[dx][4 * j + 2 * i] * a_inv, acc[dx][4 * j + 2 * i + 1] * a_inv);
+          *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[dx][4 * j + 2 * i] * w_inv, acc[dx][4 * j + 2 * i + 1] * w_inv);
       }
     }
   } else {
@@ -435,12 +468,23 @@ __global__ void __launch_bounds__(WT_THREADS, 1) wgrad_t16(const WTParams p, con
         const uint32_t dst = smem_base + (uint32_t)stage * STAGE;
         mbar_wait(empty(stage), phase ^ 1);
         mbar_expect_tx(fullD(stage), STAGE);
+        const int py = grp >> 1, px = grp & 1;
 #pragma unroll
-        for (int b = 0; b < XBOX; ++b)
-          tma_load_4d(dst + (uint32_t)(b * WT_XATOM), &x_map, ci0 + b * 64, ux * 8 - 1, uy * 8 + dyy - 1, n, fullD(stage));
+        for (int b = 0; b < XBOX; ++b) {
+          if (PH == 2)   // phase plane (py, px) of the 2x x: channel half px of the pixel pair, row parity py
+            tma_load_5d(dst + (uint32_t)(b * WT_XATOM), &x_map, px * p.Cin + ci0 + b * 64, ux * 8, py, uy * 8 + ka, n, fullD(stage));
+          else
+            tma_load_4d(dst + (uint32_t)(b * WT_XATOM), &x_map, ci0 + b * 64, ux * 8 + (PH == 1 ? px : 0) - 1,
+                        uy * 8 + (PH == 1 ? py : 0) + ka - 1, n, fullD(stage));
+        }
 #pragma unroll
-        for (int hf = 0; hf < 2; ++hf)
-          tma_load_4d(dst + (uint32_t)(XBOX * WT_XATOM + hf * WT_DYATOM), &dy_map, co0 + hf * 64, ux * 8, uy * 8, n, fullD(stage));
+        for (int hf = 0; hf < 2; ++hf) {
+          const uint32_t ddst = dst + (uint32_t)(XBOX * WT_XATOM + hf * WT_DYATOM);
+          if (PH == 1)   // phase plane (py, px) of the 2x dy
+            tma_load_5d(ddst, &dy_map, px * p.Cout + co0 + hf * 64, ux * 8, py, uy * 8, n, fullD(stage));
+          else
+            tma_load_4d(ddst, &dy_map, co0 + hf * 64, ux * 8, uy * 8, n, fullD(stage));
+        }
         if (++stage == WT_STAGES) { stage = 0; phase ^= 1; }
       }
     }
@@ -488,6 +532,39 @@ __global__ void pack_phase16(const float* __restrict__ w, __half* __restrict__ o
     for (int t = 0; t < 9; ++t)
       if ((tb.mask[g][j] >> t) & 1) s += src[t];
     out[i] = __float2half_rn(s);
+  }
+}
+
+// Upsample weight gradient from the 16 partial taps k = 4 g + j of wgrad_t16<., 1>: dw[co][ci][t] = the sum over the k whose
+// tap set tb.mask[g][j] holds t of sum_split part[split][k][co][ci], splits first, then k in ascending order - a fixed order,
+// so the result does not change from run to run. dbias sums the [split][phase] bias partials in index order.
+__global__ void conv_wgrad_fold16(const float* __restrict__ part, const float* __restrict__ bpart, int splits, int Cout, int Cin,
+                             PhaseTable tb, float* __restrict__ dw, float* __restrict__ dbias) {
+  if (bpart)
+    for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < Cout; c += gridDim.x * blockDim.x) {
+      float a = 0.f;
+      for (int s = 0; s < 4 * splits; ++s) a += bpart[(size_t)s * Cout + c];
+      dbias[c] = a;
+    }
+  const int64_t cc = (int64_t)Cout * Cin;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cc; i += (int64_t)gridDim.x * blockDim.x) {
+    float a[16], o[9];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) a[k] = 0.f;
+    for (int s = 0; s < splits; ++s)
+#pragma unroll
+      for (int k = 0; k < 16; ++k) a[k] += part[((size_t)s * 16 + k) * cc + i];
+#pragma unroll
+    for (int t = 0; t < 9; ++t) o[t] = 0.f;
+#pragma unroll
+    for (int k = 0; k < 16; ++k) {
+      const int m = tb.mask[k >> 2][k & 3];
+#pragma unroll
+      for (int t = 0; t < 9; ++t)
+        if ((m >> t) & 1) o[t] += a[k];
+    }
+#pragma unroll
+    for (int t = 0; t < 9; ++t) dw[i * 9 + t] = o[t];
   }
 }
 
@@ -714,6 +791,7 @@ int conv_wgrad_t16_launch(const void* x16, mas_tensor4 xs, const void* dy16, mas
   p.units_x = (int)(dys.w / 8); p.units_y = (int)(dys.h / 8);
   p.total_units = (int64_t)p.N * p.units_x * p.units_y;
   p.dy_amax = dy_amax;
+  p.x_amax = nullptr;
   const int nci = tc::wt_nci(p.Cin);
   const int splits = wt_splits((int64_t)(p.Cout / tc::BM) * (p.Cin / nci) * 3, p.total_units);
   p.units_per_split = cdiv(p.total_units, splits);
@@ -755,6 +833,88 @@ int conv_wgrad_t16_launch(const void* x16, mas_tensor4 xs, const void* dy16, mas
   return launched("conv_wgrad_reduce");
 }
 
+// Phase-decomposed weight gradient of the Upsample / Downsample convolution; xs / dys: the layer's input and output-gradient
+// shapes. Splits as for wgrad_t16, with wt_rows<PH> CTA rows per 128 x 128 channel block.
+static int phase_wgrad_splits(mas_tensor4 xs, mas_tensor4 dys, bool up) {
+  const mas_tensor4& lo = up ? xs : dys;
+  return wt_splits((dys.c / tc::BM) * (xs.c / 128) * (up ? tc::wt_rows<1>() : tc::wt_rows<2>()), lo.n * (lo.h / 8) * (lo.w / 8));
+}
+size_t conv_phase_wgrad_t16_ws(mas_tensor4 xs, mas_tensor4 dys, bool up) {
+  if (!conv3x3_phase_ok(xs, dys, up)) return 0;
+  const size_t splits = phase_wgrad_splits(xs, dys, up);
+  return splits * (up ? 16 : 9) * (size_t)dys.c * xs.c * sizeof(float) + splits * (up ? 4 : 1) * (size_t)dys.c * sizeof(float) + 256;
+}
+
+// fp16 NHWC map with a box of `rows` x `cols` pixels x 64 channels under the 128-byte swizzle: of the tensor itself (4-D), or
+// of its four phase planes (planes: 5-D [n][row pair][row parity][pixel pair][px * C + c], box row parity 1)
+static CUresult encode_f16_map(CUtensorMap* map, const void* t16, const mas_tensor4& s, bool planes, cuuint32_t cols, cuuint32_t rows) {
+  PFN_cuTensorMapEncodeTiled enc = tensor_map_encoder();
+  if (!enc) return CUDA_ERROR_NOT_FOUND;
+  if (planes) {
+    cuuint64_t dims[5] = {(cuuint64_t)s.c * 2, (cuuint64_t)s.w / 2, 2, (cuuint64_t)s.h / 2, (cuuint64_t)s.n};
+    cuuint64_t strides[4] = {(cuuint64_t)s.c * 4, (cuuint64_t)s.w * s.c * 2, (cuuint64_t)s.w * s.c * 4, (cuuint64_t)s.h * s.w * s.c * 2};
+    cuuint32_t box[5] = {64, cols, 1, rows, 1}, es[5] = {1, 1, 1, 1, 1};
+    return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(t16), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+               CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  }
+  cuuint64_t dims[4] = {(cuuint64_t)s.c, (cuuint64_t)s.w, (cuuint64_t)s.h, (cuuint64_t)s.n};
+  cuuint64_t strides[3] = {(cuuint64_t)s.c * 2, (cuuint64_t)s.w * s.c * 2, (cuuint64_t)s.h * s.w * s.c * 2};
+  cuuint32_t box[4] = {64, cols, rows, 1}, es[4] = {1, 1, 1, 1};
+  return enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(t16), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
+// x16: fp16 shadow of the layer input, scaled by operand_scale(*x_amax) (null: unscaled); dy16: fp16 shadow of the output
+// gradient, scaled by operand_scale(*dy_amax); dw [Cout][Cin][3][3], dbias [Cout] or null.
+int conv_phase_wgrad_t16_launch(const void* x16, mas_tensor4 xs, const float* x_amax, const void* dy16, mas_tensor4 dys,
+                                const float* dy_amax, float* dw, float* dbias, bool up, void* ws, size_t ws_bytes, cudaStream_t st) {
+  if (!conv3x3_phase_ok(xs, dys, up))
+    return fail(MAS_ERR_UNSUPPORTED, "phase wgrad: shape/layout not eligible (Cin=%lld Cout=%lld H=%lld W=%lld)", (long long)xs.c,
+                (long long)dys.c, (long long)xs.h, (long long)xs.w);
+  if (ws_bytes < conv_phase_wgrad_t16_ws(xs, dys, up)) return fail(MAS_ERR_WORKSPACE, "phase wgrad: workspace too small");
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  if (!al16(x16) || !al16(dy16) || !al16(ws)) return fail(MAS_ERR_INVALID_ARG, "phase wgrad: pointers must be 16-byte aligned");
+  const mas_tensor4& lo = up ? xs : dys;
+  tc::WTParams p;
+  p.N = (int)xs.n; p.H = (int)lo.h; p.W = (int)lo.w; p.Cin = (int)xs.c; p.Cout = (int)dys.c;
+  p.units_x = (int)(lo.w / 8); p.units_y = (int)(lo.h / 8);
+  p.total_units = (int64_t)p.N * p.units_x * p.units_y;
+  p.dy_amax = dy_amax;
+  p.x_amax = x_amax;
+  const int splits = phase_wgrad_splits(xs, dys, up);
+  const int ntap = up ? 16 : 9;
+  p.units_per_split = cdiv(p.total_units, splits);
+  p.part = (float*)ws;
+  p.bpart = dbias ? (float*)ws + (size_t)splits * ntap * p.Cout * p.Cin : nullptr;
+
+  // Upsample: the x halo from the low-resolution input, dy by phase plane; Downsample: x by phase plane, dy dense
+  CUtensorMap xmap, dmap;
+  CUresult r = encode_f16_map(&xmap, x16, xs, !up, 10, 8);
+  if (r == CUDA_SUCCESS) r = encode_f16_map(&dmap, dy16, dys, up, 8, 8);
+  if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (phase wgrad maps) failed (%d)", (int)r);
+  static std::atomic<uint64_t> configured{0};
+  if (first_on_device(configured)) {
+    cudaError_t e = cudaFuncSetAttribute(tc::wgrad_t16<128, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::wt_smem_bytes<128>());
+    if (e == cudaSuccess)
+      e = cudaFuncSetAttribute(tc::wgrad_t16<128, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)tc::wt_smem_bytes<128>());
+    if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(wgrad_t16 phase): %s", cudaGetErrorString(e));
+    mark_device(configured);
+  }
+  const int rows = up ? tc::wt_rows<1>() : tc::wt_rows<2>();
+  dim3 grid((unsigned)((p.Cin / 128) * rows), (unsigned)(p.Cout / tc::BM), (unsigned)splits);
+  if (up) tc::wgrad_t16<128, 1><<<grid, tc::WT_THREADS, tc::wt_smem_bytes<128>(), st>>>(p, xmap, dmap);
+  else tc::wgrad_t16<128, 2><<<grid, tc::WT_THREADS, tc::wt_smem_bytes<128>(), st>>>(p, xmap, dmap);
+  if (int e = launched_tc(up ? "wgrad_t16<128, up-phase>" : "wgrad_t16<128, down-phase>")) return e;
+  if (!up) {
+    conv_wgrad_reduce_launch((const float*)ws, splits, 9, p.Cout, p.Cin, dw, p.bpart, dbias, st);
+    return launched("conv_wgrad_reduce");
+  }
+  const int64_t blocks = cdiv((int64_t)p.Cout * p.Cin, 256);
+  tc::conv_wgrad_fold16<<<(unsigned)(blocks < 1184 ? blocks : 1184), 256, 0, st>>>((const float*)ws, p.bpart, splits, p.Cout, p.Cin,
+                                                                                 phase_table(true, false), dw, dbias);
+  return launched("conv_wgrad_fold16");
+}
+
 int to_half_launch(const float* x, void* y, int64_t n, const float* amax, cudaStream_t st) {
   if (n % 4 || (reinterpret_cast<uintptr_t>(x) & 15) || (reinterpret_cast<uintptr_t>(y) & 7))
     return fail(MAS_ERR_INVALID_ARG, "to_half: n %% 4 == 0 and aligned pointers required");
@@ -794,6 +954,19 @@ int mas_conv3x3_phase_tc16h(const void* x_f16, mas_tensor4 xs, const void* w_ph1
   MAS_REQUIRE(mode == MAS_CONV_UP_PHASE || mode == MAS_CONV_S2_PHASE, "conv3x3_phase_tc16h: mode %d", mode);
   return mas::conv3x3_phase_tma16_launch(x_f16, xs, w_ph16, bias, y, ys, mode == MAS_CONV_UP_PHASE, transpose != 0, x_amax,
                                          mas::S(stream));
+}
+
+size_t mas_conv3x3_phase_wgrad_tc16_ws_bytes(mas_tensor4 xs, mas_tensor4 dys, int mode) {
+  if (mode != MAS_CONV_UP_PHASE && mode != MAS_CONV_S2_PHASE) return 0;
+  return mas::conv_phase_wgrad_t16_ws(xs, dys, mode == MAS_CONV_UP_PHASE);
+}
+
+int mas_conv3x3_phase_wgrad_tc16(const void* x_f16, mas_tensor4 xs, const float* x_amax, const void* dy_f16, mas_tensor4 dys,
+                                 const float* dy_amax, float* dw_oihw, float* dbias, int mode, void* ws, size_t ws_bytes, void* stream) {
+  MAS_REQUIRE(x_f16 && dy_f16 && dw_oihw && ws, "conv3x3_phase_wgrad_tc16: null pointer");
+  MAS_REQUIRE(mode == MAS_CONV_UP_PHASE || mode == MAS_CONV_S2_PHASE, "conv3x3_phase_wgrad_tc16: mode %d", mode);
+  return mas::conv_phase_wgrad_t16_launch(x_f16, xs, x_amax, dy_f16, dys, dy_amax, dw_oihw, dbias, mode == MAS_CONV_UP_PHASE, ws,
+                                          ws_bytes, mas::S(stream));
 }
 
 }  // extern "C"

@@ -59,6 +59,8 @@ _SPEC = {
     "mas_to_half": (_I, [_P, _P, _L, _P, _P]),
     "mas_pack_conv3x3_phase16": (_I, [_P, _P, _I, _I, _I, _I, _P]),
     "mas_conv3x3_phase_tc16h": (_I, [_P, _T, _P, _P, _P, _T, _I, _I, _P, _P]),
+    "mas_conv3x3_phase_wgrad_tc16_ws_bytes": (_Z, [_T, _T, _I]),
+    "mas_conv3x3_phase_wgrad_tc16": (_I, [_P, _T, _P, _P, _T, _P, _P, _P, _I, _P, _Z, _P]),
     "mas_gn_finalize_partials": (_I, [_P, _I, _I, _I, _I, _L, _F, _P, _P, _P]),
     "mas_gn_table": (_I, [_P, _P, _P, _P, _I, _I, _I, _P, _P]),
     "mas_pack_gemm_tc": (_I, [_P, _P, _I, _I, _I, _P]),

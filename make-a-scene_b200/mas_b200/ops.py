@@ -322,7 +322,7 @@ def _packed_conv_weight(wc, weight, cout, cin, transpose, dev, prepack=False, f1
 
 def phase_mode(x, cout, mode):
     """CONV_UP_PHASE / CONV_S2_PHASE when the Upsample / Downsample convolution of dense-NHWC x runs phase-decomposed on the
-    TMA-fed kernel (forward and data gradient), else None. MAS_CONV_PHASE=0 keeps the register-staged route for A/B runs."""
+    TMA-fed kernels (forward, data and weight gradient), else None. MAS_CONV_PHASE=0 keeps the register-staged route for A/B runs."""
     if mode not in (L.CONV_UP, L.CONV_S2) or not conv_tma_on() or os.environ.get("MAS_CONV_PHASE", "1") == "0":
         return None
     if not _is_dense_nhwc(x):
@@ -350,6 +350,17 @@ def conv3x3_phase_raw(x16, weight, bias, pmode, transpose=False, x_amax=None):
         ent[key] = wt
     L.call("mas_conv3x3_phase_tc16h", x16, L.t4(x16), wt, bias, y, L.t4(y), pmode, int(transpose), x_amax)
     return y
+
+
+def conv3x3_phase_wgrad_raw(x16, x_amax, dy16, dy_amax, pmode, want_bias=True):
+    """Weight (and bias) gradient of a phase-decomposed Upsample / Downsample convolution from the fp16 shadows of its input
+    and output gradient, each scaled by the power-of-two operand scale of its device scalar (None: unscaled)."""
+    cout, cin = dy16.shape[1], x16.shape[1]
+    dw = torch.empty((cout, cin, 3, 3), dtype=torch.float32, device=x16.device)
+    db = torch.empty(cout, dtype=torch.float32, device=x16.device) if want_bias else None
+    ws = L.workspace(L.query("mas_conv3x3_phase_wgrad_tc16_ws_bytes", L.t4(x16), L.t4(dy16), pmode), x16.device)
+    L.call("mas_conv3x3_phase_wgrad_tc16", x16, L.t4(x16), x_amax, dy16, L.t4(dy16), dy_amax, dw, db, pmode, ws, ws.numel())
+    return dw, db
 
 
 def conv3x3_wgrad_raw(x, dy, cout, cin, mode, want_bias=True, table=None, silu=True, dy_amax=None):
@@ -588,11 +599,16 @@ class Conv3x3Fn(torch.autograd.Function):
         elif residual is None and not out_nchw and phase_mode(x, cout, mode) is not None:
             # Upsample / Downsample as four small convolutions over phase planes read straight from an fp16 shadow of x
             edge = 6
+            ctx.pmode = phase_mode(x, cout, mode)
             am = amax_of(x)
-            y = conv3x3_phase_raw(to_half(x, am), weight, bias, phase_mode(x, cout, mode), x_amax=am)
+            x16 = to_half(x, am)
+            y = conv3x3_phase_raw(x16, weight, bias, ctx.pmode, x_amax=am)
             if mode == L.CONV_UP:
                 # a following ResnetBlock without shortcut writes its input gradient's fp16 shadow: the data gradient here reads it
                 y._mas_res_out = True
+            # the weight gradient reads the shadow and nothing else in the backward reads x: keep half the bytes, or none
+            want_w = ctx.needs_input_grad[1] or (bias is not None and ctx.needs_input_grad[2])
+            x, ctx.x_amax = (x16, am) if want_w else (None, None)
         elif (mode == L.CONV_S2 and _tc_on() and residual is None and not out_nchw and _is_dense_nhwc(x) and cin % 8 == 0
               and cout % 128 == 0 and h % 32 == 0 and w % 16 == 0):
             edge = 3  # stride-2 conv on the stride-1 tensor kernels through space-to-depth
@@ -660,23 +676,16 @@ class Conv3x3Fn(torch.autograd.Function):
                 dwk, dbk = conv3x3_wgrad_raw(x, full, ck, cin, L.CONV_S1, True, dy_amax=am)
                 dw, db = dwk[:cout].contiguous(), dbk[:cout].contiguous()
         elif ctx.edge == 6:
+            # x is the input's fp16 shadow here (None when no weight gradient was asked for); both gradients read one dy shadow
             dy = nhwc(dy)
-            am = amax_of(dy)
+            sh = shadow_of(dy)
+            if sh is None:
+                am = amax_of(dy)
+                sh = (to_half(dy, am), am)
             if ctx.needs_input_grad[0]:
-                sh = shadow_of(dy)
-                if sh is None:
-                    sh = (to_half(dy, am), am)
-                dx = conv3x3_phase_raw(sh[0], weight, None, phase_mode(x, cout, ctx.mode), transpose=True, x_amax=sh[1])
+                dx = conv3x3_phase_raw(sh[0], weight, None, ctx.pmode, transpose=True, x_amax=sh[1])
             if want_w:
-                if ctx.mode == L.CONV_UP:
-                    dw, db = conv3x3_wgrad_raw(x, dy, cout, cin, ctx.mode, ctx.has_bias, dy_amax=am)
-                else:   # the register-staged weight gradient over the space-to-depth map
-                    n, _, h, w = x.shape
-                    x4 = empty_nhwc(n, 4 * cin, h // 2, w // 2, x)
-                    L.call("mas_space_to_depth", x, x4, n, h, w, cin)
-                    dw9, db = conv3x3_wgrad_raw(x4, dy, cout, 4 * cin, L.CONV_S1, ctx.has_bias, dy_amax=am)
-                    dw = torch.empty_like(weight)
-                    L.call("mas_s2d_unpack_wgrad", dw9, dw, cout, cin)
+                dw, db = conv3x3_phase_wgrad_raw(x, ctx.x_amax, sh[0], sh[1], ctx.pmode, ctx.has_bias)
         elif ctx.edge == 3:
             if ctx.needs_input_grad[0]:
                 dx = conv3x3_dgrad_raw(nhwc(dy), weight, ctx.mode)       # zero-stuffed map on the tensor kernel

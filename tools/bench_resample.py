@@ -1,7 +1,9 @@
 """Upsample / Downsample convolutions of the VQ-IMG model (bench.IMG_CFG) at batch 32, 256x256: times the forward, data
 gradient and weight gradient of every such layer through ops.Conv3x3Fn exactly as the model launches them (shadow
 conversions, weight packing, space-to-depth, sum-pool, unpack helpers included), once per route: MAS_CONV_PHASE=0 (the
-register-staged kernels over the nearest-x2 / space-to-depth maps) and MAS_CONV_PHASE=1 (phase-decomposed, TMA-fed fp16).
+register-staged kernels over the nearest-x2 / space-to-depth maps) and MAS_CONV_PHASE=1 (phase-decomposed, TMA-fed fp16:
+shift_gemm_t16 for the forward and data gradient, wgrad_t16 + conv_wgrad_fold16 / conv_wgrad_reduce for the weight gradient).
+The dy passed to the backward has no fp16 shadow here, so both backward passes include its amax and fp16 conversion.
 TFLOP/s are against the REFERENCE FLOP count of the layer, 2 * N * Hout * Wout * C * C * 9 per pass (what nn.Conv2d does
 on the upsampled / padded map), not against what either route executes. Layer shapes come from a batch-1 forward of the
 model with hooks on its Upsample / Downsample modules.
