@@ -497,6 +497,42 @@ int mas_bce_cl_forward(const float* logits, const float* target_nchw, const floa
 int mas_bce_cl_backward(const float* logits, const float* target_nchw, const float* pos_weight, const float* g, int N, int C,
                         int CP, int H, int W, float* grad, void* stream);
 
+
+/* ---- LPIPS perceptual loss (losses/lpips.py; csrc/lpips.cu) ------------------------------------------------------------
+ * The thirteen VGG16 3x3 convolutions (lpips.py:106-111, torchvision vgg16 features[0:30]) run on the 3x3 family above
+ * (mas_conv3x3_fprop_tc16 / mas_conv3x3_fprop, mas_edge_small_cin_fprop / mas_edge_small_cout_fprop for conv1_1); these
+ * entries are the rest of LPIPS.forward (lpips.py:66-73) and its data gradient.  Activations are channels-last fp32 over
+ * ONE batch of 2B images, real first then fake.
+ * mas_lpips_prep: ScalingLayer (lpips.py:81-82), (x - shift) / scale of NCHW real and fake [B,3,H,W] -> out [2B,H,W,3].
+ * mas_lpips_relu: nn.ReLU (features 1, 3, 6, ...) in place on n floats; amax (or NULL) = max of the result.
+ * mas_lpips_maxpool: nn.MaxPool2d(2, 2) (features 4, 9, 16, 23), floor mode: x [N,H,W,C] -> y [N,H/2,W/2,C]; amax as above.
+ * mas_lpips_head_forward: for tap [2B,H,W,C] (relu1_2 .. relu5_3), part[b][k] (k < mas_lpips_head_blocks()) = partial sums
+ *   over pixels of sum_c w_lin[c] (n_real - n_fake)^2, n = f / (sqrt(sum_c f^2) + 1e-10) (norm_tensor, lpips.py:128-135;
+ *   NetLinLayer, lpips.py:90-96; Dropout is the identity in eval mode).
+ * mas_lpips_head_finalize: out[b] = sum over the five taps, in order, of sum_k part[l][b][k] / hw_l (spatial_average and the
+ *   sum of lpips.py:73); part [5][B][mas_lpips_head_blocks()].
+ * mas_lpips_tap_backward: d p_b / d (pre-ReLU tap) for a unit seed on every p_b, for the G images g0 .. g0+G-1 of the 2B
+ *   batch (their partners: the other half), plus the gradient dpool [G,H/2,W/2,C] of the following max-pool (NULL: none)
+ *   at the first maximum of each window; ReLU mask as a select (a pixel whose tap vector is all zero writes 0).
+ *   dz [G,H,W,C]; amax (or NULL) = max|dz|.
+ * mas_lpips_relu_backward: dx = y > 0 ? dy : 0 (threshold_backward; dx may alias dy); amax as above.
+ * mas_lpips_prep_backward: ScalingLayer backward, dxp [G,H,W,3] -> J [G,3,H,W] = dxp / scale.
+ * mas_lpips_scale_jacobian: out[b, :] = g[b * g_stride] * J[b, :] (per image of `per` floats): every traversal of the
+ *   graph after the one that computed J. */
+int mas_lpips_prep(const float* real, const float* fake, const float* shift, const float* scale, float* out, int B, int H, int W,
+                   void* stream);
+int mas_lpips_relu(float* y, int64_t n, float* amax, void* stream);
+int mas_lpips_maxpool(const float* x, float* y, int N, int H, int W, int C, float* amax, void* stream);
+int mas_lpips_head_blocks(void);
+int mas_lpips_head_forward(const float* tap, const float* w_lin, int B, int H, int W, int C, double* part, void* stream);
+int mas_lpips_head_finalize(const double* part, int B, int64_t hw0, int64_t hw1, int64_t hw2, int64_t hw3, int64_t hw4, float* out,
+                            void* stream);
+int mas_lpips_tap_backward(const float* tap, const float* w_lin, int B, int H, int W, int C, int g0, int G, const float* dpool,
+                           float* dz, float* amax, void* stream);
+int mas_lpips_relu_backward(const float* dy, const float* y, float* dx, int64_t n, float* amax, void* stream);
+int mas_lpips_prep_backward(const float* dxp, const float* scale, float* J, int G, int H, int W, void* stream);
+int mas_lpips_scale_jacobian(const float* J, const float* g, int64_t g_stride, float* out, int B, int64_t per, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

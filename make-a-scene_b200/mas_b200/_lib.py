@@ -144,6 +144,16 @@ _SPEC = {
     "mas_bce_cl_forward": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _Z, _P]),
     "mas_bce_cl_backward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
     "mas_bce_logits": (_I, [_P, _T, _P, _T, _P, _P, _P, _T, _F, _P, _Z, _P]),
+    "mas_lpips_prep": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
+    "mas_lpips_relu": (_I, [_P, _L, _P, _P]),
+    "mas_lpips_maxpool": (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),
+    "mas_lpips_head_blocks": (_I, []),
+    "mas_lpips_head_forward": (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),
+    "mas_lpips_head_finalize": (_I, [_P, _I, _L, _L, _L, _L, _L, _P, _P]),
+    "mas_lpips_tap_backward": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P]),
+    "mas_lpips_relu_backward": (_I, [_P, _P, _P, _L, _P, _P]),
+    "mas_lpips_prep_backward": (_I, [_P, _P, _P, _I, _I, _I, _P]),
+    "mas_lpips_scale_jacobian": (_I, [_P, _P, _L, _P, _I, _L, _P]),
 }
 
 _lib = None

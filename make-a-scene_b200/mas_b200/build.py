@@ -10,7 +10,7 @@ ROOT = os.path.dirname(PKG)
 CSRC = os.path.join(PKG, "csrc")
 OBJ = os.path.join(PKG, "build")
 LIB = os.path.join(PKG, "lib", "libmas_b200.so")
-SOURCES = ["norm.cu", "vq.cu", "vq_tc.cu", "contract_simt.cu", "conv4x4.cu", "contract_tc.cu", "conv_tma.cu", "gemm_tma.cu", "contract_tc3.cu", "edge.cu", "edge_quad.cu", "transformer.cu", "decode.cu", "attn.cu", "attn_fused.cu", "attn_causal.cu", "probe.cu", "capi.cu"]
+SOURCES = ["norm.cu", "vq.cu", "vq_tc.cu", "contract_simt.cu", "conv4x4.cu", "lpips.cu", "contract_tc.cu", "conv_tma.cu", "gemm_tma.cu", "contract_tc3.cu", "edge.cu", "edge_quad.cu", "transformer.cu", "decode.cu", "attn.cu", "attn_fused.cu", "attn_causal.cu", "probe.cu", "capi.cu"]
 NVCC_FLAGS = ["-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
               "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 

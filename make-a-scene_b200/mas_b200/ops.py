@@ -1665,3 +1665,180 @@ class EmbedFn(torch.autograd.Function):
             L.call("mas_embed3_backward", dout, ids.contiguous(), d0, pa, d1, pb, d2, ids.shape[0] * Lg, ctx.H, Lg, ctx.total, off)
             grads += [d0, d1, d2]
         return (None, None, None) + tuple(grads)
+
+
+# ---- LPIPS perceptual loss (losses/lpips.py) -------------------------------------------------------------------------
+LPIPS_BLOCKS = (2, 2, 3, 3, 3)   # 3x3 convolutions per VGG16 block; each block ends in a tap, blocks 1-4 in a 2x2 max-pool
+
+
+def _lpips_tc_ok(n, cin, h, w, cout):
+    """Tensor route of an LPIPS convolution: fp16 operands on shift_gemm_tc, Cout padded to the 128-wide tile."""
+    if not f16_operands() or cin % 16:
+        return False
+    xs = L.Tensor4(n, h, w, cin, h * w * cin, w * cin, cin, 1)
+    ys = L.Tensor4(n, h, w, cout, h * w * cout, w * cout, cout, 1)
+    return bool(L.query("mas_conv3x3_tc16h_eligible", xs, ys))
+
+
+def _lpips_padded_pack(weight, bias, transpose):
+    """fp16 operand image of a VGG convolution (transpose: its data gradient) with the output channels zero-padded to a
+    multiple of 128, and the matching padded bias; cached per weight version like the other packs."""
+    ent = _pack_entry(weight)
+    key = ("lpips", transpose)
+    hit = ent.get(key)
+    if hit is not None and hit[0].device == weight.device:
+        return hit
+    cout, cin = weight.shape[0], weight.shape[1]
+    dev = weight.device
+    if transpose:
+        ck = _round_up(cin, 128)
+        wk = torch.zeros((cout, ck, 3, 3), dtype=torch.float32, device=dev)
+        wk[:, :cin].copy_(weight.detach())
+        wt = torch.empty(9 * cout * ck, dtype=torch.float16, device=dev)
+        L.call("mas_pack_conv3x3_tc16", wk, wt, None, cout, ck, 1)
+        bk = None
+    else:
+        ck = _round_up(cout, 128)
+        wk = torch.zeros((ck, cin, 3, 3), dtype=torch.float32, device=dev)
+        wk[:cout].copy_(weight.detach())
+        wt = torch.empty(9 * ck * cin, dtype=torch.float16, device=dev)
+        L.call("mas_pack_conv3x3_tc16", wk, wt, None, ck, cin, 0)
+        bk = torch.zeros(ck, dtype=torch.float32, device=dev)
+        bk[:cout].copy_(bias.detach())
+    ent[key] = (wt, bk)
+    return wt, bk
+
+
+def _lpips_conv(x, am, weight, bias, transpose=False):
+    """3x3 stride-1 pad-1 convolution of dense-NHWC x (transpose: the data gradient, no bias); am = max|x| on the device."""
+    n, cin, h, w = x.shape
+    cout = weight.shape[1] if transpose else weight.shape[0]
+    if _lpips_tc_ok(n, cin, h, w, cout):
+        wt, bk = _lpips_padded_pack(weight, bias, transpose)
+        y = empty_nhwc(n, cout, h, w, x)
+        L.call("mas_conv3x3_fprop_tc16", x, L.t4(x), wt, bk, None, y, L.t4(y), L.CONV_S1, None, 0, None, am)
+        return y
+    if _cfg["impl"] == L.IMPL_TC:
+        raise RuntimeError("IMPL_TC requested but the LPIPS convolution shape is not eligible for the tensor-core kernel")
+    y = empty_nhwc(n, cout, h, w, x)
+    wp = torch.empty(9 * cout * cin, dtype=torch.float32, device=x.device)
+    L.call("mas_pack_conv3x3", weight.contiguous(), wp, weight.shape[0], weight.shape[1], int(transpose), 0)
+    L.call("mas_conv3x3_fprop", x, L.t4(x), wp, None if transpose else bias, None, y, L.t4(y), L.CONV_S1, L.IMPL_SIMT)
+    return y
+
+
+def _lpips_first_dgrad_weight(weight):
+    """conv1_1's data-gradient weight (3 output channels: taps flipped, Cin <-> Cout) for mas_edge_small_cout_fprop."""
+    ent = _pack_entry(weight)
+    hit = ent.get("lpips_dgrad")
+    if hit is None or hit.device != weight.device:
+        hit = weight.detach().flip(2, 3).transpose(0, 1).contiguous()
+        ent["lpips_dgrad"] = hit
+    return hit
+
+
+class LPIPSFn(torch.autograd.Function):
+    """LPIPS.forward (losses/lpips.py:66-73) as one unit: ScalingLayer, VGG16 up to relu5_3 and the five heads over ONE
+    batch of 2B images [real; fake] -> p [B, 1, 1, 1].
+
+    p_b depends on image b alone, so d p / d fake = g.view(B, 1, 1, 1) * J with J_b = d p_b / d fake_b. The first backward
+    runs the VGG data gradient once from a unit seed, keeps J and drops the activations; every later traversal of a
+    retained graph (loss_img.py's autograd.grad(retain_graph=True), then backward()) is one scaling kernel.
+    convs: the 13 (weight, bias) pairs in layer order; lins: the five [1, C, 1, 1] head weights."""
+
+    @staticmethod
+    def forward(ctx, real, fake, shift, scale, convs, lins, keep):
+        _need_cuda(real)
+        _need_cuda(fake)
+        if real.dim() != 4 or real.shape != fake.shape or real.shape[1] != 3:
+            raise RuntimeError("LPIPS expects real and fake images of equal shape [B, 3, H, W], got %s and %s"
+                               % (tuple(real.shape), tuple(fake.shape)))
+        B, _, H, W = real.shape
+        if H < 16 or W < 16:
+            raise RuntimeError("LPIPS needs images of at least 16 x 16 pixels (four 2x2 max-pools), got %d x %d" % (H, W))
+        real, fake = real.contiguous(), fake.contiguous()
+        dev = real.device
+        x = empty_nhwc(2 * B, 3, H, W, real)
+        L.call("mas_lpips_prep", real, fake, shift, scale, x, B, H, W)
+        nblk = int(L.load().mas_lpips_head_blocks())
+        part = torch.empty((5, B, nblk), dtype=torch.float64, device=dev)
+        acts, hws = [], []
+        cur, am, ci = x, None, 0
+        for blk, nconv in enumerate(LPIPS_BLOCKS):
+            for _ in range(nconv):
+                wgt, bias = convs[ci]
+                if ci == 0:
+                    h = empty_nhwc(2 * B, wgt.shape[0], H, W, x)
+                    L.call("mas_edge_small_cin_fprop", x, L.t4(x), wgt.contiguous(), bias, h, L.t4(h), 0)
+                else:
+                    h = _lpips_conv(cur, am, wgt, bias)
+                am = torch.empty(1, dtype=torch.float32, device=dev)
+                L.call("mas_lpips_relu", h, h.numel(), am)
+                if keep:
+                    acts.append(h)
+                cur, ci = h, ci + 1
+            _, c, hh, ww = cur.shape
+            L.call("mas_lpips_head_forward", cur, lins[blk].contiguous(), B, hh, ww, c, part[blk])
+            hws.append(hh * ww)
+            if blk < len(LPIPS_BLOCKS) - 1:
+                p = empty_nhwc(2 * B, c, hh // 2, ww // 2, cur)
+                am = torch.empty(1, dtype=torch.float32, device=dev)
+                L.call("mas_lpips_maxpool", cur, p, 2 * B, hh, ww, c, am)
+                cur = p
+        out = torch.empty((B, 1, 1, 1), dtype=torch.float32, device=dev)
+        L.call("mas_lpips_head_finalize", part, B, *hws, out)
+        ctx.acts = acts if keep else None
+        ctx.convs, ctx.lins, ctx.scale, ctx.shape = convs, lins, scale, (B, H, W)
+        ctx.J = None
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        if torch.is_grad_enabled():
+            raise RuntimeError("LPIPS does not support create_graph (double backward)")
+        want_r, want_f = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        B, H, W = ctx.shape
+        if ctx.J is None:
+            if ctx.acts is None:
+                raise RuntimeError("LPIPS: the forward ran without gradient tracking; nothing was saved for a backward")
+            g0, G = (0 if want_r else B), (2 * B if want_r and want_f else B)
+            acts, convs, lins = ctx.acts, ctx.convs, ctx.lins
+            dev = acts[0].device
+            dpool, ci = None, len(convs)
+            for blk in reversed(range(len(LPIPS_BLOCKS))):
+                tap = acts[ci - 1]
+                _, c, hh, ww = tap.shape
+                dz = empty_nhwc(G, c, hh, ww, tap)
+                am = torch.empty(1, dtype=torch.float32, device=dev)
+                L.call("mas_lpips_tap_backward", tap, lins[blk].contiguous(), B, hh, ww, c, g0, G, dpool, dz, am)
+                first = ci - LPIPS_BLOCKS[blk]
+                for k in reversed(range(first, ci)):
+                    wgt = convs[k][0]
+                    if k == 0:
+                        dx = empty_nhwc(G, 3, H, W, dz)
+                        L.call("mas_edge_small_cout_fprop", dz, L.t4(dz), _lpips_first_dgrad_weight(wgt), None, dx, L.t4(dx))
+                    else:
+                        dx = _lpips_conv(dz, am, wgt, None, transpose=True)
+                    if k > first:   # the input of conv k is the ReLU output of conv k - 1: its mask, as a select
+                        am = torch.empty(1, dtype=torch.float32, device=dev)
+                        L.call("mas_lpips_relu_backward", dx, acts[k - 1][g0:g0 + G], dx, dx.numel(), am)
+                    dz = dx
+                dpool, ci = dz, first   # gradient of the block's input: the previous max-pool's output (block 0: the prep)
+            J = torch.empty((G, 3, H, W), dtype=torch.float32, device=dev)
+            L.call("mas_lpips_prep_backward", dpool, ctx.scale, J, G, H, W)
+            ctx.J, ctx.acts = J, None
+        J = ctx.J
+        if g.dtype != torch.float32 or g.dim() != 4 or g.shape[0] != B:
+            raise RuntimeError("LPIPS backward: expected a float32 [B, 1, 1, 1] gradient")
+        per = 3 * H * W
+        grads = []
+        off = 0
+        for want in (want_r, want_f):
+            if not want:
+                grads.append(None)
+                continue
+            d = torch.empty((B, 3, H, W), dtype=torch.float32, device=J.device)
+            L.call("mas_lpips_scale_jacobian", J[off:off + B], g, g.stride(0), d, B, per)
+            grads.append(d)
+            off += B
+        return grads[0], grads[1], None, None, None, None, None
