@@ -163,14 +163,18 @@ def _tc_on():
     return _cfg["impl"] != L.IMPL_SIMT
 
 
+def _nhwc4(n, h, w, c):
+    """mas_tensor4 of a dense channels-last [n, c, h, w] tensor."""
+    return L.Tensor4(n, h, w, c, h * w * c, w * c, c, 1)
+
+
 def conv_tc_eligible(x, cout, mode):
     """True when conv3x3 of dense-NHWC x with `cout` output channels runs on the tensor-core kernel."""
     if not _tc_on() or not _is_dense_nhwc(x):
         return False
     n, _, h, w = x.shape
     ho, wo = _conv_out_hw(h, w, mode)
-    ys = L.Tensor4(n, ho, wo, cout, ho * wo * cout, wo * cout, cout, 1)
-    return bool(L.query("mas_conv3x3_tc_eligible", L.t4(x), ys, mode))
+    return bool(L.query("mas_conv3x3_tc_eligible", L.t4(x), _nhwc4(n, ho, wo, cout), mode))
 
 
 def gn_table(mean, rstd, gamma, beta, n, c):
@@ -180,38 +184,49 @@ def gn_table(mean, rstd, gamma, beta, n, c):
     return t
 
 
-def _finalize_stats(part, tiles_per_image, n, c, hw):
+def _stats_part(y, want):
+    """Partial sums for the GroupNorm-statistics epilogue of the tensor-core kernel writing y: a (sum, sum of squares) pair per
+    channel and 128-pixel tile. None when no statistics are wanted or the channels do not split into 4-channel quads per group."""
+    n, c, h, w = y.shape
+    if not want or c % (4 * GN_GROUPS):
+        return None
+    return torch.empty(n * (h * w // 128) * c * 2, dtype=torch.float32, device=y.device)
+
+
+def _finalize_stats(part, n, c, hw):
+    """(mean, rstd) per (image, group) from the per-128-pixel-tile partials of a statistics epilogue (None without partials)."""
+    if part is None:
+        return None
     mean = torch.empty(n * GN_GROUPS, dtype=torch.float32, device=part.device)
     rstd = torch.empty_like(mean)
-    L.call("mas_gn_finalize_partials", part, tiles_per_image, n, c, GN_GROUPS, hw, GN_EPS, mean, rstd)
+    L.call("mas_gn_finalize_partials", part, hw // 128, n, c, GN_GROUPS, hw, GN_EPS, mean, rstd)
     return mean, rstd
 
 
 def conv3x3_raw(x, weight, bias, residual, mode, out_nchw=False, transpose=False, table=None, silu=True, want_stats=False,
-                prepack=False, x_amax=None):
+                prepack=False, x_amax=None, pad_out=False):
     """y = conv3x3(x; weight) (+bias, +residual). transpose=True applies the data-gradient operand
     (taps flipped, Cin<->Cout). Dense NHWC shapes with Cin%8==0, Cout%128==0, Hout%16==0, Wout%8==0 run on the
     tensor-core kernel; everything else (edge layers, NCHW views, small images) on the fp32 SIMT kernel.
     table: fused GroupNorm(+SiLU) prologue (tensor path only); want_stats: also return the output's GroupNorm
-    (mean, rstd) from the fused epilogue (None when the tensor path does not apply)."""
+    (mean, rstd) from the fused epilogue (None when the tensor path does not apply).
+    pad_out: the fp16 tensor-core kernel also takes an output width off the 128-wide tile. The weight and bias are zero-padded to
+    the tile, the kernel stores round_up(Cout, 4) channels and the Cout real ones come back as a channels-last view. Without
+    fp16 operands, or where even the padded shape does not fit, such a call runs on the fp32 SIMT kernel, never the TF32 one."""
     n, _, h, w = x.shape
     cout = weight.shape[1] if transpose else weight.shape[0]
     cin = weight.shape[0] if transpose else weight.shape[1]
     ho, wo = _conv_out_hw(h, w, mode)
-    if out_nchw:
-        y = torch.empty((n, cout, ho, wo), dtype=torch.float32, device=x.device)
-    else:
-        y = empty_nhwc(n, cout, ho, wo, x)
-    xs, ys = L.t4(x), L.t4(y)
-    wc = weight.contiguous()
-    stats = None
-    if _tc_on() and not out_nchw and L.query("mas_conv3x3_tc_eligible", xs, ys, mode):
-        f16 = _cfg["operands"] == "f16" and cin % 16 == 0
-        wt = _packed_conv_weight(wc, weight, cout, cin, transpose, x.device, prepack, f16)
-        part = None
-        if want_stats and cout % (4 * GN_GROUPS) == 0:
-            tiles = n * (ho // 16) * (wo // 8)
-            part = torch.empty(tiles * cout * 2, dtype=torch.float32, device=x.device)
+    xs = L.t4(x)
+    f16 = _cfg["operands"] == "f16" and cin % 16 == 0
+    ck = _round_up(cout, 128) if pad_out else cout          # output channels the tensor-core kernel computes
+    if (_tc_on() and not out_nchw and (f16 or not pad_out)
+            and L.query("mas_conv3x3_tc_eligible", xs, _nhwc4(n, ho, wo, ck), mode)):
+        y = empty_nhwc(n, _round_up(cout, 4), ho, wo, x)
+        ys = L.t4(y)
+        wt = _packed_conv_weight(weight.contiguous(), weight, ck, cin, transpose, x.device, prepack, f16)
+        bias = None if bias is None else _padded(bias, (ck,))
+        part = _stats_part(y, want_stats)
         if f16:
             # post-GroupNorm activations (prologue) are O(1) by construction; anything else (gradients above all) gets a
             # power-of-two scale from its largest magnitude
@@ -219,16 +234,22 @@ def conv3x3_raw(x, weight, bias, residual, mode, out_nchw=False, transpose=False
             L.call("mas_conv3x3_fprop_tc16", x, xs, wt, bias, residual, y, ys, mode, table, int(silu), part, xa)
         else:
             L.call("mas_conv3x3_fprop_tc", x, xs, wt, bias, residual, y, ys, mode, table, int(silu), part)
-        if part is not None:
-            stats = _finalize_stats(part, (ho // 16) * (wo // 8), n, cout, ho * wo)
+        stats = _finalize_stats(part, n, cout, ho * wo)
+        if y.shape[1] != cout:
+            y = y[:, :cout]
     else:
         if table is not None:
             raise RuntimeError("fused GroupNorm prologue requested for a shape that is not tensor-path eligible")
         if _cfg["impl"] == L.IMPL_TC:
             raise RuntimeError("IMPL_TC requested but the conv shape is not eligible for the tensor-core kernel")
+        if out_nchw:
+            y = torch.empty((n, cout, ho, wo), dtype=torch.float32, device=x.device)
+        else:
+            y = empty_nhwc(n, cout, ho, wo, x)
         wp = torch.empty(9 * cout * cin, dtype=torch.float32, device=x.device)
-        L.call("mas_pack_conv3x3", wc, wp, weight.shape[0], weight.shape[1], int(transpose), 0)
-        L.call("mas_conv3x3_fprop", x, xs, wp, bias, residual, y, ys, mode, L.IMPL_SIMT)
+        L.call("mas_pack_conv3x3", weight.contiguous(), wp, weight.shape[0], weight.shape[1], int(transpose), 0)
+        L.call("mas_conv3x3_fprop", x, xs, wp, bias, residual, y, L.t4(y), mode, L.IMPL_SIMT)
+        stats = None
     if want_stats:
         return y, stats
     return y
@@ -268,12 +289,10 @@ def conv3x3_h_raw(x16, weight, bias, residual, transpose=False, want_stats=False
     cin = weight.shape[0] if transpose else weight.shape[1]
     y = empty_nhwc(n, cout, h, w, x16)
     wt = _packed_conv_weight(weight.contiguous(), weight, cout, cin, transpose, x16.device, prepack, True)
-    part = None
-    if want_stats and cout % (4 * GN_GROUPS) == 0:
-        part = torch.empty(n * (h // 16) * (w // 8) * cout * 2, dtype=torch.float32, device=x16.device)
+    part = _stats_part(y, want_stats)
     L.call("mas_conv3x3_fprop_tc16h", x16, L.t4(x16), wt, bias, residual, y, L.t4(y), part, x_amax)
     if want_stats:
-        return y, (_finalize_stats(part, (h // 16) * (w // 8), n, cout, h * w) if part is not None else None)
+        return y, _finalize_stats(part, n, cout, h * w)
     return y
 
 
@@ -295,29 +314,51 @@ def _pack_entry(weight):
     return d
 
 
-def _packed_conv_weight(wc, weight, cout, cin, transpose, dev, prepack=False, f16=False):
-    ent = _pack_entry(weight)
-    key = ("d" if transpose else "f", f16)
+def _cached(t, key, make):
+    """The tensor stored under `key` for t's current version, built by make() when absent or not on t's device."""
+    ent = _pack_entry(t)
     hit = ent.get(key)
-    if hit is not None and hit.device == dev:
-        return hit
+    if hit is None or hit.device != t.device:
+        hit = ent[key] = make()
+    return hit
+
+
+def _padded(t, shape):
+    """t zero-padded at the end of each dimension to `shape`, cached per version of t (t itself when it has that shape)."""
+    if tuple(t.shape) == tuple(shape):
+        return t
+
+    def make():
+        p = torch.zeros(shape, dtype=t.dtype, device=t.device)
+        p[tuple(slice(0, s) for s in t.shape)] = t.detach()
+        return p
+    return _cached(t, ("pad",) + tuple(shape), make)
+
+
+def _packed_conv_weight(wc, weight, cout, cin, transpose, dev, prepack=False, f16=False):
+    """Tensor-core operand image of a 3x3 weight (wc: its contiguous form) for a convolution with `cout` output and `cin`
+    input channels (transpose: the data gradient). Extents larger than the weight's zero-pad it first: the output side to the
+    128-wide tile, the input side to the K step or to the data-gradient image's tile."""
+    rows, cols = (cin, cout) if transpose else (cout, cin)       # in the weight's [Cout, Cin] order
     dt = torch.float16 if f16 else torch.float32
-    wt = torch.empty(9 * cout * cin, dtype=dt, device=dev)
-    pair_ok = cout % 128 == 0 and cin % 128 == 0
-    if prepack and not transpose and pair_ok:
-        # forward of a training step whose backward will run the data gradient: it wants the transposed packing
-        wd = torch.empty(9 * cout * cin, dtype=dt, device=dev)
-        if f16:
-            L.call("mas_pack_conv3x3_tc16", wc, wt, wd, weight.shape[0], weight.shape[1], 0)
+
+    def make():
+        w = wc if (rows, cols) == tuple(weight.shape[:2]) else _padded(weight, (rows, cols, 3, 3))
+        wt = torch.empty(9 * rows * cols, dtype=dt, device=dev)
+        if prepack and not transpose and rows % 128 == 0 and cols % 128 == 0:
+            # forward of a training step whose backward will run the data gradient: it wants the transposed packing
+            wd = torch.empty_like(wt)
+            if f16:
+                L.call("mas_pack_conv3x3_tc16", w, wt, wd, rows, cols, 0)
+            else:
+                L.call("mas_pack_conv3x3_tc_pair", w, wt, wd, rows, cols)
+            _pack_entry(weight)[("d", f16, rows, cols)] = wd
+        elif f16:
+            L.call("mas_pack_conv3x3_tc16", w, wt, None, rows, cols, int(transpose))
         else:
-            L.call("mas_pack_conv3x3_tc_pair", wc, wt, wd, weight.shape[0], weight.shape[1])
-        ent[("d", f16)] = wd
-    elif f16:
-        L.call("mas_pack_conv3x3_tc16", wc, wt, None, weight.shape[0], weight.shape[1], int(transpose))
-    else:
-        L.call("mas_pack_conv3x3_tc", wc, wt, weight.shape[0], weight.shape[1], int(transpose))
-    ent[key] = wt
-    return wt
+            L.call("mas_pack_conv3x3_tc", w, wt, rows, cols, int(transpose))
+        return wt
+    return _cached(weight, ("d" if transpose else "f", f16, rows, cols), make)
 
 
 def phase_mode(x, cout, mode):
@@ -329,9 +370,8 @@ def phase_mode(x, cout, mode):
         return None
     n, _, h, w = x.shape
     ho, wo = _conv_out_hw(h, w, mode)
-    ys = L.Tensor4(n, ho, wo, cout, ho * wo * cout, wo * cout, cout, 1)
     pm = L.CONV_UP_PHASE if mode == L.CONV_UP else L.CONV_S2_PHASE
-    return pm if L.query("mas_conv3x3_tc_eligible", L.t4(x), ys, pm) else None
+    return pm if L.query("mas_conv3x3_tc_eligible", L.t4(x), _nhwc4(n, ho, wo, cout), pm) else None
 
 
 def conv3x3_phase_raw(x16, weight, bias, pmode, transpose=False, x_amax=None):
@@ -341,13 +381,12 @@ def conv3x3_phase_raw(x16, weight, bias, pmode, transpose=False, x_amax=None):
     cout = weight.shape[1] if transpose else weight.shape[0]
     up_side = (pmode == L.CONV_UP_PHASE) != transpose   # the destination is the 2x side
     y = empty_nhwc(n, cout, 2 * h if up_side else h // 2, 2 * w if up_side else w // 2, x16)
-    ent = _pack_entry(weight)
-    key = ("phase", pmode, transpose)
-    wt = ent.get(key)
-    if wt is None or wt.device != x16.device:
+
+    def make():
         wt = torch.empty(16 * weight.shape[0] * weight.shape[1], dtype=torch.float16, device=x16.device)
         L.call("mas_pack_conv3x3_phase16", weight.contiguous(), wt, weight.shape[0], weight.shape[1], pmode, int(transpose))
-        ent[key] = wt
+        return wt
+    wt = _cached(weight, ("phase", pmode, transpose), make)
     L.call("mas_conv3x3_phase_tc16h", x16, L.t4(x16), wt, bias, y, L.t4(y), pmode, int(transpose), x_amax)
     return y
 
@@ -570,32 +609,21 @@ class Conv3x3Fn(torch.autograd.Function):
         elif tc_pad_in:
             # channel count off the 16-wide K step of the tensor kernels (the 159-channel VQ-SEG maps; the 3-channel image of
             # conv_in, where 10x padded FLOPs on the tensor cores still beat the FFMA edge kernel 4x): zero-pad the input channels
-            # (one tiled transposing copy from the caller's NCHW tensor) and the weight, run the tensor-core kernels
+            # (one tiled transposing copy from the caller's NCHW tensor) and the weight (cached per version), run the
+            # tensor-core kernels
             edge = 4
             cp = _round_up(cin, 32)          # 32: the weight-gradient kernel's input-channel tile
             x = pad_nhwc(x, cp)
-            wp = torch.zeros((cout, cp, 3, 3), dtype=torch.float32, device=x.device)
-            wp[:, :cin].copy_(weight.detach())
-            y = conv3x3_raw(x, wp, bias, None, L.CONV_S1)
+            y = conv3x3_raw(x, _padded(weight, (cout, cp, 3, 3)), bias, None, L.CONV_S1)
         elif (mode == L.CONV_S1 and f16_operands() and residual is None and cout % 128 != 0 and cout > 128 and cin % 16 == 0
               and h % 16 == 0 and w % 8 == 0):
-            # output width off the 128-wide tile (the 159-channel VQ-SEG decoder head): the kernel runs round_up(cout, 128)
-            # channels from zero-padded weights and stores only the first round_up(cout, 4); the result is RETURNED AS A
-            # CHANNELS-LAST VIEW [N, cout, H, W] of that buffer (the weighted-BCE kernels take it as it is; `out_nchw` is
-            # not honoured here: a contiguous NCHW copy of a 1.3 GB logits tensor would cost more than the convolution)
+            # output width off the 128-wide tile (the 159-channel VQ-SEG decoder head): the result is RETURNED AS A
+            # CHANNELS-LAST VIEW [N, cout, H, W] of the round_up(cout, 4)-channel buffer the padded kernel writes (the
+            # weighted-BCE kernels take it as it is; `out_nchw` is not honoured here: a contiguous NCHW copy of a 1.3 GB
+            # logits tensor would cost more than the convolution)
             edge = 5
             x = nhwc(x)
-            cpo, ck = _round_up(cout, 4), _round_up(cout, 128)
-            wk = torch.zeros((ck, cin, 3, 3), dtype=torch.float32, device=x.device)
-            wk[:cout].copy_(weight.detach())
-            bk = torch.zeros(ck, dtype=torch.float32, device=x.device)
-            if bias is not None:
-                bk[:cout].copy_(bias.detach())
-            wt = torch.empty(9 * ck * cin, dtype=torch.float16, device=x.device)
-            L.call("mas_pack_conv3x3_tc16", wk, wt, None, ck, cin, 0)
-            full = torch.empty((n, h, w, cpo), dtype=torch.float32, device=x.device).permute(0, 3, 1, 2)
-            L.call("mas_conv3x3_fprop_tc16", x, L.t4(x), wt, bk, None, full, L.t4(full), L.CONV_S1, None, 0, None, amax_of(x))
-            y = full[:, :cout]
+            y = conv3x3_raw(x, weight, bias, None, L.CONV_S1, pad_out=True)
         elif residual is None and not out_nchw and phase_mode(x, cout, mode) is not None:
             # Upsample / Downsample as four small convolutions over phase planes read straight from an fp16 shadow of x
             edge = 6
@@ -659,21 +687,17 @@ class Conv3x3Fn(torch.autograd.Function):
                 dwp, db = conv3x3_wgrad_raw(x, dy, cout, cp, L.CONV_S1, ctx.has_bias, dy_amax=am)
                 dw = dwp[:, :cin].contiguous()
             if ctx.needs_input_grad[0]:
-                wp = torch.zeros((cout, cp, 3, 3), dtype=torch.float32, device=x.device)
-                wp[:, :cin].copy_(weight.detach())
-                dx = conv3x3_dgrad_raw(dy, wp, L.CONV_S1, am)[:, :cin]
+                dx = conv3x3_dgrad_raw(dy, _padded(weight, (cout, cp, 3, 3)), L.CONV_S1, am)[:, :cin]
         elif ctx.edge == 5:
-            cpo, ck = _round_up(cout, 4), _round_up(cout, 128)
+            cpo = _round_up(cout, 4)
             full = getattr(dy, "_mas_pad_base", None)                    # the loss kernel wrote the gradient padded already
             if full is None or full.shape[1] != cpo or full.data_ptr() != dy.data_ptr() or not _is_dense_nhwc(full):
                 full = pad_nhwc(dy.contiguous() if not dy.is_contiguous() and _cl_pitch(dy) is None else dy, cpo)
             am = amax_of(full)
             if ctx.needs_input_grad[0]:
-                w160 = torch.zeros((cpo, cin, 3, 3), dtype=torch.float32, device=x.device)
-                w160[:cout].copy_(weight.detach())
-                dx = conv3x3_raw(full, w160, None, None, L.CONV_S1, transpose=True, x_amax=am)
+                dx = conv3x3_raw(full, _padded(weight, (cpo, cin, 3, 3)), None, None, L.CONV_S1, transpose=True, x_amax=am)
             if want_w:
-                dwk, dbk = conv3x3_wgrad_raw(x, full, ck, cin, L.CONV_S1, True, dy_amax=am)
+                dwk, dbk = conv3x3_wgrad_raw(x, full, _round_up(cout, 128), cin, L.CONV_S1, True, dy_amax=am)
                 dw, db = dwk[:cout].contiguous(), dbk[:cout].contiguous()
         elif ctx.edge == 6:
             # x is the input's fp16 shadow here (None when no weight gradient was asked for); both gradients read one dy shadow
@@ -878,7 +902,7 @@ class AttnBlockFn(torch.autograd.Function):
         ctx.save_for_backward(x, mean, rstd, hn, qkv, P, O, nw, nb, qw, kw, vw, pw)
         ctx.set_materialize_grads(False)   # no zero-fill launches for the (non-differentiable) statistics outputs
         if part is not None:
-            mo, ro = _finalize_stats(part, hw // 128, n, c, hw)
+            mo, ro = _finalize_stats(part, n, c, hw)
             ctx.mark_non_differentiable(mo, ro)
             return out, mo, ro
         return out, None, None
@@ -967,16 +991,12 @@ def batchnorm_eval(x, weight, bias, running_mean, running_var, eps):
 def _packed_conv4x4_weight(weight, transpose):
     """mas_pack_conv4x4 image of a [Cout,Cin,4,4] weight, cached per parameter version (D's weights change only at its
     optimizer step, so the three forwards and the backward passes of one training step share one packing)."""
-    ent = _pack_entry(weight)
-    key = ("c4", bool(transpose))
-    hit = ent.get(key)
-    if hit is not None and hit.device == weight.device:
-        return hit
-    cout, cin = weight.shape[:2]
-    wp = torch.empty(16 * cout * cin, dtype=torch.float32, device=weight.device)
-    L.call("mas_pack_conv4x4", weight.detach().contiguous(), wp, cout, cin, int(transpose))
-    ent[key] = wp
-    return wp
+    def make():
+        cout, cin = weight.shape[:2]
+        wp = torch.empty(16 * cout * cin, dtype=torch.float32, device=weight.device)
+        L.call("mas_pack_conv4x4", weight.detach().contiguous(), wp, cout, cin, int(transpose))
+        return wp
+    return _cached(weight, ("c4", bool(transpose)), make)
 
 
 def conv4x4_out_hw(h, w, stride):
@@ -991,23 +1011,18 @@ def conv4x4_tc_route(x, cout, stride):
     n, cin, h, w = x.shape
     if stride == 2 and (h % 2 or w % 2):
         return False
-    hs, ws, c4 = h // stride, w // stride, 4 * cin
-    xs = L.Tensor4(n, hs, ws, c4, hs * ws * c4, ws * c4, c4, 1)
-    ys = L.Tensor4(n, hs, ws, cout, hs * ws * cout, ws * cout, cout, 1)
-    return cin % 4 == 0 and bool(L.query("mas_conv3x3_tc_eligible", xs, ys, L.CONV_S1))
+    hs, ws = h // stride, w // stride
+    return cin % 4 == 0 and bool(L.query("mas_conv3x3_tc_eligible", _nhwc4(n, hs, ws, 4 * cin), _nhwc4(n, hs, ws, cout), L.CONV_S1))
 
 
 def _conv4x4_as_3x3(weight, stride):
     """[Cout, 4*Cin, 3, 3] weight of the shift-map route, cached per parameter version (its own packings then stay cached)."""
-    ent = _pack_entry(weight)
-    key = ("c4to3", stride)
-    w3 = ent.get(key)
-    if w3 is None or w3.device != weight.device:
+    def make():
         cout, cin = weight.shape[:2]
         w3 = torch.empty((cout, 4 * cin, 3, 3), dtype=torch.float32, device=weight.device)
         L.call("mas_conv4x4_remap_weight", weight.detach().contiguous(), w3, cout, cin, stride, 1)
-        ent[key] = w3
-    return w3
+        return w3
+    return _cached(weight, ("c4to3", stride), make)
 
 
 class Conv4x4Fn(torch.autograd.Function):
@@ -1361,16 +1376,12 @@ def linear_f16_on(nout, kin):
 def _packed_linear_weight(weight, transpose, dev):
     """fp16 operand image of an nn.Linear weight [N,K] (transpose: of W^T, the data-gradient operand), cached per parameter
     version like the convolution packings."""
-    ent = _pack_entry(weight)
-    key = ("lin16", bool(transpose))
-    hit = ent.get(key)
-    if hit is not None and hit.device == dev:
-        return hit
-    n, k = weight.shape
-    wt = torch.empty(n * k, dtype=torch.float16, device=dev)
-    L.call("mas_pack_gemm_tc16", weight.contiguous(), wt, n, k, int(transpose))
-    ent[key] = wt
-    return wt
+    def make():
+        n, k = weight.shape
+        wt = torch.empty(n * k, dtype=torch.float16, device=dev)
+        L.call("mas_pack_gemm_tc16", weight.contiguous(), wt, n, k, int(transpose))
+        return wt
+    return _cached(weight, ("lin16", bool(transpose)), make)
 
 
 def rows_to_half(x2d):
@@ -1671,70 +1682,9 @@ class EmbedFn(torch.autograd.Function):
 LPIPS_BLOCKS = (2, 2, 3, 3, 3)   # 3x3 convolutions per VGG16 block; each block ends in a tap, blocks 1-4 in a 2x2 max-pool
 
 
-def _lpips_tc_ok(n, cin, h, w, cout):
-    """Tensor route of an LPIPS convolution: fp16 operands on shift_gemm_tc, Cout padded to the 128-wide tile."""
-    if not f16_operands() or cin % 16:
-        return False
-    xs = L.Tensor4(n, h, w, cin, h * w * cin, w * cin, cin, 1)
-    ys = L.Tensor4(n, h, w, cout, h * w * cout, w * cout, cout, 1)
-    return bool(L.query("mas_conv3x3_tc16h_eligible", xs, ys))
-
-
-def _lpips_padded_pack(weight, bias, transpose):
-    """fp16 operand image of a VGG convolution (transpose: its data gradient) with the output channels zero-padded to a
-    multiple of 128, and the matching padded bias; cached per weight version like the other packs."""
-    ent = _pack_entry(weight)
-    key = ("lpips", transpose)
-    hit = ent.get(key)
-    if hit is not None and hit[0].device == weight.device:
-        return hit
-    cout, cin = weight.shape[0], weight.shape[1]
-    dev = weight.device
-    if transpose:
-        ck = _round_up(cin, 128)
-        wk = torch.zeros((cout, ck, 3, 3), dtype=torch.float32, device=dev)
-        wk[:, :cin].copy_(weight.detach())
-        wt = torch.empty(9 * cout * ck, dtype=torch.float16, device=dev)
-        L.call("mas_pack_conv3x3_tc16", wk, wt, None, cout, ck, 1)
-        bk = None
-    else:
-        ck = _round_up(cout, 128)
-        wk = torch.zeros((ck, cin, 3, 3), dtype=torch.float32, device=dev)
-        wk[:cout].copy_(weight.detach())
-        wt = torch.empty(9 * ck * cin, dtype=torch.float16, device=dev)
-        L.call("mas_pack_conv3x3_tc16", wk, wt, None, ck, cin, 0)
-        bk = torch.zeros(ck, dtype=torch.float32, device=dev)
-        bk[:cout].copy_(bias.detach())
-    ent[key] = (wt, bk)
-    return wt, bk
-
-
-def _lpips_conv(x, am, weight, bias, transpose=False):
-    """3x3 stride-1 pad-1 convolution of dense-NHWC x (transpose: the data gradient, no bias); am = max|x| on the device."""
-    n, cin, h, w = x.shape
-    cout = weight.shape[1] if transpose else weight.shape[0]
-    if _lpips_tc_ok(n, cin, h, w, cout):
-        wt, bk = _lpips_padded_pack(weight, bias, transpose)
-        y = empty_nhwc(n, cout, h, w, x)
-        L.call("mas_conv3x3_fprop_tc16", x, L.t4(x), wt, bk, None, y, L.t4(y), L.CONV_S1, None, 0, None, am)
-        return y
-    if _cfg["impl"] == L.IMPL_TC:
-        raise RuntimeError("IMPL_TC requested but the LPIPS convolution shape is not eligible for the tensor-core kernel")
-    y = empty_nhwc(n, cout, h, w, x)
-    wp = torch.empty(9 * cout * cin, dtype=torch.float32, device=x.device)
-    L.call("mas_pack_conv3x3", weight.contiguous(), wp, weight.shape[0], weight.shape[1], int(transpose), 0)
-    L.call("mas_conv3x3_fprop", x, L.t4(x), wp, None if transpose else bias, None, y, L.t4(y), L.CONV_S1, L.IMPL_SIMT)
-    return y
-
-
 def _lpips_first_dgrad_weight(weight):
     """conv1_1's data-gradient weight (3 output channels: taps flipped, Cin <-> Cout) for mas_edge_small_cout_fprop."""
-    ent = _pack_entry(weight)
-    hit = ent.get("lpips_dgrad")
-    if hit is None or hit.device != weight.device:
-        hit = weight.detach().flip(2, 3).transpose(0, 1).contiguous()
-        ent["lpips_dgrad"] = hit
-    return hit
+    return _cached(weight, "lpips_dgrad", lambda: weight.detach().flip(2, 3).transpose(0, 1).contiguous())
 
 
 class LPIPSFn(torch.autograd.Function):
@@ -1771,7 +1721,7 @@ class LPIPSFn(torch.autograd.Function):
                     h = empty_nhwc(2 * B, wgt.shape[0], H, W, x)
                     L.call("mas_edge_small_cin_fprop", x, L.t4(x), wgt.contiguous(), bias, h, L.t4(h), 0)
                 else:
-                    h = _lpips_conv(cur, am, wgt, bias)
+                    h = conv3x3_raw(cur, wgt, bias, None, L.CONV_S1, x_amax=am, pad_out=True)
                 am = torch.empty(1, dtype=torch.float32, device=dev)
                 L.call("mas_lpips_relu", h, h.numel(), am)
                 if keep:
@@ -1818,7 +1768,7 @@ class LPIPSFn(torch.autograd.Function):
                         dx = empty_nhwc(G, 3, H, W, dz)
                         L.call("mas_edge_small_cout_fprop", dz, L.t4(dz), _lpips_first_dgrad_weight(wgt), None, dx, L.t4(dx))
                     else:
-                        dx = _lpips_conv(dz, am, wgt, None, transpose=True)
+                        dx = conv3x3_raw(dz, wgt, None, None, L.CONV_S1, transpose=True, x_amax=am, pad_out=True)
                     if k > first:   # the input of conv k is the ReLU output of conv k - 1: its mask, as a select
                         am = torch.empty(1, dtype=torch.float32, device=dev)
                         L.call("mas_lpips_relu_backward", dx, acts[k - 1][g0:g0 + G], dx, dx.numel(), am)

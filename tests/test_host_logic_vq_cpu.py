@@ -766,31 +766,40 @@ def test_img_config_model_host_logic_against_reference_fixture(vq_emu):
     assert n.count("mas_conv3x3_fprop_tc16h") == 90 and n.count("mas_attnblock_forward") == 14 and n.count("mas_vq_forward_given") == 1
 
 
+VQSEG_DD = dict(z_channels=64, in_channels=159, out_channels=159, channels=[128, 128], num_res_blocks=1, resolution=64,
+                attn_resolutions=[], dropout=0.0)
+
+
+def _vqseg_model():
+    """A segmentation-shaped VQBASE in training mode past the codebook's warm-up, a one-hot-like 159-channel map and the
+    weighted BCE's pos_weight (losses/loss_seg.py)."""
+    from models import VQBASE
+    torch.manual_seed(0)
+    m = VQBASE(VQSEG_DD, 128, 64, 10, 100)
+    with torch.no_grad():
+        m.quantize.embedding.weight.normal_()
+    m.quantize.q_counter = 10 ** 6
+    m.train()
+    seg = (torch.rand(2, 159, 64, 64, generator=torch.Generator().manual_seed(5)) > 0.9).float()
+    pw = torch.ones(159)
+    pw[153:158] = 20
+    return m, seg, pw
+
+
 def test_vqseg_step_host_logic_against_oracle(vq_emu):
     """The VQ-SEG step (159-channel maps: conv_in zero-padded to 160 input channels, conv_out run for 256 padded rows and returned
     as a channels-last view of a 160-channel buffer, weighted BCE forward / backward on that padded view, the gradient handed to
     the convolution's backward without a copy) above the emulated C-ABI against the CPU oracle (losses/loss_seg.py:6-22)."""
     from conftest import rel_err
     from mas_b200 import ops
-    from models import VQBASE
     from oracle import vqgan_oracle as O
-    dd = dict(z_channels=64, in_channels=159, out_channels=159, channels=[128, 128], num_res_blocks=1, resolution=64,
-              attn_resolutions=[], dropout=0.0)
-    torch.manual_seed(0)
-    m = VQBASE(dd, 128, 64, 10, 100)
-    with torch.no_grad():
-        m.quantize.embedding.weight.normal_()
-    m.quantize.q_counter = 10 ** 6
-    m.train()
+    m, seg, pw = _vqseg_model()
     sd = {k: v.detach().clone() for k, v in m.state_dict().items()}
     params = {k: v.requires_grad_(True) for k, v in sd.items() if v.is_floating_point() and "running" not in k}
     sd.update(params)
-    seg = (torch.rand(2, 159, 64, 64, generator=torch.Generator().manual_seed(5)) > 0.9).float()
-    dec_o, diff_o, idx_o = O.vqbase_forward(sd, dd, seg)
+    dec_o, diff_o, idx_o = O.vqbase_forward(sd, VQSEG_DD, seg)
     lo = O.bce_loss_with_quant(diff_o, seg, dec_o)
     lo.backward()
-    pw = torch.ones(159)
-    pw[153:158] = 20
     cb = m.quantize
     idx_ref = idx_o.view(-1)
 
@@ -810,6 +819,40 @@ def test_vqseg_step_host_logic_against_oracle(vq_emu):
     n = vq_emu.names
     assert n.count("mas_bce_cl_forward") == 1 and n.count("mas_bce_cl_backward") == 1 and n.count("mas_nchw_to_nhwc_pad") == 1
     assert "mas_edge_small_cin_fprop" not in n and "mas_edge_small_cout_fprop" not in n      # both edge layers on the padded tensor route
+
+
+def test_vqseg_step_packs_padded_edge_weights_once_per_version(vq_emu):
+    """The zero-padded weights of the VQ-SEG edge layers (conv_in: 160 input channels; conv_out: 256 output rows, and 160 input
+    rows for its data gradient) are packed once per parameter version: a second step with unchanged parameters packs nothing.
+    The pads the kernels receive are zero, and conv_out's padded bias follows the bias alone."""
+    from mas_b200 import ops
+    m, seg, pw = _vqseg_model()
+    packs, biases = {}, []
+    pack, fprop = vq_emu.mas_pack_conv3x3_tc16, vq_emu.mas_conv3x3_fprop_tc16
+
+    def record_pack(w, w_tc16, w_dgrad, Cout, Cin, transpose):
+        pack(w, w_tc16, w_dgrad, Cout, Cin, transpose)
+        packs[(Cout, Cin)] = vq_emu.packs[_addr(w_tc16)][1]
+
+    def record_fprop(x, xs, wpk, bias, residual, y, ys, *rest):
+        if ys.c == 160:                                    # conv_out: 159 channels stored with a pitch of 160
+            biases.append(torch.from_numpy(_f32(bias, 256).copy()))
+        fprop(x, xs, wpk, bias, residual, y, ys, *rest)
+    vq_emu.mas_pack_conv3x3_tc16, vq_emu.mas_conv3x3_fprop_tc16 = record_pack, record_fprop
+    bias = m.decoder.model[-1].bias
+
+    def step():
+        first = len(vq_emu.names)
+        dec, diff = m(seg)
+        (ops.BCELogitsFn.apply(dec, seg, pw) + diff).backward()
+        assert torch.equal(biases[-1][:159], bias.detach()) and not biases[-1][159:].any()
+        return vq_emu.names[first:]
+    assert step().count("mas_pack_conv3x3_tc16") >= 3
+    assert not packs[(256, 128)][159:].any() and not packs[(160, 128)][159:].any() and not packs[(128, 160)][:, 159:].any()
+    assert "mas_pack_conv3x3_tc16" not in step()
+    with torch.no_grad():
+        bias.add_(1.0)
+    assert "mas_pack_conv3x3_tc16" not in step()
 
 
 def test_whole_model_modes_host_logic_against_reference_fixture(vq_emu):
