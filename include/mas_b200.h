@@ -533,6 +533,52 @@ int mas_lpips_relu_backward(const float* dy, const float* y, float* dx, int64_t 
 int mas_lpips_prep_backward(const float* dxp, const float* scale, float* J, int G, int H, int W, void* stream);
 int mas_lpips_scale_jacobian(const float* J, const float* g, int64_t g_stride, float* out, int B, int64_t per, void* stream);
 
+/* VGGFace2 face loss (losses/face_loss.py; ResNet-50 "caffe" style, eval BatchNorm folded into the convolutions by the host).
+ * The 1x1 convolutions run on mas_gemm_rows_f16 and the 3x3 ones on the 3x3 family; these entries are the rest of
+ * FaceLoss.forward and its data gradient.  Activations are channels-last fp32 over ONE batch of F <= 6 faces; face p and face
+ * p + P (P = F / 2) are a pair of the L1 taps.
+ * mas_face_prepare: crop + antialiased bilinear Resize(256) + CenterCrop(254) of every face into out [F,254,254,3] from the
+ *   NCHW (any-stride, 3-channel) img / rec, zeros outside the image (face_loss.py:143-160).  tab (int32) holds 14 ints per face
+ *   (source image, side 0 = img / 1 = rec, top, left, crop height, crop width, taps per output row, per output column, then
+ *   offsets into tab of the 254 row and 254 column start indices (crop coordinates) and of the adjoint ranges, 2 ints [lo, hi)
+ *   of output rows per crop row and of output columns per crop column, and offsets into wts of the 254 x taps row and column
+ *   weights).
+ * mas_face_prepare_backward: its adjoint for faces f0 .. f0+G-1 (gradient d [G,254,254,3]) into J [B,3,H,W] (dense NCHW, every
+ *   element written) for the images of one side; per pixel a fixed-order sum over the faces (deterministic).
+ * mas_face_stem_forward: conv1, 7x7 stride 2 pad 3, 3 -> 64, no bias: x [N,H,W,3] -> y [N,(H+1)/2,(W+1)/2,64] (feature 0);
+ *   w [64,3,7,7].  mas_face_stem_backward: its data gradient dy [N,(H+1)/2,(W+1)/2,64] -> dx [N,H,W,3].
+ * mas_face_pool_forward: bn1 (bn [2][C] = per-channel scale, shift) + ReLU + MaxPool2d(3, 2) over full windows (H, W odd):
+ *   x [N,H,W,C] -> y [N,(H-3)/2+1,(W-3)/2+1,C], arg (uint8, same shape) = row-major index of the window's first maximum;
+ *   amax (or NULL) = max of y.
+ * mas_face_pool_backward: dx [G,H,W,C] = scale * relu'(x * scale + shift) * (dp routed by arg) + the seed of level 0, for the
+ *   images f0 .. f0+G-1 (x, arg, dp: their [G,...] slices; dp NULL: the seed alone).
+ * Seeds: sgn (int8 [P,H,W,C], from mas_face_l1_forward) or NULL; face f gets +coef * sgn[f] for f < P, -coef * sgn[f - P] else.
+ * mas_face_l1_forward: f [2P,H,W,C] with n = P*H*W*C: part[k] (k < mas_face_l1_blocks()) = partial sums of |f[i] - f[n + i]|,
+ *   sgn[i] (or NULL) = sign(f[i] - f[n + i]).
+ * mas_face_l1_finalize: terms[l] = c_l * sum_k part[l][k] (c_l = alpha_l / (C H W) of level l), loss = their fp32 sum in
+ *   level order; part [5][mas_face_l1_blocks()].
+ * mas_face_subsample_half: y16 [N,(H+1)/2,(W+1)/2,C] = fp16(x[:, ::2, ::2] * s) of x [N,H,W,C], s the power-of-two operand
+ *   scale of *amax (as mas_to_half): the A operand of a stride-2 1x1 convolution.
+ * mas_face_relu_seed_backward: dz = out > 0 ? dout + seed : 0 over out [G,H,W,C] (a Bottleneck's output), dout [G,H,W,C], or
+ *   with half != 0 [G,(H+1)/2,(W+1)/2,C] reaching the even positions only (a stride-2 consumer), or NULL; amax = max|dz|. */
+int mas_face_prepare(const int* tab, const float* wts, int F, const float* img, mas_tensor4 is, const float* rec, mas_tensor4 rs,
+                     float* out, void* stream);
+int mas_face_prepare_backward(const int* tab, const float* wts, int f0, int G, int side, const float* d, float* J, int B, int H,
+                              int W, void* stream);
+int mas_face_stem_forward(const float* x, const float* w, float* y, int N, int H, int W, void* stream);
+int mas_face_stem_backward(const float* dy, const float* w, float* dx, int N, int H, int W, void* stream);
+int mas_face_pool_forward(const float* x, const float* bn, float* y, uint8_t* arg, int N, int H, int W, int C, float* amax,
+                          void* stream);
+int mas_face_pool_backward(const float* x, const float* bn, const uint8_t* arg, const float* dp, const int8_t* sgn, float coef,
+                           int f0, int P, int G, int H, int W, int C, float* dx, void* stream);
+int mas_face_l1_blocks(void);
+int mas_face_l1_forward(const float* f, int64_t n, int8_t* sgn, double* part, void* stream);
+int mas_face_l1_finalize(const double* part, double c0, double c1, double c2, double c3, double c4, float* terms, float* loss,
+                         void* stream);
+int mas_face_subsample_half(const float* x, void* y16, int N, int H, int W, int C, const float* amax, void* stream);
+int mas_face_relu_seed_backward(const float* out, const float* dout, int half, const int8_t* sgn, float coef, int f0, int P, int G,
+                                int H, int W, int C, float* dz, float* amax, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

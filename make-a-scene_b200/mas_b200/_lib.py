@@ -154,6 +154,17 @@ _SPEC = {
     "mas_lpips_relu_backward": (_I, [_P, _P, _P, _L, _P, _P]),
     "mas_lpips_prep_backward": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "mas_lpips_scale_jacobian": (_I, [_P, _P, _L, _P, _I, _L, _P]),
+    "mas_face_prepare": (_I, [_P, _P, _I, _P, _T, _P, _T, _P, _P]),
+    "mas_face_prepare_backward": (_I, [_P, _P, _I, _I, _I, _P, _P, _I, _I, _I, _P]),
+    "mas_face_stem_forward": (_I, [_P, _P, _P, _I, _I, _I, _P]),
+    "mas_face_stem_backward": (_I, [_P, _P, _P, _I, _I, _I, _P]),
+    "mas_face_pool_forward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
+    "mas_face_pool_backward": (_I, [_P, _P, _P, _P, _P, _F, _I, _I, _I, _I, _I, _I, _P, _P]),
+    "mas_face_l1_blocks": (_I, []),
+    "mas_face_l1_forward": (_I, [_P, _L, _P, _P, _P]),
+    "mas_face_l1_finalize": (_I, [_P, _D, _D, _D, _D, _D, _P, _P, _P]),
+    "mas_face_subsample_half": (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),
+    "mas_face_relu_seed_backward": (_I, [_P, _P, _I, _P, _F, _I, _I, _I, _I, _I, _I, _P, _P, _P]),
 }
 
 _lib = None

@@ -1792,3 +1792,354 @@ class LPIPSFn(torch.autograd.Function):
             grads.append(d)
             off += B
         return grads[0], grads[1], None, None, None, None, None
+
+
+# ---- VGGFace2 face loss (losses/face_loss.py) -------------------------------------------------------------------------
+FACE_CROP, FACE_RESIZE, FACE_MAX = 254, 256, 6   # CenterCrop(254) after Resize(256); faces[:6]
+FACE_BN_EPS = 1e-5
+
+
+def face_pairing(n, keep=FACE_MAX):
+    """The stacked crops [gt_0 .. gt_{n-1}, gen_0 .. gen_{n-1}] that faces[:keep] keeps (keep=None: all of them), as (side, k)
+    with side 0 = img (gt), 1 = rec (gen); chunk(2) pairs entry p with entry p + len / 2."""
+    return [(0, u) if u < n else (1, u - n) for u in range(2 * n if keep is None else min(keep, 2 * n))]
+
+
+def _resize_rows(n_in, n_out, offset):
+    """Rows offset .. offset + 253 of the antialiased bilinear resize n_in -> n_out (align_corners=False, as
+    F.interpolate(antialias=True) computes its taps): per output row the first input index lo, the tap count, and the
+    normalised weights [254, K] (zero beyond the row's count)."""
+    import numpy as np
+    o = np.arange(FACE_CROP, dtype=np.float64) + offset
+    if n_in == n_out:
+        return o.astype(np.int64), np.ones(FACE_CROP, dtype=np.int64), np.ones((FACE_CROP, 1))
+    scale = n_in / n_out
+    support, inv = (scale, 1.0 / scale) if scale >= 1.0 else (1.0, 1.0)
+    center = scale * (o + 0.5)
+    lo = np.maximum(np.trunc(center - support + 0.5), 0).astype(np.int64)
+    cnt = np.minimum(np.trunc(center + support + 0.5), n_in).astype(np.int64) - lo
+    j = np.arange(int(cnt.max()))
+    w = np.maximum(0.0, 1.0 - np.abs((j[None, :] + lo[:, None] - center[:, None] + 0.5) * inv)) * (j[None, :] < cnt[:, None])
+    tot = w.sum(axis=1, keepdims=True)
+    return lo, cnt, np.divide(w, tot, out=w.copy(), where=tot != 0)
+
+
+class FacePlan:
+    """Which crops run and how each is gathered: the host side of mas_face_prepare / mas_face_prepare_backward.
+    faces: per used crop (side, source image, top, left, crop height, crop width); n: boxes over zip(img, rec, bbox)."""
+
+    def __init__(self, img_shape, rec_shape, bboxes, keep=FACE_MAX):
+        boxes = []
+        for b in range(min(img_shape[0], rec_shape[0], len(bboxes))):
+            for box in bboxes[b]:
+                x0, y0, x1, y1 = (int(v) for v in list(box)[:4])
+                if y1 - y0 <= 0 or x1 - x0 <= 0:
+                    raise ValueError("FaceLoss: box %s of image %d has zero or negative extent" % ([x0, y0, x1, y1], b))
+                boxes.append((b, y0, x0, y1 - y0, x1 - x0))
+        self.n = len(boxes)
+        self.faces = [(side,) + boxes[k] for side, k in face_pairing(self.n, keep)]
+        self.F, self.P = len(self.faces), len(self.faces) // 2
+        import numpy as np
+        meta, idx, wts = [], [], []
+        base, nidx, nw = 14 * self.F, 0, 0
+        for side, src, top, left, ch, cw in self.faces:
+            short, long_ = min(ch, cw), max(ch, cw)
+            nl = int(FACE_RESIZE * long_ / short)
+            rh, rw = (FACE_RESIZE, nl) if ch <= cw else (nl, FACE_RESIZE)
+            # (rh, rw) == (ch, cw): Resize returns the crop unchanged; _resize_rows gives the identity taps for n_in == n_out
+            ct, cl = int(round((rh - FACE_CROP) / 2.0)), int(round((rw - FACE_CROP) / 2.0))
+            axes = []
+            for n_in, n_out, off in ((ch, rh, ct), (cw, rw, cl)):
+                lo, cnt, w = _resize_rows(n_in, n_out, off)
+                # output rows reading crop row i: lo and lo + cnt are non-decreasing, so they form one range [a, b)
+                i = np.arange(n_in)
+                a, b = np.searchsorted(lo + cnt, i, side="right"), np.searchsorted(lo, i, side="right")
+                rng = np.where((b > a)[:, None], np.stack([a, b], axis=1), 0).reshape(-1)
+                axes.append((w.shape[1], lo, rng, w.reshape(-1)))
+            (ky, sy, ay, wy), (kx, sx, ax, wx) = axes
+            o_sy = base + nidx
+            o_sx, o_ay = o_sy + FACE_CROP, o_sy + 2 * FACE_CROP
+            o_ax = o_ay + len(ay)
+            idx += [sy, sx, ay, ax]
+            nidx += 2 * FACE_CROP + len(ay) + len(ax)
+            o_wy, o_wx = nw, nw + len(wy)
+            wts += [wy, wx]
+            nw += len(wy) + len(wx)
+            meta += [src, side, top, left, ch, cw, ky, kx, o_sy, o_sx, o_ay, o_ax, o_wy, o_wx]
+        self.tab = torch.from_numpy(np.concatenate([np.asarray(meta, dtype=np.int64)] + idx).astype(np.int32))
+        self.wts = torch.from_numpy(np.concatenate(wts).astype(np.float32)) if wts else torch.zeros(1)
+
+    def sides(self):
+        return {f[0] for f in self.faces}
+
+    def span(self, want_img, want_rec):
+        """[g0, g1): the crops whose gradient reaches a wanted input (img crops come first, then rec crops)."""
+        ngt = sum(1 for f in self.faces if f[0] == 0)
+        return (0 if want_img else ngt), (self.F if want_rec else ngt)
+
+
+def _face_fold(conv, bn):
+    """(weight, bias) of conv followed by eval BatchNorm bn, folded in fp64 and cached per version of all five tensors."""
+    key = ("face_fold",) + tuple((t._version, t.data_ptr()) for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
+
+    def make():
+        s = bn.weight.detach().double() / torch.sqrt(bn.running_var.double() + bn.eps)
+        w = conv.weight.detach().double() * s.view(-1, *([1] * (conv.weight.dim() - 1)))
+        b = bn.bias.detach().double() - bn.running_mean.double() * s
+        w = w.float().contiguous()
+        return (w.reshape(w.shape[0], -1) if w.shape[-1] == 1 else w), b.float()
+    ent = _pack_entry(conv.weight)
+    hit = ent.get(key)
+    if hit is None or hit[0].device != conv.weight.device:
+        hit = ent[key] = make()
+    return hit
+
+
+def _face_bn_table(bn):
+    """[2, C] = (scale, shift) of eval BatchNorm bn (bn1, applied after feature 0), cached like _face_fold."""
+    key = ("face_bn",) + tuple((t._version, t.data_ptr()) for t in (bn.weight, bn.bias, bn.running_mean, bn.running_var))
+    ent = _pack_entry(bn.weight)
+    hit = ent.get(key)
+    if hit is None or hit.device != bn.weight.device:
+        s = bn.weight.detach().double() / torch.sqrt(bn.running_var.double() + bn.eps)
+        hit = ent[key] = torch.stack([s, bn.bias.detach().double() - bn.running_mean.double() * s]).float().contiguous()
+    return hit
+
+
+def _face_gemm_pack(w2d, transpose):
+    """fp16 row-GEMM image of a folded 1x1 weight [Cout, Cin] (transpose: of W^T), the output side zero-padded to 128."""
+    def make():
+        n, k = w2d.shape
+        rows, cols = (n, _round_up(k, 128)) if transpose else (_round_up(n, 128), k)
+        wp = _padded(w2d, (rows, cols)).contiguous()
+        wt = torch.empty(rows * cols, dtype=torch.float16, device=w2d.device)
+        L.call("mas_pack_gemm_tc16", wp, wt, rows, cols, int(transpose))
+        return wt
+    return _cached(w2d, ("face16", bool(transpose)), make)
+
+
+def _face_gemm(x16, am, w2d, n, h, w, transpose=False, bias=None, residual=None):
+    """y [n, Cout, h, w] channels-last = x . W^T (+bias +residual) (transpose: x . W) from the fp16 rows x16 on mas_gemm_rows_f16."""
+    cout, cin = (w2d.shape[1], w2d.shape[0]) if transpose else (w2d.shape[0], w2d.shape[1])
+    y = empty_nhwc(n, cout, h, w, x16)
+    if bias is not None:
+        bias = _padded(bias, (_round_up(cout, 128),))
+    L.call("mas_gemm_rows_f16", x16, n * h * w, cin, _face_gemm_pack(w2d, transpose), y, cout, cout, bias, residual, am, 1.0)
+    return y
+
+
+def _new_amax(like):
+    return torch.empty(1, dtype=torch.float32, device=like.device)
+
+
+def _half_of(x, am):
+    x16 = torch.empty(x.shape[0], x.shape[2], x.shape[3], x.shape[1], dtype=torch.float16, device=x.device)
+    L.call("mas_to_half", x, x16, x.numel(), am)
+    return x16
+
+
+def face_params(model):
+    """The network of a FaceLoss module as the kernels take it: stem weight, bn1 table, and per Bottleneck its stride and
+    folded (weight, bias) pairs (1x1 weights as [Cout, Cin]); every convolution is checked against the structure run here."""
+    blocks, layers = [], []
+    for li, layer in enumerate((model.layer1, model.layer2, model.layer3, model.layer4)):
+        layers.append(len(layer))
+        for blk in layer:
+            s = blk.conv1.stride[0]
+            ok = (blk.conv1.kernel_size == (1, 1) and blk.conv2.kernel_size == (3, 3) and blk.conv2.padding == (1, 1)
+                  and blk.conv2.stride == (1, 1) and blk.conv3.kernel_size == (1, 1) and blk.conv3.stride == (1, 1))
+            if not ok:
+                raise RuntimeError("FaceLoss: unexpected Bottleneck layout in layer%d" % (li + 1))
+            ds = None
+            if blk.downsample is not None:
+                conv, bn = blk.downsample[0], blk.downsample[1]
+                if conv.kernel_size != (1, 1) or conv.stride[0] != s:
+                    raise RuntimeError("FaceLoss: unexpected downsample in layer%d" % (li + 1))
+                ds = _face_fold(conv, bn)
+            elif s != 1 or blk.conv1.in_channels != blk.conv3.out_channels:
+                raise RuntimeError("FaceLoss: a Bottleneck without downsample must keep its shape")
+            blocks.append(dict(stride=s, c1=_face_fold(blk.conv1, blk.bn1), c2=_face_fold(blk.conv2, blk.bn2),
+                               c3=_face_fold(blk.conv3, blk.bn3), ds=ds))
+    c1 = model.conv1
+    if c1.weight.shape != (64, 3, 7, 7) or c1.stride != (2, 2) or c1.padding != (3, 3) or c1.bias is not None:
+        raise RuntimeError("FaceLoss: conv1 must be Conv2d(3, 64, 7, stride 2, padding 3, bias=False)")
+    mp = model.maxpool
+    if mp.kernel_size not in (3, (3, 3)) or mp.stride not in (2, (2, 2)) or mp.padding not in (0, (0, 0)):
+        raise RuntimeError("FaceLoss: maxpool must be MaxPool2d(3, 2)")
+    return dict(stem=c1.weight.detach().contiguous(), bn1=_face_bn_table(model.bn1), blocks=blocks, layers=layers,
+                alphas=[float(a) for a in model.alphas])
+
+
+def _face_block_forward(x, am, blk):
+    n, cin, h, w = x.shape
+    s = blk["stride"]
+    ho, wo = ((h + 1) // 2, (w + 1) // 2) if s == 2 else (h, w)
+    if s == 2:
+        x16 = torch.empty((n, ho, wo, cin), dtype=torch.float16, device=x.device)
+        L.call("mas_face_subsample_half", x, x16, n, h, w, cin, am)
+    else:
+        x16 = _half_of(x, am)
+    (w1, b1), (w2, b2), (w3, b3) = blk["c1"], blk["c2"], blk["c3"]
+    h1 = _face_gemm(x16, am, w1, n, ho, wo, bias=b1)
+    am1 = _new_amax(x)
+    L.call("mas_lpips_relu", h1, h1.numel(), am1)
+    h2 = conv3x3_raw(h1, w2, b2, None, L.CONV_S1, x_amax=am1, pad_out=True)
+    am2 = _new_amax(x)
+    L.call("mas_lpips_relu", h2, h2.numel(), am2)
+    res = x if blk["ds"] is None else _face_gemm(x16, am, blk["ds"][0], n, ho, wo, bias=blk["ds"][1])
+    out = _face_gemm(_half_of(h2, am2), am2, w3, n, ho, wo, bias=b3, residual=res)
+    amo = _new_amax(x)
+    L.call("mas_lpips_relu", out, out.numel(), amo)
+    return out, amo, (h1, h2, out)
+
+
+def face_crops(img, rec, plan):
+    """The crops of a plan as one [F, 3, 254, 254] tensor (channels-last memory), no autograd."""
+    x = empty_nhwc(plan.F, 3, FACE_CROP, FACE_CROP, img)
+    L.call("mas_face_prepare", plan.tab.to(img.device, non_blocking=True), plan.wts.to(img.device, non_blocking=True), plan.F,
+           img, L.t4(img), rec, L.t4(rec), x)
+    return x
+
+
+def face_forward_raw(img, rec, plan, params, span=None):
+    """FaceLoss.forward on the kernels for a plan with at least one crop: returns the crops [F, 3, 254, 254], the five
+    features, the five level terms, the loss and (span = [g0, g1) given) what the backward of those crops needs."""
+    dev = img.device
+    F, P = plan.F, plan.P
+    tab, wts = plan.tab.to(dev, non_blocking=True), plan.wts.to(dev, non_blocking=True)
+    x = empty_nhwc(F, 3, FACE_CROP, FACE_CROP, img)
+    L.call("mas_face_prepare", tab, wts, F, img, L.t4(img), rec, L.t4(rec), x)
+    hs = (FACE_CROP - 1) // 2 + 1
+    f0 = empty_nhwc(F, 64, hs, hs, img)
+    L.call("mas_face_stem_forward", x, params["stem"], f0, F, FACE_CROP, FACE_CROP)
+    hp = (hs - 3) // 2 + 1
+    cur = empty_nhwc(F, 64, hp, hp, img)
+    arg = torch.empty((F, hp, hp, 64), dtype=torch.uint8, device=dev)
+    am = _new_amax(img)
+    L.call("mas_face_pool_forward", f0, params["bn1"], cur, arg, F, hs, hs, 64, am)
+    feats, acts, bi = [f0], [], 0
+    for nb in params["layers"]:
+        for _ in range(nb):
+            cur, am, a = _face_block_forward(cur, am, params["blocks"][bi])
+            acts.append(a)
+            bi += 1
+        feats.append(cur)
+    nblk = int(L.query("mas_face_l1_blocks"))
+    part = torch.empty((5, nblk), dtype=torch.float64, device=dev)
+    signs = []
+    for l, f in enumerate(feats):
+        n = P * f[0].numel()
+        sgn = torch.empty(n, dtype=torch.int8, device=dev) if span is not None else None
+        L.call("mas_face_l1_forward", f, n, sgn, part[l])
+        signs.append(sgn)
+    coef = [a / f[0].numel() for a, f in zip(params["alphas"], feats)]
+    terms = torch.empty(5, dtype=torch.float32, device=dev)
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    L.call("mas_face_l1_finalize", part, *coef, terms, loss)
+    out = dict(crops=x, feats=feats, terms=terms, loss=loss)
+    if span is not None:
+        g0, g1 = span
+        keep = (lambda t: t) if (g0, g1) == (0, F) else (lambda t: t[g0:g1].clone(memory_format=torch.channels_last))
+        out["saved"] = dict(tab=tab, wts=wts, f0=keep(f0), arg=arg[g0:g1].clone() if (g0, g1) != (0, F) else arg,
+                            acts=[tuple(keep(t) for t in a) for a in acts], signs=signs, coef=coef, span=span)
+    return out
+
+
+def _face_backward(sv, params, plan, want, img_shape):
+    """d loss / d img, d loss / d rec for a unit seed (dense NCHW, None where not wanted)."""
+    g0, g1 = sv["span"]
+    G, P = g1 - g0, plan.P
+    signs, coef = sv["signs"], sv["coef"]
+    d, half, bi = None, 0, len(params["blocks"])
+    ends = set()
+    k = 0
+    for nb in params["layers"]:
+        k += nb
+        ends.add(k - 1)
+    lvl = len(params["layers"])
+    for i in reversed(range(bi)):
+        blk = params["blocks"][i]
+        h1, h2, out = sv["acts"][i]
+        _, c, h, w = out.shape
+        tap = i in ends
+        dz = torch.empty_like(out)
+        am = _new_amax(out)
+        L.call("mas_face_relu_seed_backward", out, d, half, signs[lvl] if tap else None, coef[lvl] if tap else 0.0, g0, P, G, h, w, c,
+               dz, am)
+        if tap:
+            lvl -= 1
+        dz16 = _half_of(dz, am)
+        (w1, _), (w2, _), (w3, _) = blk["c1"], blk["c2"], blk["c3"]
+        dh2 = _face_gemm(dz16, am, w3, G, h, w, transpose=True)
+        am2 = _new_amax(out)
+        L.call("mas_lpips_relu_backward", dh2, h2, dh2, dh2.numel(), am2)
+        dh1 = conv3x3_raw(dh2, w2, None, None, L.CONV_S1, transpose=True, x_amax=am2, pad_out=True)
+        am1 = _new_amax(out)
+        L.call("mas_lpips_relu_backward", dh1, h1, dh1, dh1.numel(), am1)
+        r = dz if blk["ds"] is None else _face_gemm(dz16, am, blk["ds"][0], G, h, w, transpose=True)
+        d = _face_gemm(_half_of(dh1, am1), am1, w1, G, h, w, transpose=True, residual=r)
+        half = int(blk["stride"] == 2)
+    f0 = sv["f0"]
+    _, c, hs, _ = f0.shape
+    df0 = torch.empty_like(f0)
+    L.call("mas_face_pool_backward", f0, params["bn1"], sv["arg"], d, signs[0], coef[0], g0, P, G, hs, hs, c, df0)
+    dx = empty_nhwc(G, 3, FACE_CROP, FACE_CROP, f0)
+    L.call("mas_face_stem_backward", df0, params["stem"], dx, G, FACE_CROP, FACE_CROP)
+    out = []
+    for side, shp in enumerate(img_shape):
+        if not want[side]:
+            out.append(None)
+            continue
+        J = torch.empty(shp, dtype=torch.float32, device=f0.device)
+        L.call("mas_face_prepare_backward", sv["tab"], sv["wts"], g0, G, side, dx, J, shp[0], shp[2], shp[3])
+        out.append(J)
+    return out
+
+
+class FaceLossFn(torch.autograd.Function):
+    """FaceLoss.forward (face_loss.py:123-140) as one unit over a FacePlan with at least one crop -> 0-dim fp32 loss.
+
+    The loss is linear in its seeds, so d loss / d input = g * J with J its gradient for a unit seed: the first backward runs
+    the network's data gradient once for the crops whose gradient is wanted, keeps J and drops the activations; every later
+    traversal of a retained graph is one scaling kernel and gives the same result."""
+
+    @staticmethod
+    def forward(ctx, img, rec, plan, params):
+        _need_cuda(img)
+        _need_cuda(rec)
+        if not f16_operands():
+            raise RuntimeError("the face loss runs its 1x1 convolutions on the fp16-operand row GEMM; select fp16 operands")
+        for t in (img, rec):
+            if t.dim() != 4 or t.shape[1] != 3:
+                raise RuntimeError("FaceLoss expects [B, 3, H, W] images, got %s" % (tuple(t.shape),))
+        want = (ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        span = plan.span(*want) if any(want) else None
+        r = face_forward_raw(img, rec, plan, params, span if span is not None and span[1] > span[0] else None)
+        ctx.sv, ctx.plan, ctx.params = r.get("saved"), plan, params
+        ctx.shapes = (tuple(img.shape), tuple(rec.shape))
+        ctx.J = None
+        return r["loss"]
+
+    @staticmethod
+    def backward(ctx, g):
+        if torch.is_grad_enabled():
+            raise RuntimeError("FaceLoss does not support create_graph (double backward)")
+        want = (ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        if ctx.J is None:
+            if ctx.sv is None:
+                ctx.J = [None, None]
+            else:
+                ctx.J = _face_backward(ctx.sv, ctx.params, ctx.plan, want, ctx.shapes)
+            ctx.sv = None
+        grads = []
+        for side in range(2):
+            J = ctx.J[side]
+            if not want[side]:
+                grads.append(None)
+            elif J is None:
+                grads.append(torch.zeros(ctx.shapes[side], dtype=torch.float32, device=g.device))
+            else:
+                d = torch.empty_like(J)
+                L.call("mas_lpips_scale_jacobian", J, g.reshape(1).contiguous(), 0, d, 1, J.numel())
+                grads.append(d)
+        return grads[0], grads[1], None, None
