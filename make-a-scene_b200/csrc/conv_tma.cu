@@ -2,19 +2,26 @@
 // of the activation (written channels-last by the producing kernel: GroupNorm(+SiLU) apply in the forward pass, GroupNorm
 // backward in the backward pass) instead of being converted by producer warps.
 //
-//   * one persistent CTA per SM walks work items (pair of 128-pixel tiles x 128 output channels);
+//   * one persistent CTA per SM walks work items (unit of 256 pixels - one 32 x 8 tile or a pair of 16 x 8 tiles - x 64 output
+//     channels [x output phase]). Its two MMA warpgroups take the CTA's items alternately ("ping-pong"): a warpgroup runs an
+//     item's whole K loop and then its epilogue, and issues the first MMA of an item only after the other warpgroup has issued
+//     the last MMA of the previous one (one mbarrier per warpgroup). The epilogues therefore alternate instead of running in
+//     step, and one warpgroup's stores (residual loads, statistics) run while the other warpgroup keeps the tensor cores busy;
 //   * A: ONE cp.async.bulk.tensor (4-D map over [N][H][W][C] halves, box 1 x 18 x 10 x 64, 128-byte swizzle, out-of-image
-//     halo pixels zero-filled by the copy engine) per tile per 64-channel chunk.  The staged halo is [180 pixels][128 B];
+//     halo pixels zero-filled by the copy engine) per tile per 64-channel chunk, loaded again for each channel tile of the
+//     unit (from L2).  The staged halo is [180 pixels][128 B];
 //     the nine taps and the four K = 16 steps of the chunk are descriptor start-address shifts ((ty*10+tx)*128 + k*32 bytes)
 //     over that one copy: the 8-row core group is eight horizontally adjacent pixels, the group stride (SBO) one staged image
 //     row = 1280 B;
-//   * B (weights): the same pre-packed no-swizzle stages as shift_gemm_tc (mas_pack_conv3x3_tc16), one bulk copy per
-//     16-channel step, ring of three;
+//   * B (weights): the item's 64-channel half of the pre-packed no-swizzle stages of shift_gemm_tc (mas_pack_conv3x3_tc16),
+//     whose two halves interleave in every (tap, k / 8) slab of 128 channels x 16 B: one 3-D tensor-map copy per 16-channel
+//     step picks 1 KB of each slab and lands [tap][k / 8][64 channels][16 B] (LBO 1 KB, tap stride 2 KB); ring of seven;
 //   * operand roles are swapped (D^T = W x X^T: the packed weights are the M-side operand, the pixels the N side of
-//     wgmma.m64n256k16 / two m64n128k16): warpgroup g owns output channels 64 g .. 64 g + 63 of the tile, so bias and
-//     GroupNorm statistics are per-row scalars of the accumulator fragment;
+//     wgmma.m64n256k16 / two m64n128k16): the item's 64 output channels are the rows of the warpgroup's accumulator, so bias
+//     and GroupNorm statistics are per-row scalars of the fragment;
 //   * warps 0-7 MMA + epilogue (two warpgroups), warp 8 copy issuer (its warpgroup hands its registers to the MMA ones): no
-//     thread of the CTA touches the operands; the copy issuer fills the rings of the next item while the warpgroups store the current one.
+//     thread of the CTA touches the operands. The copy issuer fills the rings in item order, the order in which the
+//     warpgroups' K loops drain them, so one ring serves both warpgroups.
 //
 // Reference call sites replaced: nn.Conv2d 3x3 stride 1 (modules.py:93-104) forward and its data gradient.
 //
@@ -46,10 +53,11 @@ namespace tc {
 
 constexpr int T_MMA_WARPS = 8;
 constexpr int T_THREADS = (T_MMA_WARPS + 4) * 32;   // + the copy-issuing warpgroup
-constexpr int T_ASTAGES = 2, T_BSTAGES = 3;
+constexpr int T_ASTAGES = 2, T_BSTAGES = 7;
 constexpr int T_ATILE = 23 * 1024;                  // 18 x 10 halo pixels x 128 B = 23040, padded to the 1024-byte swizzle atom
 constexpr int T_ASTAGE = 2 * T_ATILE;               // pair of 16 x 8 tiles, or one 32 x 8 tile (34 x 10 halo = 43520 B)
-constexpr int T_BSTAGE = 9 * 2 * BN * 16;           // nine taps x 16 channels x 128 output channels (fp16)
+constexpr int T_CO = 64;                            // output channels per work item: the M extent of one warpgroup's MMAs
+constexpr int T_BSTAGE = 9 * 2 * T_CO * 16;         // nine taps x 16 channels x 64 output channels (fp16)
 
 struct HParams {
   const void* wpk;    // mas_pack_conv3x3_tc16 packing
@@ -90,15 +98,17 @@ __device__ __forceinline__ bool unit_tile(const HParams& p, int64_t u, int hf, i
 }
 
 // TALL: the unit is one 32 x 8 tile whose staged halo (34 x 10 pixels, uniform 1280-byte row pitch) is ONE N = 256 operand:
-// per K = 16 step and tap a single m64n256 MMA per warpgroup instead of two m64n128 ones over the two halos of a pair.
+// per K = 16 step and tap a single m64n256 MMA instead of two m64n128 ones over the two halos of a pair.
 // PH: 0 the nine taps of a stride-1 3x3 convolution, 1 phase-out, 2 phase-in (see the top of the file).
 template <bool TALL, int PH = 0>
-__global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, const __grid_constant__ CUtensorMap x_map) {
+__global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, const __grid_constant__ CUtensorMap x_map,
+                                                               const __grid_constant__ CUtensorMap w_map) {
   constexpr int TAPS = PH == 0 ? 9 : 4;              // phase forms: groups with fewer taps carry zero weights
   constexpr int GOUT = PH == 1 ? 4 : 1;              // output phases per work unit
   constexpr int KPL = PH == 2 ? 4 : 1;               // source planes per K loop
-  constexpr int LBO_B = BN * 16, B_TAP = 2 * LBO_B;
+  constexpr int SLAB = T_CO * 16, B_TAP = 2 * SLAB;  // staged weights: [tap][k / 8][64 channels][8 halves]
   constexpr int A_BYTES = TALL ? 34 * 10 * 128 : 2 * 18 * 10 * 128;
+  constexpr int RB = 2;                              // epilogue: image rows whose residuals are loaded together (registers)
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
@@ -112,6 +122,229 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
   auto aempty = [&](int s) { return bar_base + 8u * (T_ASTAGES + s); };
   auto bfull = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + s); };
   auto bempty = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + T_BSTAGES + s); };
+  auto order = [&](int g) { return bar_base + 8u * (2 * T_ASTAGES + 2 * T_BSTAGES + g); };   // warpgroup g may start its next mainloop
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int achunks = p.Cin / 64;
+  const int kiters = KPL * achunks;
+  const int ctiles = (p.Cstore + T_CO - 1) / T_CO;   // channel tiles with stored channels: the others are never computed
+  const int64_t nitems = p.units * ctiles * GOUT;    // channel tile (then output phase) fastest: a unit's halo is re-read from L2
+
+  if (tid == 0) {
+    for (int s = 0; s < T_ASTAGES; ++s) { mbar_init(afull(s), 1); mbar_init(aempty(s), 128); }
+    for (int s = 0; s < T_BSTAGES; ++s) { mbar_init(bfull(s), 1); mbar_init(bempty(s), 128); }
+    for (int g = 0; g < 2; ++g) mbar_init(order(g), 128);
+    fence_barrier_init();
+  }
+  __syncthreads();
+
+  if (warp < T_MMA_WARPS) {
+    wg::regs_inc<wg::MMA_REGS>();
+    // ===================== MMA warpgroups, each one its own items: mainloop, then epilogue =====================
+    // acc[64 h + 4 j + 2 i + c] = D^T[channel 16 (warp % 4) + lane / 4 + 8 i of the item][pixel 128 h + 8 j + 2 (lane % 4) + c]
+    float inv_scale = 1.f;
+    operand_scale(p.x_amax, &inv_scale);
+    const float alpha = inv_scale;
+    const int wgi = warp >> 2;
+    const int frow = (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
+    float acc[128];
+    // the CTA's items are blockIdx.x + q gridDim.x, q = 0, 1, ...: warpgroup wgi takes the q of its parity, and the rings are
+    // filled and drained in q order, kiters halo stages and 4 kiters weight stages per item
+    for (int q = wgi;; q += 2) {
+      const int64_t item = blockIdx.x + (int64_t)q * gridDim.x;
+      if (item >= nitems) break;
+      const int gout = PH == 1 ? (int)((item / ctiles) % GOUT) : 0;
+      const int a0 = q * kiters, b0 = 4 * a0;
+      int as = a0 % T_ASTAGES, bs = b0 % T_BSTAGES, prev_b = 0, prev_a = -1;
+      uint32_t aph = (uint32_t)(a0 / T_ASTAGES) & 1u, bph = (uint32_t)(b0 / T_BSTAGES) & 1u;
+      // ordered mainloops: the first MMA of item q only after the other warpgroup has issued the last one of item q - 1, so
+      // the two warpgroups' epilogues alternate instead of falling into step
+      if (q > 0) mbar_wait(order(wgi), (uint32_t)((q - 1) >> 1) & 1u);
+      for (int kk = 0; kk < kiters; ++kk) {
+        const int grp = PH == 2 ? kk / achunks : gout;
+        mbar_wait(afull(as), aph);
+        const uint64_t xd0 = wg::desc(a_base + (uint32_t)as * T_ASTAGE, 16, 1280, wg::SW_128);
+#pragma unroll 1
+        for (int sub = 0; sub < 4; ++sub) {
+          mbar_wait(bfull(bs), bph);
+          const uint64_t wd0 = wg::desc(b_base + (uint32_t)bs * T_BSTAGE, SLAB, 128);
+          const uint64_t xds = xd0 + (uint64_t)((sub * 32) >> 4);
+          const uint32_t acc0 = (kk > 0 || sub > 0) ? 1u : 0u;
+          wg::fence();
+#pragma unroll
+          for (int t = 0; t < TAPS; ++t) {
+            const uint32_t tapoff = (uint32_t)((PH == 0 ? (t / 3) * 10 + (t % 3) : p.ph_hoff[grp][t]) * 128);
+            const uint64_t wd = wd0 + (uint64_t)((t * B_TAP) >> 4);
+            const uint64_t xd = xds + (uint64_t)(tapoff >> 4);
+            // D^T = W x X^T: weights on the M side, pixels on the N side
+            if (TALL) {
+              wg::wgmma_f16_ss_n256<0, 0>(acc, wd, xd, t > 0 ? 1u : acc0);
+            } else {
+              wg::wgmma_f16_ss_n128<0, 0>(acc, wd, xd, t > 0 ? 1u : acc0);
+              wg::wgmma_f16_ss_n128<0, 0>(acc + 64, wd, xd + (uint64_t)(T_ATILE >> 4), t > 0 ? 1u : acc0);
+            }
+          }
+          wg::commit();
+          if (kk == kiters - 1 && sub == 3) mbar_arrive(order(wgi ^ 1));   // every MMA of the item is issued
+          // the previous step's MMAs have read their weight stage (and, after a chunk's last step, its halo stage)
+          wg::wait<1>();
+          if (kk > 0 || sub > 0) {
+            mbar_arrive(bempty(prev_b));
+            if (prev_a >= 0) mbar_arrive(aempty(prev_a));
+          }
+          prev_b = bs;
+          prev_a = (sub == 3) ? as : -1;
+          if (++bs == T_BSTAGES) { bs = 0; bph ^= 1; }
+        }
+        if (++as == T_ASTAGES) { as = 0; aph ^= 1; }
+      }
+      wg::wait<0>();
+      wg::fence_regs<128>(acc);
+      mbar_arrive(bempty(prev_b));
+      mbar_arrive(aempty(prev_a));
+
+      const int64_t unit = item / (ctiles * GOUT);
+      const int ch_tile = (int)(item % ctiles) * T_CO;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        int n_img, ty_, tx_;
+        const bool live = unit_tile<TALL>(p, unit, h, n_img, ty_, tx_);   // warpgroup-uniform
+        if (!live) continue;
+        const int64_t pix0 = ((int64_t)n_img * p.H + ty_ * 16) * p.W + tx_ * 8;
+        const int64_t cstep = PH == 0 ? p.ldy : p.ysw;
+        const int64_t ybase = PH == 0 ? 0 : n_img * p.ysn + (ty_ * 16) * p.ysh + (tx_ * 8) * p.ysw + (PH == 1 ? p.ph_yoff[gout] : 0);
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+          const int ch = ch_tile + frow + 8 * i;
+          const bool st_ok = ch < p.Cstore;
+          const float bv = (p.bias && st_ok) ? __ldg(p.bias + ch) : 0.f;
+#pragma unroll
+          for (int cb = 0; cb < 4; ++cb) {         // 32-pixel groups = four image rows of the 16 x 8 tile
+            float st_s = 0.f, st_q = 0.f;
+#pragma unroll
+            for (int jp = 0; jp < 4; jp += RB) {
+              float rv[RB][2];                     // residuals of RB rows, loaded together ahead of their stores
+              if (p.res && st_ok) {
+#pragma unroll
+                for (int jj = 0; jj < RB; ++jj) {
+                  const int j = cb * 4 + jp + jj;
+                  const int64_t off = PH == 0 ? (pix0 + (int64_t)j * p.W + fcol) * p.ldy + ch : ybase + j * p.ysh + fcol * p.ysw + ch;
+#pragma unroll
+                  for (int cc = 0; cc < 2; ++cc) rv[jj][cc] = __ldg(p.res + off + cc * cstep);
+                }
+              }
+#pragma unroll
+              for (int jj = 0; jj < RB; ++jj) {
+                const int j = cb * 4 + jp + jj;    // pixel row j of the tile, columns fcol, fcol + 1
+                const int64_t off = PH == 0 ? (pix0 + (int64_t)j * p.W + fcol) * p.ldy + ch : ybase + j * p.ysh + fcol * p.ysw + ch;
+#pragma unroll
+                for (int cc = 0; cc < 2; ++cc) {
+                  float o = fmaf(acc[64 * h + 4 * j + 2 * i + cc], alpha, bv);
+                  if (st_ok) {
+                    if (p.res) o += rv[jj][cc];
+                    p.y[off + cc * cstep] = o;
+                    st_s += o;
+                    st_q = fmaf(o, o, st_q);
+                  }
+                }
+              }
+            }
+            if (p.stats_part) {   // same partial layout as shift_gemm_tc: [16 x 8 tile][32-pixel group][channel quad][sum, sumsq]
+              st_s += __shfl_xor_sync(0xffffffffu, st_s, 1);   // the four lanes of a channel row: all 32 pixels
+              st_q += __shfl_xor_sync(0xffffffffu, st_q, 1);
+              st_s += __shfl_xor_sync(0xffffffffu, st_s, 2);
+              st_q += __shfl_xor_sync(0xffffffffu, st_q, 2);
+              st_s += __shfl_xor_sync(0xffffffffu, st_s, 4);   // four consecutive channel rows: the quad
+              st_q += __shfl_xor_sync(0xffffffffu, st_q, 4);
+              st_s += __shfl_xor_sync(0xffffffffu, st_s, 8);
+              st_q += __shfl_xor_sync(0xffffffffu, st_q, 8);
+              if ((lane & 15) == 0) {
+                const size_t tile = ((size_t)n_img * p.tiles_y + ty_) * p.tiles_x + tx_;
+                float* sp = p.stats_part + ((tile * 4 + cb) * (p.Cout >> 2) + (ch >> 2)) * 2;
+                sp[0] = st_s;
+                sp[1] = st_q;
+              }
+            }
+          }
+        }
+      }
+    }
+  } else {
+    // ===================== copy issuer (one thread): halos by tensor map, weight stages by tensor map =====================
+    wg::regs_dec<wg::COPY_REGS>();
+    if (warp == T_MMA_WARPS && lane == 0) {
+      int as = 0, bs = 0;
+      uint32_t aph = 0, bph = 0;
+      // weight images in 2 KB slabs (one k / 8 half of a tap, 128 channels); phase forms have one image per tap group:
+      // [group][128-channel tile][16-channel K step][tap][k / 8][128][8 halves]
+      const int tile_slabs = (p.Cin / 16) * 2 * TAPS, group_slabs = (p.Cout / BN) * tile_slabs;
+      for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
+        const int ct = (int)(item % ctiles);
+        const int gout = PH == 1 ? (int)((item / ctiles) % GOUT) : 0;
+        const int64_t unit = item / (ctiles * GOUT);
+        for (int kk = 0; kk < kiters; ++kk) {
+          const int grp = PH == 2 ? kk / achunks : gout, c = kk % achunks;
+          const int slab0 = grp * group_slabs + (ct >> 1) * tile_slabs + c * 8 * TAPS;   // the chunk's first slab
+          mbar_wait(aempty(as), aph ^ 1);
+          mbar_expect_tx(afull(as), A_BYTES);
+#pragma unroll
+          for (int hf = 0; hf < (TALL ? 1 : 2); ++hf) {
+            int n, ty_, tx_;
+            unit_tile<TALL>(p, unit, hf, n, ty_, tx_);   // a missing second tile re-reads the last one (never stored)
+            const uint32_t dst = a_base + (uint32_t)(as * T_ASTAGE + hf * T_ATILE);
+            if (PH == 2)   // plane (py, px) = grp: channel half px of the pixel pair, row parity py
+              tma_load_5d(dst, &x_map, (grp & 1) * p.Cin + c * 64, tx_ * 8 - 1, grp >> 1, ty_ * 16 - 1, n, afull(as));
+            else
+              tma_load_4d(dst, &x_map, c * 64, tx_ * 8 - 1, ty_ * 16 - 1, n, afull(as));
+          }
+          if (++as == T_ASTAGES) { as = 0; aph ^= 1; }
+          for (int sub = 0; sub < 4; ++sub) {
+            mbar_wait(bempty(bs), bph ^ 1);
+            mbar_expect_tx(bfull(bs), TAPS * B_TAP);
+            // the item's 64-channel half (ct & 1) of each of the step's 2 TAPS slabs
+            tma_load_3d(b_base + (uint32_t)bs * T_BSTAGE, &w_map, 0, ct & 1, slab0 + sub * 2 * TAPS, bfull(bs));
+            if (++bs == T_BSTAGES) { bs = 0; bph ^= 1; }
+          }
+        }
+      }
+    }
+    __syncwarp();
+  }
+}
+
+constexpr size_t t16_smem_bytes() {
+  return 1024 + (size_t)T_ASTAGES * T_ASTAGE + (size_t)T_BSTAGES * T_BSTAGE + (2 * T_ASTAGES + 2 * T_BSTAGES + 2) * 8 + 16;
+}
+static_assert(t16_smem_bytes() <= 227 * 1024, "shift_gemm_t16 rings exceed the shared memory of an SM");
+
+// Cooperative form: both MMA warpgroups work on one item of 128 output channels at the same time (warpgroup g owns channels
+// 64 g .. 64 g + 63), so their epilogues run together, with the tensor cores idle. Two warpgroups issuing together keep the
+// tensor cores busier than one, so the launchers pick this form where ping-pong has little epilogue to hide: at most two
+// items per CTA (conv3x3_fprop_tma16_launch) and the deep phase layers, whose long K loops of four-tap groups dwarf the
+// epilogue (conv3x3_phase_tma16_launch). Weights: one bulk copy of a 16-channel step for all 128 channels, ring of three.
+constexpr int TC_BSTAGES = 3;
+constexpr int TC_BSTAGE = 9 * 2 * BN * 16;          // nine taps x 16 channels x 128 output channels (fp16)
+
+template <bool TALL, int PH>
+__global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16_coop(const HParams p, const __grid_constant__ CUtensorMap x_map) {
+  constexpr int TAPS = PH == 0 ? 9 : 4;              // phase forms: groups with fewer taps carry zero weights
+  constexpr int GOUT = PH == 1 ? 4 : 1;              // output phases per work unit
+  constexpr int KPL = PH == 2 ? 4 : 1;               // source planes per K loop
+  constexpr int LBO_B = BN * 16, B_TAP = 2 * LBO_B;
+  constexpr int A_BYTES = TALL ? 34 * 10 * 128 : 2 * 18 * 10 * 128;
+
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t raw_base = smem_u32(smem_raw);
+  const uint32_t smem_base = (raw_base + 1023u) & ~1023u;           // swizzle atoms are 1024-byte aligned
+  uint8_t* smem = smem_raw + (smem_base - raw_base);
+  const uint32_t a_base = smem_base;
+  const uint32_t b_base = a_base + T_ASTAGES * T_ASTAGE;
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + T_ASTAGES * T_ASTAGE + TC_BSTAGES * TC_BSTAGE);
+  const uint32_t bar_base = smem_u32(bars);
+  auto afull = [&](int s) { return bar_base + 8u * s; };
+  auto aempty = [&](int s) { return bar_base + 8u * (T_ASTAGES + s); };
+  auto bfull = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + s); };
+  auto bempty = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + TC_BSTAGES + s); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int achunks = p.Cin / 64;
@@ -121,7 +354,7 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
 
   if (tid == 0) {
     for (int s = 0; s < T_ASTAGES; ++s) { mbar_init(afull(s), 1); mbar_init(aempty(s), T_MMA_WARPS * 32); }
-    for (int s = 0; s < T_BSTAGES; ++s) { mbar_init(bfull(s), 1); mbar_init(bempty(s), T_MMA_WARPS * 32); }
+    for (int s = 0; s < TC_BSTAGES; ++s) { mbar_init(bfull(s), 1); mbar_init(bempty(s), T_MMA_WARPS * 32); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -147,7 +380,7 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
 #pragma unroll 1
         for (int sub = 0; sub < 4; ++sub) {
           mbar_wait(bfull(bs), bph);
-          const uint64_t wd0 = wg::desc(b_base + (uint32_t)bs * T_BSTAGE + (uint32_t)(wgi * 1024), LBO_B, 128);
+          const uint64_t wd0 = wg::desc(b_base + (uint32_t)bs * TC_BSTAGE + (uint32_t)(wgi * 1024), LBO_B, 128);
           const uint64_t xds = xd0 + (uint64_t)((sub * 32) >> 4);
           const uint32_t acc0 = (kk > 0 || sub > 0) ? 1u : 0u;
           wg::fence();
@@ -173,7 +406,7 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
           }
           prev_b = bs;
           prev_a = (sub == 3) ? as : -1;
-          if (++bs == T_BSTAGES) { bs = 0; bph ^= 1; }
+          if (++bs == TC_BSTAGES) { bs = 0; bph ^= 1; }
         }
         if (++as == T_ASTAGES) { as = 0; aph ^= 1; }
       }
@@ -266,8 +499,8 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
           for (int sub = 0; sub < 4; ++sub) {
             mbar_wait(bempty(bs), bph ^ 1);
             mbar_expect_tx(bfull(bs), bstage);
-            bulk_g2s(b_base + (uint32_t)bs * T_BSTAGE, wsrc + (size_t)(c * 4 + sub) * bstage, bstage, bfull(bs));
-            if (++bs == T_BSTAGES) { bs = 0; bph ^= 1; }
+            bulk_g2s(b_base + (uint32_t)bs * TC_BSTAGE, wsrc + (size_t)(c * 4 + sub) * bstage, bstage, bfull(bs));
+            if (++bs == TC_BSTAGES) { bs = 0; bph ^= 1; }
           }
         }
       }
@@ -276,8 +509,8 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
   }
 }
 
-constexpr size_t t16_smem_bytes() {
-  return 1024 + (size_t)T_ASTAGES * T_ASTAGE + (size_t)T_BSTAGES * T_BSTAGE + (2 * T_ASTAGES + 2 * T_BSTAGES) * 8 + 16;
+constexpr size_t t16c_smem_bytes() {
+  return 1024 + (size_t)T_ASTAGES * T_ASTAGE + (size_t)TC_BSTAGES * TC_BSTAGE + (2 * T_ASTAGES + 2 * TC_BSTAGES) * 8 + 16;
 }
 
 // ------------------------------------------------------------------------------------------------------------
@@ -617,6 +850,19 @@ bool conv3x3_tma16_ok(mas_tensor4 xs, mas_tensor4 ys) {
          xs.h == ys.h && xs.w == ys.w && xs.n == ys.n;
 }
 
+// A weight image of shift_gemm_t16 (mas_pack_conv3x3_tc16 / pack_phase16: `slabs` 2 KB slabs of 128 channels x 16 B) as
+// [slab][64-channel half][1 KB]: one copy of box {1 KB, one half, 2 taps slabs} stages a half's K step. The 8-byte element
+// type only makes a half's 1 KB a single box row.
+static CUresult encode_weight_map(CUtensorMap* map, const void* wpk, int64_t slabs, int taps) {
+  PFN_cuTensorMapEncodeTiled enc = tensor_map_encoder();
+  if (!enc) return CUDA_ERROR_NOT_FOUND;
+  cuuint64_t dims[3] = {128, 2, (cuuint64_t)slabs};
+  cuuint64_t strides[2] = {1024, 2048};
+  cuuint32_t box[3] = {128, 1, (cuuint32_t)(2 * taps)}, es[3] = {1, 1, 1};
+  return enc(map, CU_TENSOR_MAP_DATA_TYPE_UINT64, 3, const_cast<void*>(wpk), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+}
+
 // x16: fp16 NHWC shadow of the (activated) input, scaled by operand_scale(*x_amax) when x_amax is given.
 int conv3x3_fprop_tma16_launch(const void* x16, mas_tensor4 xs, const void* w_tc16, const float* bias, const float* res, float* y,
                                mas_tensor4 ys, float* stats_part, const float* x_amax, cudaStream_t st) {
@@ -645,23 +891,41 @@ int conv3x3_fprop_tma16_launch(const void* x16, mas_tensor4 xs, const void* w_tc
   CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 4, const_cast<void*>(x16), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
                    CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (conv halo map) failed (%d)", (int)r);
+  CUtensorMap wmap;
+  r = encode_weight_map(&wmap, w_tc16, (int64_t)Cout * p.Cin * 9 / 1024, 9);
+  if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (conv weight map) failed (%d)", (int)r);
 
-  constexpr size_t smem = tc::t16_smem_bytes();
+  constexpr size_t smem = tc::t16_smem_bytes(), smem_c = tc::t16c_smem_bytes();
   static std::atomic<uint64_t> configured{0};
   static int sm_count = 132;
   if (first_on_device(configured)) {
-    cudaError_t e = cudaFuncSetAttribute(tc::shift_gemm_t16<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::shift_gemm_t16<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e));
+    cudaError_t e = cudaSuccess;
+    auto attr = [&](const void* f, size_t bytes) {
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    };
+    attr((const void*)tc::shift_gemm_t16<true, 0>, smem);
+    attr((const void*)tc::shift_gemm_t16<false, 0>, smem);
+    attr((const void*)tc::shift_gemm_t16_coop<true, 0>, smem_c);
+    attr((const void*)tc::shift_gemm_t16_coop<false, 0>, smem_c);
+    if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(conv): %s", cudaGetErrorString(e));
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
     mark_device(configured);
   }
-  const int64_t nitems = p.units * (Cout / tc::BN);
+  const int64_t nitems = p.units * cdiv(Cstore, tc::T_CO);   // 64-channel items; the two warpgroups of a CTA alternate
+  // At most two items per CTA (the 16 x 16 layers of the model) leave ping-pong nothing to overlap but one epilogue, and one
+  // warpgroup issuing alone runs its K loop slower than two together: both warpgroups take one 128-channel item instead.
+  if (nitems <= 2 * (int64_t)sm_count) {
+    const int64_t nc = p.units * (Cout / tc::BN);
+    const unsigned gc = (unsigned)(nc < sm_count ? nc : sm_count);
+    if (tall) tc::shift_gemm_t16_coop<true, 0><<<gc, tc::T_THREADS, smem_c, st>>>(p, map);
+    else tc::shift_gemm_t16_coop<false, 0><<<gc, tc::T_THREADS, smem_c, st>>>(p, map);
+    return launched_tc(tall ? "shift_gemm_t16_coop<tall>" : "shift_gemm_t16_coop<pair>");
+  }
   const unsigned g = (unsigned)(nitems < sm_count ? nitems : sm_count);
-  if (tall) tc::shift_gemm_t16<true><<<g, tc::T_THREADS, smem, st>>>(p, map);
-  else tc::shift_gemm_t16<false><<<g, tc::T_THREADS, smem, st>>>(p, map);
+  if (tall) tc::shift_gemm_t16<true><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
+  else tc::shift_gemm_t16<false><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
   return launched_tc(tall ? "shift_gemm_t16<tall>" : "shift_gemm_t16<pair>");
 }
 
@@ -731,30 +995,56 @@ int conv3x3_phase_tma16_launch(const void* x16, mas_tensor4 xs, const void* wpk,
             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   }
   if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (phase conv map) failed (%d)", (int)r);
+  CUtensorMap wmap;
+  r = encode_weight_map(&wmap, wpk, (int64_t)p.Cout * p.Cin / 64, 4);
+  if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (phase conv weight map) failed (%d)", (int)r);
 
-  constexpr size_t smem = tc::t16_smem_bytes();
+  constexpr size_t smem = tc::t16_smem_bytes(), smem_c = tc::t16c_smem_bytes();
   static std::atomic<uint64_t> configured{0};
   static int sm_count = 132;
   if (first_on_device(configured)) {
-    cudaError_t e = cudaFuncSetAttribute(tc::shift_gemm_t16<true, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::shift_gemm_t16<false, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::shift_gemm_t16<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(tc::shift_gemm_t16<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e));
+    cudaError_t e = cudaSuccess;
+    auto attr = [&](const void* f, size_t bytes) {
+      if (e == cudaSuccess) e = cudaFuncSetAttribute(f, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+    };
+    attr((const void*)tc::shift_gemm_t16<true, 1>, smem);
+    attr((const void*)tc::shift_gemm_t16<false, 1>, smem);
+    attr((const void*)tc::shift_gemm_t16<true, 2>, smem);
+    attr((const void*)tc::shift_gemm_t16<false, 2>, smem);
+    attr((const void*)tc::shift_gemm_t16_coop<true, 1>, smem_c);
+    attr((const void*)tc::shift_gemm_t16_coop<false, 1>, smem_c);
+    attr((const void*)tc::shift_gemm_t16_coop<true, 2>, smem_c);
+    attr((const void*)tc::shift_gemm_t16_coop<false, 2>, smem_c);
+    if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(phase conv): %s", cudaGetErrorString(e));
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
     mark_device(configured);
   }
-  const int64_t nitems = p.units * (p.Cout / tc::BN) * (phase_out ? 4 : 1);
+  // The deep layers - phase-in from 256 source channels (a K loop of 16+ chunks over the four planes), phase-out from 512 -
+  // measured slower with ping-pong warpgroups than with both warpgroups on one 128-channel item: their epilogue is a small
+  // share of an item, and the short four-tap MMA groups keep the tensor cores busier with two warpgroups issuing than with one.
+  if (p.Cin >= (phase_out ? 512 : 256)) {
+    const int64_t nitems = p.units * (p.Cout / tc::BN) * (phase_out ? 4 : 1);
+    const unsigned g = (unsigned)(nitems < sm_count ? nitems : sm_count);
+    if (phase_out) {
+      if (tall) tc::shift_gemm_t16_coop<true, 1><<<g, tc::T_THREADS, smem_c, st>>>(p, map);
+      else tc::shift_gemm_t16_coop<false, 1><<<g, tc::T_THREADS, smem_c, st>>>(p, map);
+      return launched_tc(tall ? "shift_gemm_t16_coop<tall, phase-out>" : "shift_gemm_t16_coop<pair, phase-out>");
+    }
+    if (tall) tc::shift_gemm_t16_coop<true, 2><<<g, tc::T_THREADS, smem_c, st>>>(p, map);
+    else tc::shift_gemm_t16_coop<false, 2><<<g, tc::T_THREADS, smem_c, st>>>(p, map);
+    return launched_tc(tall ? "shift_gemm_t16_coop<tall, phase-in>" : "shift_gemm_t16_coop<pair, phase-in>");
+  }
+  const int64_t nitems = p.units * (p.Cout / tc::T_CO) * (phase_out ? 4 : 1);
   const unsigned g = (unsigned)(nitems < sm_count ? nitems : sm_count);
   if (phase_out) {
-    if (tall) tc::shift_gemm_t16<true, 1><<<g, tc::T_THREADS, smem, st>>>(p, map);
-    else tc::shift_gemm_t16<false, 1><<<g, tc::T_THREADS, smem, st>>>(p, map);
+    if (tall) tc::shift_gemm_t16<true, 1><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
+    else tc::shift_gemm_t16<false, 1><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
     return launched_tc(tall ? "shift_gemm_t16<tall, phase-out>" : "shift_gemm_t16<pair, phase-out>");
   }
-  if (tall) tc::shift_gemm_t16<true, 2><<<g, tc::T_THREADS, smem, st>>>(p, map);
-  else tc::shift_gemm_t16<false, 2><<<g, tc::T_THREADS, smem, st>>>(p, map);
+  if (tall) tc::shift_gemm_t16<true, 2><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
+  else tc::shift_gemm_t16<false, 2><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
   return launched_tc(tall ? "shift_gemm_t16<tall, phase-in>" : "shift_gemm_t16<pair, phase-in>");
 }
 
