@@ -21,7 +21,12 @@
 //     and GroupNorm statistics are per-row scalars of the fragment;
 //   * warps 0-7 MMA + epilogue (two warpgroups), warp 8 copy issuer (its warpgroup hands its registers to the MMA ones): no
 //     thread of the CTA touches the operands. The copy issuer fills the rings in item order, the order in which the
-//     warpgroups' K loops drain them, so one ring serves both warpgroups.
+//     warpgroups' K loops drain them, so one ring serves both warpgroups;
+//   * epilogue input (EPI: the residual, an fp32 NHWC tensor shaped like y and read at y's offsets): warp 9 copies each
+//     item's tile of it, in the epilogue's order, into a ring of four 8 KB slabs (32 pixels = four rows of a 16 x 8 tile x 64
+//     channels, two 32-channel boxes under the 128-byte swizzle, so the fragment-order reads hit 32 distinct banks). Loads
+//     issued by the epilogue threads themselves keep too few bytes in flight and leave the epilogue waiting on HBM latency,
+//     longer than the other warpgroup's K loop; the slabs take the room of two weight stages (five instead of seven).
 //
 // Reference call sites replaced: nn.Conv2d 3x3 stride 1 (modules.py:93-104) forward and its data gradient.
 //
@@ -41,6 +46,8 @@
 #include <cuda_fp16.h>
 #include <stdlib.h>
 
+#include <type_traits>
+
 #include "mas_common.cuh"
 #include "tc_ptx.cuh"
 #include "wgmma.cuh"
@@ -58,6 +65,11 @@ constexpr int T_ATILE = 23 * 1024;                  // 18 x 10 halo pixels x 128
 constexpr int T_ASTAGE = 2 * T_ATILE;               // pair of 16 x 8 tiles, or one 32 x 8 tile (34 x 10 halo = 43520 B)
 constexpr int T_CO = 64;                            // output channels per work item: the M extent of one warpgroup's MMAs
 constexpr int T_BSTAGE = 9 * 2 * T_CO * 16;         // nine taps x 16 channels x 64 output channels (fp16)
+constexpr int T_EBSTAGES = 5, T_ESTAGES = 4;        // EPI form: weight stages, epilogue-input slabs
+constexpr int T_EBOX = 32 * 32 * 4;                 // 32 pixels x 32 channels fp32: one 128-byte-swizzled box
+constexpr int T_ESLAB = 2 * T_EBOX;                 // 32 pixels x the item's 64 channels
+template <bool EPI>
+__host__ __device__ constexpr int t16_bstages() { return EPI ? T_EBSTAGES : T_BSTAGES; }
 
 struct HParams {
   const void* wpk;    // mas_pack_conv3x3_tc16 packing
@@ -77,18 +89,19 @@ struct HParams {
   int64_t ph_yoff[4];
 };
 
-// 16 x 8 tile (n, ty, tx) of half `hf` of work unit `u`; false when the unit's second tile does not exist (odd tile count)
-template <bool TALL>
-__device__ __forceinline__ bool unit_tile(const HParams& p, int64_t u, int hf, int& n, int& ty, int& tx) {
+// 16 x 8 tile (n, ty, tx) of half `hf` of work unit `u`; false when the unit's second tile does not exist (odd tile count).
+// I: the index type of the arithmetic (uint32_t where the launcher has bounded the item count).
+template <bool TALL, typename I = int64_t>
+__device__ __forceinline__ bool unit_tile(const HParams& p, I u, int hf, int& n, int& ty, int& tx) {
   if (TALL) {
     const int ty2 = p.tiles_y >> 1;
     tx = (int)(u % p.tiles_x);
     ty = (int)((u / p.tiles_x) % ty2) * 2 + hf;
-    n = (int)(u / ((int64_t)p.tiles_x * ty2));
+    n = (int)(u / ((I)p.tiles_x * ty2));
     return true;
   }
-  const int64_t total = (int64_t)p.N * p.tiles_x * p.tiles_y;
-  int64_t t = u * 2 + hf;
+  const I total = (I)p.N * p.tiles_x * p.tiles_y;
+  I t = u * 2 + hf;
   const bool live = t < total;
   if (!live) t = total - 1;
   tx = (int)(t % p.tiles_x);
@@ -100,15 +113,21 @@ __device__ __forceinline__ bool unit_tile(const HParams& p, int64_t u, int hf, i
 // TALL: the unit is one 32 x 8 tile whose staged halo (34 x 10 pixels, uniform 1280-byte row pitch) is ONE N = 256 operand:
 // per K = 16 step and tap a single m64n256 MMA instead of two m64n128 ones over the two halos of a pair.
 // PH: 0 the nine taps of a stride-1 3x3 convolution, 1 phase-out, 2 phase-in (see the top of the file).
-template <bool TALL, int PH = 0>
+// EPI (PH 0 only): the epilogue adds the tensor of e_map (fp32 [N][H][W][Cout], p.res) staged by warp 9.
+template <bool TALL, int PH = 0, bool EPI = false>
 __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, const __grid_constant__ CUtensorMap x_map,
-                                                               const __grid_constant__ CUtensorMap w_map) {
+                                                               const __grid_constant__ CUtensorMap w_map,
+                                                               const __grid_constant__ CUtensorMap e_map) {
+  static_assert(!EPI || PH == 0, "the epilogue input is read at the offsets of a dense stride-1 output");
   constexpr int TAPS = PH == 0 ? 9 : 4;              // phase forms: groups with fewer taps carry zero weights
   constexpr int GOUT = PH == 1 ? 4 : 1;              // output phases per work unit
   constexpr int KPL = PH == 2 ? 4 : 1;               // source planes per K loop
   constexpr int SLAB = T_CO * 16, B_TAP = 2 * SLAB;  // staged weights: [tap][k / 8][64 channels][8 halves]
   constexpr int A_BYTES = TALL ? 34 * 10 * 128 : 2 * 18 * 10 * 128;
-  constexpr int RB = 2;                              // epilogue: image rows whose residuals are loaded together (registers)
+  constexpr int BST = t16_bstages<EPI>();
+  constexpr int EST = EPI ? T_ESTAGES : 0;
+  // EPI: the launcher bounds the item count to 32 bits, so item -> tile is 32-bit arithmetic (a 64-bit division is a call)
+  using Idx = typename std::conditional<EPI, uint32_t, int64_t>::type;
 
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
@@ -116,13 +135,17 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
   uint8_t* smem = smem_raw + (smem_base - raw_base);
   const uint32_t a_base = smem_base;
   const uint32_t b_base = a_base + T_ASTAGES * T_ASTAGE;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + T_ASTAGES * T_ASTAGE + T_BSTAGES * T_BSTAGE);
+  const uint32_t e_off = T_ASTAGES * T_ASTAGE + BST * T_BSTAGE;     // epilogue-input slabs (EPI)
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + e_off + EST * T_ESLAB);
   const uint32_t bar_base = smem_u32(bars);
   auto afull = [&](int s) { return bar_base + 8u * s; };
   auto aempty = [&](int s) { return bar_base + 8u * (T_ASTAGES + s); };
   auto bfull = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + s); };
-  auto bempty = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + T_BSTAGES + s); };
-  auto order = [&](int g) { return bar_base + 8u * (2 * T_ASTAGES + 2 * T_BSTAGES + g); };   // warpgroup g may start its next mainloop
+  auto bempty = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + BST + s); };
+  auto order = [&](int g) { return bar_base + 8u * (2 * T_ASTAGES + 2 * BST + g); };   // warpgroup g may start its next mainloop
+  auto efull = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + 2 * BST + 2 + s); };
+  auto eempty = [&](int s) { return bar_base + 8u * (2 * T_ASTAGES + 2 * BST + 2 + EST + s); };
+  auto eorder = [&](int g) { return bar_base + 8u * (2 * T_ASTAGES + 2 * BST + 2 + 2 * EST + g); };   // EPI: g may wait on slabs
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int achunks = p.Cin / 64;
@@ -132,8 +155,10 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
 
   if (tid == 0) {
     for (int s = 0; s < T_ASTAGES; ++s) { mbar_init(afull(s), 1); mbar_init(aempty(s), 128); }
-    for (int s = 0; s < T_BSTAGES; ++s) { mbar_init(bfull(s), 1); mbar_init(bempty(s), 128); }
+    for (int s = 0; s < BST; ++s) { mbar_init(bfull(s), 1); mbar_init(bempty(s), 128); }
     for (int g = 0; g < 2; ++g) mbar_init(order(g), 128);
+    for (int s = 0; s < EST; ++s) { mbar_init(efull(s), 1); mbar_init(eempty(s), 128); }
+    if (EPI) for (int g = 0; g < 2; ++g) mbar_init(eorder(g), 128);
     fence_barrier_init();
   }
   __syncthreads();
@@ -155,8 +180,8 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
       if (item >= nitems) break;
       const int gout = PH == 1 ? (int)((item / ctiles) % GOUT) : 0;
       const int a0 = q * kiters, b0 = 4 * a0;
-      int as = a0 % T_ASTAGES, bs = b0 % T_BSTAGES, prev_b = 0, prev_a = -1;
-      uint32_t aph = (uint32_t)(a0 / T_ASTAGES) & 1u, bph = (uint32_t)(b0 / T_BSTAGES) & 1u;
+      int as = a0 % T_ASTAGES, bs = b0 % BST, prev_b = 0, prev_a = -1;
+      uint32_t aph = (uint32_t)(a0 / T_ASTAGES) & 1u, bph = (uint32_t)(b0 / BST) & 1u;
       // ordered mainloops: the first MMA of item q only after the other warpgroup has issued the last one of item q - 1, so
       // the two warpgroups' epilogues alternate instead of falling into step
       if (q > 0) mbar_wait(order(wgi), (uint32_t)((q - 1) >> 1) & 1u);
@@ -194,7 +219,7 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
           }
           prev_b = bs;
           prev_a = (sub == 3) ? as : -1;
-          if (++bs == T_BSTAGES) { bs = 0; bph ^= 1; }
+          if (++bs == BST) { bs = 0; bph ^= 1; }
         }
         if (++as == T_ASTAGES) { as = 0; aph ^= 1; }
       }
@@ -203,75 +228,104 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
       mbar_arrive(bempty(prev_b));
       mbar_arrive(aempty(prev_a));
 
-      const int64_t unit = item / (ctiles * GOUT);
-      const int ch_tile = (int)(item % ctiles) * T_CO;
+      const Idx unit = (Idx)item / (Idx)(ctiles * GOUT);
+      const int ch_tile = (int)((Idx)item % (Idx)ctiles) * T_CO;
+      float bv[2];
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int ch = ch_tile + frow + 8 * i;
+        bv[i] = (p.bias && ch < p.Cstore) ? __ldg(p.bias + ch) : 0.f;
+      }
+      // a slab's full barrier tells two uses of its slot apart by parity only: the epilogue of item q waits on its slabs once
+      // the other warpgroup has received every slab of item q - 1, so no wait can see a phase of two uses back
+      if (EPI && q > 0) mbar_wait(eorder(wgi), (uint32_t)((q - 1) >> 1) & 1u);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         int n_img, ty_, tx_;
-        const bool live = unit_tile<TALL>(p, unit, h, n_img, ty_, tx_);   // warpgroup-uniform
-        if (!live) continue;
+        const bool live = unit_tile<TALL, Idx>(p, unit, h, n_img, ty_, tx_);   // warpgroup-uniform
         const int64_t pix0 = ((int64_t)n_img * p.H + ty_ * 16) * p.W + tx_ * 8;
         const int64_t cstep = PH == 0 ? p.ldy : p.ysw;
         const int64_t ybase = PH == 0 ? 0 : n_img * p.ysn + (ty_ * 16) * p.ysh + (tx_ * 8) * p.ysw + (PH == 1 ? p.ph_yoff[gout] : 0);
 #pragma unroll
-        for (int i = 0; i < 2; ++i) {
-          const int ch = ch_tile + frow + 8 * i;
-          const bool st_ok = ch < p.Cstore;
-          const float bv = (p.bias && st_ok) ? __ldg(p.bias + ch) : 0.f;
+        for (int cb = 0; cb < 4; ++cb) {           // 32-pixel groups = four image rows of the 16 x 8 tile
+          // the item's slabs are 8 q .. 8 q + 7 of the CTA's sequence, (h, cb) in order: on a ring of four, slot cb in phase h.
+          // A missing second tile's slabs are loaded (from the last tile) and released unread.
+          static_assert(T_ESTAGES == 4, "slab slot and phase follow from (h, cb) on a ring of four");
+          const int es = cb;
+          if (EPI) {
+            mbar_wait(efull(es), (uint32_t)h);
+            if (h == 1 && cb == 3) mbar_arrive(eorder(wgi ^ 1));
+          }
+          if (live) {
 #pragma unroll
-          for (int cb = 0; cb < 4; ++cb) {         // 32-pixel groups = four image rows of the 16 x 8 tile
-            float st_s = 0.f, st_q = 0.f;
+            for (int i = 0; i < 2; ++i) {
+              const int ch = ch_tile + frow + 8 * i;
+              const bool st_ok = ch < p.Cstore;
+              // the slab holds channel c of pixel r at box c / 32, row r, 16-byte chunk (c % 32) / 4 ^ r % 8
+              const int cl = frow + 8 * i;
+              const float* ev = reinterpret_cast<const float*>(smem + e_off + es * T_ESLAB + (cl >> 5) * T_EBOX) + (cl & 3);
+              float st_s = 0.f, st_q = 0.f;
 #pragma unroll
-            for (int jp = 0; jp < 4; jp += RB) {
-              float rv[RB][2];                     // residuals of RB rows, loaded together ahead of their stores
-              if (p.res && st_ok) {
-#pragma unroll
-                for (int jj = 0; jj < RB; ++jj) {
-                  const int j = cb * 4 + jp + jj;
-                  const int64_t off = PH == 0 ? (pix0 + (int64_t)j * p.W + fcol) * p.ldy + ch : ybase + j * p.ysh + fcol * p.ysw + ch;
-#pragma unroll
-                  for (int cc = 0; cc < 2; ++cc) rv[jj][cc] = __ldg(p.res + off + cc * cstep);
-                }
-              }
-#pragma unroll
-              for (int jj = 0; jj < RB; ++jj) {
-                const int j = cb * 4 + jp + jj;    // pixel row j of the tile, columns fcol, fcol + 1
+              for (int jj = 0; jj < 4; ++jj) {
+                const int j = cb * 4 + jj;         // pixel row j of the tile, columns fcol, fcol + 1
                 const int64_t off = PH == 0 ? (pix0 + (int64_t)j * p.W + fcol) * p.ldy + ch : ybase + j * p.ysh + fcol * p.ysw + ch;
 #pragma unroll
                 for (int cc = 0; cc < 2; ++cc) {
-                  float o = fmaf(acc[64 * h + 4 * j + 2 * i + cc], alpha, bv);
+                  float o = fmaf(acc[64 * h + 4 * j + 2 * i + cc], alpha, bv[i]);
                   if (st_ok) {
-                    if (p.res) o += rv[jj][cc];
+                    if (EPI) o += ev[(jj * 8 + fcol + cc) * 32 + ((((cl & 31) >> 2) ^ (fcol + cc)) << 2)];
                     p.y[off + cc * cstep] = o;
                     st_s += o;
                     st_q = fmaf(o, o, st_q);
                   }
                 }
               }
-            }
-            if (p.stats_part) {   // same partial layout as shift_gemm_tc: [16 x 8 tile][32-pixel group][channel quad][sum, sumsq]
-              st_s += __shfl_xor_sync(0xffffffffu, st_s, 1);   // the four lanes of a channel row: all 32 pixels
-              st_q += __shfl_xor_sync(0xffffffffu, st_q, 1);
-              st_s += __shfl_xor_sync(0xffffffffu, st_s, 2);
-              st_q += __shfl_xor_sync(0xffffffffu, st_q, 2);
-              st_s += __shfl_xor_sync(0xffffffffu, st_s, 4);   // four consecutive channel rows: the quad
-              st_q += __shfl_xor_sync(0xffffffffu, st_q, 4);
-              st_s += __shfl_xor_sync(0xffffffffu, st_s, 8);
-              st_q += __shfl_xor_sync(0xffffffffu, st_q, 8);
-              if ((lane & 15) == 0) {
-                const size_t tile = ((size_t)n_img * p.tiles_y + ty_) * p.tiles_x + tx_;
-                float* sp = p.stats_part + ((tile * 4 + cb) * (p.Cout >> 2) + (ch >> 2)) * 2;
-                sp[0] = st_s;
-                sp[1] = st_q;
+              if (p.stats_part) {   // same partial layout as shift_gemm_tc: [16 x 8 tile][32-pixel group][channel quad][sum, sumsq]
+                st_s += __shfl_xor_sync(0xffffffffu, st_s, 1);   // the four lanes of a channel row: all 32 pixels
+                st_q += __shfl_xor_sync(0xffffffffu, st_q, 1);
+                st_s += __shfl_xor_sync(0xffffffffu, st_s, 2);
+                st_q += __shfl_xor_sync(0xffffffffu, st_q, 2);
+                st_s += __shfl_xor_sync(0xffffffffu, st_s, 4);   // four consecutive channel rows: the quad
+                st_q += __shfl_xor_sync(0xffffffffu, st_q, 4);
+                st_s += __shfl_xor_sync(0xffffffffu, st_s, 8);
+                st_q += __shfl_xor_sync(0xffffffffu, st_q, 8);
+                if ((lane & 15) == 0) {
+                  const size_t tile = ((size_t)n_img * p.tiles_y + ty_) * p.tiles_x + tx_;
+                  float* sp = p.stats_part + ((tile * 4 + cb) * (p.Cout >> 2) + (ch >> 2)) * 2;
+                  sp[0] = st_s;
+                  sp[1] = st_q;
+                }
               }
             }
           }
+          if (EPI) mbar_arrive(eempty(es));
         }
       }
     }
   } else {
-    // ===================== copy issuer (one thread): halos by tensor map, weight stages by tensor map =====================
+    // ===================== copy issuers (one thread each): halos and weight stages by tensor map (warp 8), the epilogue
+    // input (warp 9, EPI) =====================
     wg::regs_dec<wg::COPY_REGS>();
+    if (EPI && warp == T_MMA_WARPS + 1 && lane == 0) {
+      int es = 0;
+      uint32_t eph = 0;
+      for (Idx item = blockIdx.x; item < (Idx)nitems; item += gridDim.x) {
+        const int ch_tile = (int)(item % (Idx)ctiles) * T_CO;
+        const Idx unit = item / (Idx)ctiles;
+        for (int h = 0; h < 2; ++h) {
+          int n, ty_, tx_;
+          unit_tile<TALL, Idx>(p, unit, h, n, ty_, tx_);   // a missing second tile re-reads the last one (never read)
+          for (int cb = 0; cb < 4; ++cb) {
+            mbar_wait(eempty(es), eph ^ 1);
+            mbar_expect_tx(efull(es), T_ESLAB);
+            const uint32_t dst = smem_base + e_off + (uint32_t)(es * T_ESLAB);
+            tma_load_4d(dst, &e_map, ch_tile, tx_ * 8, ty_ * 16 + cb * 4, n, efull(es));
+            tma_load_4d(dst + T_EBOX, &e_map, ch_tile + 32, tx_ * 8, ty_ * 16 + cb * 4, n, efull(es));
+            if (++es == T_ESTAGES) { es = 0; eph ^= 1; }
+          }
+        }
+      }
+    }
     if (warp == T_MMA_WARPS && lane == 0) {
       int as = 0, bs = 0;
       uint32_t aph = 0, bph = 0;
@@ -279,9 +333,9 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
       // [group][128-channel tile][16-channel K step][tap][k / 8][128][8 halves]
       const int tile_slabs = (p.Cin / 16) * 2 * TAPS, group_slabs = (p.Cout / BN) * tile_slabs;
       for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-        const int ct = (int)(item % ctiles);
+        const int ct = (int)((Idx)item % (Idx)ctiles);
         const int gout = PH == 1 ? (int)((item / ctiles) % GOUT) : 0;
-        const int64_t unit = item / (ctiles * GOUT);
+        const Idx unit = (Idx)item / (Idx)(ctiles * GOUT);
         for (int kk = 0; kk < kiters; ++kk) {
           const int grp = PH == 2 ? kk / achunks : gout, c = kk % achunks;
           const int slab0 = grp * group_slabs + (ct >> 1) * tile_slabs + c * 8 * TAPS;   // the chunk's first slab
@@ -290,7 +344,7 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
 #pragma unroll
           for (int hf = 0; hf < (TALL ? 1 : 2); ++hf) {
             int n, ty_, tx_;
-            unit_tile<TALL>(p, unit, hf, n, ty_, tx_);   // a missing second tile re-reads the last one (never stored)
+            unit_tile<TALL, Idx>(p, unit, hf, n, ty_, tx_);   // a missing second tile re-reads the last one (never stored)
             const uint32_t dst = a_base + (uint32_t)(as * T_ASTAGE + hf * T_ATILE);
             if (PH == 2)   // plane (py, px) = grp: channel half px of the pixel pair, row parity py
               tma_load_5d(dst, &x_map, (grp & 1) * p.Cin + c * 64, tx_ * 8 - 1, grp >> 1, ty_ * 16 - 1, n, afull(as));
@@ -303,7 +357,7 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
             mbar_expect_tx(bfull(bs), TAPS * B_TAP);
             // the item's 64-channel half (ct & 1) of each of the step's 2 TAPS slabs
             tma_load_3d(b_base + (uint32_t)bs * T_BSTAGE, &w_map, 0, ct & 1, slab0 + sub * 2 * TAPS, bfull(bs));
-            if (++bs == T_BSTAGES) { bs = 0; bph ^= 1; }
+            if (++bs == BST) { bs = 0; bph ^= 1; }
           }
         }
       }
@@ -312,10 +366,14 @@ __global__ void __launch_bounds__(T_THREADS, 1) shift_gemm_t16(const HParams p, 
   }
 }
 
+template <bool EPI = false>
 constexpr size_t t16_smem_bytes() {
-  return 1024 + (size_t)T_ASTAGES * T_ASTAGE + (size_t)T_BSTAGES * T_BSTAGE + (2 * T_ASTAGES + 2 * T_BSTAGES + 2) * 8 + 16;
+  constexpr int bst = t16_bstages<EPI>(), est = EPI ? T_ESTAGES : 0;
+  return 1024 + (size_t)T_ASTAGES * T_ASTAGE + (size_t)bst * T_BSTAGE + (size_t)est * T_ESLAB +
+         (2 * T_ASTAGES + 2 * bst + 2 + (EPI ? 2 * est + 2 : 0)) * 8 + 16;
 }
-static_assert(t16_smem_bytes() <= 227 * 1024, "shift_gemm_t16 rings exceed the shared memory of an SM");
+static_assert(t16_smem_bytes<false>() <= 227 * 1024 && t16_smem_bytes<true>() <= 227 * 1024,
+              "shift_gemm_t16 rings exceed the shared memory of an SM");
 
 // Cooperative form: both MMA warpgroups work on one item of 128 output channels at the same time (warpgroup g owns channels
 // 64 g .. 64 g + 63), so their epilogues run together, with the tensor cores idle. Two warpgroups issuing together keep the
@@ -895,7 +953,7 @@ int conv3x3_fprop_tma16_launch(const void* x16, mas_tensor4 xs, const void* w_tc
   r = encode_weight_map(&wmap, w_tc16, (int64_t)Cout * p.Cin * 9 / 1024, 9);
   if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (conv weight map) failed (%d)", (int)r);
 
-  constexpr size_t smem = tc::t16_smem_bytes(), smem_c = tc::t16c_smem_bytes();
+  constexpr size_t smem = tc::t16_smem_bytes<false>(), smem_e = tc::t16_smem_bytes<true>(), smem_c = tc::t16c_smem_bytes();
   static std::atomic<uint64_t> configured{0};
   static int sm_count = 132;
   if (first_on_device(configured)) {
@@ -905,6 +963,8 @@ int conv3x3_fprop_tma16_launch(const void* x16, mas_tensor4 xs, const void* w_tc
     };
     attr((const void*)tc::shift_gemm_t16<true, 0>, smem);
     attr((const void*)tc::shift_gemm_t16<false, 0>, smem);
+    attr((const void*)tc::shift_gemm_t16<true, 0, true>, smem_e);
+    attr((const void*)tc::shift_gemm_t16<false, 0, true>, smem_e);
     attr((const void*)tc::shift_gemm_t16_coop<true, 0>, smem_c);
     attr((const void*)tc::shift_gemm_t16_coop<false, 0>, smem_c);
     if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(conv): %s", cudaGetErrorString(e));
@@ -924,8 +984,22 @@ int conv3x3_fprop_tma16_launch(const void* x16, mas_tensor4 xs, const void* w_tc
     return launched_tc(tall ? "shift_gemm_t16_coop<tall>" : "shift_gemm_t16_coop<pair>");
   }
   const unsigned g = (unsigned)(nitems < sm_count ? nitems : sm_count);
-  if (tall) tc::shift_gemm_t16<true><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
-  else tc::shift_gemm_t16<false><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
+  CUtensorMap emap{};
+  if (res) {
+    if (nitems > (int64_t)UINT32_MAX) return fail(MAS_ERR_UNSUPPORTED, "tma conv: residual form indexes items in 32 bits");
+    // the residual as 32-channel x 8 x 4 boxes of fp32 (one half of an epilogue slab)
+    cuuint64_t edims[4] = {(cuuint64_t)Cout, (cuuint64_t)ys.w, (cuuint64_t)ys.h, (cuuint64_t)ys.n};
+    cuuint64_t estrides[3] = {(cuuint64_t)Cout * 4, (cuuint64_t)ys.w * Cout * 4, (cuuint64_t)ys.h * ys.w * Cout * 4};
+    cuuint32_t ebox[4] = {32, 8, 4, 1};
+    r = enc(&emap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(res), edims, estrides, ebox, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+            CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (conv residual map) failed (%d)", (int)r);
+    if (tall) tc::shift_gemm_t16<true, 0, true><<<g, tc::T_THREADS, smem_e, st>>>(p, map, wmap, emap);
+    else tc::shift_gemm_t16<false, 0, true><<<g, tc::T_THREADS, smem_e, st>>>(p, map, wmap, emap);
+    return launched_tc(tall ? "shift_gemm_t16<tall, residual>" : "shift_gemm_t16<pair, residual>");
+  }
+  if (tall) tc::shift_gemm_t16<true><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap, emap);
+  else tc::shift_gemm_t16<false><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap, emap);
   return launched_tc(tall ? "shift_gemm_t16<tall>" : "shift_gemm_t16<pair>");
 }
 
@@ -1038,13 +1112,14 @@ int conv3x3_phase_tma16_launch(const void* x16, mas_tensor4 xs, const void* wpk,
   }
   const int64_t nitems = p.units * (p.Cout / tc::T_CO) * (phase_out ? 4 : 1);
   const unsigned g = (unsigned)(nitems < sm_count ? nitems : sm_count);
+  const CUtensorMap emap{};   // no epilogue input
   if (phase_out) {
-    if (tall) tc::shift_gemm_t16<true, 1><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
-    else tc::shift_gemm_t16<false, 1><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
+    if (tall) tc::shift_gemm_t16<true, 1><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap, emap);
+    else tc::shift_gemm_t16<false, 1><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap, emap);
     return launched_tc(tall ? "shift_gemm_t16<tall, phase-out>" : "shift_gemm_t16<pair, phase-out>");
   }
-  if (tall) tc::shift_gemm_t16<true, 2><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
-  else tc::shift_gemm_t16<false, 2><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap);
+  if (tall) tc::shift_gemm_t16<true, 2><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap, emap);
+  else tc::shift_gemm_t16<false, 2><<<g, tc::T_THREADS, smem, st>>>(p, map, wmap, emap);
   return launched_tc(tall ? "shift_gemm_t16<tall, phase-in>" : "shift_gemm_t16<pair, phase-in>");
 }
 
