@@ -199,6 +199,14 @@ int mas_gemm_rows_f16(const void* x_f16, int64_t M, int K, const void* w_tc16, f
 size_t mas_wgrad_rows_f16_ws_bytes(int64_t M, int N, int K);
 int mas_wgrad_rows_f16(const void* x_f16, const void* dy_f16, int64_t M, int N, int K, float* dw, float* dbias,
                        const float* x_amax, const float* dy_amax, void* ws, size_t ws_bytes, void* stream);
+/* The Linear layers of a decode step at more than 8 rows (cond + uncond streams): y[R,N] = act(x[R,K] . W^T + bias) from the
+ * same operands as mas_gemm_rows_f16 (x_f16 a dense [R,K] copy scaled by the operand scale of *x_amax, w_tc16 from
+ * mas_pack_gemm_tc16, padded to 128 output features; only N columns are stored).  The rows sit on a narrow MMA side (16 .. 256)
+ * and the contraction is split so that one wave fills the GPU; the split depends on (N, K) only, its partial sums go to ws and
+ * are added in a fixed order, then bias and act (0 = none, 1 = tanh-GELU).  Needs K % 64 == 0 and 16-byte aligned operands. */
+size_t mas_linear_rows_f16_ws_bytes(int64_t R, int N, int K);
+int mas_linear_rows_f16(const void* x_f16, int64_t R, int K, const void* w_tc16, float* y, int64_t ldy, int N, const float* bias,
+                        const float* x_amax, int act, void* ws, size_t ws_bytes, void* stream);
 /* Diagnostic: wgmma D[128x32] = A[128x8].B[32x8]^T (TF32, 2 x m64) with A from shared memory (a_src=0) or registers
  * (a_src=1) and B K-major (b_layout=0) or MN-major (1; 2 = LBO/SBO fields swapped). Used by the tests to pin the
  * descriptor conventions the production kernels rely on. b_layout=99: B descriptor bits (sm_100 encoding) /
@@ -419,7 +427,7 @@ int mas_vq_gather(const float* E, const int64_t* idx, int64_t R, int K, int D, f
  * contractions go through mas_gemm_rows_packed / mas_gemm / mas_conv1x1_wgrad. */
 int mas_layernorm_forward(const float* x, const float* gamma, const float* beta, const float* residual, float* y,
                           float* mean, float* rstd, int64_t R, int H, float eps, void* stream);
-/* Two chained LayerNorms of a decode step (inference, R <= 64 rows): y1 = residual + LN1(x) (residual may be NULL) and
+/* Two chained LayerNorms of a decode step (inference, one block per row, any R): y1 = residual + LN1(x) (residual may be NULL) and
  * y2 = LN2(y1) - the sandwich LayerNorm and the next sub-layer's input LayerNorm (transformer.py:183-208) in one launch. */
 int mas_layernorm2_forward(const float* x, const float* gamma1, const float* beta1, const float* residual, float* y1,
                            const float* gamma2, const float* beta2, float* y2, int64_t R, int H, float eps1, float eps2,
@@ -474,6 +482,15 @@ int mas_attn_decode(const float* qkv, const float* kcache, const float* vcache, 
  * attends over positions 0..pos (one launch per layer instead of mas_kv_append + mas_attn_decode). */
 int mas_attn_decode_append(const float* qkv, float* kcache, float* vcache, float* ctx, int R, int heads, int hd, int Tmax,
                            int pos, void* stream);
+/* The same three with fp16 caches [R,heads,Tmax,hd] (decoding more than 8 rows): k / v are rounded to nearest once when they are
+ * stored, and the token's own k / v enter the attention as those rounded values; q, scores, softmax and ctx stay fp32
+ * (the v pass adds its partial sums in a different order from the fp32 entries': 8-element slices of d instead of 4). */
+int mas_kv_append_f16(const float* qkv, int R, int T, int heads, int hd, void* kcache, void* vcache, int Tmax, int pos0,
+                      void* stream);
+int mas_attn_decode_f16(const float* qkv, const void* kcache, const void* vcache, float* ctx, int R, int heads, int hd,
+                        int Tmax, int len, void* stream);
+int mas_attn_decode_append_f16(const float* qkv, void* kcache, void* vcache, float* ctx, int R, int heads, int hd, int Tmax,
+                               int pos, void* stream);
 int mas_cfg_mix(const float* cond, const float* uncond, float* out, int64_t n, float scale, void* stream);
 /* Token draw of the sampler (replaces the div / topk / where / softmax / multinomial chain of generate()): per row,
  * z = logits / temperature, entries below the top_k-th largest value dropped (top_k <= 0 or >= V: none), p = softmax(z),

@@ -4,10 +4,14 @@
 // 216-244): a decode step must reproduce the logits the full causal forward gives at that position.
 //   * mas_linear_small : y[r,n] = act(sum_k x[r,k] W[n,k] + b[n]) for a handful of rows (cond + uncond streams): a
 //     weight-streaming kernel — every weight is read exactly once per token, so it is HBM-bound by construction
-//     (371 M parameters = 1.48 GB per token for the 24-layer / 1024-wide model); strict fp32.
+//     (371 M parameters = 1.48 GB per token for the 24-layer / 1024-wide model); strict fp32, up to 8 rows. More rows run
+//     mas_linear_rows_f16 (gemm_tma.cu).
 //   * mas_kv_append    : scatters the k / v thirds of a fused qkv activation into the [R, heads, Tmax, hd] caches.
 //   * mas_attn_decode  : one query per (row, head) against the cache: scores, softmax, weighted sum of v.
+//     The _f16 variants of both keep the caches in fp16 (decoding more than 8 rows).
 //   * mas_cfg_mix      : classifier-free guidance, out = uncond + scale * (cond - uncond).
+#include <cuda_fp16.h>
+
 #include "mas_common.cuh"
 
 using namespace mas;
@@ -67,21 +71,52 @@ __global__ void __launch_bounds__(256) linear_small_kernel(const float* __restri
   }
 }
 
+// Cache elements: fp32 (up to 8 rows: strict fp32 decoding) or fp16 (more rows: half the cache bytes, which dominate a decode
+// step at a few hundred rows).  k / v are rounded once, to nearest, as mas_to_half rounds; everything downstream is fp32.
+__device__ __forceinline__ float to_elem(float v, float*) { return v; }
+__device__ __forceinline__ __half to_elem(float v, __half*) { return __float2half_rn(v); }
+__device__ __forceinline__ float elem_f(float v) { return v; }
+__device__ __forceinline__ float elem_f(__half v) { return __half2float(v); }
+__device__ __forceinline__ void store4(float* p, float4 v) { *reinterpret_cast<float4*>(p) = v; }
+__device__ __forceinline__ void store4(__half* p, float4 v) {
+  const __half2 a = __floats2half2_rn(v.x, v.y), b = __floats2half2_rn(v.z, v.w);
+  uint2 u;
+  u.x = *reinterpret_cast<const uint32_t*>(&a);
+  u.y = *reinterpret_cast<const uint32_t*>(&b);
+  *reinterpret_cast<uint2*>(p) = u;
+}
+// one 16-byte load: 4 fp32 or 8 fp16 elements, widened to fp32
+template <typename T> struct Vec16 { static constexpr int E = 16 / sizeof(T); };
+__device__ __forceinline__ void load16(const float* p, float* o) {
+  const float4 v = __ldg(reinterpret_cast<const float4*>(p));
+  o[0] = v.x; o[1] = v.y; o[2] = v.z; o[3] = v.w;
+}
+__device__ __forceinline__ void load16(const __half* p, float* o) {
+  const uint4 u = __ldg(reinterpret_cast<const uint4*>(p));
+  const uint32_t w[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&w[i]));
+    o[2 * i] = f.x; o[2 * i + 1] = f.y;
+  }
+}
+
 // qkv [R, T, 3H] -> kcache / vcache [R, heads, Tmax, hd] at positions pos0 .. pos0+T-1
-__global__ void kv_append_kernel(const float* __restrict__ qkv, int R, int T, int heads, int hd, float* __restrict__ kc,
-                                 float* __restrict__ vc, int Tmax, int pos0) {
+template <typename T>
+__global__ void kv_append_kernel(const float* __restrict__ qkv, int R, int T_, int heads, int hd, T* __restrict__ kc,
+                                 T* __restrict__ vc, int Tmax, int pos0) {
   const int H = heads * hd, Q = hd >> 2;
-  const int64_t total = (int64_t)R * T * heads * Q;
+  const int64_t total = (int64_t)R * T_ * heads * Q;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     int64_t r_ = i;
     const int q = (int)(r_ % Q); r_ /= Q;
     const int h = (int)(r_ % heads); r_ /= heads;
-    const int t = (int)(r_ % T);
-    const int r = (int)(r_ / T);
-    const float* src = qkv + ((size_t)r * T + t) * 3 * H + h * hd + q * 4;
+    const int t = (int)(r_ % T_);
+    const int r = (int)(r_ / T_);
+    const float* src = qkv + ((size_t)r * T_ + t) * 3 * H + h * hd + q * 4;
     const size_t dst = (((size_t)r * heads + h) * Tmax + pos0 + t) * hd + q * 4;
-    *reinterpret_cast<float4*>(kc + dst) = __ldg(reinterpret_cast<const float4*>(src + H));
-    *reinterpret_cast<float4*>(vc + dst) = __ldg(reinterpret_cast<const float4*>(src + 2 * H));
+    store4(kc + dst, __ldg(reinterpret_cast<const float4*>(src + H)));
+    store4(vc + dst, __ldg(reinterpret_cast<const float4*>(src + 2 * H)));
   }
 }
 
@@ -90,12 +125,14 @@ __global__ void kv_append_kernel(const float* __restrict__ qkv, int R, int T, in
 // flight: HD is a template parameter (fully unrolled dot products), the v pass is unrolled eight positions deep.
 // APPEND: the token's own k / v (the k and v thirds of its qkv row) are written to the caches at position len-1 by this
 // kernel (no separate mas_kv_append launch) and enter the attention from shared memory - the freshly written cache lines are
-// never read back here (the cache loads use the read-only path).
-template <int HD, bool APPEND>
-__global__ void __launch_bounds__(256) attn_decode_kernel(const float* __restrict__ qkv, float* __restrict__ kc, float* __restrict__ vc,
+// never read back here (the cache loads use the read-only path).  With an fp16 cache they enter as the rounded values stored.
+template <int HD, bool APPEND, typename T>
+__global__ void __launch_bounds__(256) attn_decode_kernel(const float* __restrict__ qkv, T* __restrict__ kc, T* __restrict__ vc,
                                                           float* __restrict__ ctx, int heads, int Tmax, int len) {
-  extern __shared__ __align__(16) float sm[];  // [HD] q, [len] scores, [32] scratch, [256/(HD/4)][HD] partial outputs, [2 HD] own k, v
-  constexpr int Q = HD / 4, GROUPS = 256 / Q;
+  // [HD] q, [len] scores, [32] scratch, [256/(HD/E)][HD] partial outputs, [2 HD] own k, v
+  extern __shared__ __align__(16) float sm[];
+  constexpr int E = Vec16<T>::E;                 // cache elements per 16-byte load
+  constexpr int Q = HD / 4, VQ = HD / E, GROUPS = 256 / VQ;
   float* qs = sm;
   float* sc = sm + HD;
   float* red = sc + ((len + 3) & ~3);
@@ -108,9 +145,9 @@ __global__ void __launch_bounds__(256) attn_decode_kernel(const float* __restric
     const float* tokrow = qkv + (size_t)r * 3 * H + h * HD + t0;
     qs[t0] = tokrow[0];
     if (APPEND) {
-      const float kv = tokrow[H], vv = tokrow[2 * H];
-      ks[t0] = kv;
-      vs[t0] = vv;
+      const T kv = to_elem(tokrow[H], (T*)nullptr), vv = to_elem(tokrow[2 * H], (T*)nullptr);
+      ks[t0] = elem_f(kv);
+      vs[t0] = elem_f(vv);
       const size_t dst = (((size_t)r * heads + h) * Tmax + (len - 1)) * HD + t0;
       kc[dst] = kv;
       vc[dst] = vv;
@@ -118,22 +155,21 @@ __global__ void __launch_bounds__(256) attn_decode_kernel(const float* __restric
   }
   __syncthreads();
   const float alpha = rsqrtf((float)HD);
-  const float* kb = kc + ((size_t)r * heads + h) * Tmax * HD;
-  const float* vb = vc + ((size_t)r * heads + h) * Tmax * HD;
+  const T* kb = kc + ((size_t)r * heads + h) * Tmax * HD;
+  const T* vb = vc + ((size_t)r * heads + h) * Tmax * HD;
   float4 q4[Q];
 #pragma unroll
   for (int i = 0; i < Q; ++i) q4[i] = *reinterpret_cast<const float4*>(qs + 4 * i);
   float mx = -INFINITY;
   for (int t = t0; t < lenc; t += 256) {
-    const float4* kr = reinterpret_cast<const float4*>(kb + (size_t)t * HD);
-    float4 kv[Q];
+    float kv[HD];
 #pragma unroll
-    for (int i = 0; i < Q; ++i) kv[i] = __ldg(kr + i);
+    for (int i = 0; i < VQ; ++i) load16(kb + (size_t)t * HD + i * E, kv + i * E);
     float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
 #pragma unroll
     for (int i = 0; i < Q; ++i) {
-      s0 = fmaf(q4[i].x, kv[i].x, s0); s1 = fmaf(q4[i].y, kv[i].y, s1);
-      s2 = fmaf(q4[i].z, kv[i].z, s2); s3 = fmaf(q4[i].w, kv[i].w, s3);
+      s0 = fmaf(q4[i].x, kv[4 * i], s0); s1 = fmaf(q4[i].y, kv[4 * i + 1], s1);
+      s2 = fmaf(q4[i].z, kv[4 * i + 2], s2); s3 = fmaf(q4[i].w, kv[4 * i + 3], s3);
     }
     const float s = ((s0 + s1) + (s2 + s3)) * alpha;
     sc[t] = s;
@@ -171,31 +207,39 @@ __global__ void __launch_bounds__(256) attn_decode_kernel(const float* __restric
 #pragma unroll
   for (int w = 0; w < 8; ++w) tot += red[8 + w];
   const float inv = 1.f / tot;
-  // ctx[d] = sum_t p_t v[t][d]: thread = (quad of d, one of GROUPS interleaved t ranges); 16-byte loads coalesced over d
-  const int dq = t0 % Q, g = t0 / Q;
-  float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
+  // ctx[d] = sum_t p_t v[t][d]: thread = (E-wide slice of d, one of GROUPS interleaved t ranges); 16-byte loads coalesced over d.
+  // GROUPS doubles for fp16 (E = 8), so the fp16 cache's partial sums are grouped and added differently from the fp32 cache's.
+  const int dq = t0 % VQ, g = t0 / VQ;
+  float o[E];
+#pragma unroll
+  for (int e = 0; e < E; ++e) o[e] = 0.f;
   int t = g;
   for (; t + 7 * GROUPS < lenc; t += 8 * GROUPS) {
-    float4 vv[8];
+    float vv[8][E];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) vv[u] = __ldg(reinterpret_cast<const float4*>(vb + (size_t)(t + u * GROUPS) * HD) + dq);
+    for (int u = 0; u < 8; ++u) load16(vb + (size_t)(t + u * GROUPS) * HD + dq * E, vv[u]);
 #pragma unroll
     for (int u = 0; u < 8; ++u) {
       const float p = sc[t + u * GROUPS];
-      o.x = fmaf(p, vv[u].x, o.x); o.y = fmaf(p, vv[u].y, o.y); o.z = fmaf(p, vv[u].z, o.z); o.w = fmaf(p, vv[u].w, o.w);
+#pragma unroll
+      for (int e = 0; e < E; ++e) o[e] = fmaf(p, vv[u][e], o[e]);
     }
   }
   for (; t < lenc; t += GROUPS) {
-    const float4 vv = __ldg(reinterpret_cast<const float4*>(vb + (size_t)t * HD) + dq);
+    float vv[E];
+    load16(vb + (size_t)t * HD + dq * E, vv);
     const float p = sc[t];
-    o.x = fmaf(p, vv.x, o.x); o.y = fmaf(p, vv.y, o.y); o.z = fmaf(p, vv.z, o.z); o.w = fmaf(p, vv.w, o.w);
+#pragma unroll
+    for (int e = 0; e < E; ++e) o[e] = fmaf(p, vv[e], o[e]);
   }
   if (APPEND && g == 0) {
-    const float4 vv = *reinterpret_cast<const float4*>(vs + 4 * dq);
     const float p = sc[len - 1];
-    o.x = fmaf(p, vv.x, o.x); o.y = fmaf(p, vv.y, o.y); o.z = fmaf(p, vv.z, o.z); o.w = fmaf(p, vv.w, o.w);
+#pragma unroll
+    for (int e = 0; e < E; ++e) o[e] = fmaf(p, vs[E * dq + e], o[e]);
   }
-  *reinterpret_cast<float4*>(po + (size_t)g * HD + 4 * dq) = o;
+#pragma unroll
+  for (int e = 0; e < E; e += 4)
+    *reinterpret_cast<float4*>(po + (size_t)g * HD + E * dq + e) = make_float4(o[e], o[e + 1], o[e + 2], o[e + 3]);
   __syncthreads();
   if (t0 < HD) {
     float v = 0.f;
@@ -399,26 +443,30 @@ int mas_linear_small(const float* x, int64_t ldx, const float* W, const float* b
   }
 }
 
-int mas_kv_append(const float* qkv, int R, int T, int heads, int hd, float* kcache, float* vcache, int Tmax, int pos0, void* stream) {
-  MAS_REQUIRE(qkv && kcache && vcache && R > 0 && T > 0 && heads > 0 && hd > 0, "kv_append: bad arguments");
+}  // extern "C"
+
+template <typename T>
+static int kv_append_run(const float* qkv, int R, int T_, int heads, int hd, T* kcache, T* vcache, int Tmax, int pos0, void* stream) {
+  MAS_REQUIRE(qkv && kcache && vcache && R > 0 && T_ > 0 && heads > 0 && hd > 0, "kv_append: bad arguments");
   if (hd % 4) return fail(MAS_ERR_UNSUPPORTED, "kv_append: head dim %% 4 != 0");
-  if (pos0 < 0 || pos0 + T > Tmax) return fail(MAS_ERR_INVALID_ARG, "kv_append: positions %d..%d outside the cache (%d)", pos0, pos0 + T, Tmax);
-  const int64_t total = (int64_t)R * T * heads * (hd / 4);
-  kv_append_kernel<<<(int)(cdiv(total, 256) < 2368 ? cdiv(total, 256) : 2368), 256, 0, S(stream)>>>(qkv, R, T, heads, hd, kcache, vcache,
-                                                                                                 Tmax, pos0);
+  if (pos0 < 0 || pos0 + T_ > Tmax) return fail(MAS_ERR_INVALID_ARG, "kv_append: positions %d..%d outside the cache (%d)", pos0, pos0 + T_, Tmax);
+  const int64_t total = (int64_t)R * T_ * heads * (hd / 4);
+  kv_append_kernel<T><<<(int)(cdiv(total, 256) < 2368 ? cdiv(total, 256) : 2368), 256, 0, S(stream)>>>(qkv, R, T_, heads, hd, kcache,
+                                                                                                    vcache, Tmax, pos0);
   return launched("kv_append");
 }
 
-static int attn_decode_run(const float* qkv, float* kcache, float* vcache, float* ctx, int R, int heads, int hd, int Tmax, int len,
+template <typename T>
+static int attn_decode_run(const float* qkv, T* kcache, T* vcache, float* ctx, int R, int heads, int hd, int Tmax, int len,
                            bool append, void* stream) {
   MAS_REQUIRE(qkv && kcache && vcache && ctx && R > 0 && heads > 0, "attn_decode: bad arguments");
   if (len <= 0 || len > Tmax) return fail(MAS_ERR_INVALID_ARG, "attn_decode: cache length %d outside (0, %d]", len, Tmax);
-  const size_t smem = (size_t)(hd + ((len + 3) & ~3) + 32 + 1024 + 2 * hd) * sizeof(float);
+  const size_t smem = (size_t)(hd + ((len + 3) & ~3) + 32 + 256 * Vec16<T>::E + 2 * hd) * sizeof(float);
   if (smem > 48 * 1024) return fail(MAS_ERR_UNSUPPORTED, "attn_decode: sequence too long for the single-pass kernel (%d)", len);
   const int grid = R * heads;
-#define MAS_AD(HD_)                                                                                                        \
-  if (append) attn_decode_kernel<HD_, true><<<grid, 256, smem, S(stream)>>>(qkv, kcache, vcache, ctx, heads, Tmax, len); \
-  else attn_decode_kernel<HD_, false><<<grid, 256, smem, S(stream)>>>(qkv, kcache, vcache, ctx, heads, Tmax, len)
+#define MAS_AD(HD_)                                                                                                           \
+  if (append) attn_decode_kernel<HD_, true, T><<<grid, 256, smem, S(stream)>>>(qkv, kcache, vcache, ctx, heads, Tmax, len); \
+  else attn_decode_kernel<HD_, false, T><<<grid, 256, smem, S(stream)>>>(qkv, kcache, vcache, ctx, heads, Tmax, len)
   switch (hd) {
     case 16: MAS_AD(16); break;
     case 32: MAS_AD(32); break;
@@ -430,15 +478,37 @@ static int attn_decode_run(const float* qkv, float* kcache, float* vcache, float
   return launched(append ? "attn_decode_append" : "attn_decode");
 }
 
+extern "C" {
+
+int mas_kv_append(const float* qkv, int R, int T, int heads, int hd, float* kcache, float* vcache, int Tmax, int pos0, void* stream) {
+  return kv_append_run(qkv, R, T, heads, hd, kcache, vcache, Tmax, pos0, stream);
+}
+
+int mas_kv_append_f16(const float* qkv, int R, int T, int heads, int hd, void* kcache, void* vcache, int Tmax, int pos0, void* stream) {
+  return kv_append_run(qkv, R, T, heads, hd, (__half*)kcache, (__half*)vcache, Tmax, pos0, stream);
+}
+
 int mas_attn_decode(const float* qkv, const float* kcache, const float* vcache, float* ctx, int R, int heads, int hd, int Tmax, int len,
                     void* stream) {
   return attn_decode_run(qkv, const_cast<float*>(kcache), const_cast<float*>(vcache), ctx, R, heads, hd, Tmax, len, false, stream);
+}
+
+int mas_attn_decode_f16(const float* qkv, const void* kcache, const void* vcache, float* ctx, int R, int heads, int hd, int Tmax, int len,
+                        void* stream) {
+  return attn_decode_run(qkv, (__half*)const_cast<void*>(kcache), (__half*)const_cast<void*>(vcache), ctx, R, heads, hd, Tmax, len, false,
+                         stream);
 }
 
 int mas_attn_decode_append(const float* qkv, float* kcache, float* vcache, float* ctx, int R, int heads, int hd, int Tmax, int pos,
                            void* stream) {
   if (pos < 0 || pos >= Tmax) return fail(MAS_ERR_INVALID_ARG, "attn_decode_append: position %d outside the cache (%d)", pos, Tmax);
   return attn_decode_run(qkv, kcache, vcache, ctx, R, heads, hd, Tmax, pos + 1, true, stream);
+}
+
+int mas_attn_decode_append_f16(const float* qkv, void* kcache, void* vcache, float* ctx, int R, int heads, int hd, int Tmax, int pos,
+                               void* stream) {
+  if (pos < 0 || pos >= Tmax) return fail(MAS_ERR_INVALID_ARG, "attn_decode_append: position %d outside the cache (%d)", pos, Tmax);
+  return attn_decode_run(qkv, (__half*)kcache, (__half*)vcache, ctx, R, heads, hd, Tmax, pos + 1, true, stream);
 }
 
 int mas_cfg_mix(const float* cond, const float* uncond, float* out, int64_t n, float scale, void* stream) {

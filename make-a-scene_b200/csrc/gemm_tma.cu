@@ -12,6 +12,8 @@
 //     from L2), 4-stage ring of 48 KB that keeps running across items while the warpgroups store the previous item;
 //   * warps 0-7 MMA + epilogue (two warpgroups), warp 8 copy issuer (its warpgroup hands its registers to the MMA ones):
 //     no thread touches an operand.
+// The rows per work item are a template parameter: 256 for training, 16 .. 256 with split-K for the sampler's decode steps
+// (mas_linear_rows_f16).
 #include <cuda.h>
 #include <cudaTypedefs.h>
 #include <cuda_fp16.h>
@@ -28,42 +30,72 @@ namespace tc {
 
 constexpr int G_MMA_WARPS = 8;
 constexpr int G_THREADS = (G_MMA_WARPS + 4) * 32;   // + the copy-issuing warpgroup
-constexpr int G_STAGES = 4;
-constexpr int G_ROWS = 256;                        // rows of x per work item (N of the MMA)
-constexpr int G_A = G_ROWS * 128;                  // 256 rows x 64 halves
+constexpr int G_ROWS = 256;                        // rows of x per work item of the training GEMM (N of the MMA)
 constexpr int G_BSUB = 2 * BN * 16;                // one K = 16 step of the packed weights: [2][128][8 halves] = 4 KB
 constexpr int G_B = 4 * G_BSUB;                    // the chunk's four steps
-constexpr int G_STAGE = G_A + G_B;                 // 48 KB
+
+// ROWS rows of x per work item (the MMA's N: 16 .. 256).  256 is the training GEMM's shape (4 stages of 48 KB); the narrow
+// decode shapes keep more stages of their smaller tiles in flight, since every stage is mostly weight bytes.
+template <int ROWS>
+struct GTile {
+  static constexpr int A = ROWS * 128;             // ROWS rows x 64 halves
+  static constexpr int STAGE = A + G_B;
+  static constexpr int STAGES = ROWS == G_ROWS ? 4 : (200 * 1024 / STAGE < 8 ? 200 * 1024 / STAGE : 8);
+  static constexpr size_t SMEM = 1024 + (size_t)STAGES * STAGE + 2 * STAGES * 8 + 16;
+  static_assert(STAGE % 1024 == 0, "stages must keep the swizzle atoms 1024-byte aligned");
+};
 
 struct GParams {
   const void* wpk;     // mas_pack_gemm_tc16 image
   const float* bias;   // [N] or null
   const float* res;    // [M, ldy] like y, or null
-  float* y;
+  float* y;            // split s writes y + s * split_stride
   int64_t M, ldy;
   int K, N, Nstore;    // N: padded to 128 (rows of the packed image), Nstore: columns actually stored
-  int64_t units;       // 256-row tiles
+  int64_t units;       // ROWS-row tiles
   const float* x_amax; // amax the fp16 copy of x was scaled from (null: unscaled)
   float alpha;
+  // decode form only
+  int splits, cps;     // split-K: splits slices of cps 64-wide chunks each
+  int act;             // 1: tanh-GELU after the bias
+  int64_t split_stride;
 };
 
+__device__ __forceinline__ float gelu_tanh(float v) {   // OpenAI tanh-GELU, transformer.py:11-14 (as mas_linear_small)
+  const float u = 0.7978845608028654f * v * (1.f + 0.044715f * v * v);
+  return 0.5f * v * (1.f + tanhf(u));
+}
+
+template <int ROWS>
+__device__ __forceinline__ void wgmma_rows(float* acc, uint64_t wd, uint64_t xd, uint32_t scale_d) {
+  if constexpr (ROWS == 256) wg::wgmma_f16_ss_n256<0, 0>(acc, wd, xd, scale_d);
+  else if constexpr (ROWS == 128) wg::wgmma_f16_ss_n128<0, 0>(acc, wd, xd, scale_d);
+  else if constexpr (ROWS == 64) wg::wgmma_f16_ss_n64<0, 0>(acc, wd, xd, scale_d);
+  else if constexpr (ROWS == 32) wg::wgmma_f16_ss_n32<0, 0>(acc, wd, xd, scale_d);
+  else wg::wgmma_f16_ss_n16<0, 0>(acc, wd, xd, scale_d);
+}
+
+// DECODE: the decode-step form (split-K slices, fused GELU); the training GEMM is <256, false>.
+template <int ROWS, bool DECODE>
 __global__ void __launch_bounds__(G_THREADS, 1) rows_gemm_t16(const GParams p, const __grid_constant__ CUtensorMap x_map) {
+  using T = GTile<ROWS>;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t raw_base = smem_u32(smem_raw);
   const uint32_t smem_base = (raw_base + 1023u) & ~1023u;           // swizzle atoms are 1024-byte aligned
   uint8_t* smem = smem_raw + (smem_base - raw_base);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)G_STAGES * G_STAGE);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)T::STAGES * T::STAGE);
   const uint32_t bar_base = smem_u32(bars);
   auto full = [&](int s) { return bar_base + 8u * s; };
-  auto empty = [&](int s) { return bar_base + 8u * (G_STAGES + s); };
+  auto empty = [&](int s) { return bar_base + 8u * (T::STAGES + s); };
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int chunks = p.K / 64;
   const int n_tiles = p.N / BN;
-  const int64_t nitems = p.units * n_tiles;
+  const int splits = DECODE ? p.splits : 1, cps = DECODE ? p.cps : chunks;
+  const int64_t nitems = p.units * splits * n_tiles;   // feature tile fastest, then the K slice, then the row tile
 
   if (tid == 0) {
-    for (int s = 0; s < G_STAGES; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), G_MMA_WARPS * 32); }
+    for (int s = 0; s < T::STAGES; ++s) { mbar_init(full(s), 1); mbar_init(empty(s), G_MMA_WARPS * 32); }
     fence_barrier_init();
   }
   __syncthreads();
@@ -78,43 +110,50 @@ __global__ void __launch_bounds__(G_THREADS, 1) rows_gemm_t16(const GParams p, c
     const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2), fcol = 2 * (lane & 3);
     int s = 0, prev = 0;
     uint32_t sph = 0;
-    float acc[G_ROWS / 2];
+    float acc[ROWS / 2];
     for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-      for (int c = 0; c < chunks; ++c) {
+      int split = 0, c0 = 0, c1 = chunks;
+      if constexpr (DECODE) {
+        split = (int)(item / n_tiles % splits);
+        c0 = split * cps;
+        c1 = min(chunks, c0 + cps);
+      }
+      for (int c = c0; c < c1; ++c) {
         mbar_wait(full(s), sph);
-        const uint32_t st = smem_base + (uint32_t)s * G_STAGE;
+        const uint32_t st = smem_base + (uint32_t)s * T::STAGE;
         const uint64_t xd0 = wg::desc(st, 16, 1024, wg::SW_128);
-        const uint64_t wd0 = wg::desc(st + G_A + (uint32_t)(wgi * 1024), BN * 16, 128);
+        const uint64_t wd0 = wg::desc(st + T::A + (uint32_t)(wgi * 1024), BN * 16, 128);
         wg::fence();
 #pragma unroll
-        for (int sub = 0; sub < 4; ++sub)   // D^T = W x X^T: weights on the M side, the 256 rows on the N side
-          wg::wgmma_f16_ss_n256<0, 0>(acc, wd0 + (uint64_t)((sub * G_BSUB) >> 4), xd0 + (uint64_t)((sub * 32) >> 4),
-                                      (c > 0 || sub > 0) ? 1u : 0u);
+        for (int sub = 0; sub < 4; ++sub)   // D^T = W x X^T: weights on the M side, the ROWS rows on the N side
+          wgmma_rows<ROWS>(acc, wd0 + (uint64_t)((sub * G_BSUB) >> 4), xd0 + (uint64_t)((sub * 32) >> 4), (c > c0 || sub > 0) ? 1u : 0u);
         wg::commit();
         wg::wait<1>();
-        if (c > 0) mbar_arrive(empty(prev));   // the previous chunk's MMAs have read their stage
+        if (c > c0) mbar_arrive(empty(prev));   // the previous chunk's MMAs have read their stage
         prev = s;
-        if (++s == G_STAGES) { s = 0; sph ^= 1; }
+        if (++s == T::STAGES) { s = 0; sph ^= 1; }
       }
       wg::wait<0>();
-      wg::fence_regs<G_ROWS / 2>(acc);
+      wg::fence_regs<ROWS / 2>(acc);
       mbar_arrive(empty(prev));
-      const int64_t unit = item / n_tiles;
-      const int64_t row0 = unit * G_ROWS + fcol;
+      const int64_t unit = DECODE ? item / n_tiles / splits : item / n_tiles;
+      const int64_t row0 = unit * ROWS + fcol;
+      float* y = DECODE ? p.y + split * p.split_stride : p.y;
 #pragma unroll
       for (int i = 0; i < 2; ++i) {
         const int ch = (int)(item % n_tiles) * BN + frow + 8 * i;
         if (ch < p.Nstore) {
           const float bv = p.bias ? __ldg(p.bias + ch) : 0.f;
 #pragma unroll
-          for (int j = 0; j < G_ROWS / 8; ++j) {
+          for (int j = 0; j < ROWS / 8; ++j) {
 #pragma unroll
             for (int cc = 0; cc < 2; ++cc) {
               const int64_t r = row0 + 8 * j + cc;
               if (r < p.M) {
                 float o = fmaf(acc[4 * j + 2 * i + cc], alpha, bv);
                 if (p.res) o += __ldg(p.res + r * p.ldy + ch);
-                p.y[r * p.ldy + ch] = o;
+                if (DECODE && p.act) o = gelu_tanh(o);
+                y[r * p.ldy + ch] = o;
               }
             }
           }
@@ -129,15 +168,16 @@ __global__ void __launch_bounds__(G_THREADS, 1) rows_gemm_t16(const GParams p, c
       uint32_t sph = 0;
       const int ksteps = p.K / 16;
       for (int64_t item = blockIdx.x; item < nitems; item += gridDim.x) {
-        const int64_t unit = item / n_tiles;
+        const int64_t unit = DECODE ? item / n_tiles / splits : item / n_tiles;
+        const int c0 = DECODE ? (int)(item / n_tiles % splits) * cps : 0, c1 = DECODE ? min(chunks, c0 + cps) : chunks;
         const uint8_t* wsrc = reinterpret_cast<const uint8_t*>(p.wpk) + (size_t)(item % n_tiles) * ksteps * G_BSUB;
-        for (int c = 0; c < chunks; ++c) {
+        for (int c = c0; c < c1; ++c) {
           mbar_wait(empty(s), sph ^ 1);
-          const uint32_t st = smem_base + (uint32_t)s * G_STAGE;
-          mbar_expect_tx(full(s), G_STAGE);
-          tma_load_2d(st, &x_map, c * 64, (int)(unit * G_ROWS), full(s));
-          bulk_g2s(st + G_A, wsrc + (size_t)c * G_B, G_B, full(s));
-          if (++s == G_STAGES) { s = 0; sph ^= 1; }
+          const uint32_t st = smem_base + (uint32_t)s * T::STAGE;
+          mbar_expect_tx(full(s), T::STAGE);
+          tma_load_2d(st, &x_map, c * 64, (int)(unit * ROWS), full(s));
+          bulk_g2s(st + T::A, wsrc + (size_t)c * G_B, G_B, full(s));
+          if (++s == T::STAGES) { s = 0; sph ^= 1; }
         }
       }
     }
@@ -145,7 +185,20 @@ __global__ void __launch_bounds__(G_THREADS, 1) rows_gemm_t16(const GParams p, c
   }
 }
 
-constexpr size_t g16_smem_bytes() { return 1024 + (size_t)G_STAGES * G_STAGE + 2 * G_STAGES * 8 + 16; }
+// y[r, n] = act(sum over the splits in order of part[s][r][n] + bias[n])
+__global__ void rows_split_reduce(const float* __restrict__ part, int splits, int64_t stride, int64_t M, int N,
+                                  const float* __restrict__ bias, int act, float* __restrict__ y, int64_t ldy) {
+  const int64_t total = M * N;
+  for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t r = i / N;
+    const int n = (int)(i % N);
+    float v = part[i];
+    for (int s = 1; s < splits; ++s) v += part[s * stride + i];
+    if (bias) v += __ldg(bias + n);
+    if (act) v = gelu_tanh(v);
+    y[r * ldy + n] = v;
+  }
+}
 
 // ------------------------------------------------------------------------------------------------------------
 // Weight gradient of a Linear layer from the two fp16 copies (activation x16 [M,K], output gradient dy16 [M,N], both scaled by
@@ -289,43 +342,101 @@ constexpr size_t rw_smem_bytes() {
 
 bool gemm_rows_f16_ok(int64_t M, int N, int K) { return M > 0 && N > 0 && K >= 64 && K % 64 == 0 && M < (1ll << 31) - 256; }
 
+template <int ROWS, bool DECODE>
+static int rows_gemm_run(tc::GParams p, const void* x16, cudaStream_t st) {
+  using T = tc::GTile<ROWS>;
+  PFN_cuTensorMapEncodeTiled enc = tensor_map_encoder();
+  if (!enc) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled entry point not available");
+  CUtensorMap map;
+  cuuint64_t dims[2] = {(cuuint64_t)p.K, (cuuint64_t)p.M};
+  cuuint64_t strides[1] = {(cuuint64_t)p.K * 2};
+  cuuint32_t box[2] = {64, (cuuint32_t)ROWS}, es[2] = {1, 1};
+  CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(x16), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (row GEMM map) failed (%d)", (int)r);
+
+  static std::atomic<uint64_t> configured{0};
+  static int sm_count = 132;
+  if (first_on_device(configured)) {
+    cudaError_t e = cudaFuncSetAttribute(tc::rows_gemm_t16<ROWS, DECODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)T::SMEM);
+    if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(smem=%zu): %s", T::SMEM, cudaGetErrorString(e));
+    int dev = 0;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
+    mark_device(configured);
+  }
+  p.units = cdiv(p.M, ROWS);
+  const int64_t nitems = p.units * (DECODE ? p.splits : 1) * (p.N / tc::BN);
+  const unsigned g = (unsigned)(nitems < sm_count ? nitems : sm_count);
+  tc::rows_gemm_t16<ROWS, DECODE><<<g, tc::G_THREADS, T::SMEM, st>>>(p, map);
+  return launched_tc("rows_gemm_t16");
+}
+
 int gemm_rows_f16_launch(const void* x16, int64_t M, int K, const void* w_tc16, float* y, int64_t ldy, int N, const float* bias,
                          const float* res, const float* x_amax, float alpha, cudaStream_t st) {
   if (!gemm_rows_f16_ok(M, N, K)) return fail(MAS_ERR_UNSUPPORTED, "gemm_rows_f16: needs K %% 64 == 0 (M=%lld N=%d K=%d)", (long long)M, N, K);
   auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
   if (!al16(x16) || !al16(w_tc16)) return fail(MAS_ERR_INVALID_ARG, "gemm_rows_f16: x16 / packed weights must be 16-byte aligned");
   tc::GParams p;
-  p.wpk = w_tc16; p.bias = bias; p.res = res; p.y = y; p.M = M; p.ldy = ldy; p.K = K;
+  p.wpk = w_tc16; p.bias = bias; p.res = res; p.y = y; p.M = M; p.ldy = ldy; p.split_stride = 0; p.K = K;
   p.N = (int)cdiv(N, tc::BN) * tc::BN; p.Nstore = N;
-  p.units = cdiv(M, tc::G_ROWS); p.x_amax = x_amax; p.alpha = alpha;
-
-  PFN_cuTensorMapEncodeTiled enc = tensor_map_encoder();
-  if (!enc) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled entry point not available");
-  CUtensorMap map;
-  cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)M};
-  cuuint64_t strides[1] = {(cuuint64_t)K * 2};
-  cuuint32_t box[2] = {64, (cuuint32_t)tc::G_ROWS}, es[2] = {1, 1};
-  CUresult r = enc(&map, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(x16), dims, strides, box, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return fail(MAS_ERR_LAUNCH, "cuTensorMapEncodeTiled (row GEMM map) failed (%d)", (int)r);
-
-  constexpr size_t smem = tc::g16_smem_bytes();
-  static std::atomic<uint64_t> configured{0};
-  static int sm_count = 132;
-  if (first_on_device(configured)) {
-    cudaError_t e = cudaFuncSetAttribute(tc::rows_gemm_t16, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "cudaFuncSetAttribute(smem=%zu): %s", smem, cudaGetErrorString(e));
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev);
-    mark_device(configured);
-  }
-  const int64_t nitems = p.units * (p.N / tc::BN);
-  const unsigned g = (unsigned)(nitems < sm_count ? nitems : sm_count);
-  tc::rows_gemm_t16<<<g, tc::G_THREADS, smem, st>>>(p, map);
-  return launched_tc("rows_gemm_t16");
+  p.splits = 1; p.cps = K / 64; p.act = 0;
+  p.x_amax = x_amax; p.alpha = alpha;
+  return rows_gemm_run<tc::G_ROWS, false>(p, x16, st);
 }
 
+// ---- decode-step Linear layers (a few to a few hundred rows): the same kernel with the rows on a narrower MMA N side and the
+// contraction split so that one wave covers the SMs.  The split factor depends on (N, K) only, never on the row count, so a
+// row's result does not depend on how many rows share the call.  ops.linear_small decides per shape and row count whether this
+// form or the training GEMM serves a decode step.
+static int linear_rows_splits(int N, int K) {
+  const int64_t tiles = cdiv(N, tc::BN);
+  const int chunks = K / 64;
+  int best = 1;
+  double best_score = -1.0;
+  for (int s = 1; s <= 16 && s <= chunks; ++s) {
+    const int cps = (int)cdiv(chunks, s), se = (int)cdiv(chunks, cps);
+    const int64_t g = tiles * se;
+    const double eff = (double)g / (double)(cdiv(g, 132) * 132) - 0.02 * se;   // partial sums cost bytes: fewer splits win ties
+    if (eff > best_score + 1e-9) { best_score = eff; best = se; }
+  }
+  return best;
+}
+static size_t linear_rows_ws(int64_t R, int N, int K) {
+  const int s = linear_rows_splits(N, K);
+  return s > 1 ? (size_t)s * R * N * sizeof(float) : 0;
+}
+
+int linear_rows_f16_launch(const void* x16, int64_t R, int K, const void* w_tc16, float* y, int64_t ldy, int N, const float* bias,
+                           const float* x_amax, int act, void* ws, size_t ws_bytes, cudaStream_t st) {
+  if (!gemm_rows_f16_ok(R, N, K)) return fail(MAS_ERR_UNSUPPORTED, "linear_rows_f16: needs K %% 64 == 0 (R=%lld N=%d K=%d)", (long long)R, N, K);
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  if (!al16(x16) || !al16(w_tc16) || !al16(ws)) return fail(MAS_ERR_INVALID_ARG, "linear_rows_f16: x16 / packed weights / workspace must be 16-byte aligned");
+  if (act != 0 && act != 1) return fail(MAS_ERR_INVALID_ARG, "linear_rows_f16: act must be 0 (none) or 1 (tanh-GELU)");
+  if (ws_bytes < linear_rows_ws(R, N, K)) return fail(MAS_ERR_WORKSPACE, "linear_rows_f16: workspace too small");
+  tc::GParams p;
+  const int splits = linear_rows_splits(N, K);
+  p.wpk = w_tc16; p.res = nullptr; p.M = R; p.K = K;
+  p.N = (int)cdiv(N, tc::BN) * tc::BN; p.Nstore = N;
+  p.splits = splits; p.cps = (int)cdiv(K / 64, splits);
+  p.x_amax = x_amax; p.alpha = 1.f;
+  if (splits > 1) {   // partial sums to the workspace, bias and activation after the ordered sum
+    p.bias = nullptr; p.act = 0; p.y = (float*)ws; p.ldy = N; p.split_stride = R * N;
+  } else {
+    p.bias = bias; p.act = act; p.y = y; p.ldy = ldy; p.split_stride = 0;
+  }
+  int e;
+  if (R <= 16) e = rows_gemm_run<16, true>(p, x16, st);
+  else if (R <= 32) e = rows_gemm_run<32, true>(p, x16, st);
+  else if (R <= 64) e = rows_gemm_run<64, true>(p, x16, st);
+  else if (R <= 128) e = rows_gemm_run<128, true>(p, x16, st);
+  else e = rows_gemm_run<256, true>(p, x16, st);
+  if (e || splits == 1) return e;
+  const int64_t total = R * N;
+  tc::rows_split_reduce<<<(unsigned)(cdiv(total, 256) < 2368 ? cdiv(total, 256) : 2368), 256, 0, st>>>((const float*)ws, splits, R * N, R, N,
+                                                                                                      bias, act, y, ldy);
+  return launched("rows_split_reduce");
+}
 
 void conv_wgrad_reduce_launch(const float* part, int splits, int ntap, int Cout, int Cin, float* dw, const float* bpart, float* dbias,
                               cudaStream_t st);   // contract_simt.cu
@@ -405,6 +516,14 @@ int mas_gemm_rows_f16(const void* x_f16, int64_t M, int K, const void* w_tc16, f
                       const float* residual, const float* x_amax, float alpha, void* stream) {
   MAS_REQUIRE(x_f16 && w_tc16 && y && ldy >= N, "gemm_rows_f16: bad arguments");
   return mas::gemm_rows_f16_launch(x_f16, M, K, w_tc16, y, ldy, N, bias, residual, x_amax, alpha, mas::S(stream));
+}
+
+size_t mas_linear_rows_f16_ws_bytes(int64_t R, int N, int K) { return mas::gemm_rows_f16_ok(R, N, K) ? mas::linear_rows_ws(R, N, K) : 0; }
+
+int mas_linear_rows_f16(const void* x_f16, int64_t R, int K, const void* w_tc16, float* y, int64_t ldy, int N, const float* bias,
+                        const float* x_amax, int act, void* ws, size_t ws_bytes, void* stream) {
+  MAS_REQUIRE(x_f16 && w_tc16 && y && ldy >= N, "linear_rows_f16: bad arguments");
+  return mas::linear_rows_f16_launch(x_f16, R, K, w_tc16, y, ldy, N, bias, x_amax, act, ws, ws_bytes, mas::S(stream));
 }
 
 size_t mas_wgrad_rows_f16_ws_bytes(int64_t M, int N, int K) { return mas::wgrad_rows_f16_ws(M, N, K); }

@@ -473,9 +473,9 @@ int mas_layernorm2_forward(const float* x, const float* gamma1, const float* bet
                            const float* gamma2, const float* beta2, float* y2, int64_t R, int H, float eps1, float eps2, void* stream) {
   MAS_REQUIRE(x && gamma1 && beta1 && y1 && gamma2 && beta2 && y2 && R > 0 && H > 0, "layernorm2_forward: bad arguments");
   auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
-  if (!(R <= 64 && H % 4 == 0 && H <= 4096 && al16(x) && al16(y1) && al16(y2) && al16(gamma1) && al16(beta1) && al16(gamma2) &&
+  if (!(R < (1ll << 31) && H % 4 == 0 && H <= 4096 && al16(x) && al16(y1) && al16(y2) && al16(gamma1) && al16(beta1) && al16(gamma2) &&
         al16(beta2) && (!residual || al16(residual))))
-    return fail(MAS_ERR_UNSUPPORTED, "layernorm2_forward: needs R <= 64, H %% 4 == 0, H <= 4096 and 16-byte aligned operands");
+    return fail(MAS_ERR_UNSUPPORTED, "layernorm2_forward: needs H %% 4 == 0, H <= 4096 and 16-byte aligned operands");
   layernorm2_fwd_block_kernel<<<(unsigned)R, 256, 0, S(stream)>>>(x, gamma1, beta1, residual, y1, gamma2, beta2, y2, H, eps1, eps2);
   return launched("layernorm2_fwd_block");
 }

@@ -64,6 +64,12 @@ __device__ __forceinline__ void wgmma_tf32_rs_n32(float* d, const uint32_t* a, u
                : WG_D16(0) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc));
 }
 template <int TA, int TB>
+__device__ __forceinline__ void wgmma_f16_ss_n16(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  asm volatile(WG_PRED(10) "wgmma.mma_async.sync.aligned.m64n16k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, %11, %12;\n\t}"
+               : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+               : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));
+}
+template <int TA, int TB>
 __device__ __forceinline__ void wgmma_f16_ss_n32(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
   asm volatile(WG_PRED(18) "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 " WG_V16 ", %16, %17, p, 1, 1, %19, %20;\n\t}"
                : WG_D16(0) : "l"(adesc), "l"(bdesc), "r"(acc), "n"(TA), "n"(TB));

@@ -1592,30 +1592,81 @@ def sample_topk(logits, temperature, top_k, u):
 
 
 # ---- autoregressive sampling (inference only; SURVEY.md 8f-3) --------------------------------------------------
+DECODE_F32_ROWS = 8   # decode steps of up to this many rows run strict fp32 (weights and KV cache); more rows run fp16 operands
+
+
+def decode_weight_image(weight):
+    """The fp16 operand image the decode steps above 8 rows read for an nn.Linear weight [N,K]: the training image
+    (mas_pack_gemm_tc16), of the weight zero-padded to 128 output features, cached per parameter version."""
+    N, K = weight.shape
+    return _packed_linear_weight(_padded(weight, (-(-N // 128) * 128, K)), False, weight.device)
+
+
+# Largest row count at which the narrow split form (mas_linear_rows_f16) beat the training GEMM, per decode shape (N, K) of the
+# 1024-wide model, timed by tools/bench_decode.py with the weights streaming from HBM (H100 SXM 80 GB, 700 W).
+# Beyond these it is the training GEMM (8-32 CTAs of 256 rows) that streams the weights faster; other shapes use the default.
+_NARROW_MAX_ROWS = {(3072, 1024): 64, (1024, 1024): 128, (4096, 1024): 128, (1024, 4096): 256, (8192, 1024): 64}
+_NARROW_MAX_ROWS_DEFAULT = 64
+
+
+def decode_narrow_rows(R, N, K):
+    """Whether a decode Linear of R rows runs the narrow split form rather than the training GEMM."""
+    return R <= _NARROW_MAX_ROWS.get((N, K), _NARROW_MAX_ROWS_DEFAULT)
+
+
 def linear_small(x, weight, bias, act=0):
-    """nn.Linear for a handful of rows ([R<=8, K] -> [R, N]): the weight-streaming decode kernel, strict fp32.
-    act=1 fuses the tanh-GELU of MLP.lin1 (transformer.py:11-14)."""
+    """nn.Linear for the rows of a decode step ([R, K] -> [R, N]); act=1 fuses the tanh-GELU of MLP.lin1 (transformer.py:11-14).
+    R <= 8: the weight-streaming kernel, strict fp32. More rows with K % 64 == 0: one fp16 copy of x (rows_to_half) and the
+    cached fp16 weight image, on the narrow-row split-K GEMM (mas_linear_rows_f16) or the training GEMM (mas_gemm_rows_f16,
+    then mas_gelu_forward for act=1), whichever decode_narrow_rows picks for the shape. Other K: the fp32 kernel over 8-row
+    chunks."""
     _need_cuda(x)
     x = x.contiguous()
     R, K = x.shape
     N = weight.shape[0]
     y = torch.empty((R, N), dtype=torch.float32, device=x.device)
-    L.call("mas_linear_small", x, K, weight.contiguous(), bias, y, N, R, N, K, int(act))
+    if R > DECODE_F32_ROWS and K % 64 == 0:
+        x16, am = rows_to_half(x)
+        wpk = decode_weight_image(weight)
+        if decode_narrow_rows(R, N, K):
+            ws = torch.empty(max(int(L.query("mas_linear_rows_f16_ws_bytes", R, N, K)), 16), dtype=torch.uint8, device=x.device)
+            L.call("mas_linear_rows_f16", x16, R, K, wpk, y, N, N, bias, am, int(act), ws, ws.numel())
+            return y
+        L.call("mas_gemm_rows_f16", x16, R, K, wpk, y, N, N, bias, None, am, 1.0)
+        if act:
+            g = torch.empty_like(y)
+            L.call("mas_gelu_forward", y, g, y.numel())
+            return g
+        return y
+    w = weight.contiguous()
+    for r0 in range(0, R, DECODE_F32_ROWS):
+        r1 = min(R, r0 + DECODE_F32_ROWS)
+        L.call("mas_linear_small", x[r0:r1], K, w, bias, y[r0:r1], N, r1 - r0, N, K, int(act))
     return y
 
 
+def _cache_entry(name, kcache):
+    """The fp32 entry for fp32 caches, its _f16 twin for fp16 ones."""
+    if kcache.dtype == torch.float16:
+        return name + "_f16"
+    if kcache.dtype != torch.float32:
+        raise RuntimeError("KV caches are float32 or float16, got %s" % kcache.dtype)
+    return name
+
+
 def kv_append(qkv, kcache, vcache, pos0):
-    """qkv [R,T,3H] (fused q|k|v activation) -> caches [R,heads,Tmax,hd] at positions pos0..pos0+T-1."""
+    """qkv [R,T,3H] (fused q|k|v activation) -> caches [R,heads,Tmax,hd] (fp32, or fp16 rounded to nearest) at positions
+    pos0..pos0+T-1."""
     R, heads, Tmax, hd = kcache.shape
     T = qkv.shape[1]
-    L.call("mas_kv_append", qkv.contiguous(), R, T, heads, hd, kcache, vcache, Tmax, int(pos0))
+    L.call(_cache_entry("mas_kv_append", kcache), qkv.contiguous(), R, T, heads, hd, kcache, vcache, Tmax, int(pos0))
 
 
 def attn_decode(qkv, kcache, vcache, length):
     """One query per (row, head) (qkv [R,3H]) against the first `length` cached positions -> ctx [R,H]."""
     R, heads, Tmax, hd = kcache.shape
     ctx = torch.empty((R, heads * hd), dtype=torch.float32, device=qkv.device)
-    L.call("mas_attn_decode", qkv.contiguous(), kcache, vcache, ctx, R, heads, hd, Tmax, int(length))
+    L.call(_cache_entry("mas_attn_decode", kcache), qkv.contiguous(), kcache, vcache, ctx, R, heads, hd, Tmax, int(length))
     return ctx
 
 
@@ -1624,12 +1675,13 @@ def attn_decode_append(qkv, kcache, vcache, pos):
     positions 0..pos -> ctx [R,H]."""
     R, heads, Tmax, hd = kcache.shape
     ctx = torch.empty((R, heads * hd), dtype=torch.float32, device=qkv.device)
-    L.call("mas_attn_decode_append", qkv.contiguous(), kcache, vcache, ctx, R, heads, hd, Tmax, int(pos))
+    L.call(_cache_entry("mas_attn_decode_append", kcache), qkv.contiguous(), kcache, vcache, ctx, R, heads, hd, Tmax, int(pos))
     return ctx
 
 
 def layernorm2(x, ln1, residual, ln2):
-    """(y1, y2) = (residual + ln1(x), ln2(y1)) for a few rows [R,H] in one launch (inference; nn.LayerNorm modules)."""
+    """(y1, y2) = (residual + ln1(x), ln2(y1)) for the rows [R,H] of a decode step in one launch (inference; nn.LayerNorm
+    modules)."""
     _need_cuda(x)
     x = x.contiguous()
     R, H = x.shape

@@ -140,20 +140,34 @@ class Transformer(nn.Module):
         return self.final_ln(x), {}
 
 
+def _param_version(model):
+    return tuple((p._version, p.data_ptr()) for p in model.parameters())
+
+
 class _GraphedDecoder:
     """KV caches + one captured CUDA graph per image position for MakeAScene.generate(use_graphs=True).
 
     A decode step is ~250 launches of a few microseconds each (24 layers x 10 kernels): launched from Python it is
     host-bound (~22 us per launch). The kernels only depend on the position through launch parameters, so each position
-    gets its own graph (captured on first use, replayed in position order afterwards; the graphs share one memory pool)."""
+    gets its own graph (captured on first use, replayed in position order afterwards; the graphs share one memory pool).
+    The caches are fp32 up to 8 rows and fp16 above (the cache read dominates a step at a few hundred rows).
+    Above 8 rows the decode Linears read the fp16 weight images of ops.decode_weight_image: they are built here, before any
+    capture, and held by the decoder, so the graphs never record a packing launch and never outlive the images they read.
+    `version` records every parameter's version and storage: generate() builds a new decoder when it changes."""
 
     def __init__(self, model, rows, dev):
         layers = model.transformer.layers
         heads = layers[0].attn.num_attn_heads
         hd = model.hidden_dim // heads
         self.model, self.rows = model, rows
-        self.kc = [torch.empty((rows, heads, model.total_length, hd), dtype=torch.float32, device=dev) for _ in layers]
+        dt = torch.float32 if rows <= ops.DECODE_F32_ROWS else torch.float16
+        self.kc = [torch.empty((rows, heads, model.total_length, hd), dtype=dt, device=dev) for _ in layers]
         self.vc = [torch.empty_like(k) for k in self.kc]
+        self.version = _param_version(model)
+        self.images = []
+        if rows > ops.DECODE_F32_ROWS:
+            lins = [m for l in layers for m in (l.attn.qkv, l.attn.out_proj, l.mlp.lin1, l.mlp.lin2)] + [model.to_logits[1]]
+            self.images = [ops.decode_weight_image(m.weight) for m in lins if m.weight.shape[1] % 64 == 0]
         self.tok = torch.zeros(rows, dtype=torch.long, device=dev)
         self.pool = torch.cuda.graph_pool_handle()
         self.graphs, self.keep = {}, {}
@@ -213,7 +227,8 @@ class MakeAScene(nn.Module):
         self.to_logits = torch.nn.Sequential(LayerNorm(hidden_dim), Linear(hidden_dim, image_vocab_size))
 
     def reset_sampler(self):
-        """Drops the cached KV buffers / CUDA graphs of generate(use_graphs=True)."""
+        """Drops the cached KV buffers / CUDA graphs of generate(use_graphs=True) (they are rebuilt by themselves when a
+        parameter changes)."""
         self._sampler = None
 
     def _init_weights(self, module):
@@ -315,12 +330,15 @@ class MakeAScene(nn.Module):
         """Autoregressive sampling of the image tokens with a KV cache; optional classifier-free guidance
         (logits = uncond + scale * (cond - uncond), the unconditional stream sees padded text; Make-A-Scene paper 3.4).
 
-        text_tokens [B,text_length], seg_tokens [B,seg_length] int64. B (x2 with guidance) <= 8 rows per call.
+        text_tokens [B,text_length], seg_tokens [B,seg_length] int64. A call decodes R = B rows (2B with guidance); memory is
+        the only limit on R. Up to 8 rows the decode steps are strict fp32 (weights and KV cache). More rows run the decode
+        Linear layers on fp16 operands with fp32 accumulation and keep K / V in fp16 caches: the arithmetic of the model's own
+        training forward. The prefix pass always runs the training kernels.
         temperature 0 = greedy; top_k keeps the k most likely codes. img_tokens (optional [B,image_length]) are fed
         instead of the sampled ones (teacher forcing — what the parity test uses). Returns tokens [B,image_length]
         (and the per-position logits [B,image_length,V] actually sampled from when return_logits=True).
         use_graphs: replay each position's decode step from a CUDA graph (captured at first use and kept on the module for
-        the same row count; call reset_sampler() after replacing parameter storage)."""
+        the same row count; captured again after any parameter changes, in place or by replaced storage)."""
         B = text_tokens.shape[0]
         dev = text_tokens.device
         cfg = guidance_scale is not None and float(guidance_scale) != 1.0
@@ -332,10 +350,8 @@ class MakeAScene(nn.Module):
         else:
             text_all, seg_all = text_tokens, seg_tokens
         R = text_all.shape[0]
-        if R > 8:
-            raise ValueError("generate: at most 8 rows per call (batch x2 with guidance)")
         dec = getattr(self, "_sampler", None)
-        if dec is None or dec.rows != R or dec.tok.device != dev or not use_graphs:
+        if dec is None or dec.rows != R or dec.tok.device != dev or not use_graphs or dec.version != _param_version(self):
             dec = _GraphedDecoder(self, R, dev)
             if use_graphs:
                 self._sampler = dec

@@ -1,16 +1,19 @@
 """Tokens/s of classifier-free-guided sampling with the KV cache (BASELINE.json configs[4]: 24 layers, 1024 wide, 16
 heads, 128 text + 256 segmentation tokens -> 256 image tokens of an 8192-code vocabulary; random-init weights).
-One JSON line; not part of bench.py's headline (the reference has no sampler to compare with: SURVEY.md 8f-3).
-Usage: python tools/bench_sampling.py [--batch B] [--reps N]"""
+One JSON line; not part of bench.py's headline (the reference has no sampler to compare with: SURVEY.md 8f-3). It carries the
+GPU's name and power limit, and the HBM bytes a decode step streams on the path actually taken: up to 8 rows fp32 weights and
+fp32 KV cache, above 8 rows fp16 weights and fp16 cache (the cache read at the mean cache length of the image positions).
+Usage: python tools/bench_sampling.py [--batch B] [--reps N] [--graphs]"""
 import argparse
 import json
 import os
+import subprocess
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, "make-a-scene_b200")]
 import torch  # noqa: E402
-from mas_b200 import _lib  # noqa: E402
+from mas_b200 import _lib, ops  # noqa: E402
 from models.transformer import MakeAScene  # noqa: E402
 
 ap = argparse.ArgumentParser()
@@ -39,8 +42,16 @@ for _ in range(args.reps):
 e1.record()
 torch.cuda.synchronize()
 sec = e0.elapsed_time(e1) * 1e-3 / args.reps
+gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, check=True)
+R = 2 * B
+elem = 4 if R <= ops.DECODE_F32_ROWS else 2
 params = sum(p.numel() for n, p in m.named_parameters() if "embedding" not in n)
+prefix, steps = 128 + 256, 255
+mean_len = prefix + (steps + 1) / 2                       # cache positions read by the step of image position t: prefix + t + 1
+weight_bytes = params * elem
+cache_bytes = args.layers * R * 2 * cfg["hidden_dim"] * mean_len * elem
 print(json.dumps({"metric": "image tokens/s, classifier-free guided sampling with KV cache", "value": B * 256 / sec, "unit": "tokens/s",
-                  "batch": B, "rows": 2 * B, "cuda_graphs": bool(args.graphs), "seconds_per_image": sec, "launches_per_image": (_lib.launch_count() - l0) // args.reps,
-                  "weight_stream_gb_per_token": params * 4 / 1e9,
-                  "weight_stream_gbs": params * 4 * 255 / sec / 1e9, "config": cfg}))
+                  "gpu": gpu.stdout.strip().splitlines()[0], "batch": B, "rows": R, "cuda_graphs": bool(args.graphs),
+                  "seconds_per_image": sec, "launches_per_image": (_lib.launch_count() - l0) // args.reps,
+                  "operand_bytes": elem, "weight_stream_gb_per_step": weight_bytes / 1e9, "cache_gb_per_step": cache_bytes / 1e9,
+                  "hbm_stream_gbs": (weight_bytes + cache_bytes) * steps / sec / 1e9, "config": cfg}))
