@@ -497,6 +497,19 @@ int mas_cfg_mix(const float* cond, const float* uncond, float* out, int64_t n, f
  * tokens[r] = first index whose running sum of p exceeds u[r] (u in [0,1): caller-supplied uniforms, device floats). */
 int mas_sample_topk(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, const float* u,
                     int64_t* tokens, void* stream);
+/* The same draw with the rest of ru-DALL-E's controls, one launch for all rows.  Per row:
+ *   1. z = logits / temperature;  2. top-k as mas_sample_topk (ties with the k-th largest kept);
+ *   3. top-p (0 < top_p < 1; top_p >= 1: off): of the entries top-k kept, an entry is kept when the softmax mass of the kept
+ *      entries with a strictly larger z is <= top_p (top_k_top_p_filtering's rule; equal z are kept or dropped together, the
+ *      largest entry always stays).  Masses are summed in 2^-40 fixed point with integer adds: the result is deterministic;
+ *   4. tokens[r] = the inverse CDF of softmax(z) over the kept set at u[r], in index order (mas_sample_topk's draw).
+ * temperature == 0: greedy, the first index of the largest logit; u is not read and may be NULL.
+ * Prompt (prompt_tokens and prompt_mask both non-NULL, or both NULL): where prompt_mask[r * prompt_ld] != 0 the token is
+ * prompt_tokens[r * prompt_ld] and nothing is drawn (u[r] is left unused).  Both are this position's column of [R, L]
+ * tensors with row stride prompt_ld (elements).  mas_sample_topk is the top_p = 1, prompt-free case: same tokens. */
+int mas_sample_filtered(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p,
+                        const float* u, const int64_t* prompt_tokens, const uint8_t* prompt_mask, int64_t prompt_ld,
+                        int64_t* tokens, void* stream);
 
 /* ---- weighted BCE-with-logits (VQ-SEG loss, losses/loss_seg.py:15-22) — "next" row ------------------
  * logits/target: strided [N,H,W,C] views; pos_weight [C]; loss_out = mean over all elements. grad may be NULL. */

@@ -257,22 +257,65 @@ __global__ void cfg_mix_kernel(const float* __restrict__ cond, const float* __re
   }
 }
 
-// Token draw (Make-A-Scene paper 3.4 / generate()): z = logits / temperature, keep the top_k largest (all values equal to the
-// k-th largest are kept, like `z < kth -> -inf`), p = softmax(z), token = inverse CDF of p at u (first index whose running
-// sum exceeds u * total).  Block per row.  The k-th largest value is found by a 4-pass radix select on order-preserving keys.
+// Token draw (Make-A-Scene paper 3.4 / generate()), block per row:
+//   1. z = logits / temperature;
+//   2. top-k: keep the top_k largest (all values equal to the k-th largest are kept, like `z < kth -> -inf`);
+//   3. top-p (top_p < 1): of the entries top-k kept, keep those whose softmax mass of kept entries with a STRICTLY larger z is
+//      <= top_p (top_k_top_p_filtering's rule, with ties decided by value: equal z are kept or dropped together; the largest
+//      entry is always kept);
+//   4. token = inverse CDF of softmax(z) over the kept set at u, in index order (first index whose running sum exceeds
+//      u * total).
+// Both filters are thresholds on order-preserving keys of z, found by 4-pass radix selects (8 bits per pass): top-k on counts,
+// top-p on masses.  The masses are exp(z - max) in 2^-40 fixed point, added with 64-bit integer atomics: associative, so the
+// threshold (and the token) is the same on every launch whatever the block's scheduling.  Quantisation moves a mass by less
+// than V * 2^-40 of the largest entry's, so only an entry whose mass above lies that close to top_p can be decided otherwise
+// than in exact arithmetic.
+// temperature == 0: greedy, the first index of the largest logit (torch.argmax's rule); u is not read.
+// Prompt (pmask != NULL): rows with pmask[r * pld] != 0 take tok = ptok[r * pld] and draw nothing.
 __device__ __forceinline__ uint32_t order_key(float f) {
   const uint32_t b = __float_as_uint(f);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
+constexpr float MASS_ONE = 1099511627776.f;          // 2^40: the largest entry's mass exp(0)
 __global__ void __launch_bounds__(256) sample_topk_kernel(const float* __restrict__ logits, int64_t ld, int V, float temperature, int top_k,
-                                                          const float* __restrict__ u, int64_t* __restrict__ tok) {
+                                                          float top_p, const float* __restrict__ u, const int64_t* __restrict__ ptok,
+                                                          const uint8_t* __restrict__ pmask, int64_t pld, int64_t* __restrict__ tok) {
   __shared__ int hist[256];
+  __shared__ unsigned long long mhist[256];
   __shared__ uint32_t s_prefix;
   __shared__ int s_remaining;
+  __shared__ unsigned long long s_above, s_budget;
   __shared__ float red[8];
+  __shared__ int redi[8];
   __shared__ float csum[256];
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const float* x = logits + (int64_t)blockIdx.x * ld;
+  if (pmask && pmask[(int64_t)blockIdx.x * pld]) {   // uniform over the block
+    if (t == 0) tok[blockIdx.x] = ptok[(int64_t)blockIdx.x * pld];
+    return;
+  }
+  if (temperature == 0.f) {                           // greedy: (value, index) maximum, ties to the lower index
+    float best = -INFINITY;
+    int bi = -1;
+    for (int c = t; c < V; c += 256) {
+      const float v = x[c];
+      if (bi < 0 || v > best) { best = v; bi = c; }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      const float ov = __shfl_down_sync(0xffffffffu, best, o);
+      const int oi = __shfl_down_sync(0xffffffffu, bi, o);
+      if (oi >= 0 && (bi < 0 || ov > best || (ov == best && oi < bi))) { best = ov; bi = oi; }
+    }
+    if (lane == 0) { red[warp] = best; redi[warp] = bi; }
+    __syncthreads();
+    if (t == 0) {
+      for (int w = 1; w < 8; ++w)
+        if (redi[w] >= 0 && (bi < 0 || red[w] > best || (red[w] == best && redi[w] < bi))) { best = red[w]; bi = redi[w]; }
+      tok[blockIdx.x] = (int64_t)bi;
+    }
+    return;
+  }
   uint32_t thr = 0;                                   // keys >= thr are kept
   if (top_k > 0 && top_k < V) {
     uint32_t prefix = 0, mask = 0;
@@ -312,6 +355,65 @@ __global__ void __launch_bounds__(256) sample_topk_kernel(const float* __restric
   mx = red[0];
 #pragma unroll
   for (int w = 1; w < 8; ++w) mx = fmaxf(mx, red[w]);
+  if (top_p < 1.f) {
+    // keys >= thr stay kept when the mass above them is <= budget = top_p * (kept mass).  Each pass picks the lowest bucket
+    // whose mass above (s_above + the buckets higher in this pass) is within the budget: the threshold key lies in it,
+    // since every key of a lower bucket has at least that bucket's mass above it.  Zero-mass buckets are skipped: exp is
+    // monotone, so they lie below every positive mass and have the whole kept mass above them.
+    uint32_t prefix = 0, mask = 0;
+    unsigned long long above = 0;
+    for (int pass = 3; pass >= 0; --pass) {
+      const int shift = pass * 8;
+      mhist[t] = 0ull;
+      __syncthreads();
+      for (int c = t; c < V; c += 256) {
+        const float z = x[c] / temperature;
+        const uint32_t key = order_key(z);
+        if (key >= thr && (key & mask) == prefix) {
+          const unsigned long long q = __float2ull_rz(expf(z - mx) * MASS_ONE);
+          if (q) atomicAdd(&mhist[(key >> shift) & 255u], q);
+        }
+      }
+      __syncthreads();
+      if (warp == 0) {                                // lane l owns buckets 8l .. 8l+7; integer sums: any order gives the same bits
+        unsigned long long m[8], loc = 0;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) loc += (m[j] = mhist[8 * lane + j]);
+        if (pass == 3) {
+          unsigned long long total = loc;
+#pragma unroll
+          for (int o = 16; o > 0; o >>= 1) total += __shfl_xor_sync(0xffffffffu, total, o);
+          if (lane == 0) s_budget = (unsigned long long)((double)total * (double)top_p);
+          __syncwarp();
+        }
+        unsigned long long suf = loc;                 // mass of lanes >= l, then of the buckets above 8l+7
+#pragma unroll
+        for (int o = 1; o < 32; o <<= 1) {
+          const unsigned long long v = __shfl_down_sync(0xffffffffu, suf, o);
+          if (lane + o < 32) suf += v;
+        }
+        const unsigned long long budget = s_budget;
+        unsigned long long run = above + (suf - loc), pick_above = 0;
+        int pick = 256;
+#pragma unroll
+        for (int j = 7; j >= 0; --j) {               // the mass above a bucket only grows downwards: the last fit is the lowest
+          if (m[j] && run <= budget) { pick = 8 * lane + j; pick_above = run; }
+          run += m[j];
+        }
+        const int low = (int)__reduce_min_sync(0xffffffffu, (unsigned)pick);
+        if (pick == low) {                            // exactly one lane; one always fits (the top bucket's mass above is <= budget)
+          s_prefix = prefix | ((uint32_t)pick << shift);
+          s_above = pick_above;
+        }
+      }
+      __syncthreads();
+      prefix = s_prefix;
+      above = s_above;
+      mask |= 0xFFu << shift;
+      __syncthreads();
+    }
+    thr = prefix;
+  }
   // contiguous chunks per thread so that the running sum follows the index order
   const int per = (V + 255) / 256, c0 = t * per, c1 = min(V, c0 + per);
   float loc = 0.f;
@@ -521,8 +623,21 @@ int mas_sample_topk(const float* logits, int64_t ld, int R, int V, float tempera
                     void* stream) {
   MAS_REQUIRE(logits && u && tokens && R > 0 && V > 0 && ld >= V, "sample_topk: bad arguments");
   if (!(temperature > 0.f)) return fail(MAS_ERR_INVALID_ARG, "sample_topk: temperature must be > 0 (greedy decoding: top_k = 1)");
-  sample_topk_kernel<<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, u, tokens);
+  sample_topk_kernel<<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, 1.f, u, nullptr, nullptr, 0, tokens);
   return launched("sample_topk");
+}
+
+int mas_sample_filtered(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, const float* u,
+                        const int64_t* prompt_tokens, const uint8_t* prompt_mask, int64_t prompt_ld, int64_t* tokens, void* stream) {
+  MAS_REQUIRE(logits && tokens && R > 0 && V > 0 && ld >= V, "sample_filtered: bad arguments");
+  if (!(temperature >= 0.f)) return fail(MAS_ERR_INVALID_ARG, "sample_filtered: temperature must be >= 0 (0: greedy)");
+  if (temperature > 0.f && !u) return fail(MAS_ERR_INVALID_ARG, "sample_filtered: sampling (temperature > 0) needs the uniforms u");
+  if (!(top_p > 0.f)) return fail(MAS_ERR_INVALID_ARG, "sample_filtered: top_p must be > 0 (>= 1: no nucleus filter)");
+  if (!prompt_tokens != !prompt_mask) return fail(MAS_ERR_INVALID_ARG, "sample_filtered: prompt tokens and prompt mask go together");
+  if (prompt_mask && prompt_ld < 0) return fail(MAS_ERR_INVALID_ARG, "sample_filtered: negative prompt row stride");
+  sample_topk_kernel<<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, top_p, u, prompt_tokens, prompt_mask, prompt_ld,
+                                               tokens);
+  return launched("sample_filtered");
 }
 
 }  // extern "C"

@@ -1580,14 +1580,37 @@ def cross_entropy(logits, target):
     return CrossEntropyFn.apply(logits, target)
 
 
-def sample_topk(logits, temperature, top_k, u):
-    """One token per row of logits [R,V]: softmax(logits / temperature) restricted to the top_k entries, drawn by inverse CDF
-    at the caller's uniforms u [R] (device fp32 in [0,1))."""
+def sample_topk(logits, temperature, top_k, u, top_p=None, prompt=None):
+    """One token per row of logits [R,V]: softmax(logits / temperature) restricted to the top_k entries, then (top_p < 1) to
+    the nucleus of mass top_p, drawn by inverse CDF at the caller's uniforms u [R] (device fp32 in [0,1)); temperature 0 is
+    greedy (u unused, may be None). prompt: (tokens int64 [R], mask bool [R]) - rows whose mask is set take the given token.
+    Without top_p < 1 and a prompt this is mas_sample_topk; otherwise mas_sample_filtered (include/mas_b200.h)."""
     _need_cuda(logits)
+    if top_p is not None:
+        top_p = float(top_p)
+        if not top_p > 0:
+            raise ValueError("top_p must be > 0 (None or >= 1: no nucleus filter), got %r" % top_p)
+        if top_p >= 1:
+            top_p = None
     logits = logits.contiguous()
     R, V = logits.shape
     tok = torch.empty(R, dtype=torch.int64, device=logits.device)
-    L.call("mas_sample_topk", logits, V, R, V, float(temperature), int(top_k) if top_k else 0, u.contiguous(), tok)
+    if top_p is None and prompt is None:
+        L.call("mas_sample_topk", logits, V, R, V, float(temperature), int(top_k) if top_k else 0, u.contiguous(), tok)
+        return tok
+    ptok = pmask = None
+    pld = 0
+    if prompt is not None:
+        ptok, pmask = prompt
+        if ptok.shape != (R,) or pmask.shape != (R,) or ptok.dtype != torch.int64 or pmask.dtype != torch.bool:
+            raise ValueError("prompt: int64 tokens and a bool mask of %d rows expected" % R)
+        if ptok.device != logits.device or pmask.device != logits.device:
+            raise ValueError("prompt: tokens and mask must be on the logits' device (%s)" % logits.device)
+        if ptok.stride(0) != pmask.stride(0):
+            ptok, pmask = ptok.contiguous(), pmask.contiguous()
+        pld = ptok.stride(0)
+    L.call("mas_sample_filtered", logits, V, R, V, float(temperature), int(top_k) if top_k else 0, 1.0 if top_p is None else top_p,
+           None if u is None else u.contiguous(), ptok, pmask, pld, tok)
     return tok
 
 

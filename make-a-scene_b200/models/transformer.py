@@ -326,7 +326,7 @@ class MakeAScene(nn.Module):
 
     @torch.no_grad()
     def generate(self, text_tokens, seg_tokens, guidance_scale=None, uncond_text_tokens=None, temperature=1.0, top_k=None,
-                 generator=None, img_tokens=None, return_logits=False, use_graphs=False):
+                 generator=None, img_tokens=None, return_logits=False, use_graphs=False, top_p=None, img_mask=None):
         """Autoregressive sampling of the image tokens with a KV cache; optional classifier-free guidance
         (logits = uncond + scale * (cond - uncond), the unconditional stream sees padded text; Make-A-Scene paper 3.4).
 
@@ -334,13 +334,36 @@ class MakeAScene(nn.Module):
         the only limit on R. Up to 8 rows the decode steps are strict fp32 (weights and KV cache). More rows run the decode
         Linear layers on fp16 operands with fp32 accumulation and keep K / V in fp16 caches: the arithmetic of the model's own
         training forward. The prefix pass always runs the training kernels.
-        temperature 0 = greedy; top_k keeps the k most likely codes. img_tokens (optional [B,image_length]) are fed
-        instead of the sampled ones (teacher forcing — what the parity test uses). Returns tokens [B,image_length]
-        (and the per-position logits [B,image_length,V] actually sampled from when return_logits=True).
+        The draw at each position, per row (ru-DALL-E's top_k_top_p_filtering chain, one kernel launch):
+          z = logits / temperature; top_k keeps the k largest (ties with the k-th kept); top_p (None or >= 1: off, <= 0:
+          ValueError) keeps, of those, every entry whose softmax mass of kept entries with a strictly larger z is <= top_p
+          (equal values are kept or dropped together; the largest always stays); the token is the inverse CDF of softmax(z)
+          over the kept set at a uniform, in index order. temperature 0 = greedy (the first index of the maximum).
+        img_tokens (optional [B,image_length] int64) are fed instead of the sampled ones at every position (teacher forcing —
+        what the parity test uses). With img_mask ([B,image_length] bool on the same device) only the positions where it is
+        set are forced (image prompts: completion, outpainting, editing a region); the others are drawn, conditioned on all
+        earlier tokens, forced or drawn. With guidance a forced token goes to both streams. When sampling with img_mask, the
+        B uniforms are drawn at every position, forced or not, so a row's random stream does not depend on the mask: an
+        all-false mask gives the tokens of the unprompted call with the same generator.
+        Returns tokens [B,image_length] (and the per-position logits [B,image_length,V], mixed and unfiltered, when
+        return_logits=True).
         use_graphs: replay each position's decode step from a CUDA graph (captured at first use and kept on the module for
         the same row count; captured again after any parameter changes, in place or by replaced storage)."""
         B = text_tokens.shape[0]
         dev = text_tokens.device
+        if top_p is not None and not float(top_p) > 0:
+            raise ValueError("top_p must be > 0 (None or >= 1: no nucleus filter), got %r" % (top_p,))
+        if img_mask is not None:
+            want = (B, self.image_length)
+            if img_tokens is None:
+                raise ValueError("img_mask selects positions of img_tokens: pass img_tokens too")
+            if not isinstance(img_mask, torch.Tensor) or img_mask.dtype != torch.bool or tuple(img_mask.shape) != want:
+                raise ValueError("img_mask must be a bool tensor of shape %s" % (want,))
+            if img_tokens.dtype != torch.int64 or tuple(img_tokens.shape) != want:
+                raise ValueError("img_tokens must be an int64 tensor of shape %s" % (want,))
+            if img_mask.device != dev or img_tokens.device != dev:
+                raise ValueError("img_tokens and img_mask must be on the device of text_tokens (%s)" % dev)
+            img_tokens, img_mask = img_tokens.contiguous(), img_mask.contiguous()
         cfg = guidance_scale is not None and float(guidance_scale) != 1.0
         if cfg:
             if uncond_text_tokens is None:
@@ -363,16 +386,19 @@ class MakeAScene(nn.Module):
             mixed = ops.cfg_mix(logits[:B], logits[B:], guidance_scale) if cfg else logits
             if return_logits:
                 kept.append(mixed)
-            if img_tokens is not None:
+            prompt = (img_tokens[:, t], img_mask[:, t]) if img_mask is not None else None
+            if img_tokens is not None and prompt is None:
                 tok = img_tokens[:, t]
-            elif not temperature:
+            elif not temperature and prompt is None:
                 tok = mixed.argmax(-1)
-            else:   # temperature, top-k filter, softmax and the draw in one kernel; torch only supplies the uniforms
-                if generator is not None and generator.device.type != dev.type:
-                    u = torch.rand(B, generator=generator).to(dev)
-                else:
-                    u = torch.rand(B, device=dev, generator=generator)
-                tok = ops.sample_topk(mixed, float(temperature), top_k, u)
+            else:   # prompt, temperature, top-k / top-p filters, softmax and the draw in one kernel; torch only supplies the uniforms
+                u = None
+                if temperature:
+                    if generator is not None and generator.device.type != dev.type:
+                        u = torch.rand(B, generator=generator).to(dev)
+                    else:
+                        u = torch.rand(B, device=dev, generator=generator)
+                tok = ops.sample_topk(mixed, float(temperature), top_k, u, top_p=top_p, prompt=prompt)
             toks.append(tok)
             if t == self.image_length - 1:
                 break

@@ -3,7 +3,9 @@ heads, 128 text + 256 segmentation tokens -> 256 image tokens of an 8192-code vo
 One JSON line; not part of bench.py's headline (the reference has no sampler to compare with: SURVEY.md 8f-3). It carries the
 GPU's name and power limit, and the HBM bytes a decode step streams on the path actually taken: up to 8 rows fp32 weights and
 fp32 KV cache, above 8 rows fp16 weights and fp16 cache (the cache read at the mean cache length of the image positions).
-Usage: python tools/bench_sampling.py [--batch B] [--reps N] [--graphs]"""
+--top-p adds the nucleus filter to the draw (top-k 64 stays); --prompt-frac F forces a random share F of the image positions
+(an image prompt, random tokens): the forced positions are still decoded one step each, so tokens/s counts every position.
+Usage: python tools/bench_sampling.py [--batch B] [--reps N] [--graphs] [--top-p P] [--prompt-frac F]"""
 import argparse
 import json
 import os
@@ -21,6 +23,8 @@ ap.add_argument("--batch", type=int, default=1)
 ap.add_argument("--reps", type=int, default=2)
 ap.add_argument("--layers", type=int, default=24)
 ap.add_argument("--graphs", action="store_true", help="replay each position's decode step from a CUDA graph")
+ap.add_argument("--top-p", type=float, default=None, help="nucleus filter of the draw (default: off)")
+ap.add_argument("--prompt-frac", type=float, default=0.0, help="share of image positions forced by a random image prompt")
 args = ap.parse_args()
 dev = torch.device("cuda:0")
 torch.manual_seed(0)
@@ -32,13 +36,17 @@ B = args.batch
 text = torch.randint(1, 40000, (B, 128), device=dev)
 seg = torch.randint(0, 1024, (B, 256), device=dev)
 gen = torch.Generator(device=dev).manual_seed(1)
-m.generate(text, seg, guidance_scale=3.0, temperature=1.0, top_k=64, generator=gen, use_graphs=args.graphs)     # warm-up (captures)
+kw = dict(guidance_scale=3.0, temperature=1.0, top_k=64, top_p=args.top_p, generator=gen, use_graphs=args.graphs)
+if args.prompt_frac > 0:
+    kw["img_tokens"] = torch.randint(0, cfg["image_vocab_size"], (B, 256), device=dev)
+    kw["img_mask"] = torch.rand(B, 256, device=dev) < args.prompt_frac
+m.generate(text, seg, **kw)     # warm-up (captures)
 torch.cuda.synchronize()
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 l0 = _lib.launch_count()
 e0.record()
 for _ in range(args.reps):
-    toks = m.generate(text, seg, guidance_scale=3.0, temperature=1.0, top_k=64, generator=gen, use_graphs=args.graphs)
+    toks = m.generate(text, seg, **kw)
 e1.record()
 torch.cuda.synchronize()
 sec = e0.elapsed_time(e1) * 1e-3 / args.reps
@@ -52,6 +60,7 @@ weight_bytes = params * elem
 cache_bytes = args.layers * R * 2 * cfg["hidden_dim"] * mean_len * elem
 print(json.dumps({"metric": "image tokens/s, classifier-free guided sampling with KV cache", "value": B * 256 / sec, "unit": "tokens/s",
                   "gpu": gpu.stdout.strip().splitlines()[0], "batch": B, "rows": R, "cuda_graphs": bool(args.graphs),
+                  "top_k": 64, "top_p": args.top_p, "prompt_frac": args.prompt_frac,
                   "seconds_per_image": sec, "launches_per_image": (_lib.launch_count() - l0) // args.reps,
                   "operand_bytes": elem, "weight_stream_gb_per_step": weight_bytes / 1e9, "cache_gb_per_step": cache_bytes / 1e9,
                   "hbm_stream_gbs": (weight_bytes + cache_bytes) * steps / sec / 1e9, "config": cfg}))
