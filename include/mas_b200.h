@@ -491,6 +491,30 @@ int mas_attn_decode_f16(const float* qkv, const void* kcache, const void* vcache
                         int Tmax, int len, void* stream);
 int mas_attn_decode_append_f16(const float* qkv, void* kcache, void* vcache, float* ctx, int R, int heads, int hd, int Tmax,
                                int pos, void* stream);
+/* mas_attn_decode_append / mas_attn_decode_append_f16 with the keys and values of each row split between a cache shared by a
+ * group of rows and one of its own (MakeAScene.generate(num_samples = n): n samples of one prompt share its text +
+ * segmentation prefix).  The R rows of qkv [R,3H] form R / n groups of n consecutive rows.  Row r attends over positions
+ * 0..prefix_len-1 of prefix row r / n (kprefix / vprefix [R/n, heads, prefix_len, hd]) and positions prefix_len..pos of its
+ * suffix cache (ksuffix / vsuffix [R, heads, Tsuf, hd], slot = position - prefix_len); its own k / v are stored at slot
+ * pos - prefix_len (prefix_len <= pos < prefix_len + Tsuf).  Each row's ctx is bit-identical to the unshared entry's on the
+ * concatenated cache.  A block serves up to rows_per_block rows of one group (1, 2 or 4; 0: chosen from R, n and the device)
+ * and reads the group's prefix once for all of them. */
+int mas_attn_decode_shared_append(const float* qkv, const float* kprefix, const float* vprefix, float* ksuffix, float* vsuffix,
+                                  float* ctx, int R, int n, int heads, int hd, int prefix_len, int Tsuf, int pos,
+                                  int rows_per_block, void* stream);
+int mas_attn_decode_shared_append_f16(const float* qkv, const void* kprefix, const void* vprefix, void* ksuffix, void* vsuffix,
+                                      float* ctx, int R, int n, int heads, int hd, int prefix_len, int Tsuf, int pos,
+                                      int rows_per_block, void* stream);
+/* The same split for mas_attn_decode / mas_attn_decode_f16 (no append): row r attends over positions 0..len-1, prefix_len < len
+ * <= prefix_len + Tsuf, all read from the caches (this token's k / v stored beforehand, e.g. by mas_kv_append(_f16) into the
+ * suffix cache at pos0 = len - 1 - prefix_len).  Each row's ctx is bit-identical to the unshared entry's on the concatenated
+ * cache; the token's own p v term is added where mas_attn_decode adds it, which is not where the _append entries add it. */
+int mas_attn_decode_shared(const float* qkv, const float* kprefix, const float* vprefix, const float* ksuffix,
+                           const float* vsuffix, float* ctx, int R, int n, int heads, int hd, int prefix_len, int Tsuf, int len,
+                           int rows_per_block, void* stream);
+int mas_attn_decode_shared_f16(const float* qkv, const void* kprefix, const void* vprefix, const void* ksuffix,
+                               const void* vsuffix, float* ctx, int R, int n, int heads, int hd, int prefix_len, int Tsuf, int len,
+                               int rows_per_block, void* stream);
 int mas_cfg_mix(const float* cond, const float* uncond, float* out, int64_t n, float scale, void* stream);
 /* Token draw of the sampler (replaces the div / topk / where / softmax / multinomial chain of generate()): per row,
  * z = logits / temperature, entries below the top_k-th largest value dropped (top_k <= 0 or >= V: none), p = softmax(z),

@@ -9,6 +9,8 @@
 //   * mas_kv_append    : scatters the k / v thirds of a fused qkv activation into the [R, heads, Tmax, hd] caches.
 //   * mas_attn_decode  : one query per (row, head) against the cache: scores, softmax, weighted sum of v.
 //     The _f16 variants of both keep the caches in fp16 (decoding more than 8 rows).
+//   * mas_attn_decode_shared(_append) : mas_attn_decode(_append) for groups of rows that share a prompt's prefix cache
+//     (generate(num_samples = n)); a block reads the group's prefix once for up to 4 of its rows.
 //   * mas_cfg_mix      : classifier-free guidance, out = uncond + scale * (cond - uncond).
 #include <cuda_fp16.h>
 
@@ -247,6 +249,208 @@ __global__ void __launch_bounds__(256) attn_decode_kernel(const float* __restric
     for (int g2 = 0; g2 < GROUPS; ++g2) v += po[g2 * HD + t0];
     ctx[(size_t)r * H + h * HD + t0] = v * inv;
   }
+}
+
+// q . k over HD in attn_decode_kernel's order: four interleaved fmaf chains, added pairwise, then scaled.
+template <int HD>
+__device__ __forceinline__ float decode_score(const float* q, const float* kv, float alpha) {
+  float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f;
+#pragma unroll
+  for (int i = 0; i < HD / 4; ++i) {
+    const float4 qv = *reinterpret_cast<const float4*>(q + 4 * i);
+    s0 = fmaf(qv.x, kv[4 * i], s0); s1 = fmaf(qv.y, kv[4 * i + 1], s1);
+    s2 = fmaf(qv.z, kv[4 * i + 2], s2); s3 = fmaf(qv.w, kv[4 * i + 3], s3);
+  }
+  return ((s0 + s1) + (s2 + s3)) * alpha;
+}
+
+// Shared-prefix decode attention (generate(num_samples = n)): the R sample rows form groups of n consecutive rows that share a
+// prompt. Row r attends over positions 0..P-1 of prompt row r / n's prefix cache (kp / vp [R/n, heads, P, HD]), then over
+// positions P..len-1 of its own suffix cache (ks / vs [R, heads, Tsuf, HD], slot = position - P).  A block serves g <= G rows of
+// one group for one head, so each 16-byte prefix load feeds g rows' scores and v partials; blocks of the same (group, head) are
+// adjacent in the grid, so the slices of one group also meet its prefix in L2.  Per row the arithmetic is
+// attn_decode_kernel<HD, APPEND, T>'s: the same thread owns the same positions in the same order in every pass (scores, max,
+// exp / sum, v pass, the GROUPS-partial reduction), so ctx is bit-identical to the unshared kernel run on the concatenated cache.
+// APPEND: this token's k / v are stored at slot len-1-P and enter from shared memory, its p v term last in partial group 0 (as
+// mas_attn_decode_append adds it).  Without APPEND, position len-1 is read from the suffix cache like every other one, so its
+// term lands in group (len-1) % GROUPS (as mas_attn_decode adds it after mas_kv_append).
+template <int HD, int G, bool APPEND, typename T>
+__global__ void __launch_bounds__(256) attn_decode_shared_kernel(const float* __restrict__ qkv, const T* __restrict__ kp,
+                                                                 const T* __restrict__ vp, T* __restrict__ ks, T* __restrict__ vs,
+                                                                 float* __restrict__ ctx, int n, int heads, int P, int Tsuf, int len) {
+  // [G][HD] q, own k, own v; [G][16] scratch; [G][len] scores; [G][GROUPS][HD] partial outputs
+  extern __shared__ __align__(16) float sm[];
+  constexpr int E = Vec16<T>::E;
+  constexpr int VQ = HD / E, GROUPS = 256 / VQ;
+  const int lenc = APPEND ? len - 1 : len, scl = (len + 3) & ~3;     // positions read from the caches
+  float* qs = sm;
+  float* kself = qs + G * HD;
+  float* vself = kself + G * HD;
+  float* red = vself + G * HD;
+  float* sc = red + G * 16;
+  float* po = sc + G * scl;
+  const int slices = (n + G - 1) / G, s = blockIdx.x % slices, h = (blockIdx.x / slices) % heads, grp = blockIdx.x / slices / heads;
+  const int r0 = grp * n + s * G, g = min(G, n - s * G), H = heads * HD, t0 = threadIdx.x, lane = t0 & 31, warp = t0 >> 5;
+  for (int i = t0; i < G * HD; i += 256) {
+    const int j = i / HD, d = i % HD;
+    float q = 0.f, kf = 0.f, vf = 0.f;
+    if (j < g) {
+      const float* tokrow = qkv + (size_t)(r0 + j) * 3 * H + h * HD + d;
+      q = tokrow[0];
+      if (APPEND) {
+        const T kv = to_elem(tokrow[H], (T*)nullptr), vv = to_elem(tokrow[2 * H], (T*)nullptr);
+        kf = elem_f(kv);
+        vf = elem_f(vv);
+        const size_t dst = (((size_t)(r0 + j) * heads + h) * Tsuf + (len - 1 - P)) * HD + d;
+        ks[dst] = kv;
+        vs[dst] = vv;
+      }
+    }
+    qs[i] = q;
+    kself[i] = kf;
+    vself[i] = vf;
+  }
+  __syncthreads();
+  const float alpha = rsqrtf((float)HD);
+  const T* kpb = kp + ((size_t)grp * heads + h) * P * HD;
+  const T* vpb = vp + ((size_t)grp * heads + h) * P * HD;
+  const size_t suf0 = ((size_t)r0 * heads + h) * Tsuf * HD, sufj = (size_t)heads * Tsuf * HD;   // row r0 + j's suffix: suf0 + j * sufj
+  float mx[G];
+#pragma unroll
+  for (int j = 0; j < G; ++j) mx[j] = -INFINITY;
+  int t = t0;
+  for (; t < P; t += 256) {                      // prefix: one load, g rows
+    float kv[HD];
+#pragma unroll
+    for (int i = 0; i < VQ; ++i) load16(kpb + (size_t)t * HD + i * E, kv + i * E);
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+      if (j < g) {
+        const float sj = decode_score<HD>(qs + j * HD, kv, alpha);
+        sc[j * scl + t] = sj;
+        mx[j] = fmaxf(mx[j], sj);
+      }
+  }
+  for (; t < lenc; t += 256) {                   // suffix: each row its own
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+      if (j < g) {
+        float kv[HD];
+#pragma unroll
+        for (int i = 0; i < VQ; ++i) load16(ks + suf0 + j * sufj + (size_t)(t - P) * HD + i * E, kv + i * E);
+        const float sj = decode_score<HD>(qs + j * HD, kv, alpha);
+        sc[j * scl + t] = sj;
+        mx[j] = fmaxf(mx[j], sj);
+      }
+  }
+  if (APPEND && t0 == 255) {
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+      if (j < g) {
+        const float sj = decode_score<HD>(qs + j * HD, kself + j * HD, alpha);
+        sc[j * scl + len - 1] = sj;
+        mx[j] = fmaxf(mx[j], sj);
+      }
+  }
+#pragma unroll
+  for (int j = 0; j < G; ++j) {
+    const float m = warp_max(mx[j]);
+    if (lane == 0) red[j * 16 + warp] = m;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < G; ++j) {
+    float m = red[j * 16];
+#pragma unroll
+    for (int w = 1; w < 8; ++w) m = fmaxf(m, red[j * 16 + w]);
+    mx[j] = m;
+  }
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < G; ++j) {
+    float sum = 0.f;
+    if (j < g)
+      for (int tt = t0; tt < len; tt += 256) {
+        const float e = expf(sc[j * scl + tt] - mx[j]);
+        sc[j * scl + tt] = e;
+        sum += e;
+      }
+    sum = warp_sum(sum);
+    if (lane == 0) red[j * 16 + 8 + warp] = sum;
+  }
+  __syncthreads();
+  float inv[G];
+#pragma unroll
+  for (int j = 0; j < G; ++j) {
+    float tot = 0.f;
+#pragma unroll
+    for (int w = 0; w < 8; ++w) tot += red[j * 16 + 8 + w];
+    inv[j] = 1.f / tot;
+  }
+  const int dq = t0 % VQ, gg = t0 / VQ;
+  float o[G][E];
+#pragma unroll
+  for (int j = 0; j < G; ++j)
+#pragma unroll
+    for (int e = 0; e < E; ++e) o[j][e] = 0.f;
+  t = gg;
+  for (; t + 7 * GROUPS < P; t += 8 * GROUPS) {
+    float vv[8][E];
+#pragma unroll
+    for (int u = 0; u < 8; ++u) load16(vpb + (size_t)(t + u * GROUPS) * HD + dq * E, vv[u]);
+#pragma unroll
+    for (int u = 0; u < 8; ++u)
+#pragma unroll
+      for (int j = 0; j < G; ++j)
+        if (j < g) {
+          const float p = sc[j * scl + t + u * GROUPS];
+#pragma unroll
+          for (int e = 0; e < E; ++e) o[j][e] = fmaf(p, vv[u][e], o[j][e]);
+        }
+  }
+  for (; t < P; t += GROUPS) {
+    float vv[E];
+    load16(vpb + (size_t)t * HD + dq * E, vv);
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+      if (j < g) {
+        const float p = sc[j * scl + t];
+#pragma unroll
+        for (int e = 0; e < E; ++e) o[j][e] = fmaf(p, vv[e], o[j][e]);
+      }
+  }
+  for (; t < lenc; t += GROUPS) {
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+      if (j < g) {
+        float vv[E];
+        load16(vs + suf0 + j * sufj + (size_t)(t - P) * HD + dq * E, vv);
+        const float p = sc[j * scl + t];
+#pragma unroll
+        for (int e = 0; e < E; ++e) o[j][e] = fmaf(p, vv[e], o[j][e]);
+      }
+  }
+#pragma unroll
+  for (int j = 0; j < G; ++j)
+    if (j < g) {
+      if (APPEND && gg == 0) {
+        const float p = sc[j * scl + len - 1];
+#pragma unroll
+        for (int e = 0; e < E; ++e) o[j][e] = fmaf(p, vself[j * HD + E * dq + e], o[j][e]);
+      }
+#pragma unroll
+      for (int e = 0; e < E; e += 4)
+        *reinterpret_cast<float4*>(po + ((size_t)j * GROUPS + gg) * HD + E * dq + e) = make_float4(o[j][e], o[j][e + 1], o[j][e + 2], o[j][e + 3]);
+    }
+  __syncthreads();
+#pragma unroll
+  for (int j = 0; j < G; ++j)
+    if (j < g && t0 < HD) {
+      float v = 0.f;
+#pragma unroll 4
+      for (int g2 = 0; g2 < GROUPS; ++g2) v += po[((size_t)j * GROUPS + g2) * HD + t0];
+      ctx[(size_t)(r0 + j) * H + h * HD + t0] = v * inv[j];
+    }
 }
 
 __global__ void cfg_mix_kernel(const float* __restrict__ cond, const float* __restrict__ uncond, float* __restrict__ out, int64_t n,
@@ -580,7 +784,103 @@ static int attn_decode_run(const float* qkv, T* kcache, T* vcache, float* ctx, i
   return launched(append ? "attn_decode_append" : "attn_decode");
 }
 
+template <typename T>
+static size_t shared_decode_smem(int G, int hd, int len) {
+  return (size_t)G * (3 * hd + 16 + ((len + 3) & ~3) + 256 * Vec16<T>::E) * sizeof(float);
+}
+
+template <int HD, int G, bool APPEND, typename T>
+static int attn_decode_shared_launch(const float* qkv, const T* kp, const T* vp, T* ks, T* vs, float* ctx, int R, int n, int heads, int P,
+                                     int Tsuf, int len, int optin, size_t smem, cudaStream_t st) {
+  static std::atomic<uint64_t> configured{0};    // per instantiation and device: allow the device's largest dynamic shared memory
+  if (first_on_device(configured)) {
+    const cudaError_t e = cudaFuncSetAttribute(attn_decode_shared_kernel<HD, G, APPEND, T>, cudaFuncAttributeMaxDynamicSharedMemorySize, optin);
+    if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "attn_decode_shared: smem attr (%d): %s", optin, cudaGetErrorString(e));
+    mark_device(configured);
+  }
+  const int grid = (R / n) * heads * ((n + G - 1) / G);
+  attn_decode_shared_kernel<HD, G, APPEND, T><<<grid, 256, smem, st>>>(qkv, kp, vp, ks, vs, ctx, n, heads, P, Tsuf, len);
+  return launched(APPEND ? "attn_decode_shared_append" : "attn_decode_shared");
+}
+
+// Rows per block: a block of G rows reads its group's prefix once for G rows, but a group of n rows then fills only
+// ceil(n / G) blocks per head. Auto (rows_per_block = 0): the smallest power of two >= n, capped at 4, halved while the grid
+// would be under two blocks per SM or the block's shared memory would exceed the device's opt-in limit.  The cap is measured
+// (tools/bench_decode.py, H100 SXM 80 GB, 700 W, 256 rows, n = 8, 16 x 64 heads, length 512): 8 rows per block took 155 us
+// against 121 us for one row, its 4 KB of v partials per row costing occupancy; 4 rows per block beat one row at every n.
+// len: positions attended (the last one is this token's, at suffix slot len-1-P: stored here when append, else already cached).
+template <typename T>
+static int attn_decode_shared_run(const float* qkv, const T* kp, const T* vp, T* ks, T* vs, float* ctx, int R, int n, int heads, int hd,
+                                  int P, int Tsuf, int len, bool append, int rows_per_block, void* stream) {
+  MAS_REQUIRE(qkv && kp && vp && ks && vs && ctx && R > 0 && heads > 0, "attn_decode_shared: bad arguments");
+  if (n < 1 || R % n) return fail(MAS_ERR_INVALID_ARG, "attn_decode_shared: %d rows are not groups of %d", R, n);
+  if (P < 1 || Tsuf < 1 || len <= P || len > P + Tsuf)
+    return fail(MAS_ERR_INVALID_ARG, "attn_decode_shared: position %d outside the suffix cache (%d..%d)", len - 1, P, P + Tsuf - 1);
+  if (rows_per_block != 0 && rows_per_block != 1 && rows_per_block != 2 && rows_per_block != 4)
+    return fail(MAS_ERR_INVALID_ARG, "attn_decode_shared: rows_per_block must be 0 (auto), 1, 2 or 4 (got %d)", rows_per_block);
+  int dev = 0, sms = 0, optin = 0;
+  cudaGetDevice(&dev);
+  cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+  cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+  int G = rows_per_block;
+  if (G == 0) {
+    G = 4;
+    while (G > 1 && G / 2 >= n) G /= 2;
+    while (G > 1 && ((size_t)(R / n) * heads * ((n + G - 1) / G) < (size_t)2 * sms || shared_decode_smem<T>(G, hd, len) > (size_t)optin)) G /= 2;
+  }
+  const size_t smem = shared_decode_smem<T>(G, hd, len);
+  if (smem > (size_t)optin)
+    return fail(MAS_ERR_UNSUPPORTED, "attn_decode_shared: %d rows per block over %d positions need %zu bytes of shared memory", G, len,
+                smem);
+  cudaStream_t st = S(stream);
+#define MAS_ADS_G(HD_, G_)                                                                                                   \
+  return append ? attn_decode_shared_launch<HD_, G_, true, T>(qkv, kp, vp, ks, vs, ctx, R, n, heads, P, Tsuf, len, optin, smem, st) \
+                : attn_decode_shared_launch<HD_, G_, false, T>(qkv, kp, vp, ks, vs, ctx, R, n, heads, P, Tsuf, len, optin, smem, st);
+#define MAS_ADS(HD_)              \
+  switch (G) {                    \
+    case 1: MAS_ADS_G(HD_, 1)     \
+    case 2: MAS_ADS_G(HD_, 2)     \
+    default: MAS_ADS_G(HD_, 4)    \
+  }
+  switch (hd) {
+    case 16: MAS_ADS(16)
+    case 32: MAS_ADS(32)
+    case 64: MAS_ADS(64)
+    case 128: MAS_ADS(128)
+    default: return fail(MAS_ERR_UNSUPPORTED, "attn_decode_shared: head dim %d (supported: 16, 32, 64, 128)", hd);
+  }
+#undef MAS_ADS
+#undef MAS_ADS_G
+}
+
 extern "C" {
+
+int mas_attn_decode_shared_append(const float* qkv, const float* kprefix, const float* vprefix, float* ksuffix, float* vsuffix, float* ctx,
+                                  int R, int n, int heads, int hd, int prefix_len, int Tsuf, int pos, int rows_per_block, void* stream) {
+  return attn_decode_shared_run(qkv, kprefix, vprefix, ksuffix, vsuffix, ctx, R, n, heads, hd, prefix_len, Tsuf, pos + 1, true,
+                                rows_per_block, stream);
+}
+
+int mas_attn_decode_shared_append_f16(const float* qkv, const void* kprefix, const void* vprefix, void* ksuffix, void* vsuffix, float* ctx,
+                                      int R, int n, int heads, int hd, int prefix_len, int Tsuf, int pos, int rows_per_block,
+                                      void* stream) {
+  return attn_decode_shared_run(qkv, (const __half*)kprefix, (const __half*)vprefix, (__half*)ksuffix, (__half*)vsuffix, ctx, R, n, heads,
+                                hd, prefix_len, Tsuf, pos + 1, true, rows_per_block, stream);
+}
+
+int mas_attn_decode_shared(const float* qkv, const float* kprefix, const float* vprefix, const float* ksuffix, const float* vsuffix,
+                           float* ctx, int R, int n, int heads, int hd, int prefix_len, int Tsuf, int len, int rows_per_block, void* stream) {
+  return attn_decode_shared_run(qkv, kprefix, vprefix, const_cast<float*>(ksuffix), const_cast<float*>(vsuffix), ctx, R, n, heads, hd,
+                                prefix_len, Tsuf, len, false, rows_per_block, stream);
+}
+
+int mas_attn_decode_shared_f16(const float* qkv, const void* kprefix, const void* vprefix, const void* ksuffix, const void* vsuffix,
+                               float* ctx, int R, int n, int heads, int hd, int prefix_len, int Tsuf, int len, int rows_per_block,
+                               void* stream) {
+  return attn_decode_shared_run(qkv, (const __half*)kprefix, (const __half*)vprefix, (__half*)const_cast<void*>(ksuffix),
+                                (__half*)const_cast<void*>(vsuffix), ctx, R, n, heads, hd, prefix_len, Tsuf, len, false, rows_per_block,
+                                stream);
+}
 
 int mas_kv_append(const float* qkv, int R, int T, int heads, int hd, float* kcache, float* vcache, int Tmax, int pos0, void* stream) {
   return kv_append_run(qkv, R, T, heads, hd, kcache, vcache, Tmax, pos0, stream);

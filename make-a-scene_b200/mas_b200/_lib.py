@@ -131,6 +131,10 @@ _SPEC = {
     "mas_kv_append_f16": (_I, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _P]),
     "mas_attn_decode_f16": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "mas_attn_decode_append_f16": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
+    "mas_attn_decode_shared_append": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "mas_attn_decode_shared_append_f16": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "mas_attn_decode_shared": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
+    "mas_attn_decode_shared_f16": (_I, [_P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _P]),
     "mas_layernorm2_forward": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _F, _F, _P]),
     "mas_sample_topk": (_I, [_P, _L, _I, _I, _F, _I, _P, _P, _P]),
     "mas_sample_filtered": (_I, [_P, _L, _I, _I, _F, _I, _F, _P, _P, _P, _L, _P, _P]),

@@ -1702,6 +1702,38 @@ def attn_decode_append(qkv, kcache, vcache, pos):
     return ctx
 
 
+def _shared_decode(entry, qkv, kprefix, vprefix, ksuffix, vsuffix, last, rows_per_block):
+    """The checks and call of the shared-prefix attention entries (the kernels index the caches from these extents)."""
+    P, heads, prefix_len, hd = kprefix.shape
+    R, heads_s, Tsuf, hd_s = ksuffix.shape
+    if (vprefix.shape != kprefix.shape or vsuffix.shape != ksuffix.shape or (heads_s, hd_s) != (heads, hd) or R % P
+            or len({t.dtype for t in (kprefix, vprefix, ksuffix, vsuffix)}) != 1
+            or not all(t.is_contiguous() and t.device == qkv.device for t in (kprefix, vprefix, ksuffix, vsuffix))):
+        raise RuntimeError("%s: prefix caches %s / %s and suffix caches %s / %s must be contiguous, of one dtype and device, agree in "
+                           "heads and head dim, and have a multiple of the prefix rows" % (entry, tuple(kprefix.shape), tuple(vprefix.shape),
+                                                                                          tuple(ksuffix.shape), tuple(vsuffix.shape)))
+    if tuple(qkv.shape) != (R, 3 * heads * hd):
+        raise RuntimeError("%s: qkv must be [%d, %d], got %s" % (entry, R, 3 * heads * hd, tuple(qkv.shape)))
+    ctx = torch.empty((R, heads * hd), dtype=torch.float32, device=qkv.device)
+    L.call(_cache_entry(entry, kprefix), qkv.contiguous(), kprefix, vprefix, ksuffix, vsuffix, ctx, R, R // P, heads, hd, prefix_len, Tsuf,
+           int(last), int(rows_per_block))
+    return ctx
+
+
+def attn_decode_shared_append(qkv, kprefix, vprefix, ksuffix, vsuffix, pos, rows_per_block=0):
+    """attn_decode_append for groups of n = R / P consecutive rows sharing a prefix: row r reads positions 0..prefix_len-1 from
+    prefix row r // n (kprefix / vprefix [P,heads,prefix_len,hd]) and the rest from its suffix cache (ksuffix / vsuffix
+    [R,heads,Tsuf,hd], slot = position - prefix_len), where this token's k / v are stored -> ctx [R,H].
+    rows_per_block: rows a block serves (0: the launcher's choice)."""
+    return _shared_decode("mas_attn_decode_shared_append", qkv, kprefix, vprefix, ksuffix, vsuffix, pos, rows_per_block)
+
+
+def attn_decode_shared(qkv, kprefix, vprefix, ksuffix, vsuffix, length, rows_per_block=0):
+    """attn_decode with the same split of the caches: positions 0..length-1, all of them already cached (the arithmetic of
+    attn_decode, which adds the last position's term differently from attn_decode_append)."""
+    return _shared_decode("mas_attn_decode_shared", qkv, kprefix, vprefix, ksuffix, vsuffix, length, rows_per_block)
+
+
 def layernorm2(x, ln1, residual, ln2):
     """(y1, y2) = (residual + ln1(x), ln2(y1)) for the rows [R,H] of a decode step in one launch (inference; nn.LayerNorm
     modules)."""

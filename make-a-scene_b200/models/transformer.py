@@ -144,6 +144,14 @@ def _param_version(model):
     return tuple((p._version, p.data_ptr()) for p in model.parameters())
 
 
+def _attend_append(qkv, kc, vc, suffix, li, pos):
+    """Layer li's attention of this token (qkv [R,3H], stored at position pos) over positions 0..pos: one cache per row, or
+    with suffix (num_samples > 1) the prefix cache of the row's prompt followed by the row's own suffix cache."""
+    if suffix is None:
+        return ops.attn_decode_append(qkv, kc[li], vc[li], pos)
+    return ops.attn_decode_shared_append(qkv, kc[li], vc[li], suffix[0][li], suffix[1][li], pos)
+
+
 class _GraphedDecoder:
     """KV caches + one captured CUDA graph per image position for MakeAScene.generate(use_graphs=True).
 
@@ -153,15 +161,25 @@ class _GraphedDecoder:
     The caches are fp32 up to 8 rows and fp16 above (the cache read dominates a step at a few hundred rows).
     Above 8 rows the decode Linears read the fp16 weight images of ops.decode_weight_image: they are built here, before any
     capture, and held by the decoder, so the graphs never record a packing launch and never outlive the images they read.
-    `version` records every parameter's version and storage: generate() builds a new decoder when it changes."""
+    `version` records every parameter's version and storage: generate() builds a new decoder when it changes.
+    samples > 1 (generate(num_samples=n)): the rows are groups of n samples of one prompt. kc / vc are then prefix caches with
+    one row per prompt [rows / n, heads, text + seg length, hd], and `suffix` holds every row's own image-position caches
+    [rows, heads, image_length, hd]; the element type still follows the row count."""
 
-    def __init__(self, model, rows, dev):
+    def __init__(self, model, rows, dev, samples=1):
         layers = model.transformer.layers
         heads = layers[0].attn.num_attn_heads
         hd = model.hidden_dim // heads
-        self.model, self.rows = model, rows
+        self.model, self.rows, self.samples = model, rows, samples
         dt = torch.float32 if rows <= ops.DECODE_F32_ROWS else torch.float16
-        self.kc = [torch.empty((rows, heads, model.total_length, hd), dtype=dt, device=dev) for _ in layers]
+        if samples == 1:
+            self.kc = [torch.empty((rows, heads, model.total_length, hd), dtype=dt, device=dev) for _ in layers]
+            self.suffix = None
+        else:
+            prefix = model.text_length + model.seg_length
+            self.kc = [torch.empty((rows // samples, heads, prefix, hd), dtype=dt, device=dev) for _ in layers]
+            ks = [torch.empty((rows, heads, model.image_length, hd), dtype=dt, device=dev) for _ in layers]
+            self.suffix = (ks, [torch.empty_like(k) for k in ks])
         self.vc = [torch.empty_like(k) for k in self.kc]
         self.version = _param_version(model)
         self.images = []
@@ -183,7 +201,7 @@ class _GraphedDecoder:
         m, R = self.model, self.rows
         emb = ops.EmbedFn.apply([(tok.view(R, 1), row, col, 0)], 1, m.hidden_dim, m.image_token_embedding.weight,
                                 m.image_row_embeddings.weight, m.image_col_embeddings.weight)
-        return m._logits_of(m._decode_step(emb.view(R, m.hidden_dim), self.kc, self.vc, pos), normed=True)
+        return m._logits_of(m._decode_step(emb.view(R, m.hidden_dim), self.kc, self.vc, pos, self.suffix), normed=True)
 
     def graphed_step(self, t, tok_all, prefix):
         self.tok.copy_(tok_all)
@@ -286,18 +304,19 @@ class MakeAScene(nn.Module):
             x = layer.second_ln_sandwich(m, residual=x) if layer.cogview_sandwich_layernorm else x + m
         return x[:, -1].contiguous()
 
-    def _decode_step(self, x, kc, vc, pos):
+    def _decode_step(self, x, kc, vc, pos, suffix=None):
         """One new token per row (x [R,H], absolute position pos) through all layers against the cache; returns
         final_ln(hidden). Seven launches per layer: qkv, attention (+ cache append), out_proj, the sandwich LayerNorm chained
-        with the next input LayerNorm (mas_layernorm2_forward), lin1 (+GELU), lin2, the second chained pair."""
+        with the next input LayerNorm (mas_layernorm2_forward), lin1 (+GELU), lin2, the second chained pair.
+        suffix: the per-row caches of _GraphedDecoder when rows share prefix caches (kc / vc) in groups."""
         layers = self.transformer.layers
         if not all(l.cogview_sandwich_layernorm for l in layers) or x.shape[-1] % 4 or x.shape[-1] > 4096:
-            return self.transformer.final_ln(self._decode_step_plain(x, kc, vc, pos))
+            return self.transformer.final_ln(self._decode_step_plain(x, kc, vc, pos, suffix))
         y = layers[0].ln_in(x)
         for li, layer in enumerate(layers):
             at, mlp = layer.attn, layer.mlp
             qkv = ops.linear_small(y, at.qkv.weight, at.qkv.bias)
-            a = ops.linear_small(ops.attn_decode_append(qkv, kc[li], vc[li], pos), at.out_proj.weight, at.out_proj.bias)
+            a = ops.linear_small(_attend_append(qkv, kc, vc, suffix, li, pos), at.out_proj.weight, at.out_proj.bias)
             x, y = ops.layernorm2(a, layer.first_ln_sandwich, x, layer.ln_out)        # x + LN(a), then the MLP's input norm
             m = ops.linear_small(y, mlp.lin1.weight, mlp.lin1.bias, act=1)
             m = ops.linear_small(m, mlp.lin2.weight, mlp.lin2.bias)
@@ -305,13 +324,18 @@ class MakeAScene(nn.Module):
             x, y = ops.layernorm2(m, layer.second_ln_sandwich, x, nxt)
         return y
 
-    def _decode_step_plain(self, x, kc, vc, pos):
+    def _decode_step_plain(self, x, kc, vc, pos, suffix=None):
         """The unfused form (configurations without the sandwich LayerNorm); returns the hidden state before final_ln."""
         for li, layer in enumerate(self.transformer.layers):
             at, mlp = layer.attn, layer.mlp
             qkv = ops.linear_small(layer.ln_in(x), at.qkv.weight, at.qkv.bias)
-            ops.kv_append(qkv.view(qkv.shape[0], 1, -1), kc[li], vc[li], pos)
-            a = ops.linear_small(ops.attn_decode(qkv, kc[li], vc[li], pos + 1), at.out_proj.weight, at.out_proj.bias)
+            if suffix is None:
+                ops.kv_append(qkv.view(qkv.shape[0], 1, -1), kc[li], vc[li], pos)
+                ctx = ops.attn_decode(qkv, kc[li], vc[li], pos + 1)
+            else:   # the same two steps on the split caches: the append entry would add this token's term in another order
+                ops.kv_append(qkv.view(qkv.shape[0], 1, -1), suffix[0][li], suffix[1][li], pos - kc[li].shape[2])
+                ctx = ops.attn_decode_shared(qkv, kc[li], vc[li], suffix[0][li], suffix[1][li], pos + 1)
+            a = ops.linear_small(ctx, at.out_proj.weight, at.out_proj.bias)
             x = layer.first_ln_sandwich(a, residual=x) if layer.cogview_sandwich_layernorm else x + a
             m = ops.linear_small(layer.ln_out(x), mlp.lin1.weight, mlp.lin1.bias, act=1)
             m = ops.linear_small(m, mlp.lin2.weight, mlp.lin2.bias)
@@ -326,7 +350,7 @@ class MakeAScene(nn.Module):
 
     @torch.no_grad()
     def generate(self, text_tokens, seg_tokens, guidance_scale=None, uncond_text_tokens=None, temperature=1.0, top_k=None,
-                 generator=None, img_tokens=None, return_logits=False, use_graphs=False, top_p=None, img_mask=None):
+                 generator=None, img_tokens=None, return_logits=False, use_graphs=False, top_p=None, img_mask=None, num_samples=1):
         """Autoregressive sampling of the image tokens with a KV cache; optional classifier-free guidance
         (logits = uncond + scale * (cond - uncond), the unconditional stream sees padded text; Make-A-Scene paper 3.4).
 
@@ -347,14 +371,26 @@ class MakeAScene(nn.Module):
         all-false mask gives the tokens of the unprompted call with the same generator.
         Returns tokens [B,image_length] (and the per-position logits [B,image_length,V], mixed and unfiltered, when
         return_logits=True).
+        num_samples=n (int >= 1) draws n images per prompt: the result is that of generate(text_tokens.repeat_interleave(n, 0),
+        seg_tokens.repeat_interleave(n, 0), ...) with the same generator state, bit for bit; output row b*n + j is sample j of
+        prompt b, so the returned shapes have B*n rows, and img_tokens / img_mask are given per output row [B*n,image_length]
+        (uncond_text_tokens stays per prompt [B,text_length]). The text + segmentation prefix runs once per prompt, its K / V
+        are cached once per prompt, and each decode step reads a prompt's prefix once for its group of samples
+        (mas_attn_decode_shared_append); the row count R = B*n (2B*n with guidance) still selects fp32 or fp16 decoding.
         use_graphs: replay each position's decode step from a CUDA graph (captured at first use and kept on the module for
         the same row count; captured again after any parameter changes, in place or by replaced storage)."""
         B = text_tokens.shape[0]
         dev = text_tokens.device
+        n = num_samples
+        if isinstance(n, bool) or not isinstance(n, int) or n < 1:
+            raise ValueError("num_samples must be an int >= 1, got %r" % (num_samples,))
+        Bn = B * n
         if top_p is not None and not float(top_p) > 0:
             raise ValueError("top_p must be > 0 (None or >= 1: no nucleus filter), got %r" % (top_p,))
+        if img_tokens is not None and n > 1 and tuple(img_tokens.shape) != (Bn, self.image_length):
+            raise ValueError("img_tokens must have one row per output row: shape %s" % ((Bn, self.image_length),))
         if img_mask is not None:
-            want = (B, self.image_length)
+            want = (Bn, self.image_length)
             if img_tokens is None:
                 raise ValueError("img_mask selects positions of img_tokens: pass img_tokens too")
             if not isinstance(img_mask, torch.Tensor) or img_mask.dtype != torch.bool or tuple(img_mask.shape) != want:
@@ -372,18 +408,21 @@ class MakeAScene(nn.Module):
             seg_all = torch.cat([seg_tokens, seg_tokens], 0)
         else:
             text_all, seg_all = text_tokens, seg_tokens
-        R = text_all.shape[0]
+        R = text_all.shape[0] * n            # rows [cond: B*n | uncond: B*n]; sample row r belongs to prompt row r // n
         dec = getattr(self, "_sampler", None)
-        if dec is None or dec.rows != R or dec.tok.device != dev or not use_graphs or dec.version != _param_version(self):
-            dec = _GraphedDecoder(self, R, dev)
+        if (dec is None or dec.rows != R or dec.samples != n or dec.tok.device != dev or not use_graphs
+                or dec.version != _param_version(self)):
+            dec = _GraphedDecoder(self, R, dev, n)
             if use_graphs:
                 self._sampler = dec
         kc, vc = dec.kc, dec.vc
         prefix = text_all.shape[1] + seg_all.shape[1]
-        logits = self._logits_of(self._prefill(self._embed(text_all, seg_all, None), kc, vc))
+        last = self._prefill(self._embed(text_all, seg_all, None), kc, vc)
+        # expanded BEFORE to_logits: linear_small picks its arithmetic by row count, and the repeated call has R rows here
+        logits = self._logits_of(last.repeat_interleave(n, 0) if n > 1 else last)
         toks, kept = [], []
         for t in range(self.image_length):
-            mixed = ops.cfg_mix(logits[:B], logits[B:], guidance_scale) if cfg else logits
+            mixed = ops.cfg_mix(logits[:Bn], logits[Bn:], guidance_scale) if cfg else logits
             if return_logits:
                 kept.append(mixed)
             prompt = (img_tokens[:, t], img_mask[:, t]) if img_mask is not None else None
@@ -395,9 +434,9 @@ class MakeAScene(nn.Module):
                 u = None
                 if temperature:
                     if generator is not None and generator.device.type != dev.type:
-                        u = torch.rand(B, generator=generator).to(dev)
+                        u = torch.rand(Bn, generator=generator).to(dev)
                     else:
-                        u = torch.rand(B, device=dev, generator=generator)
+                        u = torch.rand(Bn, device=dev, generator=generator)
                 tok = ops.sample_topk(mixed, float(temperature), top_k, u, top_p=top_p, prompt=prompt)
             toks.append(tok)
             if t == self.image_length - 1:

@@ -5,8 +5,13 @@ from HBM as they do in a decode step. One JSON line per measurement:
   * the five decode Linear shapes (qkv, out_proj, lin1 + GELU, lin2, to_logits) at R rows: the narrow split form
     mas_linear_rows_f16 against the training kernel mas_gemm_rows_f16 (+ mas_gelu_forward for lin1) on the same fp16 copy,
     as ms and weight-stream GB/s, and the form ops.linear_small selects;
-  * attention decode on the fp16 cache against the fp32 one, as ms and cache GB/s (k and v bytes read).
-Usage: python tools/bench_decode.py [--rows 16 32 64 128 256] [--iters N]"""
+  * attention decode on the fp16 cache against the fp32 one, as ms and cache GB/s (k and v bytes read);
+  * the shared-prefix decode attention of generate(num_samples=n) (a 384-position prefix cache per group of n rows, a
+    256-position suffix cache per row) against mas_attn_decode_append on the concatenated cache, at position 511 (cache length
+    512, the mean of the image positions), fp16 caches: us per launch, and GB/s of the cache bytes the step needs (the
+    shared form needs each group's prefix once). The launcher's rows per block ("auto") is timed beside one row per block,
+    where a group's prefix can only be shared through L2 hits between adjacent blocks.
+Usage: python tools/bench_decode.py [--rows 16 32 64 128 256] [--iters N] [--only linear|attn|shared] [--shared-rows 16 64 256]"""
 import argparse
 import json
 import os
@@ -21,6 +26,9 @@ from mas_b200 import _lib as L, ops  # noqa: E402
 ap = argparse.ArgumentParser()
 ap.add_argument("--rows", type=int, nargs="+", default=[16, 32, 64, 128, 256])
 ap.add_argument("--iters", type=int, default=200)
+ap.add_argument("--only", choices=["linear", "attn", "shared"], default=None)
+ap.add_argument("--shared-rows", type=int, nargs="+", default=[16, 64, 256])
+ap.add_argument("--samples", type=int, nargs="+", default=[1, 4, 8, 16])
 args = ap.parse_args()
 dev = torch.device("cuda:0")
 gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, check=True)
@@ -58,7 +66,7 @@ def timed(fn):
 H = 1024
 SHAPES = [("qkv", 3 * H, H, 0), ("out_proj", H, H, 0), ("lin1", 4 * H, H, 1), ("lin2", H, 4 * H, 0), ("to_logits", 8192, H, 0)]
 torch.manual_seed(0)
-for name, N, K, act in SHAPES:
+for name, N, K, act in (SHAPES if args.only in (None, "linear") else []):
     wb = N * K * 2
     ws_ = [torch.randn(N, K, device=dev) / K ** 0.5 for _ in range(copies(wb))]
     wpk = [ops._packed_linear_weight(w, False, dev) for w in ws_]
@@ -85,7 +93,7 @@ for name, N, K, act in SHAPES:
     del ws_, wpk
 
 heads, hd, tmax, length = 16, 64, 640, 512
-for R in args.rows:
+for R in (args.rows if args.only in (None, "attn") else []):
     qkv = torch.randn(R, 3 * heads * hd, device=dev)
     ctx = torch.empty(R, heads * hd, device=dev)
     res = {"kernel": "attn_decode", "rows": R, "heads": heads, "hd": hd, "len": length}
@@ -101,3 +109,29 @@ for R in args.rows:
         del caches
     res["f16_share_of_3350_gbs"] = round(res["f16_cache_gbs"] / 3350, 3)
     print(json.dumps(res), flush=True)
+
+prefix, tsuf, pos = 384, 256, 511
+for R in (args.shared_rows if args.only in (None, "shared") else []):
+    qkv = torch.randn(R, 3 * heads * hd, device=dev)
+    ctx = torch.empty(R, heads * hd, device=dev)
+    full = 2 * R * heads * (pos + 1) * hd * 2                                     # k + v bytes of the unshared step
+    cc = [(torch.randn(R, heads, tmax, hd, device=dev).half(), torch.randn(R, heads, tmax, hd, device=dev).half()) for _ in range(copies(full))]
+    t_ref = timed(lambda i: L.call("mas_attn_decode_append_f16", qkv, cc[i % len(cc)][0], cc[i % len(cc)][1], ctx, R, heads, hd, tmax, pos))
+    del cc
+    for n in args.samples:
+        if R % n:
+            continue
+        need = 2 * heads * hd * 2 * (R // n * prefix + R * (pos + 1 - prefix))   # each group's prefix once, every row's suffix
+        sc = [tuple(torch.randn(r, heads, t, hd, device=dev).half() for r, t in ((R // n, prefix), (R // n, prefix), (R, tsuf), (R, tsuf)))
+              for _ in range(copies(need))]
+        res = {"kernel": "attn_decode_shared_append_f16", "rows": R, "samples": n, "heads": heads, "hd": hd, "len": pos + 1,
+               "unshared_us": round(t_ref * 1e3, 2), "unshared_needed_gbs": round(full / t_ref / 1e6, 1), "copies": len(sc)}
+        for tag, rpb in (("auto", 0), ("one_row_per_block", 1)):
+            t = timed(lambda i: L.call("mas_attn_decode_shared_append_f16", qkv, *sc[i % len(sc)][:2], *sc[i % len(sc)][2:], ctx, R, n, heads,
+                                       hd, prefix, tsuf, pos, rpb))
+            res[tag + "_us"] = round(t * 1e3, 2)
+            res[tag + "_needed_gbs"] = round(need / t / 1e6, 1)
+            res[tag + "_speedup"] = round(t_ref / t, 3)
+        res["needed_bytes_share"] = round(need / full, 3)
+        print(json.dumps(res), flush=True)
+        del sc

@@ -5,7 +5,9 @@ GPU's name and power limit, and the HBM bytes a decode step streams on the path 
 fp32 KV cache, above 8 rows fp16 weights and fp16 cache (the cache read at the mean cache length of the image positions).
 --top-p adds the nucleus filter to the draw (top-k 64 stays); --prompt-frac F forces a random share F of the image positions
 (an image prompt, random tokens): the forced positions are still decoded one step each, so tokens/s counts every position.
-Usage: python tools/bench_sampling.py [--batch B] [--reps N] [--graphs] [--top-p P] [--prompt-frac F]"""
+--samples N draws N images per prompt (generate(num_samples=N)): B prompts give R = 2 B N rows that share each prompt's prefix
+cache, and cache_gb_per_step counts a prompt's prefix once per step, as the shared-prefix attention reads it.
+Usage: python tools/bench_sampling.py [--batch B] [--samples N] [--reps N] [--graphs] [--top-p P] [--prompt-frac F]"""
 import argparse
 import json
 import os
@@ -20,6 +22,7 @@ from models.transformer import MakeAScene  # noqa: E402
 
 ap = argparse.ArgumentParser()
 ap.add_argument("--batch", type=int, default=1)
+ap.add_argument("--samples", type=int, default=1, help="images per prompt (generate's num_samples)")
 ap.add_argument("--reps", type=int, default=2)
 ap.add_argument("--layers", type=int, default=24)
 ap.add_argument("--graphs", action="store_true", help="replay each position's decode step from a CUDA graph")
@@ -32,14 +35,14 @@ cfg = dict(num_layers=args.layers, hidden_dim=1024, num_attn_heads=16, image_voc
            image_tokens_per_dim=16, seg_tokens_per_dim=16, text_length=128)
 m = MakeAScene(**cfg).to(dev).eval()
 m.device = dev
-B = args.batch
+B, N = args.batch, args.samples
 text = torch.randint(1, 40000, (B, 128), device=dev)
 seg = torch.randint(0, 1024, (B, 256), device=dev)
 gen = torch.Generator(device=dev).manual_seed(1)
-kw = dict(guidance_scale=3.0, temperature=1.0, top_k=64, top_p=args.top_p, generator=gen, use_graphs=args.graphs)
+kw = dict(guidance_scale=3.0, temperature=1.0, top_k=64, top_p=args.top_p, generator=gen, use_graphs=args.graphs, num_samples=N)
 if args.prompt_frac > 0:
-    kw["img_tokens"] = torch.randint(0, cfg["image_vocab_size"], (B, 256), device=dev)
-    kw["img_mask"] = torch.rand(B, 256, device=dev) < args.prompt_frac
+    kw["img_tokens"] = torch.randint(0, cfg["image_vocab_size"], (B * N, 256), device=dev)
+    kw["img_mask"] = torch.rand(B * N, 256, device=dev) < args.prompt_frac
 m.generate(text, seg, **kw)     # warm-up (captures)
 torch.cuda.synchronize()
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -51,15 +54,16 @@ e1.record()
 torch.cuda.synchronize()
 sec = e0.elapsed_time(e1) * 1e-3 / args.reps
 gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, check=True)
-R = 2 * B
+R = 2 * B * N
 elem = 4 if R <= ops.DECODE_F32_ROWS else 2
 params = sum(p.numel() for n, p in m.named_parameters() if "embedding" not in n)
 prefix, steps = 128 + 256, 255
-mean_len = prefix + (steps + 1) / 2                       # cache positions read by the step of image position t: prefix + t + 1
+mean_suffix = (steps + 1) / 2        # the step of image position t reads prefix + t + 1 positions; its prompt's prefix once per group
 weight_bytes = params * elem
-cache_bytes = args.layers * R * 2 * cfg["hidden_dim"] * mean_len * elem
-print(json.dumps({"metric": "image tokens/s, classifier-free guided sampling with KV cache", "value": B * 256 / sec, "unit": "tokens/s",
-                  "gpu": gpu.stdout.strip().splitlines()[0], "batch": B, "rows": R, "cuda_graphs": bool(args.graphs),
+cache_bytes = args.layers * 2 * cfg["hidden_dim"] * (R // N * prefix + R * mean_suffix) * elem
+print(json.dumps({"metric": "image tokens/s, classifier-free guided sampling with KV cache", "value": B * N * 256 / sec, "unit": "tokens/s",
+                  "images_per_s": B * N / sec, "gpu": gpu.stdout.strip().splitlines()[0], "batch": B, "prompts": B, "samples": N,
+                  "rows": R, "cuda_graphs": bool(args.graphs),
                   "top_k": 64, "top_p": args.top_p, "prompt_frac": args.prompt_frac,
                   "seconds_per_image": sec, "launches_per_image": (_lib.launch_count() - l0) // args.reps,
                   "operand_bytes": elem, "weight_stream_gb_per_step": weight_bytes / 1e9, "cache_gb_per_step": cache_bytes / 1e9,
