@@ -454,6 +454,34 @@ int mas_embed3_backward(const float* dout, const int64_t* id0, float* d0, const 
  * (MAS_ERR_UNSUPPORTED otherwise: the caller runs the GEMM / softmax sequence).  2 x fp16 operand split = fp32-level accuracy. */
 int mas_attn_causal_forward(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads, int hd,
                             float scale, void* stream);
+/* ---- Dropout of the token transformer (transformer.py:90-91, 114, 139) ------------------------------------------------
+ * Element e of a dropout site is kept iff word[e & 3] of Philox4x32-10(counter = (lo32(e >> 2), hi32(e >> 2), 0, 0),
+ * key = (lo32(seed), hi32(seed))) >= floor(p * 2^32); e is the element's row-major linear index in its tensor
+ * (((b * heads + h) * S + q) * S + k for the attention probabilities, r * H + c for a [rows, H] activation), so every entry
+ * below and both backwards produce the same mask for the same seed.  seed: int64 device scalar (read by the kernels: a captured
+ * CUDA graph draws new masks at each replay).  0 <= p <= 1; kept elements are scaled by 1 / (1 - p) (0 when p = 1).
+ * mas_dropout: y = residual + x * keep * scale over n elements with the caller's scale (1 / (1 - p), or 1 to stage P * keep);
+ *   residual NULL: no add; x NULL: y = residual + keep * scale (the mask itself).  y may alias x or residual.
+ * mas_attn_causal_dropout_forward: mas_attn_causal_forward with attention dropout: P is written undropped (the backward
+ *   needs it), ctx = (P * keep) v / (1 - p).
+ * mas_softmax_causal_dropout_backward: ds = scale * p * (g - sum_visible(p * g)), g = dp * keep / (1 - p), the mask of p's
+ *   own layout; same visibility, aliasing and zero fill as mas_softmax_causal_backward.
+ * mas_layernorm_dropout_forward: y = LN(a * keep / (1 - p)) + residual (the sandwich LayerNorm fed by a dropout site); the
+ *   mask is applied on load, nothing dropped is stored.  mas_layernorm_dropout_backward regenerates it from the same seed:
+ *   da = dLN * keep / (1 - p), dgamma / dbeta as mas_layernorm_backward (same workspace size).  Both need H % 4 == 0,
+ *   H <= 4096 and 16-byte aligned operands (MAS_ERR_UNSUPPORTED otherwise). */
+int mas_dropout(const float* x, const float* residual, float* y, int64_t n, double p, float scale, const int64_t* seed,
+                void* stream);
+int mas_attn_causal_dropout_forward(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads, int hd,
+                                    float scale, double p, const int64_t* seed, void* stream);
+int mas_softmax_causal_dropout_backward(const float* p, const float* dp, float* ds, int64_t mats, int rows, int cols, float scale,
+                                        double drop_p, const int64_t* seed, void* stream);
+int mas_layernorm_dropout_forward(const float* a, const float* gamma, const float* beta, const float* residual, float* y,
+                                  float* mean, float* rstd, int64_t R, int H, float eps, double p, const int64_t* seed,
+                                  void* stream);
+int mas_layernorm_dropout_backward(const float* dy, const float* a, const float* mean, const float* rstd, const float* gamma,
+                                   float* da, float* dgamma, float* dbeta, int64_t R, int H, double p, const int64_t* seed,
+                                   void* ws, size_t ws_bytes, void* stream);
 /* Token cross-entropy, train.py:150-153 (F.cross_entropy(logits.view(-1, V), img_token.view(-1)), mean reduction):
  * logits [R, V] with row pitch ld, target int64 [R] (outside [0, V): row ignored like ignore_index).  forward writes the
  * per-row losses, the per-row logsumexp (kept for the backward) and out[0] = mean loss, out[1] = counted rows.

@@ -16,8 +16,15 @@
 //     accumulator.
 //   * shared memory: the Q tile (resident) + a 2-stage ring of K / V tiles (hi and lo images) + the P block, K-major planes
 //     [c/8][row][8 halves] for Q, K and P, MN-major planes [c/8][key][8 channels] for V (staged untransposed).
+//   * DROP (attention dropout, mas_attn_causal_dropout_forward): pass 1 still writes the undropped P (the softmax backward
+//     needs it), then zeroes the dropped fragment elements before the split into shared memory.  The factor 1 / (1 - p) is
+//     applied to ctx in the epilogue, not to P: the split keeps P * 2^14 within fp16, which P / (1 - p) would leave for large p.
+//     The keep bits come from dropout.cuh's Philox groups of four keys: the lane pair (fk, fk ^ 1) covers one group per row,
+//     so each lane generates one group per 8-key column block (row frow or frow + 8) and takes the other row's bits from its
+//     partner by a shuffle.
 #include <cuda_fp16.h>
 
+#include "dropout.cuh"
 #include "mas_common.cuh"
 #include "wgmma.cuh"
 
@@ -74,7 +81,8 @@ struct Params {
   float scale;
 };
 
-__global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p) {
+template <bool DROP>
+__global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, const DropMask dm) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* q_tile = smem;                                   // resident Q tile (hi, lo)
   uint8_t* ring = smem + TILE;                              // STAGES x TILE
@@ -199,6 +207,18 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p) {
       } else {
         // probabilities: global (fp32) and the split P block in shared memory (the previous block's P V MMAs have retired:
         // the barrier in fill() above)
+        uint32_t keep[2] = {0u, 0u};                           // DROP: bit 2 j + c <-> key 8 j + 2 fk + c of row frow + 8 i
+        if constexpr (DROP) {
+          const uint64_t seed = (uint64_t)*dm.seed;
+          const uint64_t row0 = (((uint64_t)b * heads + h) * S + q0 + frow + 8 * (fk & 1)) * S + kb * BK + 4 * (fk >> 1);
+#pragma unroll
+          for (int j = 0; j < BK / 8; ++j) {
+            const uint32_t bits = keep_bits4(seed, (row0 + 8 * j) >> 2, dm.t);
+            const uint32_t b0 = __shfl_sync(0xffffffffu, bits, lane & ~1), b1 = __shfl_sync(0xffffffffu, bits, lane | 1);
+            keep[0] |= ((b0 >> (2 * (fk & 1))) & 3u) << (2 * j);
+            keep[1] |= ((b1 >> (2 * (fk & 1))) & 3u) << (2 * j);
+          }
+        }
 #pragma unroll
         for (int i = 0; i < 2; ++i) {
           const int rit = frow + 8 * i;
@@ -210,7 +230,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p) {
             const float c = (diag && key + 1 > rit) ? 0.f : expf(sacc[4 * j + 2 * i + 1] * ss - m[i]) * rl[i];
             *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(a, c);
             uint32_t hi, lo;
-            split2(a, c, P_SCALE, &hi, &lo);
+            if constexpr (DROP)
+              split2((keep[i] >> (2 * j)) & 1u ? a : 0.f, (keep[i] >> (2 * j + 1)) & 1u ? c : 0.f, P_SCALE, &hi, &lo);
+            else
+              split2(a, c, P_SCALE, &hi, &lo);
             uint8_t* d = p_blk + (size_t)j * PITCH_P + rit * 16 + fk * 4;
             *reinterpret_cast<uint32_t*>(d) = hi;
             *reinterpret_cast<uint32_t*>(d + P_HALF) = lo;
@@ -240,7 +263,8 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p) {
     }
   }
   // ctx tile: straight from the fragment
-  const float oscale = inv_s * P_INV;
+  float oscale = inv_s * P_INV;
+  if constexpr (DROP) oscale *= dm.scale;
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
     float* orow = p.ctx + ((size_t)b * S + q0 + frow + 8 * i) * H + h * HD + 2 * fk;
@@ -260,21 +284,33 @@ bool attn_causal_fused_ok(int S, int heads, int hd) { return hd == attnc::HD && 
 
 using namespace mas;
 
-extern "C" int mas_attn_causal_forward(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads, int hd,
-                                       float scale, void* stream) {
+template <bool DROP>
+static int attn_causal_launch(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads, int hd, float scale,
+                              const DropMask& dm, void* stream) {
   MAS_REQUIRE(qkv && amax && P && ctx && B > 0, "attn_causal_forward: bad arguments");
   if (!attn_causal_fused_ok(S, heads, hd))
     return fail(MAS_ERR_UNSUPPORTED, "attn_causal_forward: needs head dim 64 and S %% 128 == 0 (got S=%d, hd=%d)", S, hd);
   if (heads > 65535 || B > 65535) return fail(MAS_ERR_UNSUPPORTED, "attn_causal_forward: heads / batch beyond the grid limits");
   static std::atomic<uint64_t> configured{0};
   if (first_on_device(configured)) {
-    cudaError_t e = cudaFuncSetAttribute(attnc::attn_causal_fwd, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attnc::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(attnc::attn_causal_fwd<DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attnc::SMEM_BYTES);
     if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "attn_causal_fwd: smem attr: %s", cudaGetErrorString(e));
     mark_device(configured);
   }
   attnc::Params p;
   p.qkv = qkv; p.P = P; p.ctx = ctx; p.amax = amax; p.S = S; p.heads = heads; p.scale = scale;
   const dim3 grid((unsigned)(S / attnc::BM), (unsigned)heads, (unsigned)B);
-  attnc::attn_causal_fwd<<<grid, attnc::NTHREADS, attnc::SMEM_BYTES, mas::S(stream)>>>(p);
-  return launched_tc("attn_causal_fwd");
+  attnc::attn_causal_fwd<DROP><<<grid, attnc::NTHREADS, attnc::SMEM_BYTES, mas::S(stream)>>>(p, dm);
+  return launched_tc(DROP ? "attn_causal_dropout_fwd" : "attn_causal_fwd");
+}
+
+extern "C" int mas_attn_causal_forward(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads, int hd,
+                                       float scale, void* stream) {
+  return attn_causal_launch<false>(qkv, amax, P, ctx, B, S, heads, hd, scale, DropMask{nullptr, 0, 1.f}, stream);
+}
+
+extern "C" int mas_attn_causal_dropout_forward(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads,
+                                               int hd, float scale, double p, const int64_t* seed, void* stream) {
+  MAS_REQUIRE(seed && p >= 0.0 && p <= 1.0, "attn_causal_dropout_forward: bad dropout arguments");
+  return attn_causal_launch<true>(qkv, amax, P, ctx, B, S, heads, hd, scale, DropMask{seed, drop_threshold(p), drop_scale(p)}, stream);
 }

@@ -3,28 +3,45 @@
 // PB-relax shift is softmax-invariant and the -10000 fill underflows to exactly 0 in fp32, so this is plain causal
 // softmax), fused token + row/column position embedding gather (transformer.py:329-364).  Linear layers and the
 // attention contractions reuse the GEMM kernels (contract_tc.cu / contract_simt.cu).  fp32 throughout.
+#include "dropout.cuh"
 #include "mas_common.cuh"
 
 namespace mas {
+
+// Dropout (dropout.cuh) of four consecutive elements 4 g .. 4 g + 3 of the row-major tensor, in place.
+__device__ __forceinline__ void drop4(float4& v, uint64_t seed, uint64_t g, const DropMask& dm) {
+  const uint32_t k = keep_bits4(seed, g, dm.t);
+  v.x = (k & 1u) ? v.x * dm.scale : 0.f;
+  v.y = (k & 2u) ? v.y * dm.scale : 0.f;
+  v.z = (k & 4u) ? v.z * dm.scale : 0.f;
+  v.w = (k & 8u) ? v.w * dm.scale : 0.f;
+}
 
 // ---------------------------------------------------------------------------------------------------- LayerNorm, few rows
 // Decode steps normalise 2-8 rows: a warp per row walks H = 1024 in 32 dependent trips per pass (13 us measured). Here a
 // 256-thread block owns one row, keeps it in registers (up to four 16-byte quads per thread: H <= 4096), and needs two
 // block reductions; same two-pass statistics (mean, then centred sum of squares) as the warp-per-row kernel.
+// DROP (mas_layernorm_dropout_forward): the LayerNorm input is x * keep * scale, masked on load (H % 4 == 0: a quad is a mask
+// group).  Any row count: the training forward uses it for every row then.
+template <bool DROP>
 __global__ void __launch_bounds__(256) layernorm_fwd_block_kernel(const float* __restrict__ x, const float* __restrict__ gamma,
                                                                   const float* __restrict__ beta, const float* __restrict__ res,
                                                                   float* __restrict__ y, float* __restrict__ mean,
-                                                                  float* __restrict__ rstd, int H, float eps) {
+                                                                  float* __restrict__ rstd, int H, float eps, const DropMask dm) {
   __shared__ float red[2][8];
   const int64_t row = blockIdx.x;
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5, Q = H >> 2;
   const float4* xr = reinterpret_cast<const float4*>(x + row * H);
   float4 v[4];
   float s = 0.f;
+  uint64_t seed = 0;
+  if constexpr (DROP) seed = (uint64_t)*dm.seed;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int q = t + 256 * i;
     v[i] = q < Q ? __ldg(xr + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+    if constexpr (DROP)
+      if (q < Q) drop4(v[i], seed, (uint64_t)row * Q + q, dm);
     s += (v[i].x + v[i].y) + (v[i].z + v[i].w);
   }
   s = warp_sum(s);
@@ -206,9 +223,13 @@ __global__ void layernorm_bwd_dx_kernel(const float* __restrict__ dy, const floa
 
 // Block-per-row form for H <= 4096 (the row's dy and x stay in registers: one pass over global memory instead of three
 // dependent warp-strided passes; the warp-per-row kernel above walked H = 1024 in 32 trips per pass).
+// DROP (mas_layernorm_dropout_backward): x is the undropped input a; the LayerNorm input a * keep * scale is rebuilt on load
+// and the data gradient is multiplied by keep * scale.
+template <bool DROP>
 __global__ void __launch_bounds__(256) layernorm_bwd_dx_block_kernel(const float* __restrict__ dy, const float* __restrict__ x,
                                                                      const float* __restrict__ mean, const float* __restrict__ rstd,
-                                                                     const float* __restrict__ gamma, float* __restrict__ dx, int H) {
+                                                                     const float* __restrict__ gamma, float* __restrict__ dx, int H,
+                                                                     const DropMask dm) {
   __shared__ float red[2][8];
   const int64_t row = blockIdx.x;
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5, Q = H >> 2;
@@ -218,11 +239,16 @@ __global__ void __launch_bounds__(256) layernorm_bwd_dx_block_kernel(const float
   const float4* g4 = reinterpret_cast<const float4*>(gamma);
   float4 g[4], xh[4];
   float a = 0.f, b = 0.f;
+  uint64_t seed = 0;
+  if constexpr (DROP) seed = (uint64_t)*dm.seed;
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int q = t + 256 * i;
     if (q < Q) {
-      const float4 d = __ldg(dr + q), xv = __ldg(xr + q), gm = __ldg(g4 + q);
+      const float4 d = __ldg(dr + q);
+      float4 xv = __ldg(xr + q);
+      const float4 gm = __ldg(g4 + q);
+      if constexpr (DROP) drop4(xv, seed, (uint64_t)row * Q + q, dm);
       g[i] = make_float4(d.x * gm.x, d.y * gm.y, d.z * gm.z, d.w * gm.w);
       xh[i] = make_float4((xv.x - m) * rs, (xv.y - m) * rs, (xv.z - m) * rs, (xv.w - m) * rs);
       a = fmaf(g[i].x, xh[i].x, a); a = fmaf(g[i].y, xh[i].y, a); a = fmaf(g[i].z, xh[i].z, a); a = fmaf(g[i].w, xh[i].w, a);
@@ -244,9 +270,12 @@ __global__ void __launch_bounds__(256) layernorm_bwd_dx_block_kernel(const float
 #pragma unroll
   for (int i = 0; i < 4; ++i) {
     const int q = t + 256 * i;
-    if (q < Q)
-      o4[q] = make_float4(rs * (g[i].x - tb - xh[i].x * ta), rs * (g[i].y - tb - xh[i].y * ta), rs * (g[i].z - tb - xh[i].z * ta),
-                          rs * (g[i].w - tb - xh[i].w * ta));
+    if (q < Q) {
+      float4 o = make_float4(rs * (g[i].x - tb - xh[i].x * ta), rs * (g[i].y - tb - xh[i].y * ta), rs * (g[i].z - tb - xh[i].z * ta),
+                             rs * (g[i].w - tb - xh[i].w * ta));
+      if constexpr (DROP) drop4(o, seed, (uint64_t)row * Q + q, dm);
+      o4[q] = o;
+    }
   }
 }
 
@@ -287,6 +316,100 @@ __global__ void layernorm_bwd_param_final(const double* __restrict__ part, int c
   }
   dgamma[c] = (float)a;
   dbeta[c] = (float)b;
+}
+
+// dgamma / dbeta partials of mas_layernorm_dropout_backward: the same partial layout as layernorm_bwd_param_partial, each
+// thread owning four adjacent columns (one mask group per row; H % 4 == 0), x = a * keep * scale rebuilt on load.
+__global__ void layernorm_dropout_bwd_param_partial(const float* __restrict__ dy, const float* __restrict__ a,
+                                                    const float* __restrict__ mean, const float* __restrict__ rstd, int64_t R, int H,
+                                                    const DropMask dm, double* __restrict__ part) {
+  __shared__ double sh[8][32][8];
+  const int Q = H >> 2, q = blockIdx.x * 32 + threadIdx.x;
+  const int64_t r0 = (int64_t)blockIdx.y * LN_ROWS, r1 = min(R, r0 + LN_ROWS);
+  const uint64_t seed = (uint64_t)*dm.seed;
+  double acc[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+  if (q < Q)
+    for (int64_t r = r0 + threadIdx.y; r < r1; r += 8) {
+      const float4 d = __ldg(reinterpret_cast<const float4*>(dy + r * H) + q);
+      float4 xv = __ldg(reinterpret_cast<const float4*>(a + r * H) + q);
+      drop4(xv, seed, (uint64_t)r * Q + q, dm);
+      const float m = mean[r], rs = rstd[r];
+      acc[0] += (double)d.x * ((xv.x - m) * rs); acc[1] += d.x;
+      acc[2] += (double)d.y * ((xv.y - m) * rs); acc[3] += d.y;
+      acc[4] += (double)d.z * ((xv.z - m) * rs); acc[5] += d.z;
+      acc[6] += (double)d.w * ((xv.w - m) * rs); acc[7] += d.w;
+    }
+#pragma unroll
+  for (int k = 0; k < 8; ++k) sh[threadIdx.y][threadIdx.x][k] = acc[k];
+  __syncthreads();
+  if (threadIdx.y == 0 && q < Q) {
+    for (int y = 1; y < 8; ++y)
+#pragma unroll
+      for (int k = 0; k < 8; ++k) acc[k] += sh[y][threadIdx.x][k];
+    double* o = part + ((size_t)blockIdx.y * H + 4 * q) * 2;
+#pragma unroll
+    for (int k = 0; k < 8; ++k) o[k] = acc[k];
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------- dropout
+// y = residual + x * keep * scale (x null: keep * scale; residual null: no add), one Philox group of four elements per
+// thread and trip (16-byte accesses when every operand is aligned).
+__global__ void dropout_kernel(const float* x, const float* res, float* y, int64_t n, const DropMask dm, bool vec) {   // y may alias x / res
+  const uint64_t seed = (uint64_t)*dm.seed;
+  const int64_t groups = (n + 3) >> 2;
+  for (int64_t g = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; g < groups; g += (int64_t)gridDim.x * blockDim.x) {
+    const int64_t e0 = 4 * g;
+    const uint32_t k = keep_bits4(seed, (uint64_t)g, dm.t);
+    if (vec && e0 + 4 <= n) {
+      float4 v = x ? reinterpret_cast<const float4*>(x)[g] : make_float4(1.f, 1.f, 1.f, 1.f);
+      v.x = (k & 1u) ? v.x * dm.scale : 0.f;
+      v.y = (k & 2u) ? v.y * dm.scale : 0.f;
+      v.z = (k & 4u) ? v.z * dm.scale : 0.f;
+      v.w = (k & 8u) ? v.w * dm.scale : 0.f;
+      if (res) {
+        const float4 r = reinterpret_cast<const float4*>(res)[g];
+        v.x = r.x + v.x; v.y = r.y + v.y; v.z = r.z + v.z; v.w = r.w + v.w;
+      }
+      reinterpret_cast<float4*>(y)[g] = v;
+    } else {
+      for (int c = 0; c < 4 && e0 + c < n; ++c) {
+        const float v = (k >> c) & 1u ? (x ? x[e0 + c] : 1.f) * dm.scale : 0.f;
+        y[e0 + c] = res ? res[e0 + c] + v : v;
+      }
+    }
+  }
+}
+
+// ds = alpha * p * (g - sum_visible(p * g)), g = dp * keep * scale, on the visible columns (0..i+cols-rows) of each row, zeros
+// beyond; the mask element of (row, c) is row * cols + c (p's layout).  Warp per row; a lane walks the row's Philox groups.
+__global__ void softmax_causal_dropout_bwd_kernel(const float* __restrict__ p, const float* dp, float* ds, int64_t total_rows, int rows,
+                                                  int cols, float alpha, const DropMask dm) {
+  const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  if (row >= total_rows) return;
+  const int lane = threadIdx.x & 31;
+  const int i = (int)(row % rows), lim = i + (cols - rows);  // columns 0..lim are visible
+  const uint64_t seed = (uint64_t)*dm.seed;
+  const int64_t e_row = row * cols;
+  const int64_t g0 = e_row >> 2, g_vis = (e_row + lim) >> 2, g_end = (e_row + cols - 1) >> 2;
+  float dot = 0.f;
+  for (int64_t g = g0 + lane; g <= g_vis; g += 32) {
+    const uint32_t k = keep_bits4(seed, (uint64_t)g, dm.t);
+    for (int c4 = 0; c4 < 4; ++c4) {
+      const int64_t c = 4 * g + c4 - e_row;
+      if (c >= 0 && c <= lim && ((k >> c4) & 1u)) dot += p[e_row + c] * (dp[e_row + c] * dm.scale);
+    }
+  }
+  dot = warp_sum(dot);
+  for (int64_t g = g0 + lane; g <= g_end; g += 32) {
+    const uint32_t k = g <= g_vis ? keep_bits4(seed, (uint64_t)g, dm.t) : 0u;
+    for (int c4 = 0; c4 < 4; ++c4) {
+      const int64_t c = 4 * g + c4 - e_row;
+      if (c < 0 || c >= cols) continue;
+      const float gv = ((k >> c4) & 1u) && c <= lim ? dp[e_row + c] * dm.scale : 0.f;
+      ds[e_row + c] = c <= lim ? p[e_row + c] * (gv - dot) * alpha : 0.f;
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------- GELU (tanh form)
@@ -463,7 +586,7 @@ int mas_layernorm_forward(const float* x, const float* gamma, const float* beta,
   MAS_REQUIRE(x && gamma && beta && y && mean && rstd && R > 0 && H > 0, "layernorm_forward: bad arguments");
   auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   if (R <= 64 && H % 4 == 0 && H <= 4096 && al16(x) && al16(y) && al16(gamma) && al16(beta) && (!residual || al16(residual))) {
-    layernorm_fwd_block_kernel<<<(unsigned)R, 256, 0, S(stream)>>>(x, gamma, beta, residual, y, mean, rstd, H, eps);
+    layernorm_fwd_block_kernel<false><<<(unsigned)R, 256, 0, S(stream)>>>(x, gamma, beta, residual, y, mean, rstd, H, eps, DropMask{});
     return launched("layernorm_fwd_block");
   }
   layernorm_fwd_kernel<<<(unsigned)cdiv(R, 8), 256, 0, S(stream)>>>(x, gamma, beta, residual, y, mean, rstd, R, H, eps);
@@ -486,7 +609,7 @@ int mas_layernorm_backward(const float* dy, const float* x, const float* mean, c
   if (ws_bytes < mas_layernorm_ws_bytes(R, H)) return fail(MAS_ERR_WORKSPACE, "layernorm_backward: workspace too small");
   auto al16 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; };
   if (H % 4 == 0 && H <= 4096 && H >= 256 && al16(dy) && al16(x) && al16(gamma) && al16(dx)) {
-    layernorm_bwd_dx_block_kernel<<<(unsigned)R, 256, 0, S(stream)>>>(dy, x, mean, rstd, gamma, dx, H);
+    layernorm_bwd_dx_block_kernel<false><<<(unsigned)R, 256, 0, S(stream)>>>(dy, x, mean, rstd, gamma, dx, H, DropMask{});
     if (int e = launched("layernorm_bwd_dx_block")) return e;
   } else {
     layernorm_bwd_dx_kernel<<<(unsigned)cdiv(R, 8), 256, 0, S(stream)>>>(dy, x, mean, rstd, gamma, dx, R, H);
@@ -500,6 +623,56 @@ int mas_layernorm_backward(const float* dy, const float* x, const float* mean, c
     return launched("layernorm_bwd_param_final");
   }
   return MAS_OK;
+}
+int mas_layernorm_dropout_forward(const float* a, const float* gamma, const float* beta, const float* residual, float* y, float* mean,
+                                  float* rstd, int64_t R, int H, float eps, double p, const int64_t* seed, void* stream) {
+  MAS_REQUIRE(a && gamma && beta && y && mean && rstd && seed && R > 0 && R < (1ll << 31) && H > 0 && p >= 0.0 && p <= 1.0,
+              "layernorm_dropout_forward: bad arguments");
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  if (!(H % 4 == 0 && H <= 4096 && al16(a) && al16(y) && al16(gamma) && al16(beta) && (!residual || al16(residual))))
+    return fail(MAS_ERR_UNSUPPORTED, "layernorm_dropout_forward: needs H %% 4 == 0, H <= 4096 and 16-byte aligned operands");
+  layernorm_fwd_block_kernel<true><<<(unsigned)R, 256, 0, S(stream)>>>(a, gamma, beta, residual, y, mean, rstd, H, eps,
+                                                                       DropMask{seed, drop_threshold(p), drop_scale(p)});
+  return launched("layernorm_dropout_fwd_block");
+}
+int mas_layernorm_dropout_backward(const float* dy, const float* a, const float* mean, const float* rstd, const float* gamma, float* da,
+                                   float* dgamma, float* dbeta, int64_t R, int H, double p, const int64_t* seed, void* ws,
+                                   size_t ws_bytes, void* stream) {
+  MAS_REQUIRE(dy && a && mean && rstd && gamma && da && seed && R > 0 && R < (1ll << 31) && H > 0 && p >= 0.0 && p <= 1.0,
+              "layernorm_dropout_backward: bad arguments");
+  if (ws_bytes < mas_layernorm_ws_bytes(R, H)) return fail(MAS_ERR_WORKSPACE, "layernorm_dropout_backward: workspace too small");
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  if (!(H % 4 == 0 && H <= 4096 && al16(dy) && al16(a) && al16(gamma) && al16(da)))
+    return fail(MAS_ERR_UNSUPPORTED, "layernorm_dropout_backward: needs H %% 4 == 0, H <= 4096 and 16-byte aligned operands");
+  const DropMask dm{seed, drop_threshold(p), drop_scale(p)};
+  layernorm_bwd_dx_block_kernel<true><<<(unsigned)R, 256, 0, S(stream)>>>(dy, a, mean, rstd, gamma, da, H, dm);
+  if (int e = launched("layernorm_dropout_bwd_dx_block")) return e;
+  if (dgamma && dbeta) {
+    const int chunks = (int)cdiv(R, LN_ROWS);
+    layernorm_dropout_bwd_param_partial<<<dim3((unsigned)cdiv(H / 4, 32), chunks), dim3(32, 8), 0, S(stream)>>>(dy, a, mean, rstd, R, H, dm,
+                                                                                                                   (double*)ws);
+    if (int e = launched("layernorm_dropout_bwd_param_partial")) return e;
+    layernorm_bwd_param_final<<<(int)cdiv(H, 128), 128, 0, S(stream)>>>((const double*)ws, chunks, H, dgamma, dbeta);
+    return launched("layernorm_bwd_param_final");
+  }
+  return MAS_OK;
+}
+int mas_dropout(const float* x, const float* residual, float* y, int64_t n, double p, float scale, const int64_t* seed, void* stream) {
+  MAS_REQUIRE(y && seed && n > 0 && p >= 0.0 && p <= 1.0, "dropout: bad arguments");
+  auto al16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  const bool vec = (!x || al16(x)) && (!residual || al16(residual)) && al16(y);
+  const int64_t groups = (n + 3) >> 2;
+  dropout_kernel<<<(unsigned)std::min<int64_t>(cdiv(groups, 256), 8 * NUM_SMS), 256, 0, S(stream)>>>(
+      x, residual, y, n, DropMask{seed, drop_threshold(p), scale}, vec);
+  return launched("dropout");
+}
+int mas_softmax_causal_dropout_backward(const float* p, const float* dp, float* ds, int64_t mats, int rows, int cols, float scale,
+                                        double drop_p, const int64_t* seed, void* stream) {
+  MAS_REQUIRE(p && dp && ds && seed && mats > 0 && rows > 0 && cols >= rows && drop_p >= 0.0 && drop_p <= 1.0,
+              "softmax_causal_dropout_backward: bad arguments");
+  softmax_causal_dropout_bwd_kernel<<<(unsigned)cdiv(mats * rows, 8), 256, 0, S(stream)>>>(
+      p, dp, ds, mats * rows, rows, cols, scale, DropMask{seed, drop_threshold(drop_p), drop_scale(drop_p)});
+  return launched("softmax_causal_dropout_bwd");
 }
 int mas_gelu_forward(const float* x, float* y, int64_t n, void* stream) {
   gelu_fwd_kernel<<<ew_grid2(n), 256, 0, S(stream)>>>(x, y, n);

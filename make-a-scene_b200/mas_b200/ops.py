@@ -1317,11 +1317,52 @@ class BCELogitsFn(torch.autograd.Function):
 
 
 # ------------------------------------------------------------------------------------------------ tier 2: token transformer
-class LayerNormFn(torch.autograd.Function):
-    """nn.LayerNorm(hidden, eps) over the last dim, optionally fused with a residual add: LN(x) + residual."""
+def dropout_seed(device):
+    """The seed of one dropout site for one call (include/mas_b200.h, dropout): an int64 device scalar drawn from torch's
+    generator, so torch.manual_seed reproduces a training step and a captured CUDA graph draws new masks at each replay.
+    Every dropout seed of the package is drawn here."""
+    return torch.randint(-2 ** 63, 2 ** 63 - 1, (1,), dtype=torch.int64, device=device)
+
+
+def dropout_scale(p):
+    """Factor of the kept elements: 1 / (1 - p), 0 for p = 1 (nn.Dropout(p=1) zeroes everything)."""
+    return 1.0 / (1.0 - p) if p < 1.0 else 0.0
+
+
+class DropoutFn(torch.autograd.Function):
+    """nn.Dropout(p) in training mode, optionally fused with a residual add: residual + x * keep / (1 - p) (mas_dropout).
+    The backward regenerates the mask from the saved seed."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias, residual, eps):
+    def forward(ctx, x, p, residual=None):
+        _need_cuda(x)
+        x = x.contiguous()
+        res = residual.contiguous() if residual is not None else None
+        if res is not None and res.shape != x.shape:
+            raise ValueError("dropout residual: shape %s vs %s" % (tuple(res.shape), tuple(x.shape)))
+        seed = dropout_seed(x.device)
+        y = torch.empty_like(x)
+        L.call("mas_dropout", x, res, y, x.numel(), float(p), dropout_scale(p), seed)
+        ctx.save_for_backward(seed)
+        ctx.p, ctx.has_res = float(p), residual is not None
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        (seed,) = ctx.saved_tensors
+        dy = dy.contiguous()
+        dx = torch.empty_like(dy)
+        L.call("mas_dropout", dy, None, dx, dy.numel(), ctx.p, dropout_scale(ctx.p), seed)
+        return dx, None, (dy if ctx.has_res else None)
+
+
+class LayerNormFn(torch.autograd.Function):
+    """nn.LayerNorm(hidden, eps) over the last dim, optionally fused with a residual add: LN(x) + residual.
+    p > 0: LN(dropout_p(x)) + residual, the mask applied on load and regenerated in the backward (the sandwich LayerNorm fed
+    by a dropout site, transformer.py:114, 139, 183-208)."""
+
+    @staticmethod
+    def forward(ctx, x, weight, bias, residual, eps, p=0.0):
         _need_cuda(x)
         x = x.contiguous()
         H = x.shape[-1]
@@ -1330,14 +1371,20 @@ class LayerNormFn(torch.autograd.Function):
         mean = torch.empty(R, dtype=torch.float32, device=x.device)
         rstd = torch.empty_like(mean)
         res = residual.contiguous() if residual is not None else None
-        L.call("mas_layernorm_forward", x, weight, bias, res, y, mean, rstd, R, H, float(eps))
-        ctx.save_for_backward(x, weight, mean, rstd)
+        ctx.p = float(p)
+        if ctx.p > 0:
+            seed = dropout_seed(x.device)
+            L.call("mas_layernorm_dropout_forward", x, weight, bias, res, y, mean, rstd, R, H, float(eps), ctx.p, seed)
+            ctx.save_for_backward(x, weight, mean, rstd, seed)
+        else:
+            L.call("mas_layernorm_forward", x, weight, bias, res, y, mean, rstd, R, H, float(eps))
+            ctx.save_for_backward(x, weight, mean, rstd)
         ctx.has_res = residual is not None
         return y
 
     @staticmethod
     def backward(ctx, dy):
-        x, weight, mean, rstd = ctx.saved_tensors
+        x, weight, mean, rstd = ctx.saved_tensors[:4]
         dy = dy.contiguous()
         H = x.shape[-1]
         R = x.numel() // H
@@ -1345,8 +1392,12 @@ class LayerNormFn(torch.autograd.Function):
         dg = torch.empty_like(weight)
         db = torch.empty_like(weight)
         ws = L.workspace(L.query("mas_layernorm_ws_bytes", R, H), x.device)
-        L.call("mas_layernorm_backward", dy, x, mean, rstd, weight, dx, dg, db, R, H, ws, ws.numel())
-        return dx, dg, db, (dy if ctx.has_res else None), None
+        if ctx.p > 0:
+            L.call("mas_layernorm_dropout_backward", dy, x, mean, rstd, weight, dx, dg, db, R, H, ctx.p, ctx.saved_tensors[4], ws,
+                   ws.numel())
+        else:
+            L.call("mas_layernorm_backward", dy, x, mean, rstd, weight, dx, dg, db, R, H, ws, ws.numel())
+        return dx, dg, db, (dy if ctx.has_res else None), None, None
 
 
 class GeluFn(torch.autograd.Function):
@@ -1491,10 +1542,12 @@ def attn_causal_fused_on(S_, hd):
 class CausalAttentionFn(torch.autograd.Function):
     """softmax_causal((q / sqrt(hd)) k^T) v per (batch, head) from the fused qkv activation [B,S,3H]
     (transformer.py:77-103; head h owns columns h*hd..(h+1)*hd of each third). Every contraction is ONE launch over all
-    (batch element, head) pairs (two-level batch strides: the heads are column slices of the fused activation)."""
+    (batch element, head) pairs (two-level batch strides: the heads are column slices of the fused activation).
+    p > 0: attention dropout on the probabilities (transformer.py:90-91), ctx = (P * keep) v / (1 - p). P is kept undropped for
+    the backward and the mask is regenerated from the saved seed; no mask tensor is stored."""
 
     @staticmethod
-    def forward(ctx, qkv, heads):
+    def forward(ctx, qkv, heads, p=0.0):
         _need_cuda(qkv)
         qkv = qkv.contiguous()
         B, S_, H3 = qkv.shape
@@ -1505,23 +1558,37 @@ class CausalAttentionFn(torch.autograd.Function):
         P = torch.empty((B, heads, S_, S_), dtype=torch.float32, device=qkv.device)
         ctxv = torch.empty((B, S_, H), dtype=torch.float32, device=qkv.device)
         SS = S_ * S_
+        p = float(p)
+        seed = dropout_seed(qkv.device) if p > 0 else None
         if attn_causal_fused_on(S_, hd):
             # scores, causal softmax and P v in one kernel per (sequence, head, 128-query tile); P is written once for the backward
-            L.call("mas_attn_causal_forward", qkv, amax(qkv), P, ctxv, B, S_, heads, hd, alpha)
+            if p > 0:
+                L.call("mas_attn_causal_dropout_forward", qkv, amax(qkv), P, ctxv, B, S_, heads, hd, alpha, p, seed)
+            else:
+                L.call("mas_attn_causal_forward", qkv, amax(qkv), P, ctxv, B, S_, heads, hd, alpha)
         else:
             # S = alpha q k^T
             gemm2(qkv, (qkv, H), P, S_, S_, hd, B, heads, H3, H3, S_, S_ * H3, S_ * H3, heads * SS, hd, hd, SS, tb=True, alpha=alpha,
                   impl=impl, causal=3)
             L.call("mas_softmax_causal_forward", P, P, B * heads, S_, S_)
-            # ctx = P v
-            gemm2(P, (qkv, 2 * H), ctxv, S_, hd, S_, B, heads, S_, H3, H, heads * SS, S_ * H3, S_ * H, SS, hd, hd, impl=impl, causal=1)
-        ctx.save_for_backward(qkv, P)
-        ctx.heads = heads
+            # ctx = P v; with dropout (P * keep) v / (1 - p), the factor in the GEMM's alpha as in the fused kernel's epilogue
+            Pv, pv_alpha = P, 1.0
+            if p > 0:
+                Pv, pv_alpha = torch.empty_like(P), dropout_scale(p)
+                L.call("mas_dropout", P, None, Pv, P.numel(), p, 1.0, seed)
+            gemm2(Pv, (qkv, 2 * H), ctxv, S_, hd, S_, B, heads, S_, H3, H, heads * SS, S_ * H3, S_ * H, SS, hd, hd, alpha=pv_alpha,
+                  impl=impl, causal=1)
+        if p > 0:
+            ctx.save_for_backward(qkv, P, seed)
+        else:
+            ctx.save_for_backward(qkv, P)
+        ctx.heads, ctx.p = heads, p
         return ctxv
 
     @staticmethod
     def backward(ctx, dctx):
-        qkv, P = ctx.saved_tensors
+        qkv, P = ctx.saved_tensors[:2]
+        p = ctx.p
         dctx = dctx.contiguous()
         heads = ctx.heads
         B, S_, H3 = qkv.shape
@@ -1535,13 +1602,23 @@ class CausalAttentionFn(torch.autograd.Function):
         oq, op_, oc = S_ * H3, heads * SS, S_ * H
         # P and dS are lower-triangular (key <= query): the contractions skip the zero blocks (causal hints of mas_gemm_batched2)
         # dV = P^T dO ; dP = dO V^T (only the entries the softmax backward reads)
-        gemm2(P, dctx, (dqkv, 2 * H), S_, hd, S_, B, heads, S_, H, H3, op_, oc, oq, SS, hd, hd, ta=True, impl=impl, causal=2)
+        if p > 0:
+            # dV = (P * keep)^T dO / (1 - p), P * keep staged in the dP buffer before the dP GEMM overwrites it
+            seed = ctx.saved_tensors[2]
+            L.call("mas_dropout", P, None, dP, P.numel(), p, 1.0, seed)
+            gemm2(dP, dctx, (dqkv, 2 * H), S_, hd, S_, B, heads, S_, H, H3, op_, oc, oq, SS, hd, hd, ta=True, alpha=dropout_scale(p),
+                  impl=impl, causal=2)
+        else:
+            gemm2(P, dctx, (dqkv, 2 * H), S_, hd, S_, B, heads, S_, H, H3, op_, oc, oq, SS, hd, hd, ta=True, impl=impl, causal=2)
         gemm2(dctx, (qkv, 2 * H), dP, S_, S_, hd, B, heads, H, H3, S_, oc, oq, op_, hd, hd, SS, tb=True, impl=impl, causal=3)
-        L.call("mas_softmax_causal_backward", P, dP, dP, B * heads, S_, S_, alpha)     # dS (already times 1/sqrt(hd)), zeros above the diagonal
+        if p > 0:   # the dropout's backward (mask regenerated) and the softmax backward in one pass
+            L.call("mas_softmax_causal_dropout_backward", P, dP, dP, B * heads, S_, S_, alpha, p, seed)
+        else:
+            L.call("mas_softmax_causal_backward", P, dP, dP, B * heads, S_, S_, alpha)     # dS (already times 1/sqrt(hd)), zeros above the diagonal
         # dQ = dS K ; dK = dS^T Q
         gemm2(dP, (qkv, H), dqkv, S_, hd, S_, B, heads, S_, H3, H3, op_, oq, oq, SS, hd, hd, impl=impl, causal=1)
         gemm2(dP, qkv, (dqkv, H), S_, hd, S_, B, heads, S_, H3, H3, op_, oq, oq, SS, hd, hd, ta=True, impl=impl, causal=2)
-        return dqkv, None
+        return dqkv, None, None
 
 
 class CrossEntropyFn(torch.autograd.Function):

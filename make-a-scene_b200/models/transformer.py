@@ -2,7 +2,8 @@
 
 Same class names, constructor signatures, attribute names and state_dict keys (including the `transformer.mask`
 buffer). Supported configuration = the reference's defaults: cogview_pb_relax=True (a softmax-invariant shift),
-sandwich LayerNorm, no prescale, no rudalle_relax, dropout 0. The reference's `cache` / `use_cache` arguments raise
+sandwich LayerNorm, no prescale, no rudalle_relax; attention and residual dropout at any 0 <= p <= 1 (masks generated inside
+the kernels, include/mas_b200.h). The reference's `cache` / `use_cache` arguments raise
 (its cache path is broken: transformer.py:73 vs :181, SURVEY.md 3.5); autoregressive sampling with a KV cache and
 classifier-free guidance is `MakeAScene.generate` (new API, SURVEY.md 8f-3: specified by the non-cached forward).
 Anything else raises — there is no fallback path.
@@ -21,13 +22,32 @@ def gelu(x):
 
 
 class LayerNorm(nn.LayerNorm):
-    def forward(self, x, residual=None):
-        return ops.LayerNormFn.apply(x, self.weight, self.bias, residual, self.eps)
+    def forward(self, x, residual=None, p=0.0):
+        """LN(x) + residual; p > 0: LN(dropout_p(x)) + residual in one kernel (the sandwich LayerNorm after a dropout site)."""
+        return ops.LayerNormFn.apply(x, self.weight, self.bias, residual, self.eps, p)
 
 
 class Linear(nn.Linear):
     def forward(self, x):
         return ops.LinearFn.apply(x, self.weight, self.bias)
+
+
+def _drop_p(mod):
+    """The probability a dropout holder (nn.Dropout) applies now: its .p in training mode, 0 in eval mode."""
+    if not mod.training:
+        return 0.0
+    p = float(mod.p)
+    if not 0.0 <= p <= 1.0:
+        raise ValueError("dropout probability has to be between 0 and 1, but got %r" % (mod.p,))
+    return p
+
+
+def _dropout(x, mod, residual=None):
+    """residual + dropout(x) with the holder's current probability (the torch add when nothing is dropped)."""
+    p = _drop_p(mod)
+    if p > 0:
+        return ops.DropoutFn.apply(x, p, residual)
+    return x if residual is None else residual + x
 
 
 class SelfAttention(nn.Module):
@@ -42,14 +62,17 @@ class SelfAttention(nn.Module):
         self.out_drop = nn.Dropout(out_dropout_prob)
         self.cogview_pb_relax = cogview_pb_relax
         self.rudalle_relax = rudalle_relax
-        if rudalle_relax or attn_dropout_prob or out_dropout_prob:
-            raise NotImplementedError("rudalle_relax / dropout>0 have no kernel (reference defaults are off)")
+        if rudalle_relax:
+            raise NotImplementedError("rudalle_relax has no kernel (reference default is off)")
 
     def forward(self, x, mask=None, use_cache=False, cache=None):
         if use_cache or cache is not None:
             raise NotImplementedError("KV cache: the reference path is broken (transformer.py:73 vs :181); no kernel")
-        ctx = ops.CausalAttentionFn.apply(self.qkv(x), self.num_attn_heads)
-        return self.out_proj(ctx), None
+        return _dropout(self.project(x), self.out_drop), None
+
+    def project(self, x):
+        """out_proj(attention) with attention dropout, before out_drop (TransformerLayer fuses out_drop into the next kernel)."""
+        return self.out_proj(ops.CausalAttentionFn.apply(self.qkv(x), self.num_attn_heads, _drop_p(self.attn_drop)))
 
 
 class MLP(nn.Module):
@@ -59,10 +82,14 @@ class MLP(nn.Module):
         self.lin2 = Linear(4 * hidden_dim, hidden_dim)
         self.dropout = nn.Dropout(dropout_prob)
         self.rudalle_relax = rudalle_relax
-        if rudalle_relax or dropout_prob:
-            raise NotImplementedError("rudalle_relax / dropout>0 have no kernel")
+        if rudalle_relax:
+            raise NotImplementedError("rudalle_relax has no kernel")
 
     def forward(self, x):
+        return _dropout(self.project(x), self.dropout)
+
+    def project(self, x):
+        """lin2(gelu(lin1(x))), before the dropout (TransformerLayer fuses it into the next kernel)."""
         return self.lin2(gelu(self.lin1(x)))
 
 
@@ -88,16 +115,18 @@ class TransformerLayer(nn.Module):
     def forward(self, x, mask=None, cache=None, use_cache=False, mlp_cache=False):
         if use_cache or cache is not None:
             raise NotImplementedError("KV cache has no kernel")
-        attn_out, _ = self.attn(self.ln_in(x))
+        # out_drop and mlp.dropout act where the reference applies them (transformer.py:114, 139), fused into the kernel that
+        # consumes their output: the sandwich LayerNorm (mask applied on load) or, without it, the residual add (mas_dropout)
+        attn_out = self.attn.project(self.ln_in(x))
         if self.cogview_sandwich_layernorm:
-            x = self.first_ln_sandwich(attn_out, residual=x)      # x + LN(attn_out), fused
+            x = self.first_ln_sandwich(attn_out, residual=x, p=_drop_p(self.attn.out_drop))      # x + LN(dropout(attn_out)), fused
         else:
-            x = x + attn_out
-        mlp_out = self.mlp(self.ln_out(x))
+            x = _dropout(attn_out, self.attn.out_drop, residual=x)
+        mlp_out = self.mlp.project(self.ln_out(x))
         if self.cogview_sandwich_layernorm:
-            x = self.second_ln_sandwich(mlp_out, residual=x)
+            x = self.second_ln_sandwich(mlp_out, residual=x, p=_drop_p(self.mlp.dropout))
         else:
-            x = x + mlp_out
+            x = _dropout(mlp_out, self.mlp.dropout, residual=x)
         return x, None
 
 
@@ -220,7 +249,10 @@ class _GraphedDecoder:
 
 class MakeAScene(nn.Module):
     def __init__(self, num_layers, hidden_dim, num_attn_heads, image_vocab_size, seg_vocab_size, text_vocab_size,
-                 image_tokens_per_dim, seg_tokens_per_dim, text_length):
+                 image_tokens_per_dim, seg_tokens_per_dim, text_length, attn_dropout_prob=0.0, out_dropout_prob=0.0):
+        """The reference's arguments, plus the dropout probabilities of every layer's attention probabilities
+        (attn_dropout_prob) and of its attention and MLP outputs (out_dropout_prob), passed to Transformer; the reference's
+        MakeAScene leaves both at 0, which the defaults keep."""
         super().__init__()
         self.image_tokens_per_dim = image_tokens_per_dim
         self.seg_tokens_per_dim = seg_tokens_per_dim
@@ -230,7 +262,8 @@ class MakeAScene(nn.Module):
         self.total_length = self.text_length + self.seg_length + self.image_length
         self.text_vocab_size = text_vocab_size
         self.hidden_dim = hidden_dim
-        self.transformer = Transformer(num_layers, hidden_dim, num_attn_heads, image_tokens_per_dim, seg_tokens_per_dim, text_length)
+        self.transformer = Transformer(num_layers, hidden_dim, num_attn_heads, image_tokens_per_dim, seg_tokens_per_dim, text_length,
+                                       attn_dropout_prob, out_dropout_prob)
         self.image_token_embedding = nn.Embedding(image_vocab_size, hidden_dim)
         self.seg_token_embedding = nn.Embedding(seg_vocab_size, hidden_dim)
         self.text_token_embedding = nn.Embedding(text_vocab_size, hidden_dim)
@@ -300,7 +333,7 @@ class MakeAScene(nn.Module):
             ops.kv_append(qkv, kc[li], vc[li], 0)
             a = layer.attn.out_proj(ops.CausalAttentionFn.apply(qkv, heads))
             x = layer.first_ln_sandwich(a, residual=x) if layer.cogview_sandwich_layernorm else x + a
-            m = layer.mlp(layer.ln_out(x))
+            m = layer.mlp.project(layer.ln_out(x))
             x = layer.second_ln_sandwich(m, residual=x) if layer.cogview_sandwich_layernorm else x + m
         return x[:, -1].contiguous()
 
@@ -378,7 +411,9 @@ class MakeAScene(nn.Module):
         are cached once per prompt, and each decode step reads a prompt's prefix once for its group of samples
         (mas_attn_decode_shared_append); the row count R = B*n (2B*n with guidance) still selects fp32 or fp16 decoding.
         use_graphs: replay each position's decode step from a CUDA graph (captured at first use and kept on the module for
-        the same row count; captured again after any parameter changes, in place or by replaced storage)."""
+        the same row count; captured again after any parameter changes, in place or by replaced storage).
+        Dropout is never applied here, in train mode as in eval mode: the prefix pass and the decode steps call the layers'
+        kernels directly, not the dropout sites, so a model trained with dropout samples as its eval-mode self."""
         B = text_tokens.shape[0]
         dev = text_tokens.device
         n = num_samples

@@ -2,7 +2,7 @@
 128 text + 256 segmentation + 256 image tokens, 8192-code image vocabulary; random-init weights, synthetic tokens):
 forward + cross-entropy over the image tokens + backward (train.py:136-153; no optimizer), CUDA-event timed.
 One JSON line; beside bench.py's headline (tier 2, SURVEY.md 8f-2).
-Usage: python tools/bench_transformer.py [--batch B] [--steps K] [--warmup W] [--layers L]"""
+Usage: python tools/bench_transformer.py [--batch B] [--steps K] [--warmup W] [--layers L] [--dropout P]"""
 import argparse
 import json
 import os
@@ -19,6 +19,7 @@ ap.add_argument("--batch", type=int, default=8)
 ap.add_argument("--steps", type=int, default=4)
 ap.add_argument("--warmup", type=int, default=2)
 ap.add_argument("--layers", type=int, default=24)
+ap.add_argument("--dropout", type=float, default=0.0, help="attention and residual dropout probability (both)")
 ap.add_argument("--profile", action="store_true", help="per-entry-point CUDA-event times of one extra step (stderr)")
 ap.add_argument("--torch-ce", action="store_true", help="F.cross_entropy on the logits instead of MakeAScene.loss (A/B of the fused entry)")
 args = ap.parse_args()
@@ -26,7 +27,7 @@ dev = torch.device("cuda:0")
 torch.manual_seed(0)
 cfg = dict(num_layers=args.layers, hidden_dim=1024, num_attn_heads=16, image_vocab_size=8192, seg_vocab_size=1024, text_vocab_size=49408,
            image_tokens_per_dim=16, seg_tokens_per_dim=16, text_length=128)
-m = MakeAScene(**cfg).to(dev).train()
+m = MakeAScene(**cfg, attn_dropout_prob=args.dropout, out_dropout_prob=args.dropout).to(dev).train()
 m.device = dev
 B = args.batch
 g = torch.Generator().manual_seed(1234)
@@ -72,6 +73,6 @@ print(json.dumps({"metric": "token transformer training step (fwd + cross-entrop
                   "unit": "tokens/s", "batch": B, "seq_len": S, "ms_per_step": sec * 1e3, "loss": float(loss),
                   "model_tflops": 3 * (lin + att) * B / sec / 1e12, "gpu_launches_per_step": (_lib.launch_count() - l0) // args.steps,
                   "tensor_core_launches_per_step": (_lib.tc_launch_count() - t0) // args.steps,
-                  "peak_mem_gb": torch.cuda.max_memory_allocated() / 1e9,
+                  "peak_mem_gb": torch.cuda.max_memory_allocated() / 1e9, "dropout": args.dropout,
                   "attention": "fused core (attn_causal_fwd)" if os.environ.get("MAS_ATTN_FUSED", "1") != "0" else "GEMM / softmax / GEMM",
                   "loss_entry": "F.cross_entropy (torch)" if args.torch_ce else "MakeAScene.loss (mas_ce_*)", "config": cfg}))
