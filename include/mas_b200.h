@@ -74,6 +74,17 @@ int mas_copy_strided(const float* x, mas_tensor4 xs, float* y, mas_tensor4 ys, v
 int mas_nchw_to_nhwc_pad(const float* x_nchw, float* y_nhwc, int N, int C, int CP, int H, int W, void* stream);
 int mas_scale_by(const float* x, const float* g, float* y, int64_t n, void* stream);
 
+/* Compact scene map: labels [N, 4, H, W] uint8, contiguous NCHW, four planes per pixel in the order of the reference's
+ * PreprocessedDataset.load_segmentation (Data/dataset_preprocessor.py:61-86):
+ *   plane 0 panoptic  seg_panoptic + 1: 0 = none, k = 1..133 sets channel k - 1
+ *   plane 1 human     seg_human + 1:    0 = none, k = 1..20  sets channel 132 + k
+ *   plane 2 face      seg_face:         0 = none, k = 1..5   sets channel 152 + k
+ *   plane 3 edges     edges_panoptic + edges_human: channel 158 = the count, 0..2
+ * A code outside its plane's range sets nothing (any byte value is safe to pass).  mas_scene_expand writes the dense map
+ * [N, C, H, W] (any strides, ys.c >= 159; channels >= 159 zero): NCHW for the 159-channel consumers, or the padded
+ * channels-last operand mas_nchw_to_nhwc_pad builds from the dense map - the same values bit for bit. */
+int mas_scene_expand(const uint8_t* labels, int N, int H, int W, float* y, mas_tensor4 ys, void* stream);
+
 /* ---- GroupNorm(32, C, eps=1e-6) + optional SiLU — Normalize / nonlinearity, modules.py:35-41 ------
  * x, y: [N, HW, C] NHWC.  mean/rstd: [N*G].  silu=1 fuses x*sigmoid(x) (modules.py:122,126,194-196).
  * round_tf32=1 rounds y to TF32 (round-to-nearest) so that a following tensor-core contraction sees
@@ -578,6 +589,13 @@ int mas_bce_cl_forward(const float* logits, const float* target_nchw, const floa
                        int W, float* loss_out, void* ws, size_t ws_bytes, void* stream);
 int mas_bce_cl_backward(const float* logits, const float* target_nchw, const float* pos_weight, const float* g, int N, int C,
                         int CP, int H, int W, float* grad, void* stream);
+/* mas_bce_cl_* with C = 159 and the target read from a compact scene map (labels [N, 4, H, W] uint8, see mas_scene_expand)
+ * instead of the dense NCHW map: loss and gradient bit-identical to mas_bce_cl_* on the expanded target.  Workspace:
+ * mas_bce_cl_ws_bytes(N, H, W). */
+int mas_bce_scene_forward(const float* logits, const uint8_t* labels, const float* pos_weight, int N, int CP, int H, int W,
+                          float* loss_out, void* ws, size_t ws_bytes, void* stream);
+int mas_bce_scene_backward(const float* logits, const uint8_t* labels, const float* pos_weight, const float* g, int N, int CP,
+                           int H, int W, float* grad, void* stream);
 
 
 /* ---- LPIPS perceptual loss (losses/lpips.py; csrc/lpips.cu) ------------------------------------------------------------

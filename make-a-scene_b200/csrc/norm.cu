@@ -724,6 +724,38 @@ __global__ void __launch_bounds__(256) nchw_to_nhwc_pad_kernel(const float* __re
     y[base + i] = c < C ? tile[c * 33 + px] : 0.f;
   }
 }
+
+// Compact scene maps (include/mas_b200.h): the dense 159-channel map's channel c is a function of one label plane's code.
+// One-hot planes: code k sets channel base + k - 1 (0 = none); edges: channel 158 holds the count.  A code outside its
+// plane's range sets nothing; channels >= 159 (tile padding) are zero.
+constexpr int SCENE_C = 159;
+__device__ __forceinline__ int scene_plane(int c) { return c < 133 ? 0 : c < 153 ? 1 : c < 158 ? 2 : 3; }
+__device__ __forceinline__ float scene_value(int c, unsigned code) {
+  if (c < 133) return code == (unsigned)c + 1u ? 1.f : 0.f;
+  if (c < 153) return code == (unsigned)c - 132u ? 1.f : 0.f;
+  if (c < 158) return code == (unsigned)c - 152u ? 1.f : 0.f;
+  return c == 158 && code <= 2u ? (float)code : 0.f;
+}
+
+// Block = up to 32 pixels of one image row: their 4 label bytes are staged in shared memory, the output is written
+// pixel-major (channels-last: one contiguous 32 x C block) or channel-major (NCHW: 128-byte rows), per the layout.
+__global__ void __launch_bounds__(256) scene_expand_kernel(const uint8_t* __restrict__ lab, int H, int W, float* __restrict__ y,
+                                                           mas_tensor4 ys) {
+  __shared__ uint8_t s[4 * 32];
+  const int w0 = blockIdx.x * 32, h = blockIdx.y, n = blockIdx.z;
+  const int npx = min(32, W - w0), C = (int)ys.c;
+  const int p = threadIdx.x >> 5, px = threadIdx.x & 31;
+  if (threadIdx.x < 128 && px < npx) s[threadIdx.x] = __ldg(lab + (((size_t)n * 4 + p) * H + h) * W + w0 + px);
+  __syncthreads();
+  float* yb = y + n * ys.sn + h * ys.sh + w0 * ys.sw;
+  const bool cl = ys.sc == 1;
+  for (int i = threadIdx.x; i < npx * C; i += 256) {
+    int q, c;
+    if (cl) { q = i / C; c = i - q * C; }
+    else { c = i / npx; q = i - c * npx; }
+    yb[q * ys.sw + c * ys.sc] = scene_value(c, s[scene_plane(c) * 32 + q]);
+  }
+}
 __global__ void scale_by_kernel(const float* __restrict__ x, const float* __restrict__ g, float* __restrict__ y, int64_t n) {
   const float s = g[0];
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) y[i] = x[i] * s;
@@ -777,18 +809,40 @@ __global__ void __launch_bounds__(256) bce_kernel(const float* __restrict__ lg, 
   }
   if (threadIdx.x == 0) part[blockIdx.x] = red[0];
 }
+// Target fetches of bce_cl_kernel for the 32 pixels of one image row a block covers: stage() fills the block's shared memory,
+// at(c, px) is the target of channel c < C at pixel px.
+struct DenseTarget {   // NCHW fp32 target: read plane by plane (128-byte rows), transposed through shared memory as [C][33]
+  const float* __restrict__ tg;
+  static size_t smem(int C) { return (size_t)C * 33 * sizeof(float); }
+  __device__ void stage(float* tile, int n, int C, int H, int W, int w0, int h) const {
+    const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    for (int c = ty; c < C; c += 8) tile[c * 33 + tx] = __ldg(tg + (((size_t)n * C + c) * H + h) * W + w0 + tx);
+  }
+  __device__ float at(const float* tile, int c, int px) const { return tile[c * 33 + px]; }
+};
+struct SceneTarget {   // compact scene map [N, 4, H, W] uint8: 4 x 32 label bytes staged, the target computed (C = 159)
+  const uint8_t* __restrict__ lab;
+  static size_t smem(int) { return 4 * 32; }
+  __device__ void stage(float* tile, int n, int, int H, int W, int w0, int h) const {
+    if (threadIdx.x < 128)
+      reinterpret_cast<uint8_t*>(tile)[threadIdx.x] = __ldg(lab + (((size_t)n * 4 + (threadIdx.x >> 5)) * H + h) * W + w0 + (threadIdx.x & 31));
+  }
+  __device__ float at(const float* tile, int c, int px) const {
+    return scene_value(c, reinterpret_cast<const uint8_t*>(tile)[scene_plane(c) * 32 + px]);
+  }
+};
+
 // Same loss for the layouts the VQ-SEG step actually has: logits channels-last with pitch CP >= C (the padded output of
-// the decoder's last convolution), target NCHW (the data loader's one-hot maps).  Block = 32 consecutive pixels of one image
-// row: the target tile is read plane by plane (128-byte rows) and transposed through shared memory, the logits / gradient
-// tile is one contiguous 32 x CP block.  MODE 0: loss partials.  MODE 1: gradient g * gscale * dl/dx (pad channels get 0).
-template <int MODE>
-__global__ void __launch_bounds__(256) bce_cl_kernel(const float* __restrict__ lg, const float* __restrict__ tg, const float* __restrict__ pw,
+// the decoder's last convolution), target NCHW (the data loader's one-hot maps) or compact scene labels.  Block = 32
+// consecutive pixels of one image row: the target is staged by the fetch, the logits / gradient tile is one contiguous
+// 32 x CP block.  MODE 0: loss partials.  MODE 1: gradient g * gscale * dl/dx (pad channels get 0).
+template <int MODE, class Target>
+__global__ void __launch_bounds__(256) bce_cl_kernel(const float* __restrict__ lg, Target tg, const float* __restrict__ pw,
                                                      int C, int CP, int H, int W, const float* __restrict__ g, float gscale,
                                                      float* __restrict__ grad, double* __restrict__ part) {
-  extern __shared__ float tile[];   // [C][33]
+  extern __shared__ float tile[];
   const int w0 = blockIdx.x * 32, h = blockIdx.y, n = blockIdx.z;
-  const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
-  for (int c = ty; c < C; c += 8) tile[c * 33 + tx] = __ldg(tg + (((size_t)n * C + c) * H + h) * W + w0 + tx);
+  tg.stage(tile, n, C, H, W, w0, h);
   __syncthreads();
   const size_t base = (((size_t)n * H + h) * W + w0) * CP;
   const float gs = MODE == 1 ? gscale * (g ? g[0] : 1.f) : 0.f;
@@ -796,7 +850,7 @@ __global__ void __launch_bounds__(256) bce_cl_kernel(const float* __restrict__ l
   for (int i = threadIdx.x; i < 32 * CP; i += 256) {
     const int px = i / CP, c = i - px * CP;
     if (c < C) {
-      const float x = __ldg(lg + base + i), t = tile[c * 33 + px];
+      const float x = __ldg(lg + base + i), t = tg.at(tile, c, px);
       const float coef = 1.0f + (__ldg(pw + c) - 1.0f) * t;
       if (MODE == 0) {
         const float sp = fmaxf(-x, 0.f) + log1pf(expf(-fabsf(x)));
@@ -836,6 +890,26 @@ __global__ void sum_final_kernel(const double* __restrict__ part, int n, double 
 static inline int ew_grid(int64_t n, int threads = 256) {
   int64_t b = cdiv(n, threads);
   return (int)(b < NUM_SMS * 16 ? (b < 1 ? 1 : b) : NUM_SMS * 16);
+}
+
+// launches of bce_cl_kernel shared by the dense (mas_bce_cl_*) and compact (mas_bce_scene_*) targets
+template <class Target>
+static int bce_cl_forward(const float* logits, Target tg, const float* pos_weight, int N, int C, int CP, int H, int W, float* loss_out,
+                          void* ws, size_t ws_bytes, void* stream) {
+  if (ws_bytes < mas_bce_cl_ws_bytes(N, H, W)) return fail(MAS_ERR_WORKSPACE, "bce_cl_forward: workspace too small");
+  const int nb = N * H * (W / 32);
+  bce_cl_kernel<0><<<dim3(W / 32, H, N), 256, Target::smem(C), S(stream)>>>(logits, tg, pos_weight, C, CP, H, W, nullptr, 0.f, nullptr,
+                                                                             (double*)ws);
+  if (int e = launched("bce_cl_loss")) return e;
+  sum_final_kernel<<<1, 256, 0, S(stream)>>>((const double*)ws, nb, 1.0 / ((double)N * C * H * W), loss_out);
+  return launched("bce_final");
+}
+template <class Target>
+static int bce_cl_backward(const float* logits, Target tg, const float* pos_weight, const float* g, int N, int C, int CP, int H, int W,
+                           float* grad, void* stream) {
+  bce_cl_kernel<1><<<dim3(W / 32, H, N), 256, Target::smem(C), S(stream)>>>(logits, tg, pos_weight, C, CP, H, W, g,
+                                                                             (float)(1.0 / ((double)N * C * H * W)), grad, nullptr);
+  return launched("bce_cl_grad");
 }
 
 }  // namespace mas
@@ -1060,6 +1134,12 @@ int mas_nchw_to_nhwc_pad(const float* x_nchw, float* y_nhwc, int N, int C, int C
   nchw_to_nhwc_pad_kernel<<<dim3((unsigned)cdiv(W, 32), H, N), 256, (size_t)C * 33 * sizeof(float), S(stream)>>>(x_nchw, y_nhwc, C, CP, H, W);
   return launched("nchw_to_nhwc_pad");
 }
+int mas_scene_expand(const uint8_t* labels, int N, int H, int W, float* y, mas_tensor4 ys, void* stream) {
+  MAS_REQUIRE(labels && y && N > 0 && H > 0 && W > 0 && ys.n == N && ys.h == H && ys.w == W && ys.c >= SCENE_C,
+              "scene_expand: bad arguments");
+  scene_expand_kernel<<<dim3((unsigned)cdiv(W, 32), H, N), 256, 0, S(stream)>>>(labels, H, W, y, ys);
+  return launched("scene_expand");
+}
 int mas_scale_by(const float* x, const float* g, float* y, int64_t n, void* stream) {
   scale_by_kernel<<<ew_grid(n), 256, 0, S(stream)>>>(x, g, y, n);
   return launched("scale_by");
@@ -1078,20 +1158,24 @@ size_t mas_bce_cl_ws_bytes(int N, int H, int W) { return (size_t)N * H * cdiv(W,
 int mas_bce_cl_forward(const float* logits, const float* target_nchw, const float* pos_weight, int N, int C, int CP, int H, int W,
                        float* loss_out, void* ws, size_t ws_bytes, void* stream) {
   MAS_REQUIRE(logits && target_nchw && pos_weight && loss_out && N > 0 && C > 0 && CP >= C && W % 32 == 0, "bce_cl_forward: bad arguments");
-  if (ws_bytes < mas_bce_cl_ws_bytes(N, H, W)) return fail(MAS_ERR_WORKSPACE, "bce_cl_forward: workspace too small");
-  const int nb = N * H * (W / 32);
-  bce_cl_kernel<0><<<dim3(W / 32, H, N), 256, (size_t)C * 33 * sizeof(float), S(stream)>>>(logits, target_nchw, pos_weight, C, CP, H, W, nullptr,
-                                                                                          0.f, nullptr, (double*)ws);
-  if (int e = launched("bce_cl_loss")) return e;
-  sum_final_kernel<<<1, 256, 0, S(stream)>>>((const double*)ws, nb, 1.0 / ((double)N * C * H * W), loss_out);
-  return launched("bce_final");
+  return bce_cl_forward(logits, DenseTarget{target_nchw}, pos_weight, N, C, CP, H, W, loss_out, ws, ws_bytes, stream);
 }
 int mas_bce_cl_backward(const float* logits, const float* target_nchw, const float* pos_weight, const float* g, int N, int C, int CP,
                         int H, int W, float* grad, void* stream) {
   MAS_REQUIRE(logits && target_nchw && pos_weight && grad && N > 0 && C > 0 && CP >= C && W % 32 == 0, "bce_cl_backward: bad arguments");
-  bce_cl_kernel<1><<<dim3(W / 32, H, N), 256, (size_t)C * 33 * sizeof(float), S(stream)>>>(
-      logits, target_nchw, pos_weight, C, CP, H, W, g, (float)(1.0 / ((double)N * C * H * W)), grad, nullptr);
-  return launched("bce_cl_grad");
+  return bce_cl_backward(logits, DenseTarget{target_nchw}, pos_weight, g, N, C, CP, H, W, grad, stream);
+}
+int mas_bce_scene_forward(const float* logits, const uint8_t* labels, const float* pos_weight, int N, int CP, int H, int W,
+                          float* loss_out, void* ws, size_t ws_bytes, void* stream) {
+  MAS_REQUIRE(logits && labels && pos_weight && loss_out && N > 0 && H > 0 && CP >= SCENE_C && W > 0 && W % 32 == 0,
+              "bce_scene_forward: bad arguments");
+  return bce_cl_forward(logits, SceneTarget{labels}, pos_weight, N, SCENE_C, CP, H, W, loss_out, ws, ws_bytes, stream);
+}
+int mas_bce_scene_backward(const float* logits, const uint8_t* labels, const float* pos_weight, const float* g, int N, int CP, int H,
+                           int W, float* grad, void* stream) {
+  MAS_REQUIRE(logits && labels && pos_weight && grad && N > 0 && H > 0 && CP >= SCENE_C && W > 0 && W % 32 == 0,
+              "bce_scene_backward: bad arguments");
+  return bce_cl_backward(logits, SceneTarget{labels}, pos_weight, g, N, SCENE_C, CP, H, W, grad, stream);
 }
 
 size_t mas_bce_ws_bytes(mas_tensor4 ls) { return (size_t)cdiv(ls.n * ls.h * ls.w * ls.c, BCE_CHUNK) * sizeof(double) + 64; }

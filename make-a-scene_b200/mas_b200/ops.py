@@ -11,6 +11,7 @@ import torch
 import torch.distributed as dist
 
 from . import _lib as L
+from . import scene
 
 GN_GROUPS = 32
 GN_EPS = 1e-6
@@ -49,12 +50,12 @@ def get_impl() -> int:
     return _cfg["impl"]
 
 
-def _need_cuda(x):
+def _need_cuda(x, dtype=torch.float32):
     if not x.is_cuda:
         raise RuntimeError("make-a-scene_b200 kernels run on CUDA (sm_90a) only; got a %s tensor — there is no CPU path"
                            % x.device.type)
-    if x.dtype != torch.float32:
-        raise RuntimeError("make-a-scene_b200 kernels take float32 tensors, got %s" % x.dtype)
+    if x.dtype != dtype:
+        raise RuntimeError("make-a-scene_b200 kernels take %s tensors here, got %s" % (dtype, x.dtype))
 
 
 def nhwc(x: torch.Tensor) -> torch.Tensor:
@@ -587,12 +588,23 @@ def _is_dense_nhwc(t):
 class Conv3x3Fn(torch.autograd.Function):
     """nn.Conv2d 3x3 / Downsample / Upsample (modules.py:44-81,93-104) with optional fused residual add.
     3-channel edge layers (conv_in reading the NCHW image, conv_out writing the NCHW reconstruction) use the
-    direct fp32 edge kernels; everything else goes through conv3x3_raw (wgmma or SIMT)."""
+    direct fp32 edge kernels; everything else goes through conv3x3_raw (wgmma or SIMT).
+    x may be a compact scene map (uint8 [N, 4, H, W], mas_b200.scene) for a 159-input-channel weight (VQ-SEG's conv_in):
+    it is expanded on the device into the operand the dense map of that shape would have become, on the same route, and
+    only the labels are kept for the weight gradient (no input gradient: the input is integer)."""
 
     @staticmethod
     def forward(ctx, x, weight, bias, residual, mode, out_nchw):
-        _need_cuda(x)
         cout, cin = weight.shape[0], weight.shape[1]
+        labels = None
+        if x.dtype == torch.uint8:
+            if cin != scene.CHANNELS or mode != L.CONV_S1 or residual is not None:
+                raise RuntimeError("a compact scene map feeds only a 3x3 stride-1 convolution with %d input channels and no "
+                                   "residual (got weight %s, mode %d)" % (scene.CHANNELS, tuple(weight.shape), mode))
+            # a stride-1, 159-input-channel layer takes either the padded tensor route or the general one below
+            labels = x = scene_labels(x)
+        else:
+            _need_cuda(x)
         n, _, h, w = x.shape
         edge = 0
         tc_pad_in = (mode == L.CONV_S1 and f16_operands() and residual is None and cout % 128 == 0 and h % 16 == 0 and w % 8 == 0
@@ -613,7 +625,7 @@ class Conv3x3Fn(torch.autograd.Function):
             # tensor-core kernels
             edge = 4
             cp = _round_up(cin, 32)          # 32: the weight-gradient kernel's input-channel tile
-            x = pad_nhwc(x, cp)
+            x = pad_nhwc(x, cp) if labels is None else scene_expand(labels, cp)
             y = conv3x3_raw(x, _padded(weight, (cout, cp, 3, 3)), bias, None, L.CONV_S1)
         elif (mode == L.CONV_S1 and f16_operands() and residual is None and cout % 128 != 0 and cout > 128 and cin % 16 == 0
               and h % 16 == 0 and w % 8 == 0):
@@ -647,9 +659,11 @@ class Conv3x3Fn(torch.autograd.Function):
             y = conv3x3_raw(x4, w9, bias, None, L.CONV_S1)
             x = x4   # saved for the weight gradient (the 4C-channel view carries the same data)
         else:
-            y = conv3x3_raw(x, weight, bias, residual, mode, out_nchw, prepack=ctx.needs_input_grad[0])
-        ctx.save_for_backward(x, weight)
+            y = conv3x3_raw(x if labels is None else scene_expand(labels), weight, bias, residual, mode, out_nchw,
+                            prepack=ctx.needs_input_grad[0])
+        ctx.save_for_backward(x if labels is None else labels, weight)
         ctx.mode, ctx.has_bias, ctx.has_res, ctx.edge = mode, bias is not None, residual is not None, edge
+        ctx.scene = labels is not None     # x saved as the labels: re-expanded for the weight gradient
         return y
 
 
@@ -680,10 +694,12 @@ class Conv3x3Fn(torch.autograd.Function):
                 ws = L.workspace(L.query("mas_edge_wgrad_ws_bytes", cin), x.device)
                 L.call("mas_edge_small_cout_wgrad", x, L.t4(x), dy, L.t4(dy), dw, db, ws, ws.numel())
         elif ctx.edge == 4:
-            cp = x.shape[1]                                              # x is the zero-padded channels-last copy
+            cp = _round_up(cin, 32)                    # x: the zero-padded channels-last copy, or the labels it was expanded from
             dy = nhwc(dy)
             am = amax_of(dy)
             if want_w:
+                if ctx.scene:
+                    x = scene_expand(x, cp)
                 dwp, db = conv3x3_wgrad_raw(x, dy, cout, cp, L.CONV_S1, ctx.has_bias, dy_amax=am)
                 dw = dwp[:, :cin].contiguous()
             if ctx.needs_input_grad[0]:
@@ -723,6 +739,8 @@ class Conv3x3Fn(torch.autograd.Function):
             if ctx.needs_input_grad[0]:
                 dx = conv3x3_dgrad_raw(dy, weight, ctx.mode, am)
             if want_w:
+                if ctx.scene:
+                    x = scene_expand(x)
                 dw, db = conv3x3_wgrad_raw(x, dy, cout, cin, ctx.mode, ctx.has_bias, dy_amax=am)
         if not ctx.has_bias:
             db = None
@@ -1258,6 +1276,29 @@ def pad_nhwc(x, cp):
     return base.permute(0, 3, 1, 2)
 
 
+def scene_labels(t, n=None, h=None, w=None):
+    """A compact scene map (mas_b200.scene) checked for the kernels: a [N, 4, H, W] uint8 CUDA tensor, made contiguous
+    NCHW; n, h, w: the extents it must have when given."""
+    if t.dim() != 4 or t.shape[1] != scene.PLANES or (n is not None and (t.shape[0], t.shape[2], t.shape[3]) != (n, h, w)):
+        raise RuntimeError("expected a compact scene map [N, %d, H, W]%s, got shape %s"
+                           % (scene.PLANES, "" if n is None else " with N, H, W = %d, %d, %d" % (n, h, w), tuple(t.shape)))
+    _need_cuda(t, torch.uint8)
+    return t.contiguous()
+
+
+def scene_expand(labels, cp=None):
+    """Compact scene map [N, 4, H, W] uint8 -> the dense 159-channel fp32 map load_segmentation builds from the same labels:
+    contiguous NCHW (cp None), or logical [N, cp, H, W] in dense channels-last memory with channels >= 159 zero (what
+    pad_nhwc makes of the dense map)."""
+    n, _, h, w = labels.shape
+    if cp is None:
+        y = torch.empty((n, scene.CHANNELS, h, w), dtype=torch.float32, device=labels.device)
+    else:
+        y = torch.empty((n, h, w, cp), dtype=torch.float32, device=labels.device).permute(0, 3, 1, 2)
+    L.call("mas_scene_expand", labels, n, h, w, y, L.t4(y))
+    return y
+
+
 def _cl_pitch(t):
     """Channel pitch if t [N,C,H,W] is a channels-last view whose pixels are `pitch` floats apart (pitch >= C), else None."""
     if t.dim() != 4 or t.stride(1) != 1:
@@ -1273,7 +1314,9 @@ class BCELogitsFn(torch.autograd.Function):
     """binary_cross_entropy_with_logits(pos_weight) mean (losses/loss_seg.py:15-19). With the VQ-SEG step's own layouts
     (channels-last logits - the padded view the decoder's last convolution returns - and an NCHW target) loss and
     gradient are two tiled kernels and the gradient is produced directly in the padded channels-last buffer the convolution's
-    backward consumes; other layouts take the generic strided kernel. Nothing of the backward runs in torch."""
+    backward consumes; other layouts take the generic strided kernel. Nothing of the backward runs in torch.
+    target may be a compact scene map (uint8 [N, 4, H, W], mas_b200.scene) for 159-channel logits: the tiled kernels read
+    the labels (mas_bce_scene_*, only the labels are saved), the generic kernel gets the target expanded on the device."""
 
     @staticmethod
     def forward(ctx, logits, target, pos_weight):
@@ -1281,12 +1324,22 @@ class BCELogitsFn(torch.autograd.Function):
         n, c, h, w = logits.shape
         loss = torch.empty((), dtype=torch.float32, device=logits.device)
         cp = _cl_pitch(logits)
-        if cp is not None and target.is_contiguous() and w % 32 == 0 and c * 33 * 4 <= 48 * 1024:
+        ctx.scene = target.dtype == torch.uint8
+        if ctx.scene:
+            if c != scene.CHANNELS:
+                raise RuntimeError("a compact scene map is the target of %d-channel logits, got %d" % (scene.CHANNELS, c))
+            target = scene_labels(target, n, h, w)
+        if cp is not None and w % 32 == 0 and (ctx.scene or (target.is_contiguous() and c * 33 * 4 <= 48 * 1024)):
             ws = L.workspace(L.query("mas_bce_cl_ws_bytes", n, h, w), logits.device)
-            L.call("mas_bce_cl_forward", logits, target, pos_weight, n, c, cp, h, w, loss, ws, ws.numel())
+            if ctx.scene:
+                L.call("mas_bce_scene_forward", logits, target, pos_weight, n, cp, h, w, loss, ws, ws.numel())
+            else:
+                L.call("mas_bce_cl_forward", logits, target, pos_weight, n, c, cp, h, w, loss, ws, ws.numel())
             ctx.save_for_backward(logits, target, pos_weight)
             ctx.cp = cp
             return loss
+        if ctx.scene:
+            target = scene_expand(target)
         grad = torch.empty_like(logits)
         nb = L.query("mas_bce_ws_bytes", L.t4(logits))
         ws = L.workspace(nb, logits.device)
@@ -1309,7 +1362,10 @@ class BCELogitsFn(torch.autograd.Function):
         logits, target, pw = ctx.saved_tensors
         n, c, h, w = logits.shape
         base = torch.empty((n, h, w, ctx.cp), dtype=torch.float32, device=logits.device)
-        L.call("mas_bce_cl_backward", logits, target, pw, g, n, c, ctx.cp, h, w, base)
+        if ctx.scene:
+            L.call("mas_bce_scene_backward", logits, target, pw, g, n, ctx.cp, h, w, base)
+        else:
+            L.call("mas_bce_cl_backward", logits, target, pw, g, n, c, ctx.cp, h, w, base)
         full = base.permute(0, 3, 1, 2)
         grad = full[:, :c]
         grad._mas_pad_base = full          # the padded tensor this view lives in (picked up by the convolution's backward)
