@@ -37,8 +37,9 @@ int launched_tc(const char* what) {
 
 // ------------------------------------------------------------------------------------------------
 // GroupNorm.  x [N, HW, C]; a block owns GN_PIX consecutive pixels of one image; thread t owns the
-// channel quad (t % U), U = C/4, and walks pixels t/U, t/U + 256/U, ...  Sums are kept in fp64
-// (cheap in an HBM-bound kernel) so that var = E[x^2]-E[x]^2 has no fp32 cancellation problem.
+// channel quad (t % U), U = C/4, and walks pixels t/U, t/U + 256/U, ...  Sums over 4 pixels are fp32, everything above
+// them fp64 (cheap in an HBM-bound kernel), so var = E[x^2]-E[x]^2 loses only what 4-term fp32 sums of x^2 lose: about
+// 2e-6 of rstd at |mean|/std = 32 (DESIGN 3.4), against ~1e-5 for the 128-element fp32 partials of the convolution epilogues.
 // ------------------------------------------------------------------------------------------------
 constexpr int GN_THREADS = 256;
 constexpr int GN_PIX = 1024;  // pixels per block for large images; small ones get smaller chunks (gn_chunks) so the grid fills the GPU

@@ -790,9 +790,10 @@ class ResnetBlockFn(torch.autograd.Function):
         fused = conv_tc_eligible(x, cout, L.CONV_S1) and cin % 8 == 0 and cout % (4 * GN_GROUPS) == 0
         # shadow mode: act(GN(.)) is written ONCE as an fp16 channels-last tensor (half the bytes of the fp32 activation the
         # unfused path stores), the convolutions read it through the copy engine (conv_tma.cu) and the backward pass feeds the
-        # same tensor to the weight-gradient kernel instead of re-materialising it
+        # same tensor to the weight-gradient kernel instead of re-materialising it. Both convolutions and both data gradients
+        # (Cout -> Cin for conv1: Cin % 128 == 0) must fit the TMA-fed kernel, which has no other fallback in backward
         hmode = (fused and conv_h_eligible(n, cin, h, w, cout) and conv_h_eligible(n, cout, h, w, cout)
-                 and wgrad_f16_on() and cin % 32 == 0)
+                 and conv_h_eligible(n, cout, h, w, cin) and wgrad_f16_on() and cin % 32 == 0)
         sc = x if sw is None else conv1x1_raw(x, sw, sb)
         if hmode:
             a1 = gn_apply_f16(x, m1, r1, n1w, n1b, True)

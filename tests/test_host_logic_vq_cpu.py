@@ -128,7 +128,8 @@ class VqEmu:
             assert dx_bound is not None and (dx_add is None or add_amax is not None)
             bound = 1.3 * float(np.abs(d).max()) + 1e-30          # any value >= max|dx| is a valid "rigorous bound"
             _f32(dx_bound, 1)[0] = bound
-            _f16(dx_f16, N * HW * C)[...] = (d.reshape(-1) * _scale(dx_bound)).astype(np.float16)
+            # the kernel scales the fp32 dx it stores (exact: a power of two), then rounds to fp16
+            _f16(dx_f16, N * HW * C)[...] = (d.reshape(-1).astype(np.float32) * np.float32(_scale(dx_bound))).astype(np.float16)
 
     # ---- fp16 copies -------------------------------------------------------------------------------------------------
     def mas_amax(self, x, n, out):
