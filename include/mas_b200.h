@@ -573,6 +573,15 @@ int mas_sample_topk(const float* logits, int64_t ld, int R, int V, float tempera
 int mas_sample_filtered(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p,
                         const float* u, const int64_t* prompt_tokens, const uint8_t* prompt_mask, int64_t prompt_ld,
                         int64_t* tokens, void* stream);
+/* mas_sample_filtered that also returns the probability each token was drawn with: the same kernel, the same tokens bit for
+ * bit, plus logp[r * logp_ld] = log p(tokens[r]) = (z_tok - max z) - log(sum of exp(z - max z) over the kept set), natural
+ * log, under the temperature-scaled, filtered distribution of steps 1-4 (the kept-set sum is the one the draw itself used:
+ * one store per row, no further pass over the logits).  A prompt row (mask set) and a greedy row (temperature 0) get 0: the
+ * token is certain under the rule that chose it.  logp is this position's column of an [R, L] tensor with row stride logp_ld
+ * (elements); it must not be NULL (mas_sample_filtered and mas_sample_topk are the no-logp cases and write nothing there). */
+int mas_sample_filtered_logp(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p,
+                             const float* u, const int64_t* prompt_tokens, const uint8_t* prompt_mask, int64_t prompt_ld,
+                             int64_t* tokens, float* logp, int64_t logp_ld, void* stream);
 
 /* ---- weighted BCE-with-logits (VQ-SEG loss, losses/loss_seg.py:15-22) — "next" row ------------------
  * logits/target: strided [N,H,W,C] views; pos_weight [C]; loss_out = mean over all elements. grad may be NULL. */

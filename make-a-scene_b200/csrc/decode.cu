@@ -476,6 +476,8 @@ __global__ void cfg_mix_kernel(const float* __restrict__ cond, const float* __re
 // than in exact arithmetic.
 // temperature == 0: greedy, the first index of the largest logit (torch.argmax's rule); u is not read.
 // Prompt (pmask != NULL): rows with pmask[r * pld] != 0 take tok = ptok[r * pld] and draw nothing.
+// logp != NULL: logp[r * lpld] = log of the probability the token was drawn with, (z_tok - mx) - log(total) with total the
+// kept-set sum the draw itself used (one store per row, no further pass over V); 0 for prompt and greedy rows (certain).
 __device__ __forceinline__ uint32_t order_key(float f) {
   const uint32_t b = __float_as_uint(f);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
@@ -483,7 +485,8 @@ __device__ __forceinline__ uint32_t order_key(float f) {
 constexpr float MASS_ONE = 1099511627776.f;          // 2^40: the largest entry's mass exp(0)
 __global__ void __launch_bounds__(256) sample_topk_kernel(const float* __restrict__ logits, int64_t ld, int V, float temperature, int top_k,
                                                           float top_p, const float* __restrict__ u, const int64_t* __restrict__ ptok,
-                                                          const uint8_t* __restrict__ pmask, int64_t pld, int64_t* __restrict__ tok) {
+                                                          const uint8_t* __restrict__ pmask, int64_t pld, int64_t* __restrict__ tok,
+                                                          float* __restrict__ logp, int64_t lpld) {
   __shared__ int hist[256];
   __shared__ unsigned long long mhist[256];
   __shared__ uint32_t s_prefix;
@@ -495,7 +498,10 @@ __global__ void __launch_bounds__(256) sample_topk_kernel(const float* __restric
   const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
   const float* x = logits + (int64_t)blockIdx.x * ld;
   if (pmask && pmask[(int64_t)blockIdx.x * pld]) {   // uniform over the block
-    if (t == 0) tok[blockIdx.x] = ptok[(int64_t)blockIdx.x * pld];
+    if (t == 0) {
+      tok[blockIdx.x] = ptok[(int64_t)blockIdx.x * pld];
+      if (logp) logp[(int64_t)blockIdx.x * lpld] = 0.f;
+    }
     return;
   }
   if (temperature == 0.f) {                           // greedy: (value, index) maximum, ties to the lower index
@@ -517,6 +523,7 @@ __global__ void __launch_bounds__(256) sample_topk_kernel(const float* __restric
       for (int w = 1; w < 8; ++w)
         if (redi[w] >= 0 && (bi < 0 || red[w] > best || (red[w] == best && redi[w] < bi))) { best = red[w]; bi = redi[w]; }
       tok[blockIdx.x] = (int64_t)bi;
+      if (logp) logp[(int64_t)blockIdx.x * lpld] = 0.f;
     }
     return;
   }
@@ -652,7 +659,9 @@ __global__ void __launch_bounds__(256) sample_topk_kernel(const float* __restric
         if (run > target) { pick = c; break; }
       }
     }
-    tok[blockIdx.x] = (int64_t)(pick >= 0 ? pick : last_kept);
+    const int drawn = pick >= 0 ? pick : last_kept;
+    tok[blockIdx.x] = (int64_t)drawn;
+    if (logp) logp[(int64_t)blockIdx.x * lpld] = (x[drawn] / temperature - mx) - logf(total);
   }
 }
 
@@ -923,21 +932,37 @@ int mas_sample_topk(const float* logits, int64_t ld, int R, int V, float tempera
                     void* stream) {
   MAS_REQUIRE(logits && u && tokens && R > 0 && V > 0 && ld >= V, "sample_topk: bad arguments");
   if (!(temperature > 0.f)) return fail(MAS_ERR_INVALID_ARG, "sample_topk: temperature must be > 0 (greedy decoding: top_k = 1)");
-  sample_topk_kernel<<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, 1.f, u, nullptr, nullptr, 0, tokens);
+  sample_topk_kernel<<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, 1.f, u, nullptr, nullptr, 0, tokens, nullptr, 0);
   return launched("sample_topk");
+}
+
+static int sample_filtered_run(const char* name, const float* logits, int64_t ld, int R, int V, float temperature, int top_k,
+                               float top_p, const float* u, const int64_t* prompt_tokens, const uint8_t* prompt_mask,
+                               int64_t prompt_ld, int64_t* tokens, float* logp, int64_t logp_ld, void* stream) {
+  if (!(logits && tokens && R > 0 && V > 0 && ld >= V)) return fail(MAS_ERR_INVALID_ARG, "%s: bad arguments", name);
+  if (!(temperature >= 0.f)) return fail(MAS_ERR_INVALID_ARG, "%s: temperature must be >= 0 (0: greedy)", name);
+  if (temperature > 0.f && !u) return fail(MAS_ERR_INVALID_ARG, "%s: sampling (temperature > 0) needs the uniforms u", name);
+  if (!(top_p > 0.f)) return fail(MAS_ERR_INVALID_ARG, "%s: top_p must be > 0 (>= 1: no nucleus filter)", name);
+  if (!prompt_tokens != !prompt_mask) return fail(MAS_ERR_INVALID_ARG, "%s: prompt tokens and prompt mask go together", name);
+  if (prompt_mask && prompt_ld < 0) return fail(MAS_ERR_INVALID_ARG, "%s: negative prompt row stride", name);
+  if (logp && logp_ld < 0) return fail(MAS_ERR_INVALID_ARG, "%s: negative log-probability row stride", name);
+  sample_topk_kernel<<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, top_p, u, prompt_tokens, prompt_mask, prompt_ld,
+                                               tokens, logp, logp_ld);
+  return launched(name);
 }
 
 int mas_sample_filtered(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p, const float* u,
                         const int64_t* prompt_tokens, const uint8_t* prompt_mask, int64_t prompt_ld, int64_t* tokens, void* stream) {
-  MAS_REQUIRE(logits && tokens && R > 0 && V > 0 && ld >= V, "sample_filtered: bad arguments");
-  if (!(temperature >= 0.f)) return fail(MAS_ERR_INVALID_ARG, "sample_filtered: temperature must be >= 0 (0: greedy)");
-  if (temperature > 0.f && !u) return fail(MAS_ERR_INVALID_ARG, "sample_filtered: sampling (temperature > 0) needs the uniforms u");
-  if (!(top_p > 0.f)) return fail(MAS_ERR_INVALID_ARG, "sample_filtered: top_p must be > 0 (>= 1: no nucleus filter)");
-  if (!prompt_tokens != !prompt_mask) return fail(MAS_ERR_INVALID_ARG, "sample_filtered: prompt tokens and prompt mask go together");
-  if (prompt_mask && prompt_ld < 0) return fail(MAS_ERR_INVALID_ARG, "sample_filtered: negative prompt row stride");
-  sample_topk_kernel<<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, top_p, u, prompt_tokens, prompt_mask, prompt_ld,
-                                               tokens);
-  return launched("sample_filtered");
+  return sample_filtered_run("sample_filtered", logits, ld, R, V, temperature, top_k, top_p, u, prompt_tokens, prompt_mask,
+                             prompt_ld, tokens, nullptr, 0, stream);
+}
+
+int mas_sample_filtered_logp(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p,
+                             const float* u, const int64_t* prompt_tokens, const uint8_t* prompt_mask, int64_t prompt_ld,
+                             int64_t* tokens, float* logp, int64_t logp_ld, void* stream) {
+  if (!logp) return fail(MAS_ERR_INVALID_ARG, "sample_filtered_logp: logp is NULL (mas_sample_filtered draws without it)");
+  return sample_filtered_run("sample_filtered_logp", logits, ld, R, V, temperature, top_k, top_p, u, prompt_tokens, prompt_mask,
+                             prompt_ld, tokens, logp, logp_ld, stream);
 }
 
 }  // extern "C"

@@ -138,6 +138,7 @@ _SPEC = {
     "mas_layernorm2_forward": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _L, _I, _F, _F, _P]),
     "mas_sample_topk": (_I, [_P, _L, _I, _I, _F, _I, _P, _P, _P]),
     "mas_sample_filtered": (_I, [_P, _L, _I, _I, _F, _I, _F, _P, _P, _P, _L, _P, _P]),
+    "mas_sample_filtered_logp": (_I, [_P, _L, _I, _I, _F, _I, _F, _P, _P, _P, _L, _P, _P, _L, _P]),
     "mas_pack_gemm_tc16": (_I, [_P, _P, _I, _I, _I, _P]),
     "mas_gemm_rows_f16": (_I, [_P, _L, _I, _P, _P, _L, _I, _P, _P, _P, _F, _P]),
     "mas_linear_rows_f16_ws_bytes": (_Z, [_L, _I, _I]),

@@ -1714,11 +1714,13 @@ def cross_entropy(logits, target):
     return CrossEntropyFn.apply(logits, target)
 
 
-def sample_topk(logits, temperature, top_k, u, top_p=None, prompt=None):
+def sample_topk(logits, temperature, top_k, u, top_p=None, prompt=None, logp=None):
     """One token per row of logits [R,V]: softmax(logits / temperature) restricted to the top_k entries, then (top_p < 1) to
     the nucleus of mass top_p, drawn by inverse CDF at the caller's uniforms u [R] (device fp32 in [0,1)); temperature 0 is
     greedy (u unused, may be None). prompt: (tokens int64 [R], mask bool [R]) - rows whose mask is set take the given token.
-    Without top_p < 1 and a prompt this is mas_sample_topk; otherwise mas_sample_filtered (include/mas_b200.h)."""
+    logp (fp32 [R], any row stride, e.g. one column of an [R, L] tensor): receives the log-probability each token was drawn
+    with under that filtered distribution (0 for prompt and greedy rows); the call is then always mas_sample_filtered_logp.
+    Without it: mas_sample_topk without top_p < 1 and a prompt, otherwise mas_sample_filtered (include/mas_b200.h)."""
     _need_cuda(logits)
     if top_p is not None:
         top_p = float(top_p)
@@ -1729,7 +1731,10 @@ def sample_topk(logits, temperature, top_k, u, top_p=None, prompt=None):
     logits = logits.contiguous()
     R, V = logits.shape
     tok = torch.empty(R, dtype=torch.int64, device=logits.device)
-    if top_p is None and prompt is None:
+    if logp is not None:
+        if logp.shape != (R,) or logp.dtype != torch.float32 or logp.device != logits.device:
+            raise ValueError("logp: an fp32 column of %d rows on the logits' device (%s) expected" % (R, logits.device))
+    if top_p is None and prompt is None and logp is None:
         L.call("mas_sample_topk", logits, V, R, V, float(temperature), int(top_k) if top_k else 0, u.contiguous(), tok)
         return tok
     ptok = pmask = None
@@ -1743,9 +1748,30 @@ def sample_topk(logits, temperature, top_k, u, top_p=None, prompt=None):
         if ptok.stride(0) != pmask.stride(0):
             ptok, pmask = ptok.contiguous(), pmask.contiguous()
         pld = ptok.stride(0)
-    L.call("mas_sample_filtered", logits, V, R, V, float(temperature), int(top_k) if top_k else 0, 1.0 if top_p is None else top_p,
-           None if u is None else u.contiguous(), ptok, pmask, pld, tok)
+    args = (logits, V, R, V, float(temperature), int(top_k) if top_k else 0, 1.0 if top_p is None else top_p,
+            None if u is None else u.contiguous(), ptok, pmask, pld, tok)
+    if logp is None:
+        L.call("mas_sample_filtered", *args)
+    else:
+        L.call("mas_sample_filtered_logp", *args, logp, logp.stride(0))
     return tok
+
+
+def token_logprobs(logits, target):
+    """log softmax(logits)[r, target[r]] for logits [R,V] fp32 (last dim contiguous) and target int64 [R] in [0, V): the
+    per-row cross-entropies mas_ce_forward writes (loss_rows), negated. No gradient; the caller checks the targets' range
+    (the entry gives a row outside [0, V) a loss of 0)."""
+    _need_cuda(logits)
+    R, V = logits.shape
+    if logits.stride(-1) != 1:
+        logits = logits.contiguous()
+    if target.shape != (R,) or target.dtype != torch.int64 or target.device != logits.device:
+        raise ValueError("token_logprobs: int64 targets of %d rows on the logits' device (%s) expected" % (R, logits.device))
+    rows = torch.empty(R, dtype=torch.float32, device=logits.device)
+    lse = torch.empty(R, dtype=torch.float32, device=logits.device)
+    out = torch.empty(2, dtype=torch.float32, device=logits.device)
+    L.call("mas_ce_forward", logits, logits.stride(0), target.contiguous(), rows, lse, out, R, V)
+    return rows.neg_()
 
 
 # ---- autoregressive sampling (inference only; SURVEY.md 8f-3) --------------------------------------------------

@@ -324,18 +324,20 @@ class MakeAScene(nn.Module):
         return ops.cross_entropy(self.forward(text_tokens, seg_tokens, img_tokens), img_tokens)
 
     # ---- sampling (SURVEY.md 8f-3) ---------------------------------------------------------------------------
-    def _prefill(self, emb, kc, vc):
-        """Full causal pass over the text+segmentation prefix with the training kernels, recording every layer's k / v."""
+    def _prefill(self, emb, kc=None, vc=None):
+        """Full causal pass over emb [B,S,H] with the training kernels and no dropout; returns every position's hidden state
+        before final_ln [B,S,H]. With kc / vc (generate's prefix pass) every layer's k / v are recorded at positions 0..S-1."""
         x = emb
         heads = self.transformer.layers[0].attn.num_attn_heads
         for li, layer in enumerate(self.transformer.layers):
             qkv = layer.attn.qkv(layer.ln_in(x))
-            ops.kv_append(qkv, kc[li], vc[li], 0)
+            if kc is not None:
+                ops.kv_append(qkv, kc[li], vc[li], 0)
             a = layer.attn.out_proj(ops.CausalAttentionFn.apply(qkv, heads))
             x = layer.first_ln_sandwich(a, residual=x) if layer.cogview_sandwich_layernorm else x + a
             m = layer.mlp.project(layer.ln_out(x))
             x = layer.second_ln_sandwich(m, residual=x) if layer.cogview_sandwich_layernorm else x + m
-        return x[:, -1].contiguous()
+        return x
 
     def _decode_step(self, x, kc, vc, pos, suffix=None):
         """One new token per row (x [R,H], absolute position pos) through all layers against the cache; returns
@@ -383,7 +385,8 @@ class MakeAScene(nn.Module):
 
     @torch.no_grad()
     def generate(self, text_tokens, seg_tokens, guidance_scale=None, uncond_text_tokens=None, temperature=1.0, top_k=None,
-                 generator=None, img_tokens=None, return_logits=False, use_graphs=False, top_p=None, img_mask=None, num_samples=1):
+                 generator=None, img_tokens=None, return_logits=False, use_graphs=False, top_p=None, img_mask=None, num_samples=1,
+                 return_logprobs=False):
         """Autoregressive sampling of the image tokens with a KV cache; optional classifier-free guidance
         (logits = uncond + scale * (cond - uncond), the unconditional stream sees padded text; Make-A-Scene paper 3.4).
 
@@ -404,6 +407,11 @@ class MakeAScene(nn.Module):
         all-false mask gives the tokens of the unprompted call with the same generator.
         Returns tokens [B,image_length] (and the per-position logits [B,image_length,V], mixed and unfiltered, when
         return_logits=True).
+        return_logprobs=True also returns logprobs fp32 [B,image_length], last: at a drawn position the natural log of the
+        probability the token was drawn with, under the mixed (guided), temperature-scaled, filtered distribution above (the
+        draw kernel's own kept-set sum; mas_sample_filtered_logp); 0 at forced positions (img_tokens, or img_mask set) and at
+        greedy ones, so a row's sum is the log-probability of its drawn part. Tokens and logits do not depend on the flag.
+        The return is then (tokens, logits, logprobs) or (tokens, logprobs).
         num_samples=n (int >= 1) draws n images per prompt: the result is that of generate(text_tokens.repeat_interleave(n, 0),
         seg_tokens.repeat_interleave(n, 0), ...) with the same generator state, bit for bit; output row b*n + j is sample j of
         prompt b, so the returned shapes have B*n rows, and img_tokens / img_mask are given per output row [B*n,image_length]
@@ -419,6 +427,8 @@ class MakeAScene(nn.Module):
         n = num_samples
         if isinstance(n, bool) or not isinstance(n, int) or n < 1:
             raise ValueError("num_samples must be an int >= 1, got %r" % (num_samples,))
+        if not isinstance(return_logprobs, bool):
+            raise ValueError("return_logprobs must be a bool, got %r" % (return_logprobs,))
         Bn = B * n
         if top_p is not None and not float(top_p) > 0:
             raise ValueError("top_p must be > 0 (None or >= 1: no nucleus filter), got %r" % (top_p,))
@@ -452,10 +462,11 @@ class MakeAScene(nn.Module):
                 self._sampler = dec
         kc, vc = dec.kc, dec.vc
         prefix = text_all.shape[1] + seg_all.shape[1]
-        last = self._prefill(self._embed(text_all, seg_all, None), kc, vc)
+        last = self._prefill(self._embed(text_all, seg_all, None), kc, vc)[:, -1].contiguous()
         # expanded BEFORE to_logits: linear_small picks its arithmetic by row count, and the repeated call has R rows here
         logits = self._logits_of(last.repeat_interleave(n, 0) if n > 1 else last)
         toks, kept = [], []
+        logprobs = torch.zeros((Bn, self.image_length), dtype=torch.float32, device=dev) if return_logprobs else None
         for t in range(self.image_length):
             mixed = ops.cfg_mix(logits[:Bn], logits[Bn:], guidance_scale) if cfg else logits
             if return_logits:
@@ -472,13 +483,55 @@ class MakeAScene(nn.Module):
                         u = torch.rand(Bn, generator=generator).to(dev)
                     else:
                         u = torch.rand(Bn, device=dev, generator=generator)
-                tok = ops.sample_topk(mixed, float(temperature), top_k, u, top_p=top_p, prompt=prompt)
+                tok = ops.sample_topk(mixed, float(temperature), top_k, u, top_p=top_p, prompt=prompt,
+                                      logp=None if logprobs is None else logprobs[:, t])
             toks.append(tok)
             if t == self.image_length - 1:
                 break
             tok_all = torch.cat([tok, tok], 0) if cfg else tok
             logits = (dec.graphed_step if use_graphs else dec.eager_step)(t, tok_all, prefix)
         tokens = torch.stack(toks, 1)
-        if return_logits:
-            return tokens, torch.stack(kept, 1)
-        return tokens
+        out = (tokens,) + ((torch.stack(kept, 1),) if return_logits else ()) + ((logprobs,) if return_logprobs else ())
+        return out if len(out) > 1 else tokens
+
+    @torch.no_grad()
+    def score(self, text_tokens, seg_tokens, img_tokens, guidance_scale=None, uncond_text_tokens=None):
+        """Teacher-forced log-likelihood of given image tokens: fp32 [B,image_length], entry [b, t] = log p(img_t | text, seg,
+        img_<t) at temperature 1 with no filters, natural log. With guidance (guidance_scale and uncond_text_tokens as in
+        generate) the distribution is softmax(u + s * (c - u)) of the unconditional and conditional streams' logits, the one
+        generate draws from at temperature 1 without top_k / top_p. Sum over t to rank candidate images.
+        One causal pass over text + seg + image (both streams in one batch with guidance; no dropout, in train mode as in
+        eval mode), to_logits on the image_length predicting positions, the guidance mix, then the per-row cross-entropies of
+        mas_ce_forward negated. text_tokens [B,text_length], seg_tokens [B,seg_length], img_tokens [B,image_length] (values in
+        [0, image_vocab_size)) and uncond_text_tokens [B,text_length]: int64 on the model's device."""
+        named = [("text_tokens", text_tokens, self.text_length), ("seg_tokens", seg_tokens, self.seg_length),
+                 ("img_tokens", img_tokens, self.image_length)]
+        if uncond_text_tokens is not None:
+            named.append(("uncond_text_tokens", uncond_text_tokens, self.text_length))
+        B = text_tokens.shape[0] if isinstance(text_tokens, torch.Tensor) and text_tokens.dim() == 2 else None
+        dev = self.image_token_embedding.weight.device
+        for name, t, length in named:
+            if not isinstance(t, torch.Tensor) or B is None or tuple(t.shape) != (B, length):
+                raise ValueError("%s must be a tensor of shape %s" % (name, (B, length)))
+            if t.dtype != torch.int64:
+                raise ValueError("%s must be int64, got %s" % (name, t.dtype))
+            if t.device != dev:
+                raise ValueError("%s must be on the model's device (%s), got %s" % (name, dev, t.device))
+        V = self.image_token_embedding.num_embeddings
+        if bool(((img_tokens < 0) | (img_tokens >= V)).any()):
+            raise ValueError("img_tokens must lie in [0, %d)" % V)
+        cfg = guidance_scale is not None and float(guidance_scale) != 1.0
+        if cfg:
+            if uncond_text_tokens is None:
+                uncond_text_tokens = torch.zeros_like(text_tokens)          # all padding, as in generate
+            text_tokens = torch.cat([text_tokens, uncond_text_tokens], 0)
+            seg_tokens, img_all = torch.cat([seg_tokens, seg_tokens], 0), torch.cat([img_tokens, img_tokens], 0)
+        else:
+            img_all = img_tokens
+        L = self.image_length
+        h = self.transformer.final_ln(self._prefill(self._embed(text_tokens, seg_tokens, img_all)))
+        h = h[:, -L - 1:-1].contiguous()                                    # forward()'s slice: the predicting positions
+        logits = self.to_logits[1](self.to_logits[0](h))
+        if cfg:
+            logits = ops.cfg_mix(logits[:B], logits[B:], guidance_scale)
+        return ops.token_logprobs(logits.view(B * L, V), img_tokens.reshape(B * L)).view(B, L)

@@ -7,7 +7,9 @@ fp32 KV cache, above 8 rows fp16 weights and fp16 cache (the cache read at the m
 (an image prompt, random tokens): the forced positions are still decoded one step each, so tokens/s counts every position.
 --samples N draws N images per prompt (generate(num_samples=N)): B prompts give R = 2 B N rows that share each prompt's prefix
 cache, and cache_gb_per_step counts a prompt's prefix once per step, as the shared-prefix attention reads it.
-Usage: python tools/bench_sampling.py [--batch B] [--samples N] [--reps N] [--graphs] [--top-p P] [--prompt-frac F]"""
+--logprobs also times the same call with return_logprobs=True next to the plain one (alternating, --reps each, after both
+are warmed up) and adds both times and the relative cost to the line; without it the line is unchanged.
+Usage: python tools/bench_sampling.py [--batch B] [--samples N] [--reps N] [--graphs] [--top-p P] [--prompt-frac F] [--logprobs]"""
 import argparse
 import json
 import os
@@ -28,6 +30,7 @@ ap.add_argument("--layers", type=int, default=24)
 ap.add_argument("--graphs", action="store_true", help="replay each position's decode step from a CUDA graph")
 ap.add_argument("--top-p", type=float, default=None, help="nucleus filter of the draw (default: off)")
 ap.add_argument("--prompt-frac", type=float, default=0.0, help="share of image positions forced by a random image prompt")
+ap.add_argument("--logprobs", action="store_true", help="also time generate(return_logprobs=True) against the plain call")
 args = ap.parse_args()
 dev = torch.device("cuda:0")
 torch.manual_seed(0)
@@ -61,10 +64,25 @@ prefix, steps = 128 + 256, 255
 mean_suffix = (steps + 1) / 2        # the step of image position t reads prefix + t + 1 positions; its prompt's prefix once per group
 weight_bytes = params * elem
 cache_bytes = args.layers * 2 * cfg["hidden_dim"] * (R // N * prefix + R * mean_suffix) * elem
-print(json.dumps({"metric": "image tokens/s, classifier-free guided sampling with KV cache", "value": B * N * 256 / sec, "unit": "tokens/s",
-                  "images_per_s": B * N / sec, "gpu": gpu.stdout.strip().splitlines()[0], "batch": B, "prompts": B, "samples": N,
-                  "rows": R, "cuda_graphs": bool(args.graphs),
-                  "top_k": 64, "top_p": args.top_p, "prompt_frac": args.prompt_frac,
-                  "seconds_per_image": sec, "launches_per_image": (_lib.launch_count() - l0) // args.reps,
-                  "operand_bytes": elem, "weight_stream_gb_per_step": weight_bytes / 1e9, "cache_gb_per_step": cache_bytes / 1e9,
-                  "hbm_stream_gbs": (weight_bytes + cache_bytes) * steps / sec / 1e9, "config": cfg}))
+res = {"metric": "image tokens/s, classifier-free guided sampling with KV cache", "value": B * N * 256 / sec, "unit": "tokens/s",
+       "images_per_s": B * N / sec, "gpu": gpu.stdout.strip().splitlines()[0], "batch": B, "prompts": B, "samples": N,
+       "rows": R, "cuda_graphs": bool(args.graphs),
+       "top_k": 64, "top_p": args.top_p, "prompt_frac": args.prompt_frac,
+       "seconds_per_image": sec, "launches_per_image": (_lib.launch_count() - l0) // args.reps,
+       "operand_bytes": elem, "weight_stream_gb_per_step": weight_bytes / 1e9, "cache_gb_per_step": cache_bytes / 1e9,
+       "hbm_stream_gbs": (weight_bytes + cache_bytes) * steps / sec / 1e9, "config": cfg}
+if args.logprobs:
+    m.generate(text, seg, return_logprobs=True, **kw)     # warm-up of the logp entry
+    times = {False: [], True: []}
+    for i in range(args.reps):
+        for flag in ((False, True) if i % 2 == 0 else (True, False)):
+            torch.cuda.synchronize()
+            e0.record()
+            m.generate(text, seg, return_logprobs=flag, **kw)
+            e1.record()
+            torch.cuda.synchronize()
+            times[flag].append(e0.elapsed_time(e1) * 1e-3)
+    plain, logp = (sorted(times[f])[len(times[f]) // 2] for f in (False, True))
+    res.update({"logprobs_seconds_per_call_median": logp, "plain_seconds_per_call_median": plain,
+                "logprobs_relative_cost": logp / plain - 1, "logprobs_seconds_all": times[True], "plain_seconds_all": times[False]})
+print(json.dumps(res))
