@@ -465,6 +465,24 @@ int mas_embed3_backward(const float* dout, const int64_t* id0, float* d0, const 
  * (MAS_ERR_UNSUPPORTED otherwise: the caller runs the GEMM / softmax sequence).  2 x fp16 operand split = fp32-level accuracy. */
 int mas_attn_causal_forward(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads, int hd,
                             float scale, void* stream);
+/* mas_attn_causal_forward_stats: the same core without P, for a backward that recomputes it: ctx is the bits of
+ * mas_attn_causal_forward (p = 0) / mas_attn_causal_dropout_forward (p > 0, same seed), and instead of P the kernel writes
+ * every row's maximum m and sum l of the scaled scores, P = exp(S - m) / l: stats = m [B,heads,S] followed by
+ * l [B,heads,S] (2 * B * heads * S floats).  0 <= p <= 1; seed may be NULL when p == 0.  Same shape limits as
+ * mas_attn_causal_forward (MAS_ERR_UNSUPPORTED off hd == 64 / S % 128 == 0; the GEMM sequence has no P-free form).
+ * mas_attn_causal_backward: the fused backward from those statistics; nothing S x S is read or written.  qkv and ctx of the
+ * forward, dctx [B,S,heads*hd] its output gradient, stats the forward's, amax = max|qkv| (the forward's device scalar),
+ * dctx_amax = max|dctx| (mas_amax), D a workspace of B * heads * S floats (row dot products dctx . ctx), p / seed those of
+ * the forward.  Writes dqkv [B,S,3*heads*hd] fully (q | k | v thirds).  P is recomputed per 128 x 64 tile from the
+ * statistics with the forward's expression, the dropout mask regenerated; dK / dV accumulate over the query blocks of a
+ * 128-key tile, dQ over the key blocks of a 128-query tile, in registers: no atomics, two calls give the same bits.
+ * 2 x fp16 operand split (fp32-level accuracy) with power-of-two scales derived on the device: max|qkv|, max|dctx|, 2^14
+ * for P, and for dS the bound 2 * hd * max|dctx| * max|qkv| / (1 - p).  Same shape limits (MAS_ERR_UNSUPPORTED). */
+int mas_attn_causal_forward_stats(const float* qkv, const float* amax, float* stats, float* ctx, int B, int S, int heads, int hd,
+                                  float scale, double p, const int64_t* seed, void* stream);
+int mas_attn_causal_backward(const float* qkv, const float* ctx, const float* dctx, const float* stats, const float* amax,
+                             const float* dctx_amax, float* D, float* dqkv, int B, int S, int heads, int hd, float scale, double p,
+                             const int64_t* seed, void* stream);
 /* ---- Dropout of the token transformer (transformer.py:90-91, 114, 139) ------------------------------------------------
  * Element e of a dropout site is kept iff word[e & 3] of Philox4x32-10(counter = (lo32(e >> 2), hi32(e >> 2), 0, 0),
  * key = (lo32(seed), hi32(seed))) >= floor(p * 2^32); e is the element's row-major linear index in its tensor

@@ -14,6 +14,9 @@
 //     scores, writes the normalised probabilities (global fp32 + split into shared memory) and accumulates ctx += P_blk v_blk.
 //     The score contraction is cheap (K = 64), recomputing it is what keeps P exactly normalised without rescaling the
 //     accumulator.
+//   * STATS (mas_attn_causal_forward_stats, the backward recomputes P: attn_causal_bwd.cu): pass 1 stores no probabilities;
+//     instead pass 0 writes every row's maximum m and sum l, P = exp(S - m) / l.  The arithmetic is the P-writing kernel's
+//     minus the store, so ctx is the same bits.
 //   * shared memory: the Q tile (resident) + a 2-stage ring of K / V tiles (hi and lo images) + the P block, K-major planes
 //     [c/8][row][8 halves] for Q, K and P, MN-major planes [c/8][key][8 channels] for V (staged untransposed).
 //   * DROP (attention dropout, mas_attn_causal_dropout_forward): pass 1 still writes the undropped P (the softmax backward
@@ -23,6 +26,8 @@
 //     so each lane generates one group per 8-key column block (row frow or frow + 8) and takes the other row's bits from its
 //     partner by a shuffle.
 #include <cuda_fp16.h>
+
+#include <type_traits>
 
 #include "dropout.cuh"
 #include "mas_common.cuh"
@@ -74,14 +79,15 @@ __device__ __forceinline__ void split8(const float4& v0, const float4& v1, float
 
 struct Params {
   const float* qkv;   // [B, S, 3H]: q | k | v, head h owns columns h*HD .. of each third
-  float* P;           // [B, heads, S, S] softmax probabilities (saved for the backward; zeros above the diagonal)
+  float* P;           // [B, heads, S, S] softmax probabilities (saved for the backward; zeros above the diagonal);
+                      // STATS: the row statistics instead, m [B, heads, S] followed by l [B, heads, S]
   float* ctx;         // [B, S, H]
   const float* amax;  // device scalar: max |qkv| (one scale for q, k and v)
   int S, heads;
   float scale;
 };
 
-template <bool DROP>
+template <bool DROP, bool STATS = false>
 __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, const DropMask dm) {
   extern __shared__ __align__(1024) uint8_t smem[];
   uint8_t* q_tile = smem;                                   // resident Q tile (hi, lo)
@@ -129,7 +135,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, c
   };
 
   // masked key blocks of the saved probabilities
-  {
+  if constexpr (!STATS) {
     float* pt0 = p.P + (((size_t)b * heads + h) * S + q0) * S;
     const int cols = S - nkb * BK;
     for (int i = tid; i < BM * (cols / 4); i += NTHREADS) {
@@ -203,6 +209,17 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, c
             }
             rl[i] = 1.0f / l[i];
           }
+          if constexpr (STATS) {
+            if (fk == 0) {
+              float* mrow = p.P + ((size_t)b * heads + h) * S + q0 + frow;
+              float* lrow = mrow + (size_t)gridDim.z * heads * S;
+#pragma unroll
+              for (int i = 0; i < 2; ++i) {
+                mrow[8 * i] = m[i];
+                lrow[8 * i] = l[i];
+              }
+            }
+          }
         }
       } else {
         // probabilities: global (fp32) and the split P block in shared memory (the previous block's P V MMAs have retired:
@@ -228,7 +245,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, c
             const int key = 8 * j + 2 * fk;
             const float a = (diag && key > rit) ? 0.f : expf(sacc[4 * j + 2 * i] * ss - m[i]) * rl[i];
             const float c = (diag && key + 1 > rit) ? 0.f : expf(sacc[4 * j + 2 * i + 1] * ss - m[i]) * rl[i];
-            *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(a, c);
+            if constexpr (!STATS) *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(a, c);
             uint32_t hi, lo;
             if constexpr (DROP)
               split2((keep[i] >> (2 * j)) & 1u ? a : 0.f, (keep[i] >> (2 * j + 1)) & 1u ? c : 0.f, P_SCALE, &hi, &lo);
@@ -276,6 +293,282 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, c
 
 constexpr size_t SMEM_BYTES = (size_t)TILE * (1 + STAGES) + 2 * (size_t)P_HALF;
 
+// ---- backward from the row statistics (mas_attn_causal_backward) --------------------------------------------------------
+// P is recomputed from qkv and the forward's m / l, nothing S x S is read.  With dO = dctx, D_q = dO_q . ctx_q (a row
+// pre-pass), keep the regenerated dropout mask and s = 1 / (1 - p):
+//     dV = (P o keep)^T dO s,  dS = P o (dO v^T o keep s - D),  dQ = dS k * scale,  dK = dS^T q * scale.
+// Two kernels of one template, no atomics (deterministic):
+//   * DKV, per (sequence, head, 128-key tile): rows = keys; K and V resident, the query blocks of 64 at or below the
+//     diagonal streamed; S^T = K Q^T and dP^T = V dO^T, then dV += (P^T o keep) dO and dK += dS^T Q, accumulated in registers.
+//   * DQ, per (sequence, head, 128-query tile): rows = queries; Q and dO resident, the causal key blocks of 64 streamed;
+//     S = Q K^T (the forward's operands and MMA order), dP = dO V^T, dQ += dS K.
+// Every contraction runs on the 2 x fp16 split with three MMAs per K step.  Power-of-two scales, all derived on the device:
+// q / k / v from max|qkv| (the forward's), dO from max|dctx|, P 2^14 (the forward's), dS from its bound
+// |dS| <= 2 hd max|dO| max|qkv| / (1 - p).  A streamed [64 rows x 64 channels] tile serves both as the K-major operand of the
+// first pair of contractions and as the MN-major operand of the second: the planes [c/8][row][8 channels] are both layouts.
+constexpr int BN = 64;                            // streamed rows per block
+constexpr int PITCH_C = BN * 16 + 32;             // bytes between 8-channel planes of a streamed tile
+constexpr int C_HALF = (HD / 8) * PITCH_C;
+constexpr int B_HALF = (BN / 8) * PITCH_P;        // a [128 rows x 64 columns] P / dS block, one image
+
+struct BwdParams {
+  const float* qkv;     // [B, S, 3H]
+  const float* dctx;    // [B, S, H]
+  const float* stats;   // m [B, heads, S] then l [B, heads, S] (mas_attn_causal_forward_stats)
+  const float* D;       // [B, heads, S] row dot products dO . ctx
+  float* dqkv;          // [B, S, 3H]
+  const float* amax;    // device scalar max|qkv|
+  const float* amax_do; // device scalar max|dctx|
+  int S, heads;
+  float scale;
+};
+
+__global__ void __launch_bounds__(256) attn_causal_bwd_rowdot(const float* __restrict__ dctx, const float* __restrict__ ctx,
+                                                              float* __restrict__ D, int S, int heads, int64_t rows) {
+  const int64_t r = (int64_t)blockIdx.x * 8 + (threadIdx.x >> 5);      // row (b, q, h) of the [B S heads, 64] view
+  if (r >= rows) return;
+  const int lane = threadIdx.x & 31;
+  const float2 a = reinterpret_cast<const float2*>(dctx + r * HD)[lane], c = reinterpret_cast<const float2*>(ctx + r * HD)[lane];
+  float v = a.x * c.x + a.y * c.y;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if (lane == 0) {
+    const int64_t b = r / ((int64_t)S * heads), rem = r - b * S * heads;
+    const int q = (int)(rem / heads), h = (int)(rem - (int64_t)q * heads);
+    D[((size_t)b * heads + h) * S + q] = v;
+  }
+}
+
+template <bool DKV, bool DROP>
+__global__ void __launch_bounds__(NTHREADS, 1) attn_causal_bwd(const BwdParams p, const DropMask dm) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  uint8_t* r1 = smem;                         // resident 128 rows: K (DKV) / Q (DQ), hi + lo
+  uint8_t* r2 = r1 + TILE;                    // resident: V / dO
+  uint8_t* c1 = r2 + TILE;                    // streamed 64 rows: Q / K
+  uint8_t* c2 = c1 + 2 * C_HALF;              // streamed: dO / V
+  uint8_t* ds_blk = c2 + 2 * C_HALF;          // dS block (A operand of dK / dQ)
+  uint8_t* p_blk = ds_blk + 2 * B_HALF;       // DKV: the P o keep block (A operand of dV)
+  const uint32_t r1_base = smem_u32(r1), r2_base = smem_u32(r2), c1_base = smem_u32(c1), c2_base = smem_u32(c2);
+  const uint32_t ds_base = smem_u32(ds_blk), p_base = smem_u32(p_blk);
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, wgi = warp >> 2, fk = lane & 3;
+  const int S = p.S, heads = p.heads, H = heads * HD, C3 = 3 * H;
+  const int t = DKV ? (int)blockIdx.x : (int)gridDim.x - 1 - (int)blockIdx.x;   // heaviest tiles first
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int r0 = t * BM;
+  const int cb0 = DKV ? r0 : 0, ncb = DKV ? (S - r0) / BN : (r0 + BM) / BN;    // causal column blocks
+  const size_t bh = (size_t)b * heads + h;
+  const float* qb = p.qkv + (size_t)b * S * C3 + h * HD;
+  const float* ob = p.dctx + (size_t)b * S * H + h * HD;
+  const float* mg = p.stats + bh * S;
+  const float* lg = mg + (size_t)gridDim.z * heads * S;
+  const float* dg = p.D + bh * S;
+  const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2);
+  const uint32_t a_rows = (uint32_t)(wgi * 64 * 16);
+  float inv_s, inv_do, inv_ds;
+  const float sc = split_scale(p.amax, &inv_s);
+  const float sdo = split_scale(p.amax_do, &inv_do);
+  const float dsc = DROP ? dm.scale : 1.f;
+  const float bound = 2.f * HD * *p.amax_do * *p.amax * dsc;
+  const float sds = split_scale(&bound, &inv_ds);
+  constexpr float P_SCALE = 16384.0f, P_INV = 1.0f / 16384.0f;
+  const float ss = p.scale * inv_s * inv_s;                 // acc1 -> scale * q.k
+  const float sdp = inv_s * inv_do;                          // acc2 -> dO . v
+
+  // [ROWS x 64 channels] fp32 rows of src (leading dimension ld) -> hi / lo images at dst, scaled by s
+  auto fill = [&](auto rows_c, uint8_t* dst, const float* src, int ld, int row0, int pitch, int half, float s) {
+    constexpr int N = decltype(rows_c)::value * 8 / NTHREADS;
+    float4 v0[N], v1[N];
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      const int itm = tid + i * NTHREADS, oct = itm & 7, r = itm >> 3;
+      const float4* g = reinterpret_cast<const float4*>(src + (size_t)(row0 + r) * ld + oct * 8);
+      v0[i] = __ldg(g);
+      v1[i] = __ldg(g + 1);
+    }
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      const int itm = tid + i * NTHREADS, oct = itm & 7, r = itm >> 3;
+      uint4 hh, ll;
+      split8(v0[i], v1[i], s, &hh, &ll);
+      uint8_t* d = dst + oct * pitch + r * 16;
+      *reinterpret_cast<uint4*>(d) = hh;
+      *reinterpret_cast<uint4*>(d + half) = ll;
+    }
+  };
+  using R128 = std::integral_constant<int, BM>;
+  using R64 = std::integral_constant<int, BN>;
+  if constexpr (DKV) {
+    fill(R128{}, r1, qb + H, C3, r0, PITCH_K, K_HALF, sc);
+    fill(R128{}, r2, qb + 2 * H, C3, r0, PITCH_K, K_HALF, sc);
+  } else {
+    fill(R128{}, r1, qb, C3, r0, PITCH_K, K_HALF, sc);
+    fill(R128{}, r2, ob, H, r0, PITCH_K, K_HALF, sdo);
+  }
+
+  // DQ: the statistics of this thread's two query rows
+  float qm[2] = {0.f, 0.f}, qrl[2] = {0.f, 0.f}, qd[2] = {0.f, 0.f};
+  if constexpr (!DKV) {
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int q = r0 + frow + 8 * i;
+      qm[i] = mg[q];
+      qrl[i] = 1.0f / lg[q];
+      qd[i] = dg[q];
+    }
+  }
+  float acc1[BN / 2], acc2[BN / 2], g1[HD / 2], g2[HD / 2];   // g1: dK / dQ, g2: dV
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) g1[i] = g2[i] = 0.f;
+  const uint64_t seed = DROP ? (uint64_t)*dm.seed : 0ull;
+
+  for (int cbi = 0; cbi < ncb; ++cbi) {
+    const int cb = cb0 + cbi * BN;
+    __syncthreads();                                  // every MMA reading c1 / c2 / the blocks has retired (wait<0> below)
+    if constexpr (DKV) {
+      fill(R64{}, c1, qb, C3, cb, PITCH_C, C_HALF, sc);
+      fill(R64{}, c2, ob, H, cb, PITCH_C, C_HALF, sdo);
+    } else {
+      fill(R64{}, c1, qb + H, C3, cb, PITCH_C, C_HALF, sc);
+      fill(R64{}, c2, qb + 2 * H, C3, cb, PITCH_C, C_HALF, sc);
+    }
+    fence_proxy_async();
+    __syncthreads();
+    // ---- acc1 = R1 C1^T (scores), acc2 = R2 C2^T (dP) ----
+    wg::fence();
+#pragma unroll
+    for (int k16 = 0; k16 < HD / 16; ++k16) {
+      const uint32_t ao = a_rows + (uint32_t)(k16 * 2 * PITCH_K), bo = (uint32_t)(k16 * 2 * PITCH_C);
+      const uint64_t ah = wg::desc(r1_base + ao, PITCH_K, 128), al = wg::desc(r1_base + K_HALF + ao, PITCH_K, 128);
+      const uint64_t bh_ = wg::desc(c1_base + bo, PITCH_C, 128), bl = wg::desc(c1_base + C_HALF + bo, PITCH_C, 128);
+      wg::wgmma_f16_ss_n64<0, 0>(acc1, ah, bh_, k16 > 0 ? 1u : 0u);
+      wg::wgmma_f16_ss_n64<0, 0>(acc1, al, bh_, 1u);
+      wg::wgmma_f16_ss_n64<0, 0>(acc1, ah, bl, 1u);
+      const uint64_t dh = wg::desc(r2_base + ao, PITCH_K, 128), dl = wg::desc(r2_base + K_HALF + ao, PITCH_K, 128);
+      const uint64_t eh = wg::desc(c2_base + bo, PITCH_C, 128), el = wg::desc(c2_base + C_HALF + bo, PITCH_C, 128);
+      wg::wgmma_f16_ss_n64<0, 0>(acc2, dh, eh, k16 > 0 ? 1u : 0u);
+      wg::wgmma_f16_ss_n64<0, 0>(acc2, dl, eh, 1u);
+      wg::wgmma_f16_ss_n64<0, 0>(acc2, dh, el, 1u);
+    }
+    wg::commit();
+    wg::wait<0>();
+    wg::fence_regs<BN / 2>(acc1);
+    wg::fence_regs<BN / 2>(acc2);
+
+    // keep bits: bit 2 j + c of keep[i] <-> element (row frow + 8 i, column 8 j + 2 fk + c) of this block
+    uint32_t keep[2] = {0u, 0u};
+    if constexpr (DROP) {
+      if constexpr (DKV) {
+        // rows are keys: the four lanes (lane >> 2) & 3 = 0..3 hold the four keys of one Philox group for every column;
+        // lane u of the four generates the groups of the combinations 4 n + u of (i, j, c) and hands them round
+        const int u = (lane >> 2) & 3;
+        const uint64_t key4 = (uint64_t)(r0 + (frow & ~3));
+        uint32_t gen[8];
+#pragma unroll
+        for (int n = 0; n < 8; ++n) {
+          const int ic = 4 * n + u, i = ic >> 4, j = (ic >> 1) & 7, c = ic & 1;
+          const uint64_t q = (uint64_t)(cb + 8 * j + 2 * fk + c);
+          gen[n] = keep_bits4(seed, ((bh * S + q) * S + key4 + 8 * i) >> 2, dm.t);
+        }
+#pragma unroll
+        for (int ic = 0; ic < 32; ++ic) {
+          const uint32_t w = __shfl_sync(0xffffffffu, gen[ic >> 2], (lane & ~12) | ((ic & 3) << 2));
+          keep[ic >> 4] |= ((w >> u) & 1u) << (ic & 15);
+        }
+      } else {
+        const uint64_t row0 = (bh * S + r0 + frow + 8 * (fk & 1)) * S + cb + 4 * (fk >> 1);
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+          const uint32_t bits = keep_bits4(seed, (row0 + 8 * j) >> 2, dm.t);
+          const uint32_t b0 = __shfl_sync(0xffffffffu, bits, lane & ~1), b1 = __shfl_sync(0xffffffffu, bits, lane | 1);
+          keep[0] |= ((b0 >> (2 * (fk & 1))) & 3u) << (2 * j);
+          keep[1] |= ((b1 >> (2 * (fk & 1))) & 3u) << (2 * j);
+        }
+      }
+    }
+    // ---- P (the forward's pass-1 expression), dS; split into the A-operand blocks ----
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      float cm[2], crl[2], cd[2];
+      if constexpr (DKV) {                          // columns are queries: their statistics
+        const int q = cb + 8 * j + 2 * fk;
+        const float2 m2 = *reinterpret_cast<const float2*>(mg + q), l2 = *reinterpret_cast<const float2*>(lg + q);
+        const float2 d2 = *reinterpret_cast<const float2*>(dg + q);
+        cm[0] = m2.x; cm[1] = m2.y; crl[0] = 1.0f / l2.x; crl[1] = 1.0f / l2.y; cd[0] = d2.x; cd[1] = d2.y;
+      }
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int rit = frow + 8 * i;
+        float dv[2], pk[2];
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int row = r0 + rit, col = cb + 8 * j + 2 * fk + c;
+          const int q = DKV ? col : row, key = DKV ? row : col;
+          const float m_ = DKV ? cm[c] : qm[i], rl_ = DKV ? crl[c] : qrl[i], d_ = DKV ? cd[c] : qd[i];
+          const int e = 4 * j + 2 * i + c;
+          const float pr = key > q ? 0.f : expf(acc1[e] * ss - m_) * rl_;
+          const bool kept = !DROP || ((keep[i] >> (2 * j + c)) & 1u);
+          const float g = kept ? acc2[e] * sdp * dsc : 0.f;
+          pk[c] = kept ? pr : 0.f;
+          dv[c] = pr * (g - d_);
+        }
+        uint32_t hi, lo;
+        split2(dv[0], dv[1], sds, &hi, &lo);
+        uint8_t* d = ds_blk + (size_t)j * PITCH_P + rit * 16 + fk * 4;
+        *reinterpret_cast<uint32_t*>(d) = hi;
+        *reinterpret_cast<uint32_t*>(d + B_HALF) = lo;
+        if constexpr (DKV) {
+          split2(pk[0], pk[1], P_SCALE, &hi, &lo);
+          uint8_t* e = p_blk + (size_t)j * PITCH_P + rit * 16 + fk * 4;
+          *reinterpret_cast<uint32_t*>(e) = hi;
+          *reinterpret_cast<uint32_t*>(e + B_HALF) = lo;
+        }
+      }
+    }
+    fence_proxy_async();
+    __syncthreads();
+    // ---- DKV: dK += dS^T Q, dV += (P o keep)^T dO; DQ: dQ += dS K (B operands MN-major from the streamed tiles) ----
+    wg::fence();
+#pragma unroll
+    for (int k16 = 0; k16 < BN / 16; ++k16) {
+      const uint32_t ao = a_rows + (uint32_t)(k16 * 2 * PITCH_P), bo = (uint32_t)(k16 * 256);
+      const uint64_t sh = wg::desc(ds_base + ao, PITCH_P, 128), sl = wg::desc(ds_base + B_HALF + ao, PITCH_P, 128);
+      const uint64_t xh = wg::desc(c1_base + bo, 128, PITCH_C), xl = wg::desc(c1_base + C_HALF + bo, 128, PITCH_C);
+      wg::wgmma_f16_ss_n64<0, 1>(g1, sh, xh, 1u);
+      wg::wgmma_f16_ss_n64<0, 1>(g1, sl, xh, 1u);
+      wg::wgmma_f16_ss_n64<0, 1>(g1, sh, xl, 1u);
+      if constexpr (DKV) {
+        const uint64_t ph = wg::desc(p_base + ao, PITCH_P, 128), pl = wg::desc(p_base + B_HALF + ao, PITCH_P, 128);
+        const uint64_t oh = wg::desc(c2_base + bo, 128, PITCH_C), ol = wg::desc(c2_base + C_HALF + bo, 128, PITCH_C);
+        wg::wgmma_f16_ss_n64<0, 1>(g2, ph, oh, 1u);
+        wg::wgmma_f16_ss_n64<0, 1>(g2, pl, oh, 1u);
+        wg::wgmma_f16_ss_n64<0, 1>(g2, ph, ol, 1u);
+      }
+    }
+    wg::commit();
+    wg::wait<0>();
+    wg::fence_regs<HD / 2>(g1);
+    if constexpr (DKV) wg::fence_regs<HD / 2>(g2);
+  }
+  // ---- epilogue: straight from the fragments into the fused [B, S, 3H] gradient ----
+  const float s1 = inv_ds * inv_s * p.scale, s2 = P_INV * inv_do * dsc;
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    float* orow = p.dqkv + ((size_t)b * S + r0 + frow + 8 * i) * C3 + h * HD + 2 * fk;
+#pragma unroll
+    for (int j = 0; j < HD / 8; ++j) {
+      if constexpr (DKV) {
+        *reinterpret_cast<float2*>(orow + H + 8 * j) = make_float2(g1[4 * j + 2 * i] * s1, g1[4 * j + 2 * i + 1] * s1);
+        *reinterpret_cast<float2*>(orow + 2 * H + 8 * j) = make_float2(g2[4 * j + 2 * i] * s2, g2[4 * j + 2 * i + 1] * s2);
+      } else {
+        *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(g1[4 * j + 2 * i] * s1, g1[4 * j + 2 * i + 1] * s1);
+      }
+    }
+  }
+}
+
+constexpr size_t BWD_SMEM_BYTES = 2 * (size_t)TILE + 4 * (size_t)C_HALF + 4 * (size_t)B_HALF;
+
 }  // namespace attnc
 
 bool attn_causal_fused_ok(int S, int heads, int hd) { return hd == attnc::HD && S % attnc::BM == 0 && S >= attnc::BM && heads > 0; }
@@ -284,7 +577,7 @@ bool attn_causal_fused_ok(int S, int heads, int hd) { return hd == attnc::HD && 
 
 using namespace mas;
 
-template <bool DROP>
+template <bool DROP, bool STATS = false>
 static int attn_causal_launch(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads, int hd, float scale,
                               const DropMask& dm, void* stream) {
   MAS_REQUIRE(qkv && amax && P && ctx && B > 0, "attn_causal_forward: bad arguments");
@@ -293,15 +586,17 @@ static int attn_causal_launch(const float* qkv, const float* amax, float* P, flo
   if (heads > 65535 || B > 65535) return fail(MAS_ERR_UNSUPPORTED, "attn_causal_forward: heads / batch beyond the grid limits");
   static std::atomic<uint64_t> configured{0};
   if (first_on_device(configured)) {
-    cudaError_t e = cudaFuncSetAttribute(attnc::attn_causal_fwd<DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)attnc::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(attnc::attn_causal_fwd<DROP, STATS>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)attnc::SMEM_BYTES);
     if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "attn_causal_fwd: smem attr: %s", cudaGetErrorString(e));
     mark_device(configured);
   }
   attnc::Params p;
   p.qkv = qkv; p.P = P; p.ctx = ctx; p.amax = amax; p.S = S; p.heads = heads; p.scale = scale;
   const dim3 grid((unsigned)(S / attnc::BM), (unsigned)heads, (unsigned)B);
-  attnc::attn_causal_fwd<DROP><<<grid, attnc::NTHREADS, attnc::SMEM_BYTES, mas::S(stream)>>>(p, dm);
-  return launched_tc(DROP ? "attn_causal_dropout_fwd" : "attn_causal_fwd");
+  attnc::attn_causal_fwd<DROP, STATS><<<grid, attnc::NTHREADS, attnc::SMEM_BYTES, mas::S(stream)>>>(p, dm);
+  return launched_tc(STATS ? (DROP ? "attn_causal_dropout_fwd_stats" : "attn_causal_fwd_stats")
+                           : (DROP ? "attn_causal_dropout_fwd" : "attn_causal_fwd"));
 }
 
 extern "C" int mas_attn_causal_forward(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads, int hd,
@@ -313,4 +608,53 @@ extern "C" int mas_attn_causal_dropout_forward(const float* qkv, const float* am
                                                int hd, float scale, double p, const int64_t* seed, void* stream) {
   MAS_REQUIRE(seed && p >= 0.0 && p <= 1.0, "attn_causal_dropout_forward: bad dropout arguments");
   return attn_causal_launch<true>(qkv, amax, P, ctx, B, S, heads, hd, scale, DropMask{seed, drop_threshold(p), drop_scale(p)}, stream);
+}
+
+extern "C" int mas_attn_causal_forward_stats(const float* qkv, const float* amax, float* stats, float* ctx, int B, int S, int heads,
+                                             int hd, float scale, double p, const int64_t* seed, void* stream) {
+  MAS_REQUIRE(p >= 0.0 && p <= 1.0 && (p == 0.0 || seed), "attn_causal_forward_stats: bad dropout arguments");
+  if (p > 0.0)
+    return attn_causal_launch<true, true>(qkv, amax, stats, ctx, B, S, heads, hd, scale,
+                                          DropMask{seed, drop_threshold(p), drop_scale(p)}, stream);
+  return attn_causal_launch<false, true>(qkv, amax, stats, ctx, B, S, heads, hd, scale, DropMask{nullptr, 0, 1.f}, stream);
+}
+
+template <bool DKV, bool DROP>
+static int attn_causal_bwd_launch(const attnc::BwdParams& p, const DropMask& dm, int B, void* stream) {
+  static std::atomic<uint64_t> configured{0};
+  if (first_on_device(configured)) {
+    cudaError_t e = cudaFuncSetAttribute(attnc::attn_causal_bwd<DKV, DROP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)attnc::BWD_SMEM_BYTES);
+    if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "attn_causal_bwd: smem attr: %s", cudaGetErrorString(e));
+    mark_device(configured);
+  }
+  const dim3 grid((unsigned)(p.S / attnc::BM), (unsigned)p.heads, (unsigned)B);
+  attnc::attn_causal_bwd<DKV, DROP><<<grid, attnc::NTHREADS, attnc::BWD_SMEM_BYTES, mas::S(stream)>>>(p, dm);
+  return launched_tc(DKV ? (DROP ? "attn_causal_dropout_bwd_dkv" : "attn_causal_bwd_dkv")
+                         : (DROP ? "attn_causal_dropout_bwd_dq" : "attn_causal_bwd_dq"));
+}
+
+extern "C" int mas_attn_causal_backward(const float* qkv, const float* ctx, const float* dctx, const float* stats, const float* amax,
+                                        const float* dctx_amax, float* D, float* dqkv, int B, int S, int heads, int hd, float scale,
+                                        double p, const int64_t* seed, void* stream) {
+  MAS_REQUIRE(qkv && ctx && dctx && stats && amax && dctx_amax && D && dqkv && B > 0, "attn_causal_backward: bad arguments");
+  MAS_REQUIRE(p >= 0.0 && p <= 1.0 && (p == 0.0 || seed), "attn_causal_backward: bad dropout arguments");
+  if (!attn_causal_fused_ok(S, heads, hd))
+    return fail(MAS_ERR_UNSUPPORTED, "attn_causal_backward: needs head dim 64 and S %% 128 == 0 (got S=%d, hd=%d)", S, hd);
+  if (heads > 65535 || B > 65535) return fail(MAS_ERR_UNSUPPORTED, "attn_causal_backward: heads / batch beyond the grid limits");
+  const int64_t rows = (int64_t)B * S * heads;
+  attnc::attn_causal_bwd_rowdot<<<(unsigned)((rows + 7) / 8), 256, 0, mas::S(stream)>>>(dctx, ctx, D, S, heads, rows);
+  int rc = launched_tc("attn_causal_bwd_rowdot");
+  if (rc != MAS_OK) return rc;
+  attnc::BwdParams bp;
+  bp.qkv = qkv; bp.dctx = dctx; bp.stats = stats; bp.D = D; bp.dqkv = dqkv; bp.amax = amax; bp.amax_do = dctx_amax;
+  bp.S = S; bp.heads = heads; bp.scale = scale;
+  if (p > 0.0) {
+    const DropMask dm{seed, drop_threshold(p), drop_scale(p)};
+    rc = attn_causal_bwd_launch<true, true>(bp, dm, B, stream);
+    return rc != MAS_OK ? rc : attn_causal_bwd_launch<false, true>(bp, dm, B, stream);
+  }
+  const DropMask dm{nullptr, 0, 1.f};
+  rc = attn_causal_bwd_launch<true, false>(bp, dm, B, stream);
+  return rc != MAS_OK ? rc : attn_causal_bwd_launch<false, false>(bp, dm, B, stream);
 }

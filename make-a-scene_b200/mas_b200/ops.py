@@ -1601,21 +1601,37 @@ class CausalAttentionFn(torch.autograd.Function):
     (transformer.py:77-103; head h owns columns h*hd..(h+1)*hd of each third). Every contraction is ONE launch over all
     (batch element, head) pairs (two-level batch strides: the heads are column slices of the fused activation).
     p > 0: attention dropout on the probabilities (transformer.py:90-91), ctx = (P * keep) v / (1 - p). P is kept undropped for
-    the backward and the mask is regenerated from the saved seed; no mask tensor is stored."""
+    the backward and the mask is regenerated from the saved seed; no mask tensor is stored.
+    recompute=True: nothing S x S is stored. The forward keeps each row's softmax maximum and sum instead of P
+    (mas_attn_causal_forward_stats, ctx the same bits) and the backward recomputes P in one fused call
+    (mas_attn_causal_backward). Only the fused core's shapes (head dim 64, S % 128 == 0, tensor path) have this route; any
+    other raises RuntimeError."""
 
     @staticmethod
-    def forward(ctx, qkv, heads, p=0.0):
+    def forward(ctx, qkv, heads, p=0.0, recompute=False):
         _need_cuda(qkv)
         qkv = qkv.contiguous()
         B, S_, H3 = qkv.shape
         H = H3 // 3
         hd = H // heads
         alpha = 1.0 / float(hd) ** 0.5
+        p = float(p)
+        ctx.heads, ctx.p, ctx.recompute = heads, p, bool(recompute)
+        if recompute:
+            if not attn_causal_fused_on(S_, hd):
+                raise RuntimeError("recomputed attention needs the fused causal core: head dim 64, S %% 128 == 0 and the tensor "
+                                   "path with MAS_ATTN_FUSED != 0 (got S=%d, head dim %d)" % (S_, hd))
+            am = amax(qkv)
+            stats = torch.empty((2, B, heads, S_), dtype=torch.float32, device=qkv.device)      # row maxima, row sums
+            ctxv = torch.empty((B, S_, H), dtype=torch.float32, device=qkv.device)
+            seed = dropout_seed(qkv.device) if p > 0 else None
+            L.call("mas_attn_causal_forward_stats", qkv, am, stats, ctxv, B, S_, heads, hd, alpha, p, seed)
+            ctx.save_for_backward(qkv, ctxv, stats, am, seed)
+            return ctxv
         impl = _attn_impl(S_, hd)
         P = torch.empty((B, heads, S_, S_), dtype=torch.float32, device=qkv.device)
         ctxv = torch.empty((B, S_, H), dtype=torch.float32, device=qkv.device)
         SS = S_ * S_
-        p = float(p)
         seed = dropout_seed(qkv.device) if p > 0 else None
         if attn_causal_fused_on(S_, hd):
             # scores, causal softmax and P v in one kernel per (sequence, head, 128-query tile); P is written once for the backward
@@ -1639,15 +1655,23 @@ class CausalAttentionFn(torch.autograd.Function):
             ctx.save_for_backward(qkv, P, seed)
         else:
             ctx.save_for_backward(qkv, P)
-        ctx.heads, ctx.p = heads, p
         return ctxv
 
     @staticmethod
     def backward(ctx, dctx):
-        qkv, P = ctx.saved_tensors[:2]
         p = ctx.p
         dctx = dctx.contiguous()
         heads = ctx.heads
+        if ctx.recompute:
+            qkv, ctxv, stats, am, seed = ctx.saved_tensors
+            B, S_, H3 = qkv.shape
+            hd = H3 // 3 // heads
+            dqkv = torch.empty_like(qkv)
+            D = torch.empty((B, heads, S_), dtype=torch.float32, device=qkv.device)
+            L.call("mas_attn_causal_backward", qkv, ctxv, dctx, stats, am, amax(dctx), D, dqkv, B, S_, heads, hd,
+                   1.0 / float(hd) ** 0.5, p, seed)
+            return dqkv, None, None, None
+        qkv, P = ctx.saved_tensors[:2]
         B, S_, H3 = qkv.shape
         H = H3 // 3
         hd = H // heads
@@ -1675,7 +1699,7 @@ class CausalAttentionFn(torch.autograd.Function):
         # dQ = dS K ; dK = dS^T Q
         gemm2(dP, (qkv, H), dqkv, S_, hd, S_, B, heads, S_, H3, H3, op_, oq, oq, SS, hd, hd, impl=impl, causal=1)
         gemm2(dP, qkv, (dqkv, H), S_, hd, S_, B, heads, S_, H3, H3, op_, oq, oq, SS, hd, hd, ta=True, impl=impl, causal=2)
-        return dqkv, None, None
+        return dqkv, None, None, None
 
 
 class CrossEntropyFn(torch.autograd.Function):

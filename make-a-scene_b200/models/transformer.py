@@ -51,8 +51,12 @@ def _dropout(x, mod, residual=None):
 
 
 class SelfAttention(nn.Module):
-    def __init__(self, hidden_dim, num_attn_heads, attn_dropout_prob, out_dropout_prob, cogview_pb_relax=True, rudalle_relax=False):
+    def __init__(self, hidden_dim, num_attn_heads, attn_dropout_prob, out_dropout_prob, cogview_pb_relax=True, rudalle_relax=False,
+                 recompute_attention=False):
+        """recompute_attention: the attention stores no S x S probabilities for the backward and recomputes them there
+        (ops.CausalAttentionFn(recompute=True)); less memory for more arithmetic. Needs head dim 64 and S % 128 == 0."""
         super().__init__()
+        self.recompute_attention = recompute_attention
         self.hidden_dim = hidden_dim
         self.num_attn_heads = num_attn_heads
         self.d = math.sqrt(self.hidden_dim // self.num_attn_heads)
@@ -72,7 +76,8 @@ class SelfAttention(nn.Module):
 
     def project(self, x):
         """out_proj(attention) with attention dropout, before out_drop (TransformerLayer fuses out_drop into the next kernel)."""
-        return self.out_proj(ops.CausalAttentionFn.apply(self.qkv(x), self.num_attn_heads, _drop_p(self.attn_drop)))
+        return self.out_proj(ops.CausalAttentionFn.apply(self.qkv(x), self.num_attn_heads, _drop_p(self.attn_drop),
+                                                          self.recompute_attention))
 
 
 class MLP(nn.Module):
@@ -95,7 +100,7 @@ class MLP(nn.Module):
 
 class TransformerLayer(nn.Module):
     def __init__(self, hidden_dim, num_attn_heads, attn_dropout_prop, out_dropout_prob, cogview_pb_relax=True,
-                 cogview_sandwich_layernorm=True, cogview_layernorm_prescale=False, rudalle_relax=False):
+                 cogview_sandwich_layernorm=True, cogview_layernorm_prescale=False, rudalle_relax=False, recompute_attention=False):
         super().__init__()
         self.cogview_pb_relax = cogview_pb_relax
         self.cogview_sandwich_layernorm = cogview_sandwich_layernorm
@@ -109,7 +114,8 @@ class TransformerLayer(nn.Module):
             self.first_ln_sandwich = LayerNorm(hidden_dim, eps=1e-5)
             self.second_ln_sandwich = LayerNorm(hidden_dim, eps=1e-5)
         self.attn = SelfAttention(hidden_dim=hidden_dim, num_attn_heads=num_attn_heads, attn_dropout_prob=attn_dropout_prop,
-                                  out_dropout_prob=out_dropout_prob, cogview_pb_relax=cogview_pb_relax, rudalle_relax=rudalle_relax)
+                                  out_dropout_prob=out_dropout_prob, cogview_pb_relax=cogview_pb_relax, rudalle_relax=rudalle_relax,
+                                  recompute_attention=recompute_attention)
         self.mlp = MLP(hidden_dim=hidden_dim, dropout_prob=out_dropout_prob, rudalle_relax=rudalle_relax)
 
     def forward(self, x, mask=None, cache=None, use_cache=False, mlp_cache=False):
@@ -133,14 +139,15 @@ class TransformerLayer(nn.Module):
 class Transformer(nn.Module):
     def __init__(self, num_layers, hidden_dim, num_attn_heads, image_tokens_per_dim, seg_tokens_per_dim, text_length,
                  attn_dropout_prop=0, out_dropout_prob=0, cogview_pb_relax=True, cogview_sandwich_layernorm=True,
-                 cogview_layernorm_prescale=False, rudalle_relax=False):
+                 cogview_layernorm_prescale=False, rudalle_relax=False, recompute_attention=False):
         super().__init__()
         self.num_layers = num_layers
         self.cogview_pb_relax = cogview_pb_relax
         self.rudalle_relax = rudalle_relax
         self.layers = nn.ModuleList([
             TransformerLayer(hidden_dim, num_attn_heads, attn_dropout_prop, out_dropout_prob, cogview_pb_relax,
-                             cogview_sandwich_layernorm, cogview_layernorm_prescale, rudalle_relax) for _ in range(num_layers)])
+                             cogview_sandwich_layernorm, cogview_layernorm_prescale, rudalle_relax, recompute_attention)
+            for _ in range(num_layers)])
         self.register_buffer("mask", self._create_mask(text_length, seg_tokens_per_dim, image_tokens_per_dim))
         self.final_ln = LayerNorm(hidden_dim, eps=1e-5)
 
@@ -249,10 +256,15 @@ class _GraphedDecoder:
 
 class MakeAScene(nn.Module):
     def __init__(self, num_layers, hidden_dim, num_attn_heads, image_vocab_size, seg_vocab_size, text_vocab_size,
-                 image_tokens_per_dim, seg_tokens_per_dim, text_length, attn_dropout_prob=0.0, out_dropout_prob=0.0):
+                 image_tokens_per_dim, seg_tokens_per_dim, text_length, attn_dropout_prob=0.0, out_dropout_prob=0.0,
+                 recompute_attention=False):
         """The reference's arguments, plus the dropout probabilities of every layer's attention probabilities
         (attn_dropout_prob) and of its attention and MLP outputs (out_dropout_prob), passed to Transformer; the reference's
-        MakeAScene leaves both at 0, which the defaults keep."""
+        MakeAScene leaves both at 0, which the defaults keep.
+        recompute_attention=True: training stores no attention probabilities (S x S per head and sequence) for the backward,
+        which recomputes them from per-row statistics; the loss is the same bits, the gradients agree to fp32 rounding.
+        Needs head dim 64 and a sequence length that is a multiple of 128 (RuntimeError otherwise). Not a parameter or
+        buffer: the state_dict is unchanged."""
         super().__init__()
         self.image_tokens_per_dim = image_tokens_per_dim
         self.seg_tokens_per_dim = seg_tokens_per_dim
@@ -263,7 +275,7 @@ class MakeAScene(nn.Module):
         self.text_vocab_size = text_vocab_size
         self.hidden_dim = hidden_dim
         self.transformer = Transformer(num_layers, hidden_dim, num_attn_heads, image_tokens_per_dim, seg_tokens_per_dim, text_length,
-                                       attn_dropout_prob, out_dropout_prob)
+                                       attn_dropout_prob, out_dropout_prob, recompute_attention=recompute_attention)
         self.image_token_embedding = nn.Embedding(image_vocab_size, hidden_dim)
         self.seg_token_embedding = nn.Embedding(seg_vocab_size, hidden_dim)
         self.text_token_embedding = nn.Embedding(text_vocab_size, hidden_dim)
@@ -326,14 +338,16 @@ class MakeAScene(nn.Module):
     # ---- sampling (SURVEY.md 8f-3) ---------------------------------------------------------------------------
     def _prefill(self, emb, kc=None, vc=None):
         """Full causal pass over emb [B,S,H] with the training kernels and no dropout; returns every position's hidden state
-        before final_ln [B,S,H]. With kc / vc (generate's prefix pass) every layer's k / v are recorded at positions 0..S-1."""
+        before final_ln [B,S,H]. With kc / vc (generate's prefix pass) every layer's k / v are recorded at positions 0..S-1.
+        Where the fused core runs, the attention writes no probabilities (nothing reads them here): the same outputs."""
         x = emb
         heads = self.transformer.layers[0].attn.num_attn_heads
+        stats_only = ops.attn_causal_fused_on(x.shape[1], self.hidden_dim // heads)
         for li, layer in enumerate(self.transformer.layers):
             qkv = layer.attn.qkv(layer.ln_in(x))
             if kc is not None:
                 ops.kv_append(qkv, kc[li], vc[li], 0)
-            a = layer.attn.out_proj(ops.CausalAttentionFn.apply(qkv, heads))
+            a = layer.attn.out_proj(ops.CausalAttentionFn.apply(qkv, heads, 0.0, stats_only))
             x = layer.first_ln_sandwich(a, residual=x) if layer.cogview_sandwich_layernorm else x + a
             m = layer.mlp.project(layer.ln_out(x))
             x = layer.second_ln_sandwich(m, residual=x) if layer.cogview_sandwich_layernorm else x + m

@@ -2,7 +2,10 @@
 128 text + 256 segmentation + 256 image tokens, 8192-code image vocabulary; random-init weights, synthetic tokens):
 forward + cross-entropy over the image tokens + backward (train.py:136-153; no optimizer), CUDA-event timed.
 One JSON line; beside bench.py's headline (tier 2, SURVEY.md 8f-2).
-Usage: python tools/bench_transformer.py [--batch B] [--steps K] [--warmup W] [--layers L] [--dropout P]"""
+--image-tokens-per-dim 32 runs the sequence the VQ configs produce (128 + 16^2 + 32^2 = 1408 tokens); --recompute-attention
+trains with MakeAScene(recompute_attention=True) (no stored attention probabilities).
+Usage: python tools/bench_transformer.py [--batch B] [--steps K] [--warmup W] [--layers L] [--dropout P]
+       [--image-tokens-per-dim N] [--recompute-attention]"""
 import argparse
 import json
 import os
@@ -22,18 +25,22 @@ ap.add_argument("--layers", type=int, default=24)
 ap.add_argument("--dropout", type=float, default=0.0, help="attention and residual dropout probability (both)")
 ap.add_argument("--profile", action="store_true", help="per-entry-point CUDA-event times of one extra step (stderr)")
 ap.add_argument("--torch-ce", action="store_true", help="F.cross_entropy on the logits instead of MakeAScene.loss (A/B of the fused entry)")
+ap.add_argument("--image-tokens-per-dim", type=int, default=16, help="image tokens per side (sequence = 128 + 256 + N^2)")
+ap.add_argument("--recompute-attention", action="store_true", help="store no attention probabilities; the backward recomputes them")
 args = ap.parse_args()
 dev = torch.device("cuda:0")
 torch.manual_seed(0)
 cfg = dict(num_layers=args.layers, hidden_dim=1024, num_attn_heads=16, image_vocab_size=8192, seg_vocab_size=1024, text_vocab_size=49408,
-           image_tokens_per_dim=16, seg_tokens_per_dim=16, text_length=128)
-m = MakeAScene(**cfg, attn_dropout_prob=args.dropout, out_dropout_prob=args.dropout).to(dev).train()
+           image_tokens_per_dim=args.image_tokens_per_dim, seg_tokens_per_dim=16, text_length=128)
+m = MakeAScene(**cfg, attn_dropout_prob=args.dropout, out_dropout_prob=args.dropout,
+               recompute_attention=args.recompute_attention).to(dev).train()
+IMG = args.image_tokens_per_dim ** 2
 m.device = dev
 B = args.batch
 g = torch.Generator().manual_seed(1234)
 text = torch.randint(1, 40000, (B, 128), generator=g).to(dev)
 seg = torch.randint(0, 1024, (B, 256), generator=g).to(dev)
-img = torch.randint(0, 8192, (B, 256), generator=g).to(dev)
+img = torch.randint(0, 8192, (B, IMG), generator=g).to(dev)
 
 
 def step():
@@ -66,13 +73,14 @@ if args.profile:
     for k, (c, t) in sorted(rep.items(), key=lambda kv: -kv[1][1])[:24]:
         print("  %-36s n=%4d  %8.2f ms  %5.1f%%  %7.3f ms/call" % (k, c, t, 100 * t / tot, t / c), file=sys.stderr)
     print("  total %.2f ms in %d calls" % (tot, sum(c for c, _ in rep.values())), file=sys.stderr)
-S, H, L, V = 640, 1024, args.layers, 8192
-lin = 2 * S * (12 * H * H) * L + 2 * 256 * H * V           # Linear layers, forward, per sequence
+S, H, L, V = 128 + 256 + IMG, 1024, args.layers, 8192
+lin = 2 * S * (12 * H * H) * L + 2 * IMG * H * V           # Linear layers, forward, per sequence
 att = 2 * 2 * S * S * H * L                                # QK^T and PV over the full (masked) square, forward
 print(json.dumps({"metric": "token transformer training step (fwd + cross-entropy + bwd), sequence tokens/s", "value": B * S / sec,
                   "unit": "tokens/s", "batch": B, "seq_len": S, "ms_per_step": sec * 1e3, "loss": float(loss),
                   "model_tflops": 3 * (lin + att) * B / sec / 1e12, "gpu_launches_per_step": (_lib.launch_count() - l0) // args.steps,
                   "tensor_core_launches_per_step": (_lib.tc_launch_count() - t0) // args.steps,
                   "peak_mem_gb": torch.cuda.max_memory_allocated() / 1e9, "dropout": args.dropout,
-                  "attention": "fused core (attn_causal_fwd)" if os.environ.get("MAS_ATTN_FUSED", "1") != "0" else "GEMM / softmax / GEMM",
+                  "attention": ("recomputed P (attn_causal_fwd_stats + attn_causal_bwd)" if args.recompute_attention else
+                                "fused core (attn_causal_fwd)" if os.environ.get("MAS_ATTN_FUSED", "1") != "0" else "GEMM / softmax / GEMM"),
                   "loss_entry": "F.cross_entropy (torch)" if args.torch_ce else "MakeAScene.loss (mas_ce_*)", "config": cfg}))
