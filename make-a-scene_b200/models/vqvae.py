@@ -7,9 +7,14 @@ initial weights and checkpoints load in both directions.
 import torch
 from torch import nn
 
-from mas_b200 import ops
+from mas_b200 import ops, scene
 
-from .modules import Codebook, Conv2d, Decoder, Encoder
+from .modules import Codebook, Conv2d, Decoder, Downsample, Encoder
+
+
+def _kernel_device(t):
+    """Whether t lives where the kernels run."""
+    return t.is_cuda
 
 
 class QuantBatchNorm(nn.SyncBatchNorm):
@@ -52,6 +57,48 @@ class VQBASE(nn.Module):
             shape = (b, h, w, self.quantize.codebook_dim)
         quant_b = self.quantize.get_codebook_entry(code_b.reshape(-1), shape)
         return self.decode(quant_b)
+
+    def encode_code(self, x):
+        """Codebook indices of an input: the counterpart of decode_code, for tokenizing images and scene maps for the token
+        transformer (MakeAScene's img_tokens / seg_tokens are encode_code(x).flatten(1)).
+
+        x: an fp32 image batch [B, in_channels, H, W], a dense fp32 scene map [B, 159, H, W] or a compact scene map uint8
+        [B, 4, H, W] (mas_b200.scene; only when conv_in takes 159 channels), a CUDA tensor on the model's device, H and W
+        multiples of the encoder's downsampling factor f = 2^(len(channels) - 2).
+        Returns int64 [B, H/f, W/f], row-major: flatten(1) puts position (i, j) at t = i * w + j, which is where MakeAScene
+        adds row embedding i and column embedding j, and decode_code(tokens) is the inverse.
+
+        Always the eval-mode encoding, whatever the module's mode: encoder -> quant_conv[0] -> BatchNorm with the running
+        statistics -> codebook arg-min (the forward's kernels). Codebook.forward and QuantBatchNorm.forward are not called,
+        so nothing changes: no step counter, reservoir, k-means re-initialisation, running statistics or collective, and the
+        module's mode is left alone. No autograd graph is recorded, even under torch.enable_grad(). Raises ValueError on a
+        tensor off the model's device or not on CUDA, a wrong dtype or channel count, or H / W off the downsampling factor."""
+        conv_in = self.encoder.model[0]
+        dev = conv_in.weight.device
+        if not isinstance(x, torch.Tensor) or x.dim() != 4:
+            raise ValueError("encode_code expects a 4-D [B, C, H, W] tensor, got %s"
+                             % (str(tuple(x.shape)) if isinstance(x, torch.Tensor) else type(x).__name__))
+        if not _kernel_device(x) or x.device != dev:
+            raise ValueError("encode_code needs a CUDA tensor on the model's device (%s), got one on %s" % (dev, x.device))
+        b, c, h, w = x.shape
+        if x.dtype == torch.uint8:
+            if conv_in.in_channels != scene.CHANNELS or c != scene.PLANES:
+                raise ValueError("a uint8 input is a compact scene map [B, %d, H, W] for a model whose conv_in takes %d "
+                                 "channels; got shape %s for conv_in with %d" % (scene.PLANES, scene.CHANNELS, tuple(x.shape),
+                                                                                 conv_in.in_channels))
+        elif x.dtype != torch.float32:
+            raise ValueError("encode_code takes float32 images / scene maps or uint8 compact scene maps, got %s" % x.dtype)
+        elif c != conv_in.in_channels:
+            raise ValueError("expected %d input channels (conv_in), got shape %s" % (conv_in.in_channels, tuple(x.shape)))
+        f = 2 ** sum(isinstance(m, Downsample) for m in self.encoder.model)
+        if b == 0 or h == 0 or w == 0 or h % f or w % f:
+            raise ValueError("encode_code needs a non-empty batch with H and W multiples of %d, got shape %s" % (f, tuple(x.shape)))
+        bn = self.quant_conv[1]
+        with torch.no_grad():
+            z = self.quant_conv[0](self.encoder(x))
+            z = ops.batchnorm_eval(z, bn.weight, bn.bias, bn.running_mean, bn.running_var, bn.eps)
+            _, _, idx = ops.VQFn.apply(z, self.quantize.embedding.weight, self.quantize.beta)
+        return idx.view(b, h // f, w // f)
 
     def forward(self, input):
         """-> (dec, diff) exactly like vqvae.py:36-39 (train.py:84 unpacks this pair)."""
