@@ -59,6 +59,12 @@ const char* mas_last_error(void);
 int64_t mas_launch_count(void);
 /* ... of which kernels that issue wgmma tensor-core MMAs (the driver's evidence that the tensor path ran). */
 int64_t mas_tc_launch_count(void);
+/* Launch trace (a test and measurement aid): mas_launch_trace(1) clears the trace and records the name of every kernel the
+ * library launches from then on (host side, in launch order, one per line; hd-128 attention kernels carry a "<128>"
+ * suffix); mas_launch_trace(0) clears it and stops.  mas_launch_trace_read copies the trace, NUL-terminated and cut to
+ * cap - 1 bytes, into buf (may be NULL) and returns its full length in bytes. */
+int mas_launch_trace(int on);
+int64_t mas_launch_trace_read(char* buf, int64_t cap);
 
 /* Measurement aid for bench.py: runs a pure-FFMA kernel (16 independent chains per thread, 148*4 blocks of 512 threads,
  * 128*iters FMAs per thread); *flops_out_host (HOST pointer, may be NULL) receives the FLOPs of one launch. `scratch`
@@ -461,7 +467,7 @@ int mas_embed3_backward(const float* dout, const int64_t* id0, float* d0, const 
 /* Causal self-attention core of the token transformer, fused (transformer.py:77-103; csrc/attn_causal.cu): per (sequence,
  * head, 128-query tile) S = q k^T * scale in registers -> causal softmax on the accumulator fragment -> P (written once, [B,heads,S,S],
  * zeros above the diagonal: the backward reads it) -> ctx = P v accumulated in registers.  qkv [B,S,3*heads*hd] fused
- * q|k|v, ctx [B,S,heads*hd], amax = device scalar max|qkv| (mas_amax).  Needs hd == 64 and S % 128 == 0
+ * q|k|v, ctx [B,S,heads*hd], amax = device scalar max|qkv| (mas_amax).  Needs hd == 64 or 128 and S % 128 == 0
  * (MAS_ERR_UNSUPPORTED otherwise: the caller runs the GEMM / softmax sequence).  2 x fp16 operand split = fp32-level accuracy. */
 int mas_attn_causal_forward(const float* qkv, const float* amax, float* P, float* ctx, int B, int S, int heads, int hd,
                             float scale, void* stream);
@@ -469,11 +475,11 @@ int mas_attn_causal_forward(const float* qkv, const float* amax, float* P, float
  * mas_attn_causal_forward (p = 0) / mas_attn_causal_dropout_forward (p > 0, same seed), and instead of P the kernel writes
  * every row's maximum m and sum l of the scaled scores, P = exp(S - m) / l: stats = m [B,heads,S] followed by
  * l [B,heads,S] (2 * B * heads * S floats).  0 <= p <= 1; seed may be NULL when p == 0.  Same shape limits as
- * mas_attn_causal_forward (MAS_ERR_UNSUPPORTED off hd == 64 / S % 128 == 0; the GEMM sequence has no P-free form).
+ * mas_attn_causal_forward (MAS_ERR_UNSUPPORTED off hd == 64 or 128 / S % 128 == 0; the GEMM sequence has no P-free form).
  * mas_attn_causal_backward: the fused backward from those statistics; nothing S x S is read or written.  qkv and ctx of the
  * forward, dctx [B,S,heads*hd] its output gradient, stats the forward's, amax = max|qkv| (the forward's device scalar),
  * dctx_amax = max|dctx| (mas_amax), D a workspace of B * heads * S floats (row dot products dctx . ctx), p / seed those of
- * the forward.  Writes dqkv [B,S,3*heads*hd] fully (q | k | v thirds).  P is recomputed per 128 x 64 tile from the
+ * the forward.  Writes dqkv [B,S,3*heads*hd] fully (q | k | v thirds).  P is recomputed per 128 x 64 tile (128 x 32 at hd 128) from the
  * statistics with the forward's expression, the dropout mask regenerated; dK / dV accumulate over the query blocks of a
  * 128-key tile, dQ over the key blocks of a 128-query tile, in registers: no atomics, two calls give the same bits.
  * 2 x fp16 operand split (fp32-level accuracy) with power-of-two scales derived on the device: max|qkv|, max|dctx|, 2^14

@@ -5,6 +5,10 @@
 
 #include <cuda_fp16.h>
 #include <stdlib.h>
+#include <string.h>
+
+#include <mutex>
+#include <string>
 
 #include "mas_common.cuh"
 #include "tc_ptx.cuh"
@@ -23,8 +27,18 @@ int fail(int code, const char* fmt, ...) {
   return code;
 }
 
+// mas_launch_trace: the names of the kernels launched while it is on, one per line, in launch order
+static std::atomic<int> g_trace_on{0};
+static std::mutex g_trace_mu;
+static std::string g_trace;
+
 int launched(const char* what) {
   g_launches.fetch_add(1, std::memory_order_relaxed);
+  if (g_trace_on.load(std::memory_order_relaxed)) {
+    std::lock_guard<std::mutex> lk(g_trace_mu);
+    g_trace += what;
+    g_trace += '\n';
+  }
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "%s: %s", what, cudaGetErrorString(e));
   return MAS_OK;
@@ -923,6 +937,22 @@ int mas_version(void) { return 100; }
 const char* mas_last_error(void) { return g_err; }
 int64_t mas_launch_count(void) { return g_launches.load(); }
 int64_t mas_tc_launch_count(void) { return g_tc_launches.load(); }
+int mas_launch_trace(int on) {
+  std::lock_guard<std::mutex> lk(g_trace_mu);
+  g_trace.clear();
+  g_trace_on.store(on ? 1 : 0);
+  return MAS_OK;
+}
+int64_t mas_launch_trace_read(char* buf, int64_t cap) {
+  std::lock_guard<std::mutex> lk(g_trace_mu);
+  const int64_t n = (int64_t)g_trace.size();
+  if (buf && cap > 0) {
+    const int64_t c = n < cap - 1 ? n : cap - 1;
+    memcpy(buf, g_trace.data(), (size_t)c);
+    buf[c] = 0;
+  }
+  return n;
+}
 
 static int gn_check(int N, int HW, int C, int G) {
   if (N <= 0 || HW <= 0 || C <= 0 || G <= 0 || C % G != 0) return fail(MAS_ERR_INVALID_ARG, "groupnorm: bad shape N=%d HW=%d C=%d G=%d", N, HW, C, G);

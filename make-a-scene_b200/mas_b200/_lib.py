@@ -6,6 +6,7 @@ CUDA stream cross the boundary.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import os
 
@@ -32,6 +33,8 @@ _SPEC = {
     "mas_last_error": (ctypes.c_char_p, []),
     "mas_launch_count": (_L, []),
     "mas_tc_launch_count": (_L, []),
+    "mas_launch_trace": (_I, [_I]),
+    "mas_launch_trace_read": (_L, [_P, _L]),
     "mas_ffma_probe": (_I, [_P, _I, _P, _P]),
     "mas_copy_strided": (_I, [_P, _T, _P, _T, _P]),
     "mas_nchw_to_nhwc_pad": (_I, [_P, _P, _I, _I, _I, _I, _I, _P]),
@@ -293,6 +296,23 @@ def launch_count() -> int:
 def tc_launch_count() -> int:
     """Launches of kernels that issue tensor-core (wgmma) MMAs (subset of launch_count)."""
     return int(load().mas_tc_launch_count())
+
+
+@contextlib.contextmanager
+def launch_trace():
+    """Yields a list that, when the block ends, holds the name of every kernel the library launched inside it, in launch
+    order (mas_launch_trace: recorded on the host at launch, so no profiler is needed and none can drop an entry)."""
+    lib = load()
+    names = []
+    lib.mas_launch_trace(1)
+    try:
+        yield names
+    finally:
+        n = int(lib.mas_launch_trace_read(None, 0))
+        buf = ctypes.create_string_buffer(n + 1)
+        lib.mas_launch_trace_read(buf, n + 1)
+        lib.mas_launch_trace(0)
+        names.extend(buf.value.decode().splitlines())
 
 
 def t4(x: torch.Tensor) -> Tensor4:

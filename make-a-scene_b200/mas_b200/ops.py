@@ -1591,9 +1591,9 @@ def gemm2(A, B, C, M, N, K, outer, batch, lda, ldb, ldc, osa, osb, osc, sa, sb, 
 
 
 def attn_causal_fused_on(S_, hd):
-    """The fused wgmma forward core (csrc/attn_causal.cu): head dim 64, S % 128 == 0, tensor path enabled.
+    """The fused wgmma causal-attention kernels (csrc/attn_causal.cu): head dim 64 or 128, S % 128 == 0, tensor path enabled.
     MAS_ATTN_FUSED=0 selects the GEMM / softmax / GEMM sequence instead."""
-    return _tc_on() and hd == 64 and S_ % 128 == 0 and S_ >= 128 and os.environ.get("MAS_ATTN_FUSED", "1") != "0"
+    return _tc_on() and hd in (64, 128) and S_ % 128 == 0 and S_ >= 128 and os.environ.get("MAS_ATTN_FUSED", "1") != "0"
 
 
 class CausalAttentionFn(torch.autograd.Function):
@@ -1604,8 +1604,8 @@ class CausalAttentionFn(torch.autograd.Function):
     the backward and the mask is regenerated from the saved seed; no mask tensor is stored.
     recompute=True: nothing S x S is stored. The forward keeps each row's softmax maximum and sum instead of P
     (mas_attn_causal_forward_stats, ctx the same bits) and the backward recomputes P in one fused call
-    (mas_attn_causal_backward). Only the fused core's shapes (head dim 64, S % 128 == 0, tensor path) have this route; any
-    other raises RuntimeError."""
+    (mas_attn_causal_backward). Only the fused core's shapes (head dim 64 or 128, S % 128 == 0, tensor path) have this route;
+    any other raises RuntimeError."""
 
     @staticmethod
     def forward(ctx, qkv, heads, p=0.0, recompute=False):
@@ -1619,8 +1619,9 @@ class CausalAttentionFn(torch.autograd.Function):
         ctx.heads, ctx.p, ctx.recompute = heads, p, bool(recompute)
         if recompute:
             if not attn_causal_fused_on(S_, hd):
-                raise RuntimeError("recomputed attention needs the fused causal core: head dim 64, S %% 128 == 0 and the tensor "
-                                   "path with MAS_ATTN_FUSED != 0 (got S=%d, head dim %d)" % (S_, hd))
+                raise RuntimeError("recomputed attention needs the fused causal core: head dim 64, S %% 128 == 0 (or head dim "
+                                   "128, S %% 128 == 0) and the tensor path with MAS_ATTN_FUSED != 0 (got S=%d, head dim %d)"
+                                   % (S_, hd))
             am = amax(qkv)
             stats = torch.empty((2, B, heads, S_), dtype=torch.float32, device=qkv.device)      # row maxima, row sums
             ctxv = torch.empty((B, S_, H), dtype=torch.float32, device=qkv.device)

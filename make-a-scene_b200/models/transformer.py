@@ -54,7 +54,7 @@ class SelfAttention(nn.Module):
     def __init__(self, hidden_dim, num_attn_heads, attn_dropout_prob, out_dropout_prob, cogview_pb_relax=True, rudalle_relax=False,
                  recompute_attention=False):
         """recompute_attention: the attention stores no S x S probabilities for the backward and recomputes them there
-        (ops.CausalAttentionFn(recompute=True)); less memory for more arithmetic. Needs head dim 64 and S % 128 == 0."""
+        (ops.CausalAttentionFn(recompute=True)); less memory for more arithmetic. Needs head dim 64 or 128 and S % 128 == 0."""
         super().__init__()
         self.recompute_attention = recompute_attention
         self.hidden_dim = hidden_dim
@@ -263,7 +263,7 @@ class MakeAScene(nn.Module):
         MakeAScene leaves both at 0, which the defaults keep.
         recompute_attention=True: training stores no attention probabilities (S x S per head and sequence) for the backward,
         which recomputes them from per-row statistics; the loss is the same bits, the gradients agree to fp32 rounding.
-        Needs head dim 64 and a sequence length that is a multiple of 128 (RuntimeError otherwise). Not a parameter or
+        Needs head dim 64 or 128 and a sequence length that is a multiple of 128 (RuntimeError otherwise). Not a parameter or
         buffer: the state_dict is unchanged."""
         super().__init__()
         self.image_tokens_per_dim = image_tokens_per_dim

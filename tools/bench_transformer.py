@@ -3,9 +3,10 @@
 forward + cross-entropy over the image tokens + backward (train.py:136-153; no optimizer), CUDA-event timed.
 One JSON line; beside bench.py's headline (tier 2, SURVEY.md 8f-2).
 --image-tokens-per-dim 32 runs the sequence the VQ configs produce (128 + 16^2 + 32^2 = 1408 tokens); --recompute-attention
-trains with MakeAScene(recompute_attention=True) (no stored attention probabilities).
+trains with MakeAScene(recompute_attention=True) (no stored attention probabilities); --hidden / --heads change the width and
+the head count (--hidden 2048 --heads 16 and --hidden 1024 --heads 8: heads of 128).
 Usage: python tools/bench_transformer.py [--batch B] [--steps K] [--warmup W] [--layers L] [--dropout P]
-       [--image-tokens-per-dim N] [--recompute-attention]"""
+       [--image-tokens-per-dim N] [--recompute-attention] [--hidden H] [--heads N]"""
 import argparse
 import json
 import os
@@ -27,10 +28,12 @@ ap.add_argument("--profile", action="store_true", help="per-entry-point CUDA-eve
 ap.add_argument("--torch-ce", action="store_true", help="F.cross_entropy on the logits instead of MakeAScene.loss (A/B of the fused entry)")
 ap.add_argument("--image-tokens-per-dim", type=int, default=16, help="image tokens per side (sequence = 128 + 256 + N^2)")
 ap.add_argument("--recompute-attention", action="store_true", help="store no attention probabilities; the backward recomputes them")
+ap.add_argument("--hidden", type=int, default=1024, help="model width")
+ap.add_argument("--heads", type=int, default=16, help="attention heads (head dim = hidden / heads)")
 args = ap.parse_args()
 dev = torch.device("cuda:0")
 torch.manual_seed(0)
-cfg = dict(num_layers=args.layers, hidden_dim=1024, num_attn_heads=16, image_vocab_size=8192, seg_vocab_size=1024, text_vocab_size=49408,
+cfg = dict(num_layers=args.layers, hidden_dim=args.hidden, num_attn_heads=args.heads, image_vocab_size=8192, seg_vocab_size=1024, text_vocab_size=49408,
            image_tokens_per_dim=args.image_tokens_per_dim, seg_tokens_per_dim=16, text_length=128)
 m = MakeAScene(**cfg, attn_dropout_prob=args.dropout, out_dropout_prob=args.dropout,
                recompute_attention=args.recompute_attention).to(dev).train()
@@ -73,7 +76,7 @@ if args.profile:
     for k, (c, t) in sorted(rep.items(), key=lambda kv: -kv[1][1])[:24]:
         print("  %-36s n=%4d  %8.2f ms  %5.1f%%  %7.3f ms/call" % (k, c, t, 100 * t / tot, t / c), file=sys.stderr)
     print("  total %.2f ms in %d calls" % (tot, sum(c for c, _ in rep.values())), file=sys.stderr)
-S, H, L, V = 128 + 256 + IMG, 1024, args.layers, 8192
+S, H, L, V = 128 + 256 + IMG, args.hidden, args.layers, 8192
 lin = 2 * S * (12 * H * H) * L + 2 * IMG * H * V           # Linear layers, forward, per sequence
 att = 2 * 2 * S * S * H * L                                # QK^T and PV over the full (masked) square, forward
 print(json.dumps({"metric": "token transformer training step (fwd + cross-entropy + bwd), sequence tokens/s", "value": B * S / sec,
