@@ -579,6 +579,10 @@ int mas_attn_decode_shared_f16(const float* qkv, const void* kprefix, const void
                                const void* vsuffix, float* ctx, int R, int n, int heads, int hd, int prefix_len, int Tsuf, int len,
                                int rows_per_block, void* stream);
 int mas_cfg_mix(const float* cond, const float* uncond, float* out, int64_t n, float scale, void* stream);
+/* mas_cfg_mix with one scale per row: cond / uncond / out are R contiguous rows of V elements, and row r is
+ * fmaf(scale[r], cond - uncond, uncond), mas_cfg_mix's expression, so it is bit-identical to mas_cfg_mix at scale[r].
+ * scale: fp32 [R] in device memory. */
+int mas_cfg_mix_rows(const float* cond, const float* uncond, float* out, int R, int64_t V, const float* scale, void* stream);
 /* Token draw of the sampler (replaces the div / topk / where / softmax / multinomial chain of generate()): per row,
  * z = logits / temperature, entries below the top_k-th largest value dropped (top_k <= 0 or >= V: none), p = softmax(z),
  * tokens[r] = first index whose running sum of p exceeds u[r] (u in [0,1): caller-supplied uniforms, device floats). */
@@ -606,6 +610,22 @@ int mas_sample_filtered(const float* logits, int64_t ld, int R, int V, float tem
 int mas_sample_filtered_logp(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, float top_p,
                              const float* u, const int64_t* prompt_tokens, const uint8_t* prompt_mask, int64_t prompt_ld,
                              int64_t* tokens, float* logp, int64_t logp_ld, void* stream);
+/* The draw of mas_sample_filtered_logp with per-row controls, one launch for all rows: row r uses temperature[r] (0:
+ * greedy), top_k[r] (<= 0 or >= V: off) and top_p[r] (>= 1: off), device arrays of R fp32 / int32 / fp32 values, and gets
+ * the tokens and logp that mas_sample_filtered_logp gives it at those values, bit for bit (the same kernel code reads the
+ * row's values instead of the scalars).  The caller guarantees temperature[r] >= 0 and finite and top_p[r] > 0: the values
+ * are in device memory and are not checked here.  The prompt columns are those of mas_sample_filtered; logp may be NULL
+ * (nothing written).
+ * Uniforms: exactly one of u and seeds is non-NULL.  u [R]: the caller's uniforms, as mas_sample_filtered reads them.
+ * seeds (int64 [R], device): row r's uniform is
+ *     u = (word0 >> 8) * 2^-24 in [0, 1),  word0 = word 0 of Philox4x32-10(counter = (lo32(position), hi32(position), 0, 0),
+ *                                                                  key = (lo32(seeds[r]), hi32(seeds[r])))
+ * (the generator of the dropout masks below), so a row's uniform at a position depends on its seed and the position alone,
+ * never on its place in the batch, the row count or the other rows; rows with equal seeds draw with equal uniforms.
+ * MakeAScene.generate passes the image position 0 .. image_length-1 as position. */
+int mas_sample_rows(const float* logits, int64_t ld, int R, int V, const float* temperature, const int* top_k, const float* top_p,
+                    const float* u, const int64_t* seeds, int64_t position, const int64_t* prompt_tokens,
+                    const uint8_t* prompt_mask, int64_t prompt_ld, int64_t* tokens, float* logp, int64_t logp_ld, void* stream);
 
 /* ---- weighted BCE-with-logits (VQ-SEG loss, losses/loss_seg.py:15-22) — "next" row ------------------
  * logits/target: strided [N,H,W,C] views; pos_weight [C]; loss_out = mean over all elements. grad may be NULL. */

@@ -11,9 +11,11 @@
 //     The _f16 variants of both keep the caches in fp16 (decoding more than 8 rows).
 //   * mas_attn_decode_shared(_append) : mas_attn_decode(_append) for groups of rows that share a prompt's prefix cache
 //     (generate(num_samples = n)); a block reads the group's prefix once for up to 4 of its rows.
-//   * mas_cfg_mix      : classifier-free guidance, out = uncond + scale * (cond - uncond).
+//   * mas_cfg_mix      : classifier-free guidance, out = uncond + scale * (cond - uncond); mas_cfg_mix_rows: one scale per row.
+//   * mas_sample_topk / _filtered / _filtered_logp / _rows : the token draw (mas_sample_rows: per-row controls and seeds).
 #include <cuda_fp16.h>
 
+#include "dropout.cuh"
 #include "mas_common.cuh"
 
 using namespace mas;
@@ -461,6 +463,19 @@ __global__ void cfg_mix_kernel(const float* __restrict__ cond, const float* __re
   }
 }
 
+// cfg_mix_kernel with one scale per row of V elements: row r is cfg_mix_kernel's expression at scale[r], bit for bit.
+__global__ void cfg_mix_rows_kernel(const float* __restrict__ cond, const float* __restrict__ uncond, float* __restrict__ out, int R,
+                                    int64_t V, const float* __restrict__ scale) {
+  for (int r = blockIdx.y; r < R; r += gridDim.y) {
+    const float s = scale[r];
+    const size_t o = (size_t)r * V;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < V; i += (int64_t)gridDim.x * blockDim.x) {
+      const float u = uncond[o + i];
+      out[o + i] = fmaf(s, cond[o + i] - u, u);
+    }
+  }
+}
+
 // Token draw (Make-A-Scene paper 3.4 / generate()), block per row:
 //   1. z = logits / temperature;
 //   2. top-k: keep the top_k largest (all values equal to the k-th largest are kept, like `z < kth -> -inf`);
@@ -478,15 +493,36 @@ __global__ void cfg_mix_kernel(const float* __restrict__ cond, const float* __re
 // Prompt (pmask != NULL): rows with pmask[r * pld] != 0 take tok = ptok[r * pld] and draw nothing.
 // logp != NULL: logp[r * lpld] = log of the probability the token was drawn with, (z_tok - mx) - log(total) with total the
 // kept-set sum the draw itself used (one store per row, no further pass over V); 0 for prompt and greedy rows (certain).
+// ROWS (mas_sample_rows): the row reads its temperature, top_k and top_p from rc's arrays instead of the scalar arguments, and
+// with rc.seeds its uniform from seeded_uniform instead of u; everything after those reads is the scalar kernel's code, so a row
+// gets the bits the scalar entries give it at its own values.  ROWS = false compiles to the kernel of the scalar entries.
 __device__ __forceinline__ uint32_t order_key(float f) {
   const uint32_t b = __float_as_uint(f);
   return (b & 0x80000000u) ? ~b : (b | 0x80000000u);
 }
 constexpr float MASS_ONE = 1099511627776.f;          // 2^40: the largest entry's mass exp(0)
+
+struct RowControls {
+  const float* temperature;   // [R]
+  const int* top_k;           // [R]
+  const float* top_p;         // [R], >= 1: off
+  const int64_t* seeds;       // [R] or NULL (then u)
+  int64_t position;
+};
+
+// The uniform of a row with this seed at this position (include/mas_b200.h, mas_sample_rows): the top 24 bits of word 0 of
+// Philox4x32-10(counter = (lo32(position), hi32(position), 0, 0), key = (lo32(seed), hi32(seed))), times 2^-24: in [0, 1).
+__device__ __forceinline__ float seeded_uniform(int64_t seed, int64_t position) {
+  const uint64_t s = (uint64_t)seed, p = (uint64_t)position;
+  const uint4 w = philox4x32_10(make_uint4((uint32_t)p, (uint32_t)(p >> 32), 0u, 0u), (uint32_t)s, (uint32_t)(s >> 32));
+  return (float)(w.x >> 8) * 5.9604644775390625e-8f;
+}
+
+template <bool ROWS>
 __global__ void __launch_bounds__(256) sample_topk_kernel(const float* __restrict__ logits, int64_t ld, int V, float temperature, int top_k,
                                                           float top_p, const float* __restrict__ u, const int64_t* __restrict__ ptok,
                                                           const uint8_t* __restrict__ pmask, int64_t pld, int64_t* __restrict__ tok,
-                                                          float* __restrict__ logp, int64_t lpld) {
+                                                          float* __restrict__ logp, int64_t lpld, RowControls rc) {
   __shared__ int hist[256];
   __shared__ unsigned long long mhist[256];
   __shared__ uint32_t s_prefix;
@@ -503,6 +539,11 @@ __global__ void __launch_bounds__(256) sample_topk_kernel(const float* __restric
       if (logp) logp[(int64_t)blockIdx.x * lpld] = 0.f;
     }
     return;
+  }
+  if (ROWS) {
+    temperature = rc.temperature[blockIdx.x];
+    top_k = rc.top_k[blockIdx.x];
+    top_p = rc.top_p[blockIdx.x];
   }
   if (temperature == 0.f) {                           // greedy: (value, index) maximum, ties to the lower index
     float best = -INFINITY;
@@ -637,7 +678,8 @@ __global__ void __launch_bounds__(256) sample_topk_kernel(const float* __restric
   if (t == 0) {
     float total = 0.f;
     for (int j = 0; j < 256; ++j) total += csum[j];
-    const float target = u[blockIdx.x] * total;
+    const float ur = (ROWS && rc.seeds) ? seeded_uniform(rc.seeds[blockIdx.x], rc.position) : u[blockIdx.x];
+    const float target = ur * total;
     float run = 0.f;
     int j = 0, last_chunk = 0;
     for (; j < 256; ++j) {
@@ -928,11 +970,21 @@ int mas_cfg_mix(const float* cond, const float* uncond, float* out, int64_t n, f
   return launched("cfg_mix");
 }
 
+int mas_cfg_mix_rows(const float* cond, const float* uncond, float* out, int R, int64_t V, const float* scale, void* stream) {
+  MAS_REQUIRE(cond && uncond && out && scale && R > 0 && V > 0, "cfg_mix_rows: bad arguments");
+  const int gy = R < 65535 ? R : 65535;
+  const int64_t gx_max = 1184 / gy > 0 ? 1184 / gy : 1;
+  const int gx = (int)(cdiv(V, 256) < gx_max ? cdiv(V, 256) : gx_max);
+  cfg_mix_rows_kernel<<<dim3(gx, gy), 256, 0, S(stream)>>>(cond, uncond, out, R, V, scale);
+  return launched("cfg_mix_rows");
+}
+
 int mas_sample_topk(const float* logits, int64_t ld, int R, int V, float temperature, int top_k, const float* u, int64_t* tokens,
                     void* stream) {
   MAS_REQUIRE(logits && u && tokens && R > 0 && V > 0 && ld >= V, "sample_topk: bad arguments");
   if (!(temperature > 0.f)) return fail(MAS_ERR_INVALID_ARG, "sample_topk: temperature must be > 0 (greedy decoding: top_k = 1)");
-  sample_topk_kernel<<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, 1.f, u, nullptr, nullptr, 0, tokens, nullptr, 0);
+  sample_topk_kernel<false><<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, 1.f, u, nullptr, nullptr, 0, tokens, nullptr, 0,
+                                                      RowControls{});
   return launched("sample_topk");
 }
 
@@ -946,8 +998,8 @@ static int sample_filtered_run(const char* name, const float* logits, int64_t ld
   if (!prompt_tokens != !prompt_mask) return fail(MAS_ERR_INVALID_ARG, "%s: prompt tokens and prompt mask go together", name);
   if (prompt_mask && prompt_ld < 0) return fail(MAS_ERR_INVALID_ARG, "%s: negative prompt row stride", name);
   if (logp && logp_ld < 0) return fail(MAS_ERR_INVALID_ARG, "%s: negative log-probability row stride", name);
-  sample_topk_kernel<<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, top_p, u, prompt_tokens, prompt_mask, prompt_ld,
-                                               tokens, logp, logp_ld);
+  sample_topk_kernel<false><<<R, 256, 0, S(stream)>>>(logits, ld, V, temperature, top_k, top_p, u, prompt_tokens, prompt_mask,
+                                                      prompt_ld, tokens, logp, logp_ld, RowControls{});
   return launched(name);
 }
 
@@ -963,6 +1015,20 @@ int mas_sample_filtered_logp(const float* logits, int64_t ld, int R, int V, floa
   if (!logp) return fail(MAS_ERR_INVALID_ARG, "sample_filtered_logp: logp is NULL (mas_sample_filtered draws without it)");
   return sample_filtered_run("sample_filtered_logp", logits, ld, R, V, temperature, top_k, top_p, u, prompt_tokens, prompt_mask,
                              prompt_ld, tokens, logp, logp_ld, stream);
+}
+
+int mas_sample_rows(const float* logits, int64_t ld, int R, int V, const float* temperature, const int* top_k, const float* top_p,
+                    const float* u, const int64_t* seeds, int64_t position, const int64_t* prompt_tokens, const uint8_t* prompt_mask,
+                    int64_t prompt_ld, int64_t* tokens, float* logp, int64_t logp_ld, void* stream) {
+  if (!(logits && tokens && R > 0 && V > 0 && ld >= V)) return fail(MAS_ERR_INVALID_ARG, "sample_rows: bad arguments");
+  if (!(temperature && top_k && top_p)) return fail(MAS_ERR_INVALID_ARG, "sample_rows: temperature, top_k and top_p are [R] arrays");
+  if (!u == !seeds) return fail(MAS_ERR_INVALID_ARG, "sample_rows: give exactly one source of uniforms, u or seeds");
+  if (!prompt_tokens != !prompt_mask) return fail(MAS_ERR_INVALID_ARG, "sample_rows: prompt tokens and prompt mask go together");
+  if (prompt_mask && prompt_ld < 0) return fail(MAS_ERR_INVALID_ARG, "sample_rows: negative prompt row stride");
+  if (logp && logp_ld < 0) return fail(MAS_ERR_INVALID_ARG, "sample_rows: negative log-probability row stride");
+  sample_topk_kernel<true><<<R, 256, 0, S(stream)>>>(logits, ld, V, 0.f, 0, 1.f, u, prompt_tokens, prompt_mask, prompt_ld, tokens, logp,
+                                                     logp_ld, RowControls{temperature, top_k, top_p, seeds, position});
+  return launched("sample_rows");
 }
 
 }  // extern "C"

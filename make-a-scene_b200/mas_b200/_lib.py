@@ -130,6 +130,7 @@ _SPEC = {
     "mas_kv_append": (_I, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _P]),
     "mas_attn_decode": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "mas_cfg_mix": (_I, [_P, _P, _P, _L, _F, _P]),
+    "mas_cfg_mix_rows": (_I, [_P, _P, _P, _I, _L, _P, _P]),
     "mas_attn_decode_append": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
     "mas_kv_append_f16": (_I, [_P, _I, _I, _I, _I, _P, _P, _I, _I, _P]),
     "mas_attn_decode_f16": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P]),
@@ -142,6 +143,7 @@ _SPEC = {
     "mas_sample_topk": (_I, [_P, _L, _I, _I, _F, _I, _P, _P, _P]),
     "mas_sample_filtered": (_I, [_P, _L, _I, _I, _F, _I, _F, _P, _P, _P, _L, _P, _P]),
     "mas_sample_filtered_logp": (_I, [_P, _L, _I, _I, _F, _I, _F, _P, _P, _P, _L, _P, _P, _L, _P]),
+    "mas_sample_rows": (_I, [_P, _L, _I, _I, _P, _P, _P, _P, _P, _L, _P, _P, _L, _P, _P, _L, _P]),
     "mas_pack_gemm_tc16": (_I, [_P, _P, _I, _I, _I, _P]),
     "mas_gemm_rows_f16": (_I, [_P, _L, _I, _P, _P, _L, _I, _P, _P, _P, _F, _P]),
     "mas_linear_rows_f16_ws_bytes": (_Z, [_L, _I, _I]),

@@ -1762,23 +1762,53 @@ def sample_topk(logits, temperature, top_k, u, top_p=None, prompt=None, logp=Non
     if top_p is None and prompt is None and logp is None:
         L.call("mas_sample_topk", logits, V, R, V, float(temperature), int(top_k) if top_k else 0, u.contiguous(), tok)
         return tok
-    ptok = pmask = None
-    pld = 0
-    if prompt is not None:
-        ptok, pmask = prompt
-        if ptok.shape != (R,) or pmask.shape != (R,) or ptok.dtype != torch.int64 or pmask.dtype != torch.bool:
-            raise ValueError("prompt: int64 tokens and a bool mask of %d rows expected" % R)
-        if ptok.device != logits.device or pmask.device != logits.device:
-            raise ValueError("prompt: tokens and mask must be on the logits' device (%s)" % logits.device)
-        if ptok.stride(0) != pmask.stride(0):
-            ptok, pmask = ptok.contiguous(), pmask.contiguous()
-        pld = ptok.stride(0)
+    ptok, pmask, pld = _prompt_columns(prompt, R, logits.device)
     args = (logits, V, R, V, float(temperature), int(top_k) if top_k else 0, 1.0 if top_p is None else top_p,
             None if u is None else u.contiguous(), ptok, pmask, pld, tok)
     if logp is None:
         L.call("mas_sample_filtered", *args)
     else:
         L.call("mas_sample_filtered_logp", *args, logp, logp.stride(0))
+    return tok
+
+
+def _prompt_columns(prompt, R, dev):
+    """(tokens, mask, row stride) of a prompt (int64 tokens [R], bool mask [R]) for the sampler entries, or Nones."""
+    if prompt is None:
+        return None, None, 0
+    ptok, pmask = prompt
+    if ptok.shape != (R,) or pmask.shape != (R,) or ptok.dtype != torch.int64 or pmask.dtype != torch.bool:
+        raise ValueError("prompt: int64 tokens and a bool mask of %d rows expected" % R)
+    if ptok.device != dev or pmask.device != dev:
+        raise ValueError("prompt: tokens and mask must be on the logits' device (%s)" % dev)
+    if ptok.stride(0) != pmask.stride(0):
+        ptok, pmask = ptok.contiguous(), pmask.contiguous()
+    return ptok, pmask, ptok.stride(0)
+
+
+def sample_rows(logits, temperature, top_k, top_p, u=None, seeds=None, position=0, prompt=None, logp=None):
+    """sample_topk with per-row controls (mas_sample_rows): temperature fp32 [R] (0: greedy), top_k int32 [R] (<= 0: off) and
+    top_p fp32 [R] (>= 1: off), on the logits' device. Row r draws what sample_topk draws at its own three values, bit for bit.
+    The uniforms are u fp32 [R] or, with seeds int64 [R], Philox4x32-10 of (seed, position) (include/mas_b200.h): exactly one
+    of the two. prompt / logp as in sample_topk. The values are not read back here: the caller validates them (temperature
+    finite and >= 0, top_p > 0)."""
+    _need_cuda(logits)
+    logits = logits.contiguous()
+    R, V = logits.shape
+    dev = logits.device
+    for name, t, dt in (("temperature", temperature, torch.float32), ("top_k", top_k, torch.int32), ("top_p", top_p, torch.float32),
+                        ("u", u, torch.float32), ("seeds", seeds, torch.int64)):
+        if t is not None and (t.shape != (R,) or t.dtype != dt or t.device != dev):
+            raise ValueError("%s: a %s tensor of %d rows on the logits' device (%s) expected" % (name, dt, R, dev))
+    if (u is None) == (seeds is None):
+        raise ValueError("sample_rows: give exactly one of u and seeds")
+    if logp is not None and (logp.shape != (R,) or logp.dtype != torch.float32 or logp.device != dev):
+        raise ValueError("logp: an fp32 column of %d rows on the logits' device (%s) expected" % (R, dev))
+    ptok, pmask, pld = _prompt_columns(prompt, R, dev)
+    tok = torch.empty(R, dtype=torch.int64, device=dev)
+    c = lambda t: None if t is None else t.contiguous()
+    L.call("mas_sample_rows", logits, V, R, V, c(temperature), c(top_k), c(top_p), c(u), c(seeds), int(position), ptok, pmask, pld,
+           tok, logp, 0 if logp is None else logp.stride(0))
     return tok
 
 
@@ -1935,6 +1965,17 @@ def cfg_mix(cond, uncond, scale):
     """Classifier-free guidance on logits: uncond + scale * (cond - uncond)."""
     out = torch.empty_like(cond)
     L.call("mas_cfg_mix", cond.contiguous(), uncond.contiguous(), out, cond.numel(), float(scale))
+    return out
+
+
+def cfg_mix_rows(cond, uncond, scale):
+    """cfg_mix with one scale per row (mas_cfg_mix_rows): cond / uncond [R, ...] fp32, scale fp32 [R] on their device; row r
+    is bit-identical to cfg_mix at scale[r]."""
+    R = cond.shape[0]
+    if scale.shape != (R,) or scale.dtype != torch.float32 or scale.device != cond.device:
+        raise ValueError("scale: an fp32 tensor of %d rows on the logits' device (%s) expected" % (R, cond.device))
+    out = torch.empty_like(cond, memory_format=torch.contiguous_format)
+    L.call("mas_cfg_mix_rows", cond.contiguous(), uncond.contiguous(), out, R, cond.numel() // R, scale.contiguous())
     return out
 
 

@@ -180,6 +180,33 @@ def _param_version(model):
     return tuple((p._version, p.data_ptr()) for p in model.parameters())
 
 
+def _is_per_row(v):
+    """A sampling control given per row (a 1-D tensor or a sequence) rather than one value for the call."""
+    return isinstance(v, (list, tuple)) or (isinstance(v, torch.Tensor) and v.dim() > 0)
+
+
+def _row_values(name, v, n, dev, integer=False):
+    """The n per-row values of a sampling control as (fp64 host copy, device tensor fp32 or, integer, int32). A scalar is
+    repeated; a 1-D tensor must hold n values of a floating (integer: integer) dtype on dev; a sequence is read on the host.
+    ValueError otherwise."""
+    if isinstance(v, torch.Tensor) and v.dim() > 0:
+        ok = not v.dtype.is_floating_point and not v.dtype.is_complex and v.dtype != torch.bool if integer else v.dtype.is_floating_point
+        if v.dim() != 1 or v.shape[0] != n or not ok or v.device != dev:
+            raise ValueError("%s: one value per output row expected: a 1-D %s tensor of %d values on %s, got %s %s on %s" % (
+                name, "integer" if integer else "floating-point", n, dev, v.dtype, tuple(v.shape), v.device))
+        host = v.detach().to("cpu", torch.float64)
+    elif isinstance(v, (list, tuple)):
+        if len(v) != n or not all(isinstance(x, (int, float)) and not isinstance(x, bool) for x in v) or (
+                integer and not all(isinstance(x, int) for x in v)):
+            raise ValueError("%s: a sequence of %d %s expected, got %r" % (name, n, "ints" if integer else "numbers", v))
+        host = torch.tensor([float(x) for x in v], dtype=torch.float64)
+    else:
+        host = torch.full((n,), float(v), dtype=torch.float64)
+    if integer:
+        return host, host.clamp(-2 ** 31, 2 ** 31 - 1).to(torch.int32).to(dev)
+    return host, host.to(torch.float32).to(dev)
+
+
 def _attend_append(qkv, kc, vc, suffix, li, pos):
     """Layer li's attention of this token (qkv [R,3H], stored at position pos) over positions 0..pos: one cache per row, or
     with suffix (num_samples > 1) the prefix cache of the row's prompt followed by the row's own suffix cache."""
@@ -400,7 +427,7 @@ class MakeAScene(nn.Module):
     @torch.no_grad()
     def generate(self, text_tokens, seg_tokens, guidance_scale=None, uncond_text_tokens=None, temperature=1.0, top_k=None,
                  generator=None, img_tokens=None, return_logits=False, use_graphs=False, top_p=None, img_mask=None, num_samples=1,
-                 return_logprobs=False):
+                 return_logprobs=False, seeds=None):
         """Autoregressive sampling of the image tokens with a KV cache; optional classifier-free guidance
         (logits = uncond + scale * (cond - uncond), the unconditional stream sees padded text; Make-A-Scene paper 3.4).
 
@@ -435,7 +462,20 @@ class MakeAScene(nn.Module):
         use_graphs: replay each position's decode step from a CUDA graph (captured at first use and kept on the module for
         the same row count; captured again after any parameter changes, in place or by replaced storage).
         Dropout is never applied here, in train mode as in eval mode: the prefix pass and the decode steps call the layers'
-        kernels directly, not the dropout sites, so a model trained with dropout samples as its eval-mode self."""
+        kernels directly, not the dropout sites, so a model trained with dropout samples as its eval-mode self.
+        Per-row controls: temperature, top_k, top_p and guidance_scale each take one value for the call, or one per output row
+        (a 1-D tensor on the model's device, or a sequence, of B*n values; row b*n + j as img_tokens). A row then draws and
+        mixes exactly as a call with its values as scalars would (mas_sample_rows / mas_cfg_mix_rows, bit for bit), so one
+        call can sweep settings over the samples of a prompt, or batch requests with different settings. ValueError for a
+        wrong length, dtype or device, a temperature that is negative or not finite, top_k < 0, top_p <= 0 or a guidance
+        scale that is not finite. With per-row scales both streams run for every row unless every scale is 1 (then the call
+        is unguided); a row at scale 1 then gets fmaf(1, cond - uncond, uncond), within rounding of its conditional logits
+        but not always bitwise equal to them (and the doubled row count may decode in fp16 where the unguided call would not).
+        seeds (int64 [B*n] on the model's device; not together with generator): row r draws at image position t with the
+        uniform of Philox4x32-10 keyed by seeds[r] at counter t (include/mas_b200.h, mas_sample_rows), which depends on the
+        seed and t alone: rows with equal seeds draw with equal uniforms, in this call or another (common random numbers, so
+        a sweep compares settings, not noise). Any per-row control or seeds routes the draw to mas_sample_rows; a call with
+        scalars only and no seeds issues the entries it always did."""
         B = text_tokens.shape[0]
         dev = text_tokens.device
         n = num_samples
@@ -444,8 +484,33 @@ class MakeAScene(nn.Module):
         if not isinstance(return_logprobs, bool):
             raise ValueError("return_logprobs must be a bool, got %r" % (return_logprobs,))
         Bn = B * n
-        if top_p is not None and not float(top_p) > 0:
+        if top_p is not None and not _is_per_row(top_p) and not float(top_p) > 0:
             raise ValueError("top_p must be > 0 (None or >= 1: no nucleus filter), got %r" % (top_p,))
+        mdev = self.image_token_embedding.weight.device
+        rows = None          # per-row draw: (temperature, top_k, top_p) device tensors [B*n]
+        if seeds is not None or any(_is_per_row(v) for v in (temperature, top_k, top_p)):
+            if seeds is not None:
+                if generator is not None:
+                    raise ValueError("seeds and generator are two sources of uniforms: pass one of them")
+                if not isinstance(seeds, torch.Tensor) or seeds.dtype != torch.int64 or tuple(seeds.shape) != (Bn,) or seeds.device != mdev:
+                    raise ValueError("seeds must be an int64 tensor of shape %s on the model's device (%s)" % ((Bn,), mdev))
+            temp_h, temp_d = _row_values("temperature", 0.0 if temperature is None else temperature, Bn, mdev)
+            topk_h, topk_d = _row_values("top_k", 0 if top_k is None else top_k, Bn, mdev, integer=True)
+            topp_h, topp_d = _row_values("top_p", 1.0 if top_p is None else top_p, Bn, mdev)
+            if not bool((torch.isfinite(temp_h) & (temp_h >= 0)).all()):
+                raise ValueError("temperature must be finite and >= 0 in every row (0: greedy), got %s" % temp_h.tolist())
+            if not bool((topk_h >= 0).all()):
+                raise ValueError("top_k must be >= 0 in every row (0: off), got %s" % topk_h.tolist())
+            if not bool((topp_h > 0).all()):
+                raise ValueError("top_p must be > 0 in every row (>= 1: off), got %s" % topp_h.tolist())
+            rows = (temp_d, topk_d, topp_d)
+            drawing = bool((temp_h > 0).any())
+        scale_rows = None    # per-row guidance: fp32 [B*n] device tensor
+        if _is_per_row(guidance_scale):
+            scale_h, scale_d = _row_values("guidance_scale", guidance_scale, Bn, mdev)
+            if not bool(torch.isfinite(scale_h).all()):
+                raise ValueError("guidance_scale must be finite in every row, got %s" % scale_h.tolist())
+            scale_rows = scale_d if bool((scale_h != 1.0).any()) else None
         if img_tokens is not None and n > 1 and tuple(img_tokens.shape) != (Bn, self.image_length):
             raise ValueError("img_tokens must have one row per output row: shape %s" % ((Bn, self.image_length),))
         if img_mask is not None:
@@ -459,7 +524,10 @@ class MakeAScene(nn.Module):
             if img_mask.device != dev or img_tokens.device != dev:
                 raise ValueError("img_tokens and img_mask must be on the device of text_tokens (%s)" % dev)
             img_tokens, img_mask = img_tokens.contiguous(), img_mask.contiguous()
-        cfg = guidance_scale is not None and float(guidance_scale) != 1.0
+        if _is_per_row(guidance_scale):
+            cfg = scale_rows is not None
+        else:
+            cfg = guidance_scale is not None and float(guidance_scale) != 1.0
         if cfg:
             if uncond_text_tokens is None:
                 uncond_text_tokens = torch.zeros_like(text_tokens)          # all padding -> the per-position pad ids
@@ -481,22 +549,34 @@ class MakeAScene(nn.Module):
         logits = self._logits_of(last.repeat_interleave(n, 0) if n > 1 else last)
         toks, kept = [], []
         logprobs = torch.zeros((Bn, self.image_length), dtype=torch.float32, device=dev) if return_logprobs else None
+
+        def uniforms():
+            if generator is not None and generator.device.type != dev.type:
+                return torch.rand(Bn, generator=generator).to(dev)
+            return torch.rand(Bn, device=dev, generator=generator)
+
+        # per-row draw without seeds and without a sampling row: no uniform is read, none is drawn (as a scalar temperature 0)
+        u_none = torch.zeros(Bn, dtype=torch.float32, device=dev) if rows is not None and seeds is None and not drawing else None
         for t in range(self.image_length):
-            mixed = ops.cfg_mix(logits[:Bn], logits[Bn:], guidance_scale) if cfg else logits
+            if not cfg:
+                mixed = logits
+            elif scale_rows is not None:
+                mixed = ops.cfg_mix_rows(logits[:Bn], logits[Bn:], scale_rows)
+            else:
+                mixed = ops.cfg_mix(logits[:Bn], logits[Bn:], guidance_scale)
             if return_logits:
                 kept.append(mixed)
             prompt = (img_tokens[:, t], img_mask[:, t]) if img_mask is not None else None
             if img_tokens is not None and prompt is None:
                 tok = img_tokens[:, t]
+            elif rows is not None:    # per-row controls or seeds: mas_sample_rows, the uniforms of the seeds or of the generator
+                u = uniforms() if seeds is None and drawing else u_none
+                tok = ops.sample_rows(mixed, *rows, u=u, seeds=seeds, position=t, prompt=prompt,
+                                      logp=None if logprobs is None else logprobs[:, t])
             elif not temperature and prompt is None:
                 tok = mixed.argmax(-1)
             else:   # prompt, temperature, top-k / top-p filters, softmax and the draw in one kernel; torch only supplies the uniforms
-                u = None
-                if temperature:
-                    if generator is not None and generator.device.type != dev.type:
-                        u = torch.rand(Bn, generator=generator).to(dev)
-                    else:
-                        u = torch.rand(Bn, device=dev, generator=generator)
+                u = uniforms() if temperature else None
                 tok = ops.sample_topk(mixed, float(temperature), top_k, u, top_p=top_p, prompt=prompt,
                                       logp=None if logprobs is None else logprobs[:, t])
             toks.append(tok)
@@ -517,7 +597,10 @@ class MakeAScene(nn.Module):
         One causal pass over text + seg + image (both streams in one batch with guidance; no dropout, in train mode as in
         eval mode), to_logits on the image_length predicting positions, the guidance mix, then the per-row cross-entropies of
         mas_ce_forward negated. text_tokens [B,text_length], seg_tokens [B,seg_length], img_tokens [B,image_length] (values in
-        [0, image_vocab_size)) and uncond_text_tokens [B,text_length]: int64 on the model's device."""
+        [0, image_vocab_size)) and uncond_text_tokens [B,text_length]: int64 on the model's device.
+        guidance_scale may also give one scale per row (a 1-D tensor on the model's device, or a sequence, of B values, as in
+        generate): row b is then the guided log-likelihood at its own scale, bit for bit the row of a call with that scale, so
+        candidates can be reranked at several scales in one pass (a row at scale 1 in a guided call: see generate)."""
         named = [("text_tokens", text_tokens, self.text_length), ("seg_tokens", seg_tokens, self.seg_length),
                  ("img_tokens", img_tokens, self.image_length)]
         if uncond_text_tokens is not None:
@@ -531,10 +614,16 @@ class MakeAScene(nn.Module):
                 raise ValueError("%s must be int64, got %s" % (name, t.dtype))
             if t.device != dev:
                 raise ValueError("%s must be on the model's device (%s), got %s" % (name, dev, t.device))
+        scale_rows = None
+        if _is_per_row(guidance_scale):
+            scale_h, scale_d = _row_values("guidance_scale", guidance_scale, B, dev)
+            if not bool(torch.isfinite(scale_h).all()):
+                raise ValueError("guidance_scale must be finite in every row, got %s" % scale_h.tolist())
+            scale_rows = scale_d if bool((scale_h != 1.0).any()) else None
         V = self.image_token_embedding.num_embeddings
         if bool(((img_tokens < 0) | (img_tokens >= V)).any()):
             raise ValueError("img_tokens must lie in [0, %d)" % V)
-        cfg = guidance_scale is not None and float(guidance_scale) != 1.0
+        cfg = scale_rows is not None if _is_per_row(guidance_scale) else guidance_scale is not None and float(guidance_scale) != 1.0
         if cfg:
             if uncond_text_tokens is None:
                 uncond_text_tokens = torch.zeros_like(text_tokens)          # all padding, as in generate
@@ -546,6 +635,8 @@ class MakeAScene(nn.Module):
         h = self.transformer.final_ln(self._prefill(self._embed(text_tokens, seg_tokens, img_all)))
         h = h[:, -L - 1:-1].contiguous()                                    # forward()'s slice: the predicting positions
         logits = self.to_logits[1](self.to_logits[0](h))
-        if cfg:
+        if scale_rows is not None:
+            logits = ops.cfg_mix_rows(logits[:B], logits[B:], scale_rows)
+        elif cfg:
             logits = ops.cfg_mix(logits[:B], logits[B:], guidance_scale)
         return ops.token_logprobs(logits.view(B * L, V), img_tokens.reshape(B * L)).view(B, L)

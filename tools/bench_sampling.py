@@ -9,8 +9,14 @@ fp32 KV cache, above 8 rows fp16 weights and fp16 cache (the cache read at the m
 cache, and cache_gb_per_step counts a prompt's prefix once per step, as the shared-prefix attention reads it.
 --logprobs also times the same call with return_logprobs=True next to the plain one (alternating, --reps each, after both
 are warmed up) and adds both times and the relative cost to the line; without it the line is unchanged.
-Usage: python tools/bench_sampling.py [--batch B] [--samples N] [--reps N] [--graphs] [--top-p P] [--prompt-frac F] [--logprobs]"""
+--sweep N times a guidance sweep over N scales two ways, alternating, --reps each after both are warmed up: one call with
+num_samples=N and one guidance scale per sample (per-row controls: one prefix pass, N x the decode rows) against N calls at
+num_samples=1, one per scale. It also times the draw kernel alone, mas_sample_rows (per-row values, u or seeds) against
+mas_sample_filtered_logp with the same values as scalars, at R = 8, 128, 256 rows of V = 8192 (the bench's top-k 64).
+Usage: python tools/bench_sampling.py [--batch B] [--samples N] [--reps N] [--graphs] [--top-p P] [--prompt-frac F] [--logprobs]
+                                      [--sweep N]"""
 import argparse
+import copy
 import json
 import os
 import subprocess
@@ -31,6 +37,7 @@ ap.add_argument("--graphs", action="store_true", help="replay each position's de
 ap.add_argument("--top-p", type=float, default=None, help="nucleus filter of the draw (default: off)")
 ap.add_argument("--prompt-frac", type=float, default=0.0, help="share of image positions forced by a random image prompt")
 ap.add_argument("--logprobs", action="store_true", help="also time generate(return_logprobs=True) against the plain call")
+ap.add_argument("--sweep", type=int, default=0, help="time a sweep over N guidance scales: one per-row call against N calls")
 args = ap.parse_args()
 dev = torch.device("cuda:0")
 torch.manual_seed(0)
@@ -85,4 +92,55 @@ if args.logprobs:
     plain, logp = (sorted(times[f])[len(times[f]) // 2] for f in (False, True))
     res.update({"logprobs_seconds_per_call_median": logp, "plain_seconds_per_call_median": plain,
                 "logprobs_relative_cost": logp / plain - 1, "logprobs_seconds_all": times[True], "plain_seconds_all": times[False]})
+if args.sweep:
+    scales = [1.5 + 3.5 * j / max(args.sweep - 1, 1) for j in range(args.sweep)]
+    sweep_kw = dict(kw, num_samples=args.sweep, guidance_scale=torch.tensor([s for _ in range(B) for s in scales], device=dev))
+    m_rows = copy.copy(m)     # the same parameters, its own sampler cache: with --graphs neither arm recaptures the other's graphs
+    arms = {"per_row": lambda: m_rows.generate(text, seg, **sweep_kw),
+            "scalar_calls": lambda: [m.generate(text, seg, **dict(kw, num_samples=1, guidance_scale=s)) for s in scales]}
+    for f in arms.values():                                          # warm-up (and graph captures) of both arms
+        f()
+    times = {k: [] for k in arms}
+    for i in range(args.reps):
+        for k in (("per_row", "scalar_calls") if i % 2 == 0 else ("scalar_calls", "per_row")):
+            torch.cuda.synchronize()
+            e0.record()
+            arms[k]()
+            e1.record()
+            torch.cuda.synchronize()
+            times[k].append(e0.elapsed_time(e1) * 1e-3)
+    med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
+    # the draw kernel alone: per-row arrays (u or seeds) against the scalar entry at the same values, alternating
+    kern = {}
+    V = cfg["image_vocab_size"]
+    for Rk in (8, 128, 256):
+        lg = torch.randn(Rk, V, device=dev) * 2.5
+        u = torch.rand(Rk, device=dev)
+        tok, lp = torch.empty(Rk, dtype=torch.int64, device=dev), torch.empty(Rk, device=dev)
+        tt, kk, pp = (torch.full((Rk,), 1.0, device=dev), torch.full((Rk,), 64, dtype=torch.int32, device=dev),
+                      torch.full((Rk,), 1.0 if args.top_p is None else args.top_p, device=dev))
+        sd = torch.arange(Rk, dtype=torch.int64, device=dev)
+        p = 1.0 if args.top_p is None else args.top_p
+        calls = {"scalar": lambda: _lib.call("mas_sample_filtered_logp", lg, V, Rk, V, 1.0, 64, p, u, None, None, 0, tok, lp, 1),
+                 "rows_u": lambda: _lib.call("mas_sample_rows", lg, V, Rk, V, tt, kk, pp, u, None, 0, None, None, 0, tok, lp, 1),
+                 "rows_seeds": lambda: _lib.call("mas_sample_rows", lg, V, Rk, V, tt, kk, pp, None, sd, 7, None, None, 0, tok, lp, 1)}
+        per = {k: [] for k in calls}
+        for f in calls.values():
+            for _ in range(20):
+                f()
+        for i in range(7):
+            for k in (list(calls) if i % 2 == 0 else list(calls)[::-1]):
+                torch.cuda.synchronize()
+                e0.record()
+                for _ in range(200):
+                    calls[k]()
+                e1.record()
+                torch.cuda.synchronize()
+                per[k].append(e0.elapsed_time(e1) * 1e3 / 200)
+        kern[str(Rk)] = {k: sorted(v)[len(v) // 2] for k, v in per.items()}
+    res.update({"sweep": args.sweep, "sweep_scales": scales, "sweep_images": B * args.sweep,
+                "sweep_per_row_seconds_median": med["per_row"], "sweep_scalar_calls_seconds_median": med["scalar_calls"],
+                "sweep_per_row_images_per_s": B * args.sweep / med["per_row"],
+                "sweep_scalar_calls_images_per_s": B * args.sweep / med["scalar_calls"],
+                "sweep_seconds_all": times, "sampler_us_per_launch_median_V8192": kern})
 print(json.dumps(res))
