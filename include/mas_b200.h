@@ -686,6 +686,41 @@ int mas_lpips_relu_backward(const float* dy, const float* y, float* dx, int64_t 
 int mas_lpips_prep_backward(const float* dxp, const float* scale, float* J, int G, int H, int W, void* stream);
 int mas_lpips_scale_jacobian(const float* J, const float* g, int64_t g_stride, float* out, int B, int64_t per, void* stream);
 
+/* Object-aware loss (losses/object_loss.py; csrc/lpips.cu): LPIPS of every box crop, batched by size class.  A class is one
+ * channels-last batch of 2K canvases [2K,Hc,Wc,C] (the K crops of img, then the same K of rec), each crop at the canvas
+ * origin.  tab (int32) holds 6 ints per crop (image b, y0, x0, h, w, global box index k), then B+1 row offsets: the rows of
+ * image b are [tab[6K + b], tab[6K + b + 1]).  At pooling level l crop r is valid on (h >> l) x (w >> l); every entry below
+ * holds activations outside that region at zero, so the 3x3 convolutions (the LPIPS ones, unchanged) see the crop's own zero
+ * padding.  wts (fp32) [number of boxes]: w_k = 1 / (n_b + 1) by global index.
+ * mas_object_gather: out [2K,Hc,Wc,3] = (crop - shift) / scale inside the extent, img / rec NCHW dense [*,3,H,W], pixels of
+ *   the box outside the image read 0 (before scaling); 0 outside the extent.
+ * mas_object_relu: ReLU of y [2K,H,W,C] in place, 0 outside the level's extent; amax (or NULL) = max of the result.
+ * mas_object_maxpool: x [2K,H,W,C] at level `level` -> y [2K,H/2,W/2,C], 2x2 floor max-pool inside the extent of level + 1,
+ *   0 outside it; amax as above.
+ * mas_object_head_forward: mas_lpips_head_forward over the extent of crop r only: part [K][mas_lpips_head_blocks()].
+ * mas_object_head_finalize: p[k of crop r] = sum over the five levels, in order, of sum_j part[l][r][j] / (valid area of l);
+ *   part [5][K][mas_lpips_head_blocks()].
+ * mas_object_tap_backward: mas_lpips_tap_backward per canvas, for canvases g0 .. g0+G-1 (partner (t + K) mod 2K): the head
+ *   mean over the crop's valid area, dpool [G,H/2,W/2,C] (or NULL) read only inside the extent of level + 1, dz = 0 outside
+ *   the extent of `level`.
+ * mas_object_scatter: ScalingLayer backward and crop adjoint of the prep gradient dxp [G,Hc,Wc,3] (canvases g0 .. g0+G-1,
+ *   which must hold all K crops of `side`, 0 = img, 1 = rec): J[b,c,y,x] (+= with accumulate, else =) the sum over the rows
+ *   of image b, in row order, covering the pixel, of w_k * dxp[.., y - y0, x - x0, c] / scale[c]; J dense [B,3,H,W], every
+ *   element written; no atomics.
+ * mas_object_loss: out = sum_k wts[k] * p[k], in fp64 in index order, rounded to fp32. */
+int mas_object_gather(const int* tab, int K, const float* img, const float* rec, const float* shift, const float* scale, float* out,
+                      int H, int W, int Hc, int Wc, void* stream);
+int mas_object_relu(float* y, const int* tab, int K, int H, int W, int C, int level, float* amax, void* stream);
+int mas_object_maxpool(const float* x, float* y, const int* tab, int K, int H, int W, int C, int level, float* amax, void* stream);
+int mas_object_head_forward(const float* tap, const float* w_lin, const int* tab, int K, int H, int W, int C, int level, double* part,
+                            void* stream);
+int mas_object_head_finalize(const double* part, const int* tab, int K, float* p, void* stream);
+int mas_object_tap_backward(const float* tap, const float* w_lin, const int* tab, int K, int H, int W, int C, int level, int g0, int G,
+                            const float* dpool, float* dz, float* amax, void* stream);
+int mas_object_scatter(const float* dxp, const float* scale, const int* tab, const float* wts, int K, int g0, int G, int side, int Hc,
+                       int Wc, float* J, int B, int H, int W, int accumulate, void* stream);
+int mas_object_loss(const float* p, const float* wts, int K, float* out, void* stream);
+
 /* VGGFace2 face loss (losses/face_loss.py; ResNet-50 "caffe" style, eval BatchNorm folded into the convolutions by the host).
  * The 1x1 convolutions run on mas_gemm_rows_f16 and the 3x3 ones on the 3x3 family; these entries are the rest of
  * FaceLoss.forward and its data gradient.  Activations are channels-last fp32 over ONE batch of F <= 6 faces; face p and face

@@ -127,6 +127,14 @@ class LPIPS(nn.Module):
 
     def forward(self, real_x, fake_x):
         """-> [B, 1, 1, 1] fp32: sum over relu1_2 .. relu5_3 of the spatial mean of lin((n(real) - n(fake))^2)."""
+        self.check()
+        lins = [lin.model[1].weight for lin in self.lins]
+        keep = torch.is_grad_enabled() and (real_x.requires_grad or fake_x.requires_grad)
+        return ops.LPIPSFn.apply(real_x, fake_x, self.scaling_layer.shift, self.scaling_layer.scale, self.vgg.convs(), lins,
+                                 keep)
+
+    def check(self):
+        """Refuses what has no kernel: training-mode Dropout and trainable parameters."""
         if self.training:
             raise RuntimeError("LPIPS: Dropout(p=0.5) in training mode has no kernel; call .eval() on the loss "
                                "(as losses/loss_img.py does)")
@@ -134,7 +142,3 @@ class LPIPS(nn.Module):
         if trainable:
             raise RuntimeError("LPIPS computes no weight gradients; its parameters must have requires_grad=False "
                                "(got %s)" % ", ".join(trainable))
-        lins = [lin.model[1].weight for lin in self.lins]
-        keep = torch.is_grad_enabled() and (real_x.requires_grad or fake_x.requires_grad)
-        return ops.LPIPSFn.apply(real_x, fake_x, self.scaling_layer.shift, self.scaling_layer.scale, self.vgg.convs(), lins,
-                                 keep)

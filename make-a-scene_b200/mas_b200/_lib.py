@@ -180,6 +180,14 @@ _SPEC = {
     "mas_lpips_relu_backward": (_I, [_P, _P, _P, _L, _P, _P]),
     "mas_lpips_prep_backward": (_I, [_P, _P, _P, _I, _I, _I, _P]),
     "mas_lpips_scale_jacobian": (_I, [_P, _P, _L, _P, _I, _L, _P]),
+    "mas_object_gather": (_I, [_P, _I, _P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "mas_object_relu": (_I, [_P, _P, _I, _I, _I, _I, _I, _P, _P]),
+    "mas_object_maxpool": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
+    "mas_object_head_forward": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
+    "mas_object_head_finalize": (_I, [_P, _P, _I, _P, _P]),
+    "mas_object_tap_backward": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _P, _P, _P, _P]),
+    "mas_object_scatter": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _P, _I, _I, _I, _I, _P]),
+    "mas_object_loss": (_I, [_P, _P, _I, _P, _P]),
     "mas_face_prepare": (_I, [_P, _P, _I, _P, _T, _P, _T, _P, _P]),
     "mas_face_prepare_backward": (_I, [_P, _P, _I, _I, _I, _P, _P, _I, _I, _I, _P]),
     "mas_face_stem_forward": (_I, [_P, _P, _P, _I, _I, _I, _P]),

@@ -2127,6 +2127,193 @@ class LPIPSFn(torch.autograd.Function):
         return grads[0], grads[1], None, None, None, None, None
 
 
+# ---- object-aware loss (losses/object_loss.py) ------------------------------------------------------------------------
+OBJECT_MIN_SIDE = 16    # four 2x2 floor pools leave at least one pixel
+OBJECT_ROW = 6          # ints per crop in a class table: image, y0, x0, h, w, global box index
+
+
+def object_class_side(n):
+    """Canvas side of a crop side n: the next power of two >= n, at least OBJECT_MIN_SIDE."""
+    return max(OBJECT_MIN_SIDE, 1 << (int(n) - 1).bit_length())
+
+
+class ObjectPlan:
+    """The host side of the object-aware loss: which boxes count, their weights and their size classes.
+
+    boxes: per kept box (image b, y0, x0, h, w) in global index order (image by image, box order within an image); w: the
+    weight 1 / (n_b + 1) of each; n_img: n_b per image; dropped: (b, box) of the boxes under OBJECT_MIN_SIDE on a side.
+    classes: per size class, in (Hc, Wc) order, (Hc, Wc, rows, offset into tab) with rows the global indices of its crops.
+    tab: one int32 tensor with every class table (mas_object_* layout) followed by the fp32 weights' bits."""
+
+    def __init__(self, img_shape, rec_shape, bboxes):
+        import numpy as np
+        nb = min(img_shape[0], rec_shape[0], len(bboxes))
+        self.boxes, self.dropped, self.n_img = [], [], []
+        for b in range(nb):
+            bb = bboxes[b]
+            if isinstance(bb, torch.Tensor):
+                bb = bb.detach().cpu().tolist()
+            kept = 0
+            for box in bb:
+                x0, y0, x1, y1 = (int(v) for v in list(box)[:4])
+                if y1 - y0 <= 0 or x1 - x0 <= 0:
+                    raise ValueError("ObjectLoss: box %s of image %d has zero or negative extent" % ([x0, y0, x1, y1], b))
+                if y1 - y0 < OBJECT_MIN_SIDE or x1 - x0 < OBJECT_MIN_SIDE:
+                    self.dropped.append((b, [x0, y0, x1, y1]))
+                    continue
+                self.boxes.append((b, y0, x0, y1 - y0, x1 - x0))
+                kept += 1
+            self.n_img.append(kept)
+        self.K = len(self.boxes)
+        self.w = [1.0 / (self.n_img[b] + 1) for b, *_ in self.boxes]
+        by = {}
+        for k, (_, _, _, h, w) in enumerate(self.boxes):
+            by.setdefault((object_class_side(h), object_class_side(w)), []).append(k)
+        nimg = max(img_shape[0], rec_shape[0])
+        parts, self.classes, off = [], [], 0
+        for (hc, wc), rows in sorted(by.items()):
+            t = np.array([list(self.boxes[k]) + [k] for k in rows], dtype=np.int64).reshape(-1)
+            img_of = np.array([self.boxes[k][0] for k in rows], dtype=np.int64)
+            offs = np.searchsorted(img_of, np.arange(nimg + 1), side="left")
+            parts += [t, offs]
+            self.classes.append((hc, wc, rows, off))
+            off += len(t) + len(offs)
+        self.w_off = off
+        wbits = np.asarray(self.w, dtype=np.float32).view(np.int32)
+        self.tab = torch.from_numpy(np.concatenate(parts + [wbits.astype(np.int64)]).astype(np.int32)) if self.K else None
+
+    def device_tables(self, device):
+        """(tab, wts) on the device: one non-blocking copy; wts is the fp32 view of the weights' bits."""
+        t = self.tab.to(device, non_blocking=True)
+        return t, t[self.w_off:self.w_off + self.K].view(torch.float32)
+
+
+def object_forward_raw(img, rec, plan, shift, scale, convs, lins, keep):
+    """The object-aware loss on the kernels for a plan with at least one box -> dict(p [K] per box by global index, loss (0-dim),
+    saved: per class the activations (keep) for the backward, and the device tables)."""
+    dev = img.device
+    tab, wts = plan.device_tables(dev)
+    _, _, H, W = img.shape
+    nblk = int(L.query("mas_lpips_head_blocks"))
+    p = torch.empty(plan.K, dtype=torch.float32, device=dev)
+    saved = []
+    for hc, wc, rows, off in plan.classes:
+        K, t = len(rows), tab[off:]
+        x = empty_nhwc(2 * K, 3, hc, wc, img)
+        L.call("mas_object_gather", t, K, img, rec, shift, scale, x, H, W, hc, wc)
+        part = torch.empty((5, K, nblk), dtype=torch.float64, device=dev)
+        acts, cur, am, ci = [], x, None, 0
+        for blk, nconv in enumerate(LPIPS_BLOCKS):
+            for _ in range(nconv):
+                wgt, bias = convs[ci]
+                if ci == 0:
+                    h = empty_nhwc(2 * K, wgt.shape[0], hc, wc, x)
+                    L.call("mas_edge_small_cin_fprop", x, L.t4(x), wgt.contiguous(), bias, h, L.t4(h), 0)
+                else:
+                    h = conv3x3_raw(cur, wgt, bias, None, L.CONV_S1, x_amax=am, pad_out=True)
+                _, c, hh, ww = h.shape
+                am = torch.empty(1, dtype=torch.float32, device=dev)
+                L.call("mas_object_relu", h, t, K, hh, ww, c, blk, am)
+                if keep:
+                    acts.append(h)
+                cur, ci = h, ci + 1
+            _, c, hh, ww = cur.shape
+            L.call("mas_object_head_forward", cur, lins[blk].contiguous(), t, K, hh, ww, c, blk, part[blk])
+            if blk < len(LPIPS_BLOCKS) - 1:
+                pool = empty_nhwc(2 * K, c, hh // 2, ww // 2, cur)
+                am = torch.empty(1, dtype=torch.float32, device=dev)
+                L.call("mas_object_maxpool", cur, pool, t, K, hh, ww, c, blk, am)
+                cur = pool
+        L.call("mas_object_head_finalize", part, t, K, p)
+        saved.append(acts if keep else None)
+    loss = torch.empty((), dtype=torch.float32, device=dev)
+    L.call("mas_object_loss", p, wts, plan.K, loss)
+    return dict(p=p, loss=loss, saved=saved if keep else None, tab=tab, wts=wts)
+
+
+def _object_backward(r, plan, convs, lins, scale, want, shapes):
+    """Unit-seed gradients [J_img, J_rec] (None where not wanted) of the loss: per class the VGG data gradient of the wanted
+    canvases from the kept activations, then one scatter per wanted side, accumulated in class order."""
+    tab, wts = r["tab"], r["wts"]
+    dev = tab.device
+    J = [torch.empty(shapes[s], dtype=torch.float32, device=dev) if want[s] else None for s in range(2)]
+    for ic, ((hc, wc, rows, off), acts) in enumerate(zip(plan.classes, r["saved"])):
+        K, t = len(rows), tab[off:]
+        g0, G = (0 if want[0] else K), (2 * K if want[0] and want[1] else K)
+        dpool, ci = None, len(convs)
+        for blk in reversed(range(len(LPIPS_BLOCKS))):
+            tap = acts[ci - 1]
+            _, c, hh, ww = tap.shape
+            dz = empty_nhwc(G, c, hh, ww, tap)
+            am = torch.empty(1, dtype=torch.float32, device=dev)
+            L.call("mas_object_tap_backward", tap, lins[blk].contiguous(), t, K, hh, ww, c, blk, g0, G, dpool, dz, am)
+            first = ci - LPIPS_BLOCKS[blk]
+            for k in reversed(range(first, ci)):
+                wgt = convs[k][0]
+                if k == 0:
+                    dx = empty_nhwc(G, 3, hc, wc, dz)
+                    L.call("mas_edge_small_cout_fprop", dz, L.t4(dz), _lpips_first_dgrad_weight(wgt), None, dx, L.t4(dx))
+                else:
+                    dx = conv3x3_raw(dz, wgt, None, None, L.CONV_S1, transpose=True, x_amax=am, pad_out=True)
+                if k > first:   # the ReLU mask of conv k - 1's output (zero outside the extent: the kept activation is)
+                    am = torch.empty(1, dtype=torch.float32, device=dev)
+                    L.call("mas_lpips_relu_backward", dx, acts[k - 1][g0:g0 + G], dx, dx.numel(), am)
+                dz = dx
+            dpool, ci = dz, first
+        for s in range(2):
+            if want[s]:
+                B, _, H, W = shapes[s]
+                L.call("mas_object_scatter", dpool, scale, t, wts, K, g0, G, s, hc, wc, J[s], B, H, W, int(ic > 0))
+    return J
+
+
+class ObjectLossFn(torch.autograd.Function):
+    """The object-aware loss, sum_b 1 / (n_b + 1) sum_k LPIPS(crop(img_b, box_bk), crop(rec_b, box_bk)), as one unit over an
+    ObjectPlan with at least one box -> 0-dim fp32 loss. Every size class of the plan is one masked LPIPS pass.
+
+    The loss is linear in its seed, so d loss / d input = g * J with J its gradient for a unit seed: the first backward runs
+    the VGG data gradient once per class for the wanted side(s), keeps J and drops the activations; every later traversal
+    of a retained graph is one scaling kernel per wanted input and gives the same result."""
+
+    @staticmethod
+    def forward(ctx, img, rec, plan, shift, scale, convs, lins, keep):
+        _need_cuda(img)
+        _need_cuda(rec)
+        for t in (img, rec):
+            if t.dim() != 4 or t.shape[1] != 3:
+                raise RuntimeError("ObjectLoss expects [B, 3, H, W] images, got %s" % (tuple(t.shape),))
+        if img.shape[2:] != rec.shape[2:]:
+            raise RuntimeError("ObjectLoss expects images and reconstructions of one size, got %s and %s"
+                               % (tuple(img.shape), tuple(rec.shape)))
+        r = object_forward_raw(img.contiguous(), rec.contiguous(), plan, shift, scale, convs, lins, keep)
+        ctx.r = r if keep else None
+        ctx.plan, ctx.convs, ctx.lins, ctx.scale = plan, convs, lins, scale
+        ctx.shapes = (tuple(img.shape), tuple(rec.shape))
+        ctx.J = None
+        return r["loss"]
+
+    @staticmethod
+    def backward(ctx, g):
+        if torch.is_grad_enabled():
+            raise RuntimeError("ObjectLoss does not support create_graph (double backward)")
+        want = (ctx.needs_input_grad[0], ctx.needs_input_grad[1])
+        if ctx.J is None:
+            if ctx.r is None:
+                raise RuntimeError("ObjectLoss: the forward ran without gradient tracking; nothing was saved for a backward")
+            ctx.J = _object_backward(ctx.r, ctx.plan, ctx.convs, ctx.lins, ctx.scale, want, ctx.shapes)
+            ctx.r = None
+        grads = []
+        for s in range(2):
+            J = ctx.J[s]
+            if not want[s]:
+                grads.append(None)
+                continue
+            d = torch.empty_like(J)
+            L.call("mas_lpips_scale_jacobian", J, g.reshape(1).contiguous(), 0, d, 1, J.numel())
+            grads.append(d)
+        return grads[0], grads[1], None, None, None, None, None, None
+
+
 # ---- VGGFace2 face loss (losses/face_loss.py) -------------------------------------------------------------------------
 FACE_CROP, FACE_RESIZE, FACE_MAX = 254, 256, 6   # CenterCrop(254) after Resize(256); faces[:6]
 FACE_BN_EPS = 1e-5
