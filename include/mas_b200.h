@@ -489,6 +489,16 @@ int mas_attn_causal_forward_stats(const float* qkv, const float* amax, float* st
 int mas_attn_causal_backward(const float* qkv, const float* ctx, const float* dctx, const float* stats, const float* amax,
                              const float* dctx_amax, float* D, float* dqkv, int B, int S, int heads, int hd, float scale, double p,
                              const int64_t* seed, void* stream);
+/* mas_attn_causal_prefix_forward: the same core for suffix queries over a shared prefix (MakeAScene.score(num_samples = n)).
+ * qkv [P*n,L,3*heads*hd] is the fused q|k|v of L suffix positions per row, qkv_prefix [P,Lp,3*heads*hd] that of the Lp
+ * prefix positions per prompt; row r's query at suffix position i sits at absolute position Lp + i and attends to keys
+ * 0..Lp-1 of prefix row r / n and Lp..Lp+i of its own row.  Writes ctx [P*n,L,heads*hd] only (no P, no statistics; no
+ * backward).  amax: device scalar max|.| over BOTH qkv tensors.  Same tiles, key blocks and block order as the query tile at
+ * Lp + i of the concatenated sequence, so each row's ctx is the bits mas_attn_causal_forward writes at positions Lp.. of
+ * [P*n,Lp+L,3*heads*hd] (prefix rows repeated n times) with the same amax.  Needs hd == 64 or 128, Lp % 128 == 0 and
+ * L % 128 == 0 (MAS_ERR_UNSUPPORTED otherwise). */
+int mas_attn_causal_prefix_forward(const float* qkv_prefix, const float* qkv, const float* amax, float* ctx, int P, int n, int Lp,
+                                   int L, int heads, int hd, float scale, void* stream);
 /* ---- Dropout of the token transformer (transformer.py:90-91, 114, 139) ------------------------------------------------
  * Element e of a dropout site is kept iff word[e & 3] of Philox4x32-10(counter = (lo32(e >> 2), hi32(e >> 2), 0, 0),
  * key = (lo32(seed), hi32(seed))) >= floor(p * 2^32); e is the element's row-major linear index in its tensor

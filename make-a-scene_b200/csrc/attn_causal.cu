@@ -26,6 +26,11 @@
 //     The keep bits come from dropout.cuh's Philox groups of four keys: the lane pair (fk, fk ^ 1) covers one group per row,
 //     so each lane generates one group per 8-key column block (row frow or frow + 8) and takes the other row's bits from its
 //     partner by a shuffle.
+//   * PREFIX (mas_attn_causal_prefix_forward, MakeAScene.score(num_samples=n)): the queries are the L suffix positions of
+//     row r (qkv [R, L, 3H]), at absolute positions Lp + i, and the keys 0 .. Lp - 1 come from the shared prefix row r / n
+//     (qkv_prefix [P, Lp, 3H]).  The tile, the key blocks and their order are those of the query tile at Lp + i of the
+//     concatenated sequence; only fill() picks the source row of a block (prefix or suffix).  Nothing but ctx is written, so
+//     ctx is the bits mas_attn_causal_forward gives there.
 #include <cuda_fp16.h>
 
 #include <type_traits>
@@ -107,6 +112,8 @@ struct Params {
   const float* amax;  // device scalar: max |qkv| (one scale for q, k and v)
   int S, heads;
   float scale;
+  const float* qkvp;  // PREFIX: the shared prefix [P, Lp, 3H]; S is then the suffix length L, row b reads prefix row b / n
+  int Lp, n;
 };
 
 // D += A B over one K step of 16, N columns (f16 operands, fp32 accumulators); TB = 1: B is MN-major
@@ -117,8 +124,9 @@ __device__ __forceinline__ void mma(float* d, uint64_t a, uint64_t b, uint32_t a
   else wg::wgmma_f16_ss_n128<0, TB>(d, a, b, acc);
 }
 
-template <int HD, bool DROP, bool STATS = false>
+template <int HD, bool DROP, bool STATS = false, bool PREFIX = false>
 __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, const DropMask dm) {
+  static_assert(!PREFIX || (!DROP && !STATS), "the prefix form writes ctx only");
   using C = Cfg<HD>;
   constexpr int BK = C::BK, PITCH_Q = C::PITCH_Q, Q_HALF = C::Q_HALF, PITCH_K = C::PITCH_K, K_HALF = C::K_HALF;
   constexpr int PITCH_V = C::PITCH_V, V_HALF = C::V_HALF, TILE = C::TILE, P_HALF = C::P_HALF;
@@ -132,8 +140,10 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, c
   const int S = p.S, heads = p.heads, H = heads * HD, C3 = 3 * H;
   const int qt = (int)gridDim.x - 1 - (int)blockIdx.x;      // heaviest query tiles first
   const int h = blockIdx.y, b = blockIdx.z;
-  const int q0 = qt * BM, nkb = (qt + 1) * (BM / BK);       // causal: the key blocks up to the tile's last query
+  const int qa = PREFIX ? qt + p.Lp / BM : qt;              // PREFIX: the tile's absolute position in prefix + suffix
+  const int q0 = qa * BM, nkb = (qa + 1) * (BM / BK);       // causal: the key blocks up to the tile's last query
   const float* base = p.qkv + (size_t)b * S * C3 + h * HD;
+  const float* pbase = PREFIX ? p.qkvp + (size_t)(b / p.n) * p.Lp * C3 + h * HD : nullptr;
   const int frow = wgi * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows frow, frow + 8 (query within the tile)
   const uint32_t a_rows = (uint32_t)(wgi * 64 * 16);          // this warpgroup's rows inside a K-major plane
   float inv_s;
@@ -144,13 +154,19 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, c
   // a [ROWS x HD] fp32 tile of the q / k / v third -> hi / lo images; ROWS * HD / 8 items of 8 channels: item = (row, oct)
   // with oct fastest, so HD / 8 lanes read one row's contiguous bytes; all loads of a tile in flight together.
   // The caller has retired every MMA that read dst (wait<0> in both warpgroups, then the barrier below).
+  // row0 is absolute: PREFIX reads rows below Lp from the prefix row, the others from this row's suffix.
   auto fill = [&](auto rows_c, uint8_t* dst, int third, int row0, int pitch, int half) {
     constexpr int N = decltype(rows_c)::value * (HD / 8) / NPROD, OCT_LOG = HD == 64 ? 3 : 4;
+    const float* fb = base;
+    if constexpr (PREFIX) {
+      if (row0 < p.Lp) fb = pbase;
+      else row0 -= p.Lp;
+    }
     float4 v0[N], v1[N];
 #pragma unroll
     for (int i = 0; i < N; ++i) {
       const int itm = pt + i * NPROD, oct = itm & (HD / 8 - 1), r = itm >> OCT_LOG;
-      const float4* src = reinterpret_cast<const float4*>(base + (size_t)(row0 + r) * C3 + third * H + oct * 8);
+      const float4* src = reinterpret_cast<const float4*>(fb + (size_t)(row0 + r) * C3 + third * H + oct * 8);
       v0[i] = __ldg(src);
       v1[i] = __ldg(src + 1);
     }
@@ -171,7 +187,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, c
   using RK = std::integral_constant<int, BK>;
 
   // masked key blocks of the saved probabilities
-  if constexpr (!STATS) {
+  if constexpr (!STATS && !PREFIX) {
     float* pt0 = p.P + (((size_t)b * heads + h) * S + q0) * S;
     const int cols = S - nkb * BK;
     for (int i = tid; i < BM * (cols / 4); i += NTHREADS) {
@@ -210,7 +226,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, c
       if (++stage == STAGES) stage = 0;
       // the blocks with masked entries: key kb * BK + key > query q0 + rit for some row of the tile
       const int koff = BK == BM ? 0 : kb * BK - q0;          // the block's first key relative to the tile's first query
-      const bool diag = BK == BM ? kb == qt : koff >= 0;
+      const bool diag = BK == BM ? kb == qa : koff >= 0;
       if (pass == 0) {
         // online maximum / sum over this thread's columns of its two rows; the four lanes of a row are combined at the end
 #pragma unroll
@@ -283,7 +299,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, c
             const int key = 8 * j + 2 * fk + koff;
             const float a = (diag && key > rit) ? 0.f : expf(sacc[4 * j + 2 * i] * ss - m[i]) * rl[i];
             const float c = (diag && key + 1 > rit) ? 0.f : expf(sacc[4 * j + 2 * i + 1] * ss - m[i]) * rl[i];
-            if constexpr (!STATS) *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(a, c);
+            if constexpr (!STATS && !PREFIX) *reinterpret_cast<float2*>(prow + 8 * j) = make_float2(a, c);
             uint32_t hi, lo;
             if constexpr (DROP)
               split2((keep[i] >> (2 * j)) & 1u ? a : 0.f, (keep[i] >> (2 * j + 1)) & 1u ? c : 0.f, P_SCALE, &hi, &lo);
@@ -322,7 +338,7 @@ __global__ void __launch_bounds__(NTHREADS, 1) attn_causal_fwd(const Params p, c
   if constexpr (DROP) oscale *= dm.scale;
 #pragma unroll
   for (int i = 0; i < 2; ++i) {
-    float* orow = p.ctx + ((size_t)b * S + q0 + frow + 8 * i) * H + h * HD + 2 * fk;
+    float* orow = p.ctx + ((size_t)b * S + q0 - (PREFIX ? p.Lp : 0) + frow + 8 * i) * H + h * HD + 2 * fk;
 #pragma unroll
     for (int j = 0; j < HD / 8; ++j)
       *reinterpret_cast<float2*>(orow + 8 * j) = make_float2(oacc[4 * j + 2 * i] * oscale, oacc[4 * j + 2 * i + 1] * oscale);
@@ -623,17 +639,18 @@ bool attn_causal_fused_ok(int S, int heads, int hd) { return (hd == 64 || hd == 
 
 using namespace mas;
 
-template <int HD, bool DROP, bool STATS>
+template <int HD, bool DROP, bool STATS, bool PREFIX = false>
 static int attn_causal_launch_hd(const attnc::Params& p, const DropMask& dm, int B, void* stream) {
   static std::atomic<uint64_t> configured{0};
   constexpr size_t smem = attnc::Cfg<HD>::SMEM_BYTES;
   if (first_on_device(configured)) {
-    cudaError_t e = cudaFuncSetAttribute(attnc::attn_causal_fwd<HD, DROP, STATS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(attnc::attn_causal_fwd<HD, DROP, STATS, PREFIX>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return fail(MAS_ERR_LAUNCH, "attn_causal_fwd: smem attr: %s", cudaGetErrorString(e));
     mark_device(configured);
   }
   const dim3 grid((unsigned)(p.S / attnc::BM), (unsigned)p.heads, (unsigned)B);
-  attnc::attn_causal_fwd<HD, DROP, STATS><<<grid, attnc::NTHREADS, smem, mas::S(stream)>>>(p, dm);
+  attnc::attn_causal_fwd<HD, DROP, STATS, PREFIX><<<grid, attnc::NTHREADS, smem, mas::S(stream)>>>(p, dm);
+  if (PREFIX) return launched_tc(HD == 128 ? "attn_causal_prefix_fwd<128>" : "attn_causal_prefix_fwd");
   if (HD == 128)
     return launched_tc(STATS ? (DROP ? "attn_causal_dropout_fwd_stats<128>" : "attn_causal_fwd_stats<128>")
                              : (DROP ? "attn_causal_dropout_fwd<128>" : "attn_causal_fwd<128>"));
@@ -650,6 +667,7 @@ static int attn_causal_launch(const float* qkv, const float* amax, float* P, flo
   if (heads > 65535 || B > 65535) return fail(MAS_ERR_UNSUPPORTED, "attn_causal_forward: heads / batch beyond the grid limits");
   attnc::Params p;
   p.qkv = qkv; p.P = P; p.ctx = ctx; p.amax = amax; p.S = S; p.heads = heads; p.scale = scale;
+  p.qkvp = nullptr; p.Lp = 0; p.n = 1;
   return hd == 64 ? attn_causal_launch_hd<64, DROP, STATS>(p, dm, B, stream) : attn_causal_launch_hd<128, DROP, STATS>(p, dm, B, stream);
 }
 
@@ -671,6 +689,22 @@ extern "C" int mas_attn_causal_forward_stats(const float* qkv, const float* amax
     return attn_causal_launch<true, true>(qkv, amax, stats, ctx, B, S, heads, hd, scale,
                                           DropMask{seed, drop_threshold(p), drop_scale(p)}, stream);
   return attn_causal_launch<false, true>(qkv, amax, stats, ctx, B, S, heads, hd, scale, DropMask{nullptr, 0, 1.f}, stream);
+}
+
+extern "C" int mas_attn_causal_prefix_forward(const float* qkv_prefix, const float* qkv, const float* amax, float* ctx, int P, int n,
+                                              int Lp, int L, int heads, int hd, float scale, void* stream) {
+  MAS_REQUIRE(qkv_prefix && qkv && amax && ctx && P > 0 && n > 0, "attn_causal_prefix_forward: bad arguments");
+  if (!(hd == 64 || hd == 128) || heads <= 0 || Lp <= 0 || L <= 0 || Lp % attnc::BM || L % attnc::BM)
+    return fail(MAS_ERR_UNSUPPORTED, "attn_causal_prefix_forward: needs head dim 64 or 128, Lp %% 128 == 0 and L %% 128 == 0 "
+                "(got Lp=%d, L=%d, hd=%d)", Lp, L, hd);
+  if (heads > 65535 || (int64_t)P * n > 65535)
+    return fail(MAS_ERR_UNSUPPORTED, "attn_causal_prefix_forward: heads / rows beyond the grid limits");
+  attnc::Params p;
+  p.qkv = qkv; p.P = nullptr; p.ctx = ctx; p.amax = amax; p.S = L; p.heads = heads; p.scale = scale;
+  p.qkvp = qkv_prefix; p.Lp = Lp; p.n = n;
+  const DropMask dm{nullptr, 0, 1.f};
+  return hd == 64 ? attn_causal_launch_hd<64, false, false, true>(p, dm, P * n, stream)
+                  : attn_causal_launch_hd<128, false, false, true>(p, dm, P * n, stream);
 }
 
 template <int HD, bool DKV, bool DROP>

@@ -153,6 +153,7 @@ _SPEC = {
     "mas_attn_causal_forward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "mas_attn_causal_forward_stats": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _D, _P, _P]),
     "mas_attn_causal_backward": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _D, _P, _P]),
+    "mas_attn_causal_prefix_forward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _F, _P]),
     "mas_dropout": (_I, [_P, _P, _P, _L, _D, _F, _P, _P]),
     "mas_attn_causal_dropout_forward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _D, _P, _P]),
     "mas_softmax_causal_dropout_backward": (_I, [_P, _P, _P, _L, _I, _I, _F, _D, _P, _P]),

@@ -1492,12 +1492,35 @@ def _packed_linear_weight(weight, transpose, dev):
     return _cached(weight, ("lin16", bool(transpose)), make)
 
 
-def rows_to_half(x2d):
-    """(fp16 copy of a dense [M,K] matrix under the power-of-two scale of its max|.|, that maximum as a device scalar)."""
-    am = amax(x2d)
+def rows_to_half(x2d, am=None):
+    """(fp16 copy of a dense [M,K] matrix under the power-of-two scale of its max|.|, that maximum as a device scalar).
+    am: a given device maximum instead (one at least max|x2d|, e.g. amax_joint over the blocks of a larger operand)."""
+    if am is None:
+        am = amax(x2d)
     x16 = torch.empty(x2d.shape, dtype=torch.float16, device=x2d.device)
     L.call("mas_to_half", x2d, x16, x2d.numel(), am)
     return x16, am
+
+
+def amax_joint(*parts):
+    """max|.| over several tensors as one device scalar: the max of their concatenation, bit for bit (mas_amax of every part,
+    then of the part maxima). For one operand that is computed in blocks but has to be scaled as a whole."""
+    each = torch.empty(len(parts), dtype=torch.float32, device=parts[0].device)
+    for i, x in enumerate(parts):
+        L.call("mas_amax", x, x.numel(), each[i:])
+    return amax(each)
+
+
+def linear_joint(parts, weight, bias):
+    """nn.Linear on the fp16 route (linear_f16_on) of several row blocks under the ONE operand scale of their
+    concatenation: each block's output is the bits of those rows of LinearFn on the concatenated rows (the row GEMM
+    mas_gemm_rows_f16 computes every row alone). parts: contiguous fp32 tensors [..., K]; returns their outputs [..., N]."""
+    N, K = weight.shape
+    if not linear_f16_on(N, K):
+        raise RuntimeError("linear_joint: the fp16 Linear route is off for [%d, %d]" % (N, K))
+    rows = [x.reshape(-1, K) for x in parts]
+    am = amax_joint(*rows)
+    return [gemm_rows_f16(rows_to_half(r, am)[0], am, weight, False, bias).view(x.shape[:-1] + (N,)) for x, r in zip(parts, rows)]
 
 
 def gemm_rows_f16(x16, am, weight, transpose=False, bias=None):
@@ -1594,6 +1617,36 @@ def attn_causal_fused_on(S_, hd):
     """The fused wgmma causal-attention kernels (csrc/attn_causal.cu): head dim 64 or 128, S % 128 == 0, tensor path enabled.
     MAS_ATTN_FUSED=0 selects the GEMM / softmax / GEMM sequence instead."""
     return _tc_on() and hd in (64, 128) and S_ % 128 == 0 and S_ >= 128 and os.environ.get("MAS_ATTN_FUSED", "1") != "0"
+
+
+def attn_causal_given_amax(qkv, heads, am):
+    """The P-free fused causal attention (mas_attn_causal_forward_stats, no dropout) of qkv [B,S,3H] under a given device
+    max am >= max|qkv| instead of qkv's own: ctx [B,S,H]; the statistics are not kept. Inference only."""
+    B, S_, H3 = qkv.shape
+    hd = H3 // 3 // heads
+    if not attn_causal_fused_on(S_, hd):
+        raise RuntimeError("attn_causal_given_amax: needs the fused causal core (S=%d, head dim %d)" % (S_, hd))
+    stats = torch.empty((2, B, heads, S_), dtype=torch.float32, device=qkv.device)
+    ctxv = torch.empty((B, S_, H3 // 3), dtype=torch.float32, device=qkv.device)
+    L.call("mas_attn_causal_forward_stats", qkv.contiguous(), am, stats, ctxv, B, S_, heads, hd, 1.0 / float(hd) ** 0.5, 0.0, None)
+    return ctxv
+
+
+def attn_causal_prefix(qkv_prefix, qkv, am, heads):
+    """Causal attention of suffix queries over a shared prefix (mas_attn_causal_prefix_forward): qkv [R,L,3H] holds L suffix
+    positions per row, qkv_prefix [P,Lp,3H] the prefix of each prompt; row r (of R = P * n) is the continuation of prefix
+    row r // n and its query i sits at position Lp + i. am: device max|.| over both tensors. Returns ctx [R,L,H], the bits
+    of the fused forward on the concatenated [R,Lp+L,3H] rows at positions Lp.. under the same am. Inference only."""
+    P, Lp, H3 = qkv_prefix.shape
+    R, L_, H3s = qkv.shape
+    if H3s != H3 or R % P or H3 % (3 * heads):
+        raise ValueError("attn_causal_prefix: qkv %s must continue the rows of qkv_prefix %s in groups (%d heads)"
+                         % (tuple(qkv.shape), tuple(qkv_prefix.shape), heads))
+    hd = H3 // 3 // heads
+    ctxv = torch.empty((R, L_, H3 // 3), dtype=torch.float32, device=qkv.device)
+    L.call("mas_attn_causal_prefix_forward", qkv_prefix.contiguous(), qkv.contiguous(), am, ctxv, P, R // P, Lp, L_, heads, hd,
+           1.0 / float(hd) ** 0.5)
+    return ctxv
 
 
 class CausalAttentionFn(torch.autograd.Function):

@@ -176,6 +176,13 @@ class Transformer(nn.Module):
         return self.final_ln(x), {}
 
 
+# score(num_samples=n) computes each prompt's prefix once only from this many candidate rows on (B*n, twice that with
+# guidance). Below it both forms are bound by the host's launch rate, and the shared form, with two launches per kernel of a
+# layer, is the slower (24 layers, 1024 wide, H100 80GB HBM3 at 700 W: 0.68x at 16 rows, 1.06x at 24, 1.8x from 48;
+# tools/bench_score.py). The result is the same bits either way.
+SCORE_SHARED_MIN_ROWS = 24
+
+
 def _param_version(model):
     return tuple((p._version, p.data_ptr()) for p in model.parameters())
 
@@ -379,6 +386,41 @@ class MakeAScene(nn.Module):
             m = layer.mlp.project(layer.ln_out(x))
             x = layer.second_ln_sandwich(m, residual=x) if layer.cogview_sandwich_layernorm else x + m
         return x
+
+    def _score_shares_prefix(self, rows=None):
+        """Whether score(num_samples > 1) runs the prefix once per prompt (_prefill_shared): the fused causal core for the
+        prefix and the image lengths, the fp16 Linear route for the layers' widths and (when given) at least
+        SCORE_SHARED_MIN_ROWS candidate rows. Elsewhere it repeats the prompts."""
+        if rows is not None and rows < SCORE_SHARED_MIN_ROWS:
+            return False
+        heads = self.transformer.layers[0].attn.num_attn_heads
+        hd, H = self.hidden_dim // heads, self.hidden_dim
+        prefix = self.text_length + self.seg_length
+        return (ops.attn_causal_fused_on(prefix, hd) and ops.attn_causal_fused_on(self.image_length, hd)
+                and all(ops.linear_f16_on(n, k) for n, k in ((3 * H, H), (H, H), (4 * H, H), (H, 4 * H))))
+
+    def _prefill_shared(self, xp, xs, n):
+        """_prefill of prefix rows xp [P,Lp,H] continued by suffix rows xs [P*n,L,H] (row r continues prefix row r // n), in
+        lockstep through every layer: each row's hidden states are the bits _prefill gives on the concatenated [P*n,Lp+L,H]
+        sequence (prefix rows repeated). Those scale every fp16 operand by max|.| over the whole tensor, prefix rows included,
+        so each Linear and attention call here takes the joint maximum of both parts (ops.amax_joint). Returns (xp, xs)."""
+        heads = self.transformer.layers[0].attn.num_attn_heads
+
+        def sandwich(ln, a, x):
+            return ln(a, residual=x) if ln is not None else x + a
+        for layer in self.transformer.layers:
+            at, mlp = layer.attn, layer.mlp
+            qp, qs = ops.linear_joint([layer.ln_in(xp), layer.ln_in(xs)], at.qkv.weight, at.qkv.bias)
+            am = ops.amax_joint(qp, qs)
+            cp, cs = ops.attn_causal_given_amax(qp, heads, am), ops.attn_causal_prefix(qp, qs, am, heads)
+            ap, as_ = ops.linear_joint([cp, cs], at.out_proj.weight, at.out_proj.bias)
+            ln1 = layer.first_ln_sandwich if layer.cogview_sandwich_layernorm else None
+            xp, xs = sandwich(ln1, ap, xp), sandwich(ln1, as_, xs)
+            mp, ms = ops.linear_joint([layer.ln_out(xp), layer.ln_out(xs)], mlp.lin1.weight, mlp.lin1.bias)
+            mp, ms = ops.linear_joint([gelu(mp), gelu(ms)], mlp.lin2.weight, mlp.lin2.bias)
+            ln2 = layer.second_ln_sandwich if layer.cogview_sandwich_layernorm else None
+            xp, xs = sandwich(ln2, mp, xp), sandwich(ln2, ms, xs)
+        return xp, xs
 
     def _decode_step(self, x, kc, vc, pos, suffix=None):
         """One new token per row (x [R,H], absolute position pos) through all layers against the cache; returns
@@ -589,7 +631,7 @@ class MakeAScene(nn.Module):
         return out if len(out) > 1 else tokens
 
     @torch.no_grad()
-    def score(self, text_tokens, seg_tokens, img_tokens, guidance_scale=None, uncond_text_tokens=None):
+    def score(self, text_tokens, seg_tokens, img_tokens, guidance_scale=None, uncond_text_tokens=None, num_samples=1):
         """Teacher-forced log-likelihood of given image tokens: fp32 [B,image_length], entry [b, t] = log p(img_t | text, seg,
         img_<t) at temperature 1 with no filters, natural log. With guidance (guidance_scale and uncond_text_tokens as in
         generate) the distribution is softmax(u + s * (c - u)) of the unconditional and conditional streams' logits, the one
@@ -600,23 +642,36 @@ class MakeAScene(nn.Module):
         [0, image_vocab_size)) and uncond_text_tokens [B,text_length]: int64 on the model's device.
         guidance_scale may also give one scale per row (a 1-D tensor on the model's device, or a sequence, of B values, as in
         generate): row b is then the guided log-likelihood at its own scale, bit for bit the row of a call with that scale, so
-        candidates can be reranked at several scales in one pass (a row at scale 1 in a guided call: see generate)."""
-        named = [("text_tokens", text_tokens, self.text_length), ("seg_tokens", seg_tokens, self.seg_length),
-                 ("img_tokens", img_tokens, self.image_length)]
-        if uncond_text_tokens is not None:
-            named.append(("uncond_text_tokens", uncond_text_tokens, self.text_length))
+        candidates can be reranked at several scales in one pass (a row at scale 1 in a guided call: see generate).
+        num_samples=n (int >= 1) scores n candidates per prompt, as generate(num_samples=n) draws them: text_tokens,
+        seg_tokens and uncond_text_tokens stay per prompt [B,·], img_tokens and the result have B*n rows (row b*n + j is
+        candidate j of prompt b), a per-row guidance_scale has B*n values. The result is bit for bit that of
+        score(text_tokens.repeat_interleave(n, 0), seg_tokens.repeat_interleave(n, 0), img_tokens, ...) (uncond_text_tokens
+        repeated likewise). Where the fused causal-attention core and the fp16 Linear route run (head dim 64 or 128, text +
+        seg and image lengths multiples of 128, hidden width a multiple of 128) and the call has at least
+        SCORE_SHARED_MIN_ROWS candidate rows (B*n, 2*B*n with guidance), the text + seg prefix is computed once per prompt
+        and each candidate's image positions attend to it (mas_attn_causal_prefix_forward): about half the Linear work and
+        half the activation memory of the repeated call at the paper's lengths. Elsewhere the prompts are repeated."""
+        n = num_samples
+        if isinstance(n, bool) or not isinstance(n, int) or n < 1:
+            raise ValueError("num_samples must be an int >= 1, got %r" % (num_samples,))
         B = text_tokens.shape[0] if isinstance(text_tokens, torch.Tensor) and text_tokens.dim() == 2 else None
+        Bn = None if B is None else B * n
+        named = [("text_tokens", text_tokens, self.text_length, B), ("seg_tokens", seg_tokens, self.seg_length, B),
+                 ("img_tokens", img_tokens, self.image_length, Bn)]
+        if uncond_text_tokens is not None:
+            named.append(("uncond_text_tokens", uncond_text_tokens, self.text_length, B))
         dev = self.image_token_embedding.weight.device
-        for name, t, length in named:
-            if not isinstance(t, torch.Tensor) or B is None or tuple(t.shape) != (B, length):
-                raise ValueError("%s must be a tensor of shape %s" % (name, (B, length)))
+        for name, t, length, rows in named:
+            if not isinstance(t, torch.Tensor) or B is None or tuple(t.shape) != (rows, length):
+                raise ValueError("%s must be a tensor of shape %s" % (name, (rows, length)))
             if t.dtype != torch.int64:
                 raise ValueError("%s must be int64, got %s" % (name, t.dtype))
             if t.device != dev:
                 raise ValueError("%s must be on the model's device (%s), got %s" % (name, dev, t.device))
         scale_rows = None
         if _is_per_row(guidance_scale):
-            scale_h, scale_d = _row_values("guidance_scale", guidance_scale, B, dev)
+            scale_h, scale_d = _row_values("guidance_scale", guidance_scale, Bn, dev)
             if not bool(torch.isfinite(scale_h).all()):
                 raise ValueError("guidance_scale must be finite in every row, got %s" % scale_h.tolist())
             scale_rows = scale_d if bool((scale_h != 1.0).any()) else None
@@ -624,6 +679,9 @@ class MakeAScene(nn.Module):
         if bool(((img_tokens < 0) | (img_tokens >= V)).any()):
             raise ValueError("img_tokens must lie in [0, %d)" % V)
         cfg = scale_rows is not None if _is_per_row(guidance_scale) else guidance_scale is not None and float(guidance_scale) != 1.0
+        if n > 1 and not self._score_shares_prefix(Bn * (2 if cfg else 1)):
+            rep = lambda t: None if t is None else t.repeat_interleave(n, 0)
+            return self.score(rep(text_tokens), rep(seg_tokens), img_tokens, guidance_scale, rep(uncond_text_tokens))
         if cfg:
             if uncond_text_tokens is None:
                 uncond_text_tokens = torch.zeros_like(text_tokens)          # all padding, as in generate
@@ -632,11 +690,21 @@ class MakeAScene(nn.Module):
         else:
             img_all = img_tokens
         L = self.image_length
-        h = self.transformer.final_ln(self._prefill(self._embed(text_tokens, seg_tokens, img_all)))
-        h = h[:, -L - 1:-1].contiguous()                                    # forward()'s slice: the predicting positions
+        if n == 1:
+            h = self.transformer.final_ln(self._prefill(self._embed(text_tokens, seg_tokens, img_all)))
+            h = h[:, -L - 1:-1].contiguous()                                # forward()'s slice: the predicting positions
+        else:
+            # prefix rows [cond B | uncond B], candidate rows [cond B*n | uncond B*n]: row r continues prefix row r // n
+            ar = torch.arange(L, dtype=torch.long, device=dev)
+            ip = self.image_tokens_per_dim
+            xs = ops.EmbedFn.apply([(img_all, ar // ip, ar % ip, 0)], L, self.hidden_dim, self.image_token_embedding.weight,
+                                   self.image_row_embeddings.weight, self.image_col_embeddings.weight)
+            xp, xs = self._prefill_shared(self._embed(text_tokens, seg_tokens, None), xs, n)
+            # the predicting positions: the prefix's last one (for image token 0), then image positions 0 .. L-2
+            h = self.transformer.final_ln(torch.cat([xp[:, -1:].repeat_interleave(n, 0), xs[:, :-1]], 1))
         logits = self.to_logits[1](self.to_logits[0](h))
         if scale_rows is not None:
-            logits = ops.cfg_mix_rows(logits[:B], logits[B:], scale_rows)
+            logits = ops.cfg_mix_rows(logits[:Bn], logits[Bn:], scale_rows)
         elif cfg:
-            logits = ops.cfg_mix(logits[:B], logits[B:], guidance_scale)
-        return ops.token_logprobs(logits.view(B * L, V), img_tokens.reshape(B * L)).view(B, L)
+            logits = ops.cfg_mix(logits[:Bn], logits[Bn:], guidance_scale)
+        return ops.token_logprobs(logits.view(Bn * L, V), img_tokens.reshape(Bn * L)).view(Bn, L)
