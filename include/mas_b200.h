@@ -660,6 +660,26 @@ int mas_bce_scene_forward(const float* logits, const uint8_t* labels, const floa
 int mas_bce_scene_backward(const float* logits, const uint8_t* labels, const float* pos_weight, const float* g, int N, int CP,
                            int H, int W, float* grad, void* stream);
 
+/* ---- weighted BCE-with-logits + MSE of the sigmoid (VQVAEWithBCELoss, losses/loss_seg.py:34-41) -------------------------
+ * mse_loss(sigmoid(x), t) and the weighted BCE are means over the same N*C*H*W elements, so the loss is one mean:
+ *   loss = mean[ (1 + (pw_c - 1) t) softplus(-x) + (1 - t) x + (sigmoid(x) - t)^2 ]
+ *   dloss/dx = ( (1 + (pw_c - 1) t) sigmoid(x) - pw_c t + 2 (sigmoid(x) - t) sigmoid(x) (1 - sigmoid(x)) ) / (N*C*H*W)
+ * Each entry takes the arguments, layouts, limits and workspace (mas_bce_cl_ws_bytes / mas_bce_ws_bytes) of the weighted-BCE
+ * entry of the same name without "_mse", and reduces the same way (per-block fp64 partials, one fixed-order fp64 total).
+ * mas_bce_mse_cl_*: also MAS_ERR_UNSUPPORTED when the staged target tile (C * 33 floats) exceeds 48 KB.
+ * mas_bce_mse_scene_*: loss and gradient bit-identical to mas_bce_mse_cl_* on the expanded target.
+ * mas_bce_mse_logits: grad (may be NULL) = grad_scale * dl/dx, the target and grad views of the logits' extents. */
+int mas_bce_mse_cl_forward(const float* logits, const float* target_nchw, const float* pos_weight, int N, int C, int CP, int H,
+                           int W, float* loss_out, void* ws, size_t ws_bytes, void* stream);
+int mas_bce_mse_cl_backward(const float* logits, const float* target_nchw, const float* pos_weight, const float* g, int N, int C,
+                            int CP, int H, int W, float* grad, void* stream);
+int mas_bce_mse_scene_forward(const float* logits, const uint8_t* labels, const float* pos_weight, int N, int CP, int H, int W,
+                              float* loss_out, void* ws, size_t ws_bytes, void* stream);
+int mas_bce_mse_scene_backward(const float* logits, const uint8_t* labels, const float* pos_weight, const float* g, int N, int CP,
+                               int H, int W, float* grad, void* stream);
+int mas_bce_mse_logits(const float* logits, mas_tensor4 ls, const float* target, mas_tensor4 ts, const float* pos_weight,
+                       float* loss_out, float* grad, mas_tensor4 gs, float grad_scale, void* ws, size_t ws_bytes, void* stream);
+
 
 /* ---- LPIPS perceptual loss (losses/lpips.py; csrc/lpips.cu) ------------------------------------------------------------
  * The thirteen VGG16 3x3 convolutions (lpips.py:106-111, torchvision vgg16 features[0:30]) run on the 3x3 family above

@@ -791,7 +791,11 @@ __global__ void sumpool2x2_kernel(const float* __restrict__ x, float* __restrict
 
 // weighted BCE-with-logits (loss_seg.py:15-19): l = -[pw*t*log(sig(x)) + (1-t)*log(1-sig(x))]
 //   = (1-t)*x + (1+(pw-1)*t) * softplus(-x);  dl/dx = (1-t) - (1+(pw-1)*t)*sigmoid(-x)
+// MSE adds VQVAEWithBCELoss's term (loss_seg.py:34-41): both are means over the same N*C*H*W elements, so the sum is one mean
+// of l + (sig(x)-t)^2, with dl/dx + 2*(sig(x)-t)*sig(x)*sig(-x).  MSE = false is the BCE kernel alone, instruction for
+// instruction.
 constexpr int BCE_CHUNK = 256 * 8;
+template <bool MSE>
 __global__ void __launch_bounds__(256) bce_kernel(const float* __restrict__ lg, mas_tensor4 ls, const float* __restrict__ tg,
                                                   mas_tensor4 ts, const float* __restrict__ pw, float* __restrict__ grad,
                                                   mas_tensor4 gs, float gscale, double* __restrict__ part, int64_t total) {
@@ -807,11 +811,22 @@ __global__ void __launch_bounds__(256) bce_kernel(const float* __restrict__ lg, 
       float x = lg[n * ls.sn + h * ls.sh + w * ls.sw + c * ls.sc];
       float t = tg[n * ts.sn + h * ts.sh + w * ts.sw + c * ts.sc];
       float coef = 1.0f + (pw[c] - 1.0f) * t;
-      float sp = fmaxf(-x, 0.f) + log1pf(expf(-fabsf(x)));  // softplus(-x)
-      acc += (double)((1.0f - t) * x + coef * sp);
+      float e = expf(-fabsf(x));
+      float sp = fmaxf(-x, 0.f) + log1pf(e);  // softplus(-x)
+      float l = (1.0f - t) * x + coef * sp;
+      if (MSE) {
+        float d = (x >= 0.f ? 1.0f : e) / (1.0f + e) - t;  // sigmoid(x) - t
+        l += d * d;
+      }
+      acc += (double)l;
       if (grad) {
         float sg = 1.0f / (1.0f + expf(x));  // sigmoid(-x)
-        grad[n * gs.sn + h * gs.sh + w * gs.sw + c * gs.sc] = gscale * ((1.0f - t) - coef * sg);
+        float dl = (1.0f - t) - coef * sg;
+        if (MSE) {
+          float s = 1.0f / (1.0f + expf(-x));  // sigmoid(x)
+          dl += 2.0f * (s - t) * s * sg;
+        }
+        grad[n * gs.sn + h * gs.sh + w * gs.sw + c * gs.sc] = gscale * dl;
       }
     }
   }
@@ -850,8 +865,8 @@ struct SceneTarget {   // compact scene map [N, 4, H, W] uint8: 4 x 32 label byt
 // Same loss for the layouts the VQ-SEG step actually has: logits channels-last with pitch CP >= C (the padded output of
 // the decoder's last convolution), target NCHW (the data loader's one-hot maps) or compact scene labels.  Block = 32
 // consecutive pixels of one image row: the target is staged by the fetch, the logits / gradient tile is one contiguous
-// 32 x CP block.  MODE 0: loss partials.  MODE 1: gradient g * gscale * dl/dx (pad channels get 0).
-template <int MODE, class Target>
+// 32 x CP block.  MODE 0: loss partials.  MODE 1: gradient g * gscale * dl/dx (pad channels get 0).  MSE: as bce_kernel.
+template <int MODE, class Target, bool MSE = false>
 __global__ void __launch_bounds__(256) bce_cl_kernel(const float* __restrict__ lg, Target tg, const float* __restrict__ pw,
                                                      int C, int CP, int H, int W, const float* __restrict__ g, float gscale,
                                                      float* __restrict__ grad, double* __restrict__ part) {
@@ -868,11 +883,22 @@ __global__ void __launch_bounds__(256) bce_cl_kernel(const float* __restrict__ l
       const float x = __ldg(lg + base + i), t = tg.at(tile, c, px);
       const float coef = 1.0f + (__ldg(pw + c) - 1.0f) * t;
       if (MODE == 0) {
-        const float sp = fmaxf(-x, 0.f) + log1pf(expf(-fabsf(x)));
-        acc += (double)((1.0f - t) * x + coef * sp);
+        const float e = expf(-fabsf(x));
+        const float sp = fmaxf(-x, 0.f) + log1pf(e);
+        float l = (1.0f - t) * x + coef * sp;
+        if (MSE) {
+          const float d = (x >= 0.f ? 1.0f : e) / (1.0f + e) - t;
+          l += d * d;
+        }
+        acc += (double)l;
       } else {
         const float sg = 1.0f / (1.0f + expf(x));
-        grad[base + i] = gs * ((1.0f - t) - coef * sg);
+        float dl = (1.0f - t) - coef * sg;
+        if (MSE) {
+          const float s = 1.0f / (1.0f + expf(-x));
+          dl += 2.0f * (s - t) * s * sg;
+        }
+        grad[base + i] = gs * dl;
       }
     } else if (MODE == 1) {
       grad[base + i] = 0.f;
@@ -907,24 +933,37 @@ static inline int ew_grid(int64_t n, int threads = 256) {
   return (int)(b < NUM_SMS * 16 ? (b < 1 ? 1 : b) : NUM_SMS * 16);
 }
 
-// launches of bce_cl_kernel shared by the dense (mas_bce_cl_*) and compact (mas_bce_scene_*) targets
-template <class Target>
+// launches of bce_cl_kernel shared by the dense (mas_bce_cl_*, mas_bce_mse_cl_*) and compact (mas_bce_scene_*,
+// mas_bce_mse_scene_*) targets
+template <bool MSE, class Target>
 static int bce_cl_forward(const float* logits, Target tg, const float* pos_weight, int N, int C, int CP, int H, int W, float* loss_out,
                           void* ws, size_t ws_bytes, void* stream) {
   if (ws_bytes < mas_bce_cl_ws_bytes(N, H, W)) return fail(MAS_ERR_WORKSPACE, "bce_cl_forward: workspace too small");
   const int nb = N * H * (W / 32);
-  bce_cl_kernel<0><<<dim3(W / 32, H, N), 256, Target::smem(C), S(stream)>>>(logits, tg, pos_weight, C, CP, H, W, nullptr, 0.f, nullptr,
-                                                                             (double*)ws);
-  if (int e = launched("bce_cl_loss")) return e;
+  bce_cl_kernel<0, Target, MSE><<<dim3(W / 32, H, N), 256, Target::smem(C), S(stream)>>>(logits, tg, pos_weight, C, CP, H, W, nullptr,
+                                                                                          0.f, nullptr, (double*)ws);
+  if (int e = launched(MSE ? "bce_mse_cl_loss" : "bce_cl_loss")) return e;
   sum_final_kernel<<<1, 256, 0, S(stream)>>>((const double*)ws, nb, 1.0 / ((double)N * C * H * W), loss_out);
   return launched("bce_final");
 }
-template <class Target>
+template <bool MSE, class Target>
 static int bce_cl_backward(const float* logits, Target tg, const float* pos_weight, const float* g, int N, int C, int CP, int H, int W,
                            float* grad, void* stream) {
-  bce_cl_kernel<1><<<dim3(W / 32, H, N), 256, Target::smem(C), S(stream)>>>(logits, tg, pos_weight, C, CP, H, W, g,
-                                                                             (float)(1.0 / ((double)N * C * H * W)), grad, nullptr);
-  return launched("bce_cl_grad");
+  bce_cl_kernel<1, Target, MSE><<<dim3(W / 32, H, N), 256, Target::smem(C), S(stream)>>>(logits, tg, pos_weight, C, CP, H, W, g,
+                                                                                          (float)(1.0 / ((double)N * C * H * W)), grad,
+                                                                                          nullptr);
+  return launched(MSE ? "bce_mse_cl_grad" : "bce_cl_grad");
+}
+template <bool MSE>
+static int bce_logits(const float* logits, mas_tensor4 ls, const float* target, mas_tensor4 ts, const float* pos_weight,
+                      float* loss_out, float* grad, mas_tensor4 gs, float grad_scale, void* ws, size_t ws_bytes, void* stream) {
+  int64_t total = ls.n * ls.h * ls.w * ls.c;
+  if (ws_bytes < mas_bce_ws_bytes(ls)) return fail(MAS_ERR_WORKSPACE, "bce: workspace too small");
+  int blocks = (int)cdiv(total, BCE_CHUNK);
+  bce_kernel<MSE><<<blocks, 256, 0, S(stream)>>>(logits, ls, target, ts, pos_weight, grad, gs, grad_scale, (double*)ws, total);
+  if (int e = launched(MSE ? "bce_mse" : "bce")) return e;
+  sum_final_kernel<<<1, 256, 0, S(stream)>>>((const double*)ws, blocks, 1.0 / (double)total, loss_out);
+  return launched("bce_final");
 }
 
 }  // namespace mas
@@ -1189,36 +1228,66 @@ size_t mas_bce_cl_ws_bytes(int N, int H, int W) { return (size_t)N * H * cdiv(W,
 int mas_bce_cl_forward(const float* logits, const float* target_nchw, const float* pos_weight, int N, int C, int CP, int H, int W,
                        float* loss_out, void* ws, size_t ws_bytes, void* stream) {
   MAS_REQUIRE(logits && target_nchw && pos_weight && loss_out && N > 0 && C > 0 && CP >= C && W % 32 == 0, "bce_cl_forward: bad arguments");
-  return bce_cl_forward(logits, DenseTarget{target_nchw}, pos_weight, N, C, CP, H, W, loss_out, ws, ws_bytes, stream);
+  return bce_cl_forward<false>(logits, DenseTarget{target_nchw}, pos_weight, N, C, CP, H, W, loss_out, ws, ws_bytes, stream);
 }
 int mas_bce_cl_backward(const float* logits, const float* target_nchw, const float* pos_weight, const float* g, int N, int C, int CP,
                         int H, int W, float* grad, void* stream) {
   MAS_REQUIRE(logits && target_nchw && pos_weight && grad && N > 0 && C > 0 && CP >= C && W % 32 == 0, "bce_cl_backward: bad arguments");
-  return bce_cl_backward(logits, DenseTarget{target_nchw}, pos_weight, g, N, C, CP, H, W, grad, stream);
+  return bce_cl_backward<false>(logits, DenseTarget{target_nchw}, pos_weight, g, N, C, CP, H, W, grad, stream);
 }
 int mas_bce_scene_forward(const float* logits, const uint8_t* labels, const float* pos_weight, int N, int CP, int H, int W,
                           float* loss_out, void* ws, size_t ws_bytes, void* stream) {
   MAS_REQUIRE(logits && labels && pos_weight && loss_out && N > 0 && H > 0 && CP >= SCENE_C && W > 0 && W % 32 == 0,
               "bce_scene_forward: bad arguments");
-  return bce_cl_forward(logits, SceneTarget{labels}, pos_weight, N, SCENE_C, CP, H, W, loss_out, ws, ws_bytes, stream);
+  return bce_cl_forward<false>(logits, SceneTarget{labels}, pos_weight, N, SCENE_C, CP, H, W, loss_out, ws, ws_bytes, stream);
 }
 int mas_bce_scene_backward(const float* logits, const uint8_t* labels, const float* pos_weight, const float* g, int N, int CP, int H,
                            int W, float* grad, void* stream) {
   MAS_REQUIRE(logits && labels && pos_weight && grad && N > 0 && H > 0 && CP >= SCENE_C && W > 0 && W % 32 == 0,
               "bce_scene_backward: bad arguments");
-  return bce_cl_backward(logits, SceneTarget{labels}, pos_weight, g, N, SCENE_C, CP, H, W, grad, stream);
+  return bce_cl_backward<false>(logits, SceneTarget{labels}, pos_weight, g, N, SCENE_C, CP, H, W, grad, stream);
 }
 
 size_t mas_bce_ws_bytes(mas_tensor4 ls) { return (size_t)cdiv(ls.n * ls.h * ls.w * ls.c, BCE_CHUNK) * sizeof(double) + 64; }
 int mas_bce_logits(const float* logits, mas_tensor4 ls, const float* target, mas_tensor4 ts, const float* pos_weight,
                    float* loss_out, float* grad, mas_tensor4 gs, float grad_scale, void* ws, size_t ws_bytes, void* stream) {
-  int64_t total = ls.n * ls.h * ls.w * ls.c;
-  if (ws_bytes < mas_bce_ws_bytes(ls)) return fail(MAS_ERR_WORKSPACE, "bce: workspace too small");
-  int blocks = (int)cdiv(total, BCE_CHUNK);
-  bce_kernel<<<blocks, 256, 0, S(stream)>>>(logits, ls, target, ts, pos_weight, grad, gs, grad_scale, (double*)ws, total);
-  if (int e = launched("bce")) return e;
-  sum_final_kernel<<<1, 256, 0, S(stream)>>>((const double*)ws, blocks, 1.0 / (double)total, loss_out);
-  return launched("bce_final");
+  return bce_logits<false>(logits, ls, target, ts, pos_weight, loss_out, grad, gs, grad_scale, ws, ws_bytes, stream);
+}
+
+// BCE + MSE of the sigmoid (VQVAEWithBCELoss, losses/loss_seg.py:34-41): the same launches, extents and workspaces as the
+// weighted-BCE entries above, on the MSE instantiations of their kernels
+int mas_bce_mse_cl_forward(const float* logits, const float* target_nchw, const float* pos_weight, int N, int C, int CP, int H,
+                           int W, float* loss_out, void* ws, size_t ws_bytes, void* stream) {
+  MAS_REQUIRE(logits && target_nchw && pos_weight && loss_out && N > 0 && C > 0 && CP >= C && H > 0 && W > 0 && W % 32 == 0,
+              "bce_mse_cl_forward: bad arguments");
+  if ((size_t)C * 33 * sizeof(float) > 48 * 1024) return fail(MAS_ERR_UNSUPPORTED, "bce_mse_cl_forward: C=%d too large", C);
+  return bce_cl_forward<true>(logits, DenseTarget{target_nchw}, pos_weight, N, C, CP, H, W, loss_out, ws, ws_bytes, stream);
+}
+int mas_bce_mse_cl_backward(const float* logits, const float* target_nchw, const float* pos_weight, const float* g, int N, int C,
+                            int CP, int H, int W, float* grad, void* stream) {
+  MAS_REQUIRE(logits && target_nchw && pos_weight && grad && N > 0 && C > 0 && CP >= C && H > 0 && W > 0 && W % 32 == 0,
+              "bce_mse_cl_backward: bad arguments");
+  if ((size_t)C * 33 * sizeof(float) > 48 * 1024) return fail(MAS_ERR_UNSUPPORTED, "bce_mse_cl_backward: C=%d too large", C);
+  return bce_cl_backward<true>(logits, DenseTarget{target_nchw}, pos_weight, g, N, C, CP, H, W, grad, stream);
+}
+int mas_bce_mse_scene_forward(const float* logits, const uint8_t* labels, const float* pos_weight, int N, int CP, int H, int W,
+                              float* loss_out, void* ws, size_t ws_bytes, void* stream) {
+  MAS_REQUIRE(logits && labels && pos_weight && loss_out && N > 0 && H > 0 && CP >= SCENE_C && W > 0 && W % 32 == 0,
+              "bce_mse_scene_forward: bad arguments");
+  return bce_cl_forward<true>(logits, SceneTarget{labels}, pos_weight, N, SCENE_C, CP, H, W, loss_out, ws, ws_bytes, stream);
+}
+int mas_bce_mse_scene_backward(const float* logits, const uint8_t* labels, const float* pos_weight, const float* g, int N, int CP,
+                               int H, int W, float* grad, void* stream) {
+  MAS_REQUIRE(logits && labels && pos_weight && grad && N > 0 && H > 0 && CP >= SCENE_C && W > 0 && W % 32 == 0,
+              "bce_mse_scene_backward: bad arguments");
+  return bce_cl_backward<true>(logits, SceneTarget{labels}, pos_weight, g, N, SCENE_C, CP, H, W, grad, stream);
+}
+int mas_bce_mse_logits(const float* logits, mas_tensor4 ls, const float* target, mas_tensor4 ts, const float* pos_weight,
+                       float* loss_out, float* grad, mas_tensor4 gs, float grad_scale, void* ws, size_t ws_bytes, void* stream) {
+  MAS_REQUIRE(logits && target && pos_weight && loss_out && ls.n > 0 && ls.c > 0 && ls.h > 0 && ls.w > 0 && ts.n == ls.n &&
+              ts.c == ls.c && ts.h == ls.h && ts.w == ls.w && (!grad || (gs.n == ls.n && gs.c == ls.c && gs.h == ls.h && gs.w == ls.w)),
+              "bce_mse_logits: bad arguments");
+  return bce_logits<true>(logits, ls, target, ts, pos_weight, loss_out, grad, gs, grad_scale, ws, ws_bytes, stream);
 }
 
 }  // extern "C"

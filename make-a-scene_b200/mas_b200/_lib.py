@@ -171,6 +171,11 @@ _SPEC = {
     "mas_scene_expand": (_I, [_P, _I, _I, _I, _P, _T, _P]),
     "mas_bce_scene_forward": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P]),
     "mas_bce_scene_backward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
+    "mas_bce_mse_cl_forward": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _Z, _P]),
+    "mas_bce_mse_cl_backward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
+    "mas_bce_mse_scene_forward": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P]),
+    "mas_bce_mse_scene_backward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
+    "mas_bce_mse_logits": (_I, [_P, _T, _P, _T, _P, _P, _P, _T, _F, _P, _Z, _P]),
     "mas_lpips_prep": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _P]),
     "mas_lpips_relu": (_I, [_P, _L, _P, _P]),
     "mas_lpips_maxpool": (_I, [_P, _P, _I, _I, _I, _I, _P, _P]),

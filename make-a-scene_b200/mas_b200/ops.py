@@ -1311,6 +1311,61 @@ def _cl_pitch(t):
     return pitch
 
 
+def _bce_forward(ctx, entry, logits, target, pos_weight):
+    """Forward of BCELogitsFn (entry "mas_bce") and BCEMSELogitsFn ("mas_bce_mse"): the tiled <entry>_cl_* / <entry>_scene_*
+    kernels for padded channels-last logits, else <entry>_logits, which also writes the unit-seed gradient."""
+    _need_cuda(logits)
+    n, c, h, w = logits.shape
+    loss = torch.empty((), dtype=torch.float32, device=logits.device)
+    cp = _cl_pitch(logits)
+    ctx.entry = entry
+    ctx.scene = target.dtype == torch.uint8
+    if ctx.scene:
+        if c != scene.CHANNELS:
+            raise RuntimeError("a compact scene map is the target of %d-channel logits, got %d" % (scene.CHANNELS, c))
+        target = scene_labels(target, n, h, w)
+    if cp is not None and w % 32 == 0 and (ctx.scene or (target.is_contiguous() and c * 33 * 4 <= 48 * 1024)):
+        ws = L.workspace(L.query("mas_bce_cl_ws_bytes", n, h, w), logits.device)
+        if ctx.scene:
+            L.call(entry + "_scene_forward", logits, target, pos_weight, n, cp, h, w, loss, ws, ws.numel())
+        else:
+            L.call(entry + "_cl_forward", logits, target, pos_weight, n, c, cp, h, w, loss, ws, ws.numel())
+        ctx.save_for_backward(logits, target, pos_weight)
+        ctx.cp = cp
+        return loss
+    if ctx.scene:
+        target = scene_expand(target)
+    grad = torch.empty_like(logits)
+    nb = L.query("mas_bce_ws_bytes", L.t4(logits))
+    ws = L.workspace(nb, logits.device)
+    L.call(entry + "_logits", logits, L.t4(logits), target, L.t4(target), pos_weight, loss, grad, L.t4(grad),
+           1.0 / logits.numel(), ws, ws.numel())
+    ctx.save_for_backward(grad)
+    ctx.cp = None
+    return loss
+
+
+def _bce_backward(ctx, g):
+    g = g.contiguous()
+    if ctx.cp is None:
+        (grad,) = ctx.saved_tensors
+        src = grad if grad.is_contiguous() or grad.is_contiguous(memory_format=torch.channels_last) else grad.contiguous()
+        out = torch.empty_like(src)
+        L.call("mas_scale_by", src, g, out, src.numel())
+        return out, None, None
+    logits, target, pw = ctx.saved_tensors
+    n, c, h, w = logits.shape
+    base = torch.empty((n, h, w, ctx.cp), dtype=torch.float32, device=logits.device)
+    if ctx.scene:
+        L.call(ctx.entry + "_scene_backward", logits, target, pw, g, n, ctx.cp, h, w, base)
+    else:
+        L.call(ctx.entry + "_cl_backward", logits, target, pw, g, n, c, ctx.cp, h, w, base)
+    full = base.permute(0, 3, 1, 2)
+    grad = full[:, :c]
+    grad._mas_pad_base = full          # the padded tensor this view lives in (picked up by the convolution's backward)
+    return grad, None, None
+
+
 class BCELogitsFn(torch.autograd.Function):
     """binary_cross_entropy_with_logits(pos_weight) mean (losses/loss_seg.py:15-19). With the VQ-SEG step's own layouts
     (channels-last logits - the padded view the decoder's last convolution returns - and an NCHW target) loss and
@@ -1321,56 +1376,25 @@ class BCELogitsFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, logits, target, pos_weight):
-        _need_cuda(logits)
-        n, c, h, w = logits.shape
-        loss = torch.empty((), dtype=torch.float32, device=logits.device)
-        cp = _cl_pitch(logits)
-        ctx.scene = target.dtype == torch.uint8
-        if ctx.scene:
-            if c != scene.CHANNELS:
-                raise RuntimeError("a compact scene map is the target of %d-channel logits, got %d" % (scene.CHANNELS, c))
-            target = scene_labels(target, n, h, w)
-        if cp is not None and w % 32 == 0 and (ctx.scene or (target.is_contiguous() and c * 33 * 4 <= 48 * 1024)):
-            ws = L.workspace(L.query("mas_bce_cl_ws_bytes", n, h, w), logits.device)
-            if ctx.scene:
-                L.call("mas_bce_scene_forward", logits, target, pos_weight, n, cp, h, w, loss, ws, ws.numel())
-            else:
-                L.call("mas_bce_cl_forward", logits, target, pos_weight, n, c, cp, h, w, loss, ws, ws.numel())
-            ctx.save_for_backward(logits, target, pos_weight)
-            ctx.cp = cp
-            return loss
-        if ctx.scene:
-            target = scene_expand(target)
-        grad = torch.empty_like(logits)
-        nb = L.query("mas_bce_ws_bytes", L.t4(logits))
-        ws = L.workspace(nb, logits.device)
-        L.call("mas_bce_logits", logits, L.t4(logits), target, L.t4(target), pos_weight, loss, grad, L.t4(grad),
-               1.0 / logits.numel(), ws, ws.numel())
-        ctx.save_for_backward(grad)
-        ctx.cp = None
-        return loss
+        return _bce_forward(ctx, "mas_bce", logits, target, pos_weight)
 
     @staticmethod
     def backward(ctx, g):
-        g = g.contiguous()
-        if ctx.cp is None:
-            (grad,) = ctx.saved_tensors
-            out = torch.empty_like(grad)
-            src = grad if grad.is_contiguous() or grad.is_contiguous(memory_format=torch.channels_last) else grad.contiguous()
-            out = torch.empty_like(src)
-            L.call("mas_scale_by", src, g, out, src.numel())
-            return out, None, None
-        logits, target, pw = ctx.saved_tensors
-        n, c, h, w = logits.shape
-        base = torch.empty((n, h, w, ctx.cp), dtype=torch.float32, device=logits.device)
-        if ctx.scene:
-            L.call("mas_bce_scene_backward", logits, target, pw, g, n, ctx.cp, h, w, base)
-        else:
-            L.call("mas_bce_cl_backward", logits, target, pw, g, n, c, ctx.cp, h, w, base)
-        full = base.permute(0, 3, 1, 2)
-        grad = full[:, :c]
-        grad._mas_pad_base = full          # the padded tensor this view lives in (picked up by the convolution's backward)
-        return grad, None, None
+        return _bce_backward(ctx, g)
+
+
+class BCEMSELogitsFn(torch.autograd.Function):
+    """mse_loss(logits.sigmoid(), target) + binary_cross_entropy_with_logits(pos_weight) mean, the VQ-SEG objective of
+    VQVAEWithBCELoss (losses/loss_seg.py:34-41), as one mean over N*C*H*W computed by one kernel per direction. Layouts,
+    routing, compact targets and the padded gradient are those of BCELogitsFn, on the mas_bce_mse_* entries."""
+
+    @staticmethod
+    def forward(ctx, logits, target, pos_weight):
+        return _bce_forward(ctx, "mas_bce_mse", logits, target, pos_weight)
+
+    @staticmethod
+    def backward(ctx, g):
+        return _bce_backward(ctx, g)
 
 
 # ------------------------------------------------------------------------------------------------ tier 2: token transformer
