@@ -91,6 +91,26 @@ int mas_scale_by(const float* x, const float* g, float* y, int64_t n, void* stre
  * channels-last operand mas_nchw_to_nhwc_pad builds from the dense map - the same values bit for bit. */
 int mas_scene_expand(const uint8_t* labels, int N, int H, int W, float* y, mas_tensor4 ys, void* stream);
 
+/* The inverse direction (csrc/scene.cu).  mas_scene_decode: VQ-SEG logits x [B, 159, H, W] fp32 (any strides; the fast case
+ * is the decoder's padded channels-last view, xs.sc == 1, whose pad channels are never read) -> planes [B, 4, H, W] uint8,
+ * contiguous, by the rule of the BCE decision boundary (a channel is on when its logit is > 0):
+ *   plane 0  1 + argmax(x[0:133])   if that maximum is > 0, else 0
+ *   plane 1  1 + argmax(x[133:153]) if > 0, else 0
+ *   plane 2  1 + argmax(x[153:158]) if > 0, else 0
+ *   plane 3  1 if x[158] > 0, else 0
+ * Ties go to the lowest channel; -0 ties with +0; a NaN never wins an argmax and is never > 0 (an all-NaN group decodes to 0).
+ * Every logit is read once, no atomics: the output is the same bytes on every call.  B, H <= 65535.  On a dense map
+ * mas_scene_expand wrote it returns the labels, with an edge count of 2 as 1.
+ * mas_scene_confusion: pred and target [B, 4, pixels_per_image] uint8 (contiguous compact maps) -> conf, OVERWRITTEN with
+ * 18438 int64 counts, target row x prediction column, in this order: panoptic 134 x 134, human 21 x 21, face 6 x 6, edges 2 x 2
+ * (an edge count of 1 or 2 is an edge), then the number of pixels with a plane counted in no cell because its target or
+ * prediction byte lies outside the plane's range (codes above 133 / 20 / 5 / 2; a pixel counts once however many of its
+ * planes are out of range; the other planes of that pixel are counted).  Integer atomics: the same counts on every call.  No workspace is needed at present (the size query returns 0 and ws may be NULL). */
+int mas_scene_decode(const float* x, mas_tensor4 xs, uint8_t* planes, void* stream);
+size_t mas_scene_confusion_ws_bytes(int64_t pixels_per_image, int B);
+int mas_scene_confusion(const uint8_t* pred, const uint8_t* target, int64_t pixels_per_image, int B, int64_t* conf, void* ws,
+                        size_t ws_bytes, void* stream);
+
 /* ---- GroupNorm(32, C, eps=1e-6) + optional SiLU — Normalize / nonlinearity, modules.py:35-41 ------
  * x, y: [N, HW, C] NHWC.  mean/rstd: [N*G].  silu=1 fuses x*sigmoid(x) (modules.py:122,126,194-196).
  * round_tf32=1 rounds y to TF32 (round-to-nearest) so that a following tensor-core contraction sees

@@ -169,6 +169,9 @@ _SPEC = {
     "mas_bce_cl_backward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P]),
     "mas_bce_logits": (_I, [_P, _T, _P, _T, _P, _P, _P, _T, _F, _P, _Z, _P]),
     "mas_scene_expand": (_I, [_P, _I, _I, _I, _P, _T, _P]),
+    "mas_scene_decode": (_I, [_P, _T, _P, _P]),
+    "mas_scene_confusion_ws_bytes": (_Z, [_L, _I]),
+    "mas_scene_confusion": (_I, [_P, _P, _L, _I, _P, _P, _Z, _P]),
     "mas_bce_scene_forward": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P]),
     "mas_bce_scene_backward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
     "mas_bce_mse_cl_forward": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _Z, _P]),

@@ -100,6 +100,33 @@ class VQBASE(nn.Module):
             _, _, idx = ops.VQFn.apply(z, self.quantize.embedding.weight, self.quantize.beta)
         return idx.view(b, h // f, w // f)
 
+    def decode_scene(self, code_b):
+        """Seg tokens -> the compact scene map they stand for: scene.decode(decode_code(code_b)), uint8 [B, 4, H, W] on the
+        model's device (mas_b200.scene: 1 + the argmax of each one-hot group where its maximum logit is > 0, else 0; edges 0 / 1).
+        The counterpart of encode_code for a VQ-SEG model: decode_scene(encode_code(labels)) is its round trip, and
+        scene.iou(scene.confusion(decode_scene(encode_code(labels)), labels)) its quality.
+
+        code_b: int64 [B, h, w] codebook indices on the model's device.  Only for a model whose decoder's last convolution has
+        159 outputs.  The decoder has no mode-dependent layer, so this is the eval-mode decoding in either mode; nothing of the
+        module changes and no autograd graph is recorded.  Raises ValueError on another model, a tensor off the model's
+        device or not [B, h, w] int64."""
+        conv_out = self.decoder.model[-1]
+        dev = conv_out.weight.device
+        if conv_out.out_channels != scene.CHANNELS:
+            raise ValueError("decode_scene needs a VQ-SEG model (decoder output %d channels), this one has %d"
+                             % (scene.CHANNELS, conv_out.out_channels))
+        if not isinstance(code_b, torch.Tensor) or code_b.dim() != 3 or code_b.dtype != torch.int64 or 0 in code_b.shape:
+            raise ValueError("decode_scene expects int64 tokens [B, h, w], got %s" % (
+                "%s %s" % (tuple(code_b.shape), code_b.dtype) if isinstance(code_b, torch.Tensor) else type(code_b).__name__))
+        if not _kernel_device(code_b) or code_b.device != dev:
+            raise ValueError("decode_scene needs a CUDA tensor on the model's device (%s), got one on %s" % (dev, code_b.device))
+        f = 2 ** sum(isinstance(m, Downsample) for m in self.encoder.model)
+        b, h, w = code_b.shape
+        if b > 65535 or h * f > 65535:
+            raise ValueError("decode_scene needs B and H * %d at most 65535, got tokens of shape %s" % (f, tuple(code_b.shape)))
+        with torch.no_grad():
+            return scene.decode(self.decode_code(code_b))
+
     def forward(self, input):
         """-> (dec, diff) exactly like vqvae.py:36-39 (train.py:84 unpacks this pair)."""
         z_q, diff = self.encode(input)
