@@ -111,6 +111,29 @@ size_t mas_scene_confusion_ws_bytes(int64_t pixels_per_image, int B);
 int mas_scene_confusion(const uint8_t* pred, const uint8_t* target, int64_t pixels_per_image, int B, int64_t* conf, void* ws,
                         size_t ws_bytes, void* stream);
 
+/* Reconstruction quality of images (csrc/image_quality.cu): psnr[b] and ssim[b] (fp32, B each) of rec against ref.
+ *   Inputs:  rec and ref are logical [B, C, H, W] fp32 tensors read through their mas_tensor4 strides (rs.n = B, rs.c = C).
+ *   Mapping: every value is clamped to [-1, 1] and mapped to [0, 1] by v -> (v + 1) / 2.
+ *   NaN:     a NaN anywhere in an image makes that image's PSNR and SSIM NaN.
+ *   PSNR:    psnr[b] = 10 log10(1 / MSE_b), MSE_b over all C*H*W mapped elements; +inf when MSE_b = 0.
+ *   SSIM (Wang et al. 2004), for each channel separately:
+ *     window     a Gaussian, sigma = 1.5, 11 taps, w_k ~ exp(-k^2 / (2 sigma^2)) for k = -5..5, normalised to sum 1 in fp64
+ *                and then rounded once to fp32;
+ *     constants  C1 = (0.01)^2, C2 = (0.03)^2;
+ *     moments    mu_x = G*x; population moments sigma_x^2 = G*x^2 - mu_x^2, sigma_xy = G*(xy) - mu_x mu_y;
+ *     map        ((2 mu_x mu_y + C1)(2 sigma_xy + C2)) / ((mu_x^2 + mu_y^2 + C1)(sigma_x^2 + sigma_y^2 + C2)), taken at every
+ *                pixel whose 11 x 11 window lies inside the image: (H - 10)(W - 10) pixels per channel;
+ *     result     ssim[b] is the mean over channels of each channel's mean over those pixels.
+ *   This equals scikit-image's structural_similarity(gaussian_weights=True, sigma=1.5, use_sample_covariance=False,
+ *   data_range=1, channel_axis=0).
+ *   Determinism: no floating-point atomics; partial sums are fp64 and added in an order that depends only on logical indices,
+ *   so every call returns the same bits, whatever the strides of the inputs.
+ * Needs B, C >= 1, H, W >= 11, B, C <= 65535 and a workspace of mas_image_quality_ws_bytes(B, C, H, W) bytes (0 for extents
+ * it refuses). */
+size_t mas_image_quality_ws_bytes(int B, int C, int64_t H, int64_t W);
+int mas_image_quality(const float* rec, mas_tensor4 rs, const float* ref, mas_tensor4 fs, float* psnr, float* ssim, void* ws,
+                      size_t ws_bytes, void* stream);
+
 /* ---- GroupNorm(32, C, eps=1e-6) + optional SiLU — Normalize / nonlinearity, modules.py:35-41 ------
  * x, y: [N, HW, C] NHWC.  mean/rstd: [N*G].  silu=1 fuses x*sigmoid(x) (modules.py:122,126,194-196).
  * round_tf32=1 rounds y to TF32 (round-to-nearest) so that a following tensor-core contraction sees

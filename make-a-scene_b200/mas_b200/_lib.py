@@ -172,6 +172,8 @@ _SPEC = {
     "mas_scene_decode": (_I, [_P, _T, _P, _P]),
     "mas_scene_confusion_ws_bytes": (_Z, [_L, _I]),
     "mas_scene_confusion": (_I, [_P, _P, _L, _I, _P, _P, _Z, _P]),
+    "mas_image_quality_ws_bytes": (_Z, [_I, _I, _L, _L]),
+    "mas_image_quality": (_I, [_P, _T, _P, _T, _P, _P, _P, _Z, _P]),
     "mas_bce_scene_forward": (_I, [_P, _P, _P, _I, _I, _I, _I, _P, _P, _Z, _P]),
     "mas_bce_scene_backward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _P]),
     "mas_bce_mse_cl_forward": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _Z, _P]),

@@ -43,6 +43,21 @@ def load_planes(name, size):
     return lab[:, top:top + size, left:left + size].contiguous()
 
 
+def load_model(config, checkpoint, dev):
+    """The VQBASE of a yaml config's model block with a checkpoint's weights, in eval mode on dev.  The checkpoint is a
+    state_dict (train.py's checkpoint.pt / final.pt) or a resumable checkpoint with a "model" entry."""
+    import yaml
+    from mas_b200 import scene
+    from models import VQBASE
+    cfg = yaml.safe_load(open(config))["model"]
+    cfg.pop("_target_", None)
+    cfg["ddconfig"].setdefault("out_channels", cfg["ddconfig"].get("out_ch", scene.CHANNELS))   # seg_config omits it
+    m = VQBASE(**cfg)
+    sd = torch.load(checkpoint, map_location="cpu", weights_only=False)
+    m.load_state_dict(sd["model"] if "model" in sd else sd)
+    return m.to(dev).eval()
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--checkpoint", required=True)
@@ -52,17 +67,9 @@ def main():
     ap.add_argument("--size", type=int, default=256)
     ap.add_argument("--limit", type=int, default=0)
     a = ap.parse_args()
-    import yaml
     from mas_b200 import scene
-    from models import VQBASE
     dev = torch.device("cuda:0")
-    cfg = yaml.safe_load(open(a.config))["model"]
-    cfg.pop("_target_", None)
-    cfg["ddconfig"].setdefault("out_channels", cfg["ddconfig"].get("out_ch", scene.CHANNELS))
-    m = VQBASE(**cfg)
-    sd = torch.load(a.checkpoint, map_location="cpu", weights_only=False)
-    m.load_state_dict(sd["model"] if "model" in sd else sd)
-    m = m.to(dev).eval()
+    m = load_model(a.config, a.checkpoint, dev)
     names = find_maps(a.data)
     if a.limit:
         names = names[:a.limit]
