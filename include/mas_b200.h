@@ -259,6 +259,33 @@ int mas_gemm_rows_f16(const void* x_f16, int64_t M, int K, const void* w_tc16, f
 size_t mas_wgrad_rows_f16_ws_bytes(int64_t M, int N, int K);
 int mas_wgrad_rows_f16(const void* x_f16, const void* dy_f16, int64_t M, int N, int K, float* dw, float* dbias,
                        const float* x_amax, const float* dy_amax, void* ws, size_t ws_bytes, void* stream);
+/* FP8 Linear layers (csrc/gemm_f8.cu; opt-in training route of the token transformer, MakeAScene(fp8_linear=True)).
+ * Formats: activations and weights e4m3 (MAS_FP8_E4M3, max 448), output gradients e5m2 (MAS_FP8_E5M2, max 57344).  Scale:
+ * one power of two per tensor, derived on the device from the exact max|.| (*amax, from mas_amax), that puts max|.| in the top
+ * full binade below the format's maximum: [2^7, 2^8) for e4m3, [2^14, 2^15) for e5m2, so nothing saturates.  Zero or
+ * non-finite amax -> scale 1.  Conversion rounds to nearest even (cvt.rn.satfinite); NaN stays NaN.  fp32 accumulation:
+ * the sum of every 128 K elements (four k32 MMAs) is promoted into fp32 registers.  Every call gives the same bits.
+ * mas_to_fp8: x fp32 [M,K] (K % 16 == 0) -> y_rows [M,K] (row-major, or NULL) and / or y_cols [K,M'] (transposed, M' = M rounded
+ *   up to 16, columns M .. M'-1 zero; or NULL) in format fmt; colsum [K] (or NULL) = fp32 column sums of the unscaled x, added in a
+ *   fixed order, which needs ws of mas_to_fp8_ws_bytes(M, K) bytes.
+ * mas_pack_gemm_f8: the weight image of W [N,K] (N, K % 16 == 0) in both orientations under the weight's own scale: *amax =
+ *   max|W|, w_f8 [N,K] = e4m3(W s) for the forward, wt_f8 [K,N] = its transpose for the data gradient.
+ * mas_gemm_rows_f8: y[M,N] = x . W^T (+bias), x_f8 [M,K] in x_fmt scaled from *x_amax, w_f8 [N,K] e4m3 scaled from *w_amax (the
+ *   forward: x e4m3, w_f8 from mas_pack_gemm_f8; the data gradient dx = dy . W: x = dy e5m2 [M,N], w_f8 = wt_f8, N <-> K).
+ *   Needs K % 16 == 0.
+ * mas_wgrad_rows_f8: dw[N,K] = dy^T . x from the transposed copies xt_f8 [K,M'] (e4m3, *x_amax) and dyt_f8 [N,M'] (e5m2,
+ *   *dy_amax) of mas_to_fp8; split-K partials in ws, added in a fixed order.  The bias gradient is mas_to_fp8's colsum of dy. */
+#define MAS_FP8_E4M3 0
+#define MAS_FP8_E5M2 1
+size_t mas_to_fp8_ws_bytes(int64_t M, int K);
+int mas_to_fp8(const float* x, int64_t M, int K, int fmt, const float* amax, void* y_rows, void* y_cols, float* colsum, void* ws,
+               size_t ws_bytes, void* stream);
+int mas_pack_gemm_f8(const float* w_nk, int N, int K, void* w_f8, void* wt_f8, float* amax, void* stream);
+int mas_gemm_rows_f8(const void* x_f8, int64_t M, int K, int x_fmt, const float* x_amax, const void* w_f8, int N, const float* w_amax,
+                     const float* bias, float* y, int64_t ldy, void* stream);
+size_t mas_wgrad_rows_f8_ws_bytes(int64_t M, int N, int K);
+int mas_wgrad_rows_f8(const void* xt_f8, const void* dyt_f8, int64_t M, int N, int K, const float* x_amax, const float* dy_amax,
+                      float* dw, void* ws, size_t ws_bytes, void* stream);
 /* The Linear layers of a decode step at more than 8 rows (cond + uncond streams): y[R,N] = act(x[R,K] . W^T + bias) from the
  * same operands as mas_gemm_rows_f16 (x_f16 a dense [R,K] copy scaled by the operand scale of *x_amax, w_tc16 from
  * mas_pack_gemm_tc16, padded to 128 output features; only N columns are stored).  The rows sit on a narrow MMA side (16 .. 256)

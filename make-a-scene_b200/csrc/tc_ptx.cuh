@@ -78,13 +78,15 @@ __device__ __forceinline__ uint32_t pack_h2(float a, float b) {
 // power-of-two operand scale for an fp16 operand tensor from its largest magnitude (device scalar; null = 1):
 // amax * s lands in [2^14, 2^15), so the whole fp16 normal range (30 binades) sits below the largest element and
 // nothing overflows. *inv receives 1/s (exact). Zero / non-finite amax -> s = 1.
+// TOP: the binade [2^TOP, 2^(TOP+1)) amax * s lands in: 14 for fp16 and FP8 e5m2 (max 57344), 7 for FP8 e4m3 (max 448).
+template <int TOP = 14>
 __device__ __forceinline__ float operand_scale(const float* amax, float* inv) {
   float s = 1.f, i = 1.f;
   if (amax) {
     const uint32_t b = __float_as_uint(*amax);
     const int e = (int)((b >> 23) & 0xff);            // biased exponent of amax (0 = zero/denormal, 255 = inf/nan)
     if (e > 0 && e < 255) {
-      int se = 127 + 14 - (e - 127);                  // biased exponent of s = 2^(14 - floor(log2 amax))
+      int se = 127 + TOP - (e - 127);                 // biased exponent of s = 2^(TOP - floor(log2 amax))
       se = se < 1 ? 1 : (se > 254 ? 254 : se);
       s = __uint_as_float((uint32_t)se << 23);
       i = __uint_as_float((uint32_t)(254 - se) << 23);

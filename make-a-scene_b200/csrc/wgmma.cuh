@@ -120,6 +120,16 @@ __device__ __forceinline__ void wgmma_tf32_rs_n128(float* d, const uint32_t* a, 
   asm volatile(WG_PRED(69) "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 " WG_V64 ", {%64,%65,%66,%67}, %68, p, 1, 1;\n\t}"
                : WG_D64 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(acc));
 }
+// FP8 (K = 32 per MMA): A is e4m3, B is e4m3 or (B_E5M2) e5m2.  8-bit operands have no transpose bit: both are K-major.
+template <bool B_E5M2>
+__device__ __forceinline__ void wgmma_f8_ss_n128(float* d, uint64_t adesc, uint64_t bdesc, uint32_t acc) {
+  if constexpr (B_E5M2)
+    asm volatile(WG_PRED(66) "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e5m2 " WG_V64 ", %64, %65, p, 1, 1;\n\t}"
+                 : WG_D64 : "l"(adesc), "l"(bdesc), "r"(acc));
+  else
+    asm volatile(WG_PRED(66) "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 " WG_V64 ", %64, %65, p, 1, 1;\n\t}"
+                 : WG_D64 : "l"(adesc), "l"(bdesc), "r"(acc));
+}
 
 }  // namespace wg
 }  // namespace mas

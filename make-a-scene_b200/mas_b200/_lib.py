@@ -150,6 +150,12 @@ _SPEC = {
     "mas_linear_rows_f16": (_I, [_P, _L, _I, _P, _P, _L, _I, _P, _P, _I, _P, _Z, _P]),
     "mas_wgrad_rows_f16_ws_bytes": (_Z, [_L, _I, _I]),
     "mas_wgrad_rows_f16": (_I, [_P, _P, _L, _I, _I, _P, _P, _P, _P, _P, _Z, _P]),
+    "mas_to_fp8_ws_bytes": (_Z, [_L, _I]),
+    "mas_to_fp8": (_I, [_P, _L, _I, _I, _P, _P, _P, _P, _P, _Z, _P]),
+    "mas_pack_gemm_f8": (_I, [_P, _I, _I, _P, _P, _P, _P]),
+    "mas_gemm_rows_f8": (_I, [_P, _L, _I, _I, _P, _P, _I, _P, _P, _P, _L, _P]),
+    "mas_wgrad_rows_f8_ws_bytes": (_Z, [_L, _I, _I]),
+    "mas_wgrad_rows_f8": (_I, [_P, _P, _L, _I, _I, _P, _P, _P, _P, _Z, _P]),
     "mas_attn_causal_forward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _P]),
     "mas_attn_causal_forward_stats": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _F, _D, _P, _P]),
     "mas_attn_causal_backward": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _F, _D, _P, _P]),

@@ -1567,20 +1567,100 @@ def wgrad_rows_f16(x16, am_x, dy16, am_dy, want_bias=True):
     return dw, db
 
 
+FP8_E4M3, FP8_E5M2 = 0, 1   # MAS_FP8_E4M3 / MAS_FP8_E5M2
+
+
+def linear_fp8_on(nout, kin):
+    """The FP8 Linear kernels (csrc/gemm_f8.cu) serve an [nout, kin] weight exactly where the fp16 route does (linear_f16_on):
+    both widths multiples of 128, fp16 operand format, MAS_LINEAR_F16 not 0. With the TF32 operand format or MAS_LINEAR_F16=0
+    a layer's fp8 flag has no effect."""
+    return linear_f16_on(nout, kin)
+
+
+def linear(x, weight, bias, fp8=False):
+    """nn.Linear on the last dim through LinearFn. fp8=True takes the FP8 route (e4m3 activations and weights, e5m2 output
+    gradients, per-tensor power-of-two scales from the device-side max|.|) only when the call records an autograd graph
+    (grad mode on and x or the weight requiring a gradient) and linear_fp8_on holds; every other call - generate, score, any
+    no-grad forward - runs exactly as with fp8=False."""
+    N, K = weight.shape
+    fp8 = bool(fp8) and torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad) and linear_fp8_on(N, K)
+    return LinearFn.apply(x, weight, bias, fp8)
+
+
+def to_fp8(x2d, fmt, rows=True, cols=False, colsum=False, am=None):
+    """(row-major fp8 [M,K] or None, transposed fp8 [K, M rounded up to 16] zero-padded or None, fp32 column sums [K] of x2d or
+    None, max|x2d| device scalar) from one mas_to_fp8 pass over the dense fp32 [M,K] x2d. fmt: FP8_E4M3 / FP8_E5M2; the bytes
+    (uint8 tensors) are x2d times the format's power-of-two scale of the maximum."""
+    M, K = x2d.shape
+    if am is None:
+        am = amax(x2d)
+    dev = x2d.device
+    r = torch.empty((M, K), dtype=torch.uint8, device=dev) if rows else None
+    c = torch.empty((K, _round_up(M, 16)), dtype=torch.uint8, device=dev) if cols else None
+    s = torch.empty(K, dtype=torch.float32, device=dev) if colsum else None
+    ws = L.workspace(L.query("mas_to_fp8_ws_bytes", M, K), dev) if colsum else None
+    L.call("mas_to_fp8", x2d, M, K, fmt, am, r, c, s, ws, 0 if ws is None else ws.numel())
+    return r, c, s, am
+
+
+def fp8_weight(weight):
+    """(e4m3 [N,K] for the forward, e4m3 [K,N] for the data gradient, max|W| as a device scalar): the FP8 image of an nn.Linear
+    weight under its own scale (mas_pack_gemm_f8), cached per parameter version like the fp16 images."""
+    ent = _pack_entry(weight)
+    hit = ent.get("lin8")
+    if hit is None or hit[0].device != weight.device:
+        N, K = weight.shape
+        buf = torch.empty(2 * N * K + 16, dtype=torch.uint8, device=weight.device)
+        hit = ent["lin8"] = (buf[:N * K].view(N, K), buf[N * K:2 * N * K].view(K, N), buf[2 * N * K:2 * N * K + 4].view(torch.float32))
+        L.call("mas_pack_gemm_f8", weight.detach().contiguous(), N, K, hit[0], hit[1], hit[2])
+    return hit
+
+
+def gemm_rows_f8(x8, am, fmt, w8, am_w, bias=None):
+    """y[M,N] = x[M,K] . W^T (+bias) on mas_gemm_rows_f8 from the fp8 copy x8 (format fmt, scaled from am) and an e4m3 [N,K]
+    image w8 (scaled from am_w)."""
+    M, K = x8.shape
+    N = w8.shape[0]
+    y = torch.empty((M, N), dtype=torch.float32, device=x8.device)
+    L.call("mas_gemm_rows_f8", x8, M, K, fmt, am, w8, N, am_w, bias, y, N)
+    return y
+
+
+def wgrad_rows_f8(x8t, am_x, dy8t, am_dy, M):
+    """dW [N,K] = dy^T . x from the transposed fp8 copies x8t [K,M'] (e4m3) and dy8t [N,M'] (e5m2) (mas_wgrad_rows_f8)."""
+    K, N = x8t.shape[0], dy8t.shape[0]
+    dw = torch.empty((N, K), dtype=torch.float32, device=x8t.device)
+    ws = L.workspace(L.query("mas_wgrad_rows_f8_ws_bytes", M, N, K), x8t.device)
+    L.call("mas_wgrad_rows_f8", x8t, dy8t, M, N, K, am_x, am_dy, dw, ws, ws.numel())
+    return dw
+
+
 class LinearFn(torch.autograd.Function):
     """nn.Linear on the last dim. Both widths % 128 == 0: the TMA-fed fp16 kernels - the input is converted ONCE to fp16 (kept
     for the weight gradient instead of the fp32 tensor), the output gradient once for both the data and the weight gradient.
-    Else the register-staged TF32 row GEMM (out % 128 == 0, in % 32 == 0), else fp32 SIMT."""
+    Else the register-staged TF32 row GEMM (out % 128 == 0, in % 32 == 0), else fp32 SIMT.
+    fp8=True (decided by ops.linear): the FP8 kernels of csrc/gemm_f8.cu. The input is cast once to e4m3 in both layouts: the
+    row-major copy feeds the forward, the transposed one (1 byte per element) is all that is kept for the weight gradient. The
+    output gradient is cast once to e5m2 in both layouts, with the bias gradient (fp32 column sums) from the same pass."""
 
     @staticmethod
-    def forward(ctx, x, weight, bias):
+    def forward(ctx, x, weight, bias, fp8=False):
         _need_cuda(x)
         x = x.contiguous()
         K, N = x.shape[-1], weight.shape[0]
         R = x.numel() // K
-        ctx.f16 = linear_f16_on(N, K)
+        ctx.fp8 = bool(fp8)
+        ctx.f16 = linear_f16_on(N, K) and not ctx.fp8
         ctx.has_bias = bias is not None
         ctx.xshape = x.shape
+        if ctx.fp8:
+            if not linear_fp8_on(N, K):
+                raise RuntimeError("LinearFn: the FP8 route is off for [%d, %d] (linear_fp8_on)" % (N, K))
+            w8, _, am_w = fp8_weight(weight)
+            x8, x8t, _, am_x = to_fp8(x.view(R, K), FP8_E4M3, rows=True, cols=True)
+            y = gemm_rows_f8(x8, am_x, FP8_E4M3, w8, am_w, bias).view(x.shape[:-1] + (N,))
+            ctx.save_for_backward(x8t, am_x, weight)
+            return y
         if ctx.f16:
             x16, am = rows_to_half(x.view(R, K))
             y = gemm_rows_f16(x16, am, weight, False, bias).view(x.shape[:-1] + (N,))
@@ -1594,6 +1674,17 @@ class LinearFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         dy = dy.contiguous()
+        if ctx.fp8:
+            x8t, am_x, weight = ctx.saved_tensors
+            N, K = weight.shape
+            R = dy.numel() // N
+            want_dx = ctx.needs_input_grad[0]
+            dy8, dy8t, db, am_dy = to_fp8(dy.view(R, N), FP8_E5M2, rows=want_dx, cols=True, colsum=ctx.has_bias)
+            dx = None
+            if want_dx:
+                _, w8t, am_w = fp8_weight(weight)
+                dx = gemm_rows_f8(dy8, am_dy, FP8_E5M2, w8t, am_w).view(ctx.xshape)
+            return dx, wgrad_rows_f8(x8t, am_x, dy8t, am_dy, R), db, None
         if ctx.f16:
             x16, am_x, weight = ctx.saved_tensors
             N, K = weight.shape
@@ -1601,7 +1692,7 @@ class LinearFn(torch.autograd.Function):
             dy16, am_dy = rows_to_half(dy.view(R, N))
             dx = gemm_rows_f16(dy16, am_dy, weight, True).view(ctx.xshape) if ctx.needs_input_grad[0] else None
             dw, db = wgrad_rows_f16(x16, am_x, dy16, am_dy, ctx.has_bias)
-            return dx, dw, db
+            return dx, dw, db, None
         x, weight = ctx.saved_tensors
         K, N = x.shape[-1], weight.shape[0]
         R = x.numel() // K
@@ -1610,7 +1701,7 @@ class LinearFn(torch.autograd.Function):
             dx = torch.empty_like(x)
             gemm_w(dy, N, weight, dx, K, R, transpose=True)
         dw, db = conv1x1_wgrad_raw(x, dy, R, K, N, ctx.has_bias)
-        return dx, dw.view(N, K), db
+        return dx, dw.view(N, K), db, None
 
 
 def _attn_impl(S_, hd):

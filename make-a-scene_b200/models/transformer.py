@@ -28,8 +28,13 @@ class LayerNorm(nn.LayerNorm):
 
 
 class Linear(nn.Linear):
+    """fp8: a plain attribute (not a parameter or buffer, so the state_dict is unchanged). True runs the layer's training calls on
+    the FP8 kernels (ops.linear: only calls that record an autograd graph, only where ops.linear_fp8_on holds); every other call
+    runs exactly as with False. MakeAScene(fp8_linear=True) sets it on the four Linear layers of every TransformerLayer."""
+    fp8 = False
+
     def forward(self, x):
-        return ops.LinearFn.apply(x, self.weight, self.bias)
+        return ops.linear(x, self.weight, self.bias, self.fp8)
 
 
 def _drop_p(mod):
@@ -139,8 +144,11 @@ class TransformerLayer(nn.Module):
 class Transformer(nn.Module):
     def __init__(self, num_layers, hidden_dim, num_attn_heads, image_tokens_per_dim, seg_tokens_per_dim, text_length,
                  attn_dropout_prop=0, out_dropout_prob=0, cogview_pb_relax=True, cogview_sandwich_layernorm=True,
-                 cogview_layernorm_prescale=False, rudalle_relax=False, recompute_attention=False):
+                 cogview_layernorm_prescale=False, rudalle_relax=False, recompute_attention=False, fp8_linear=False):
+        """fp8_linear: see MakeAScene."""
         super().__init__()
+        if not isinstance(fp8_linear, bool):
+            raise ValueError("fp8_linear must be a bool, got %r" % (fp8_linear,))
         self.num_layers = num_layers
         self.cogview_pb_relax = cogview_pb_relax
         self.rudalle_relax = rudalle_relax
@@ -148,6 +156,9 @@ class Transformer(nn.Module):
             TransformerLayer(hidden_dim, num_attn_heads, attn_dropout_prop, out_dropout_prob, cogview_pb_relax,
                              cogview_sandwich_layernorm, cogview_layernorm_prescale, rudalle_relax, recompute_attention)
             for _ in range(num_layers)])
+        for layer in self.layers:
+            for lin in (layer.attn.qkv, layer.attn.out_proj, layer.mlp.lin1, layer.mlp.lin2):
+                lin.fp8 = fp8_linear
         self.register_buffer("mask", self._create_mask(text_length, seg_tokens_per_dim, image_tokens_per_dim))
         self.final_ln = LayerNorm(hidden_dim, eps=1e-5)
 
@@ -291,14 +302,20 @@ class _GraphedDecoder:
 class MakeAScene(nn.Module):
     def __init__(self, num_layers, hidden_dim, num_attn_heads, image_vocab_size, seg_vocab_size, text_vocab_size,
                  image_tokens_per_dim, seg_tokens_per_dim, text_length, attn_dropout_prob=0.0, out_dropout_prob=0.0,
-                 recompute_attention=False):
+                 recompute_attention=False, fp8_linear=False):
         """The reference's arguments, plus the dropout probabilities of every layer's attention probabilities
         (attn_dropout_prob) and of its attention and MLP outputs (out_dropout_prob), passed to Transformer; the reference's
         MakeAScene leaves both at 0, which the defaults keep.
         recompute_attention=True: training stores no attention probabilities (S x S per head and sequence) for the backward,
         which recomputes them from per-row statistics; the loss is the same bits, the gradients agree to fp32 rounding.
         Needs head dim 64 or 128 and a sequence length that is a multiple of 128 (RuntimeError otherwise). Not a parameter or
-        buffer: the state_dict is unchanged."""
+        buffer: the state_dict is unchanged.
+        fp8_linear=True: the four Linear layers of every TransformerLayer (attn.qkv, attn.out_proj, mlp.lin1, mlp.lin2) train on
+        FP8 tensor cores: e4m3 activations and weights, e5m2 output gradients, one power-of-two scale per tensor from its exact
+        max|.| on the device (DESIGN §3.5). It sets the plain attribute `fp8` of those modules (setting `lin.fp8` by hand toggles
+        one layer; the state_dict is unchanged). Only calls that record an autograd graph take the FP8 route, so generate, score
+        and no-grad forwards return the same bits as with the flag off. to_logits, the embeddings, the LayerNorms and attention
+        stay as they are. With the TF32 operand format or MAS_LINEAR_F16=0 the flag has no effect. ValueError unless a bool."""
         super().__init__()
         self.image_tokens_per_dim = image_tokens_per_dim
         self.seg_tokens_per_dim = seg_tokens_per_dim
@@ -309,7 +326,8 @@ class MakeAScene(nn.Module):
         self.text_vocab_size = text_vocab_size
         self.hidden_dim = hidden_dim
         self.transformer = Transformer(num_layers, hidden_dim, num_attn_heads, image_tokens_per_dim, seg_tokens_per_dim, text_length,
-                                       attn_dropout_prob, out_dropout_prob, recompute_attention=recompute_attention)
+                                       attn_dropout_prob, out_dropout_prob, recompute_attention=recompute_attention,
+                                       fp8_linear=fp8_linear)
         self.image_token_embedding = nn.Embedding(image_vocab_size, hidden_dim)
         self.seg_token_embedding = nn.Embedding(seg_vocab_size, hidden_dim)
         self.text_token_embedding = nn.Embedding(text_vocab_size, hidden_dim)
